@@ -105,7 +105,8 @@ int se2gpu_orb_level_dims(se2gpu_orb* h, int level, int* w, int* hgt, int* pitch
 int se2gpu_orb_get_level(se2gpu_orb* h, int frame, int level, int blurred, uint8_t* out);
 
 /* per-kernel device timing (CUDA events on the launching stream) for bench.py's roofline line.
- * groups: 0 pyramid (orb_pyr0 + orb_resize), 1 orb_fast_cells, 2 orb_select, 3 orb_blur, 4 orb_orient_describe.
+ * groups: 0 pyramid (orb_pyr0 + orb_resize_w), 1 FAST (orb_fast_cells or orb_fast_cells_big), 2 orb_select, 3 orb_blur,
+ * 4 orb_orient_describe.
  * enable!=0 starts/restarts accumulation; read returns accumulated milliseconds and launch counts per group
  * (synchronises the events it reads). */
 #define SE2GPU_ORB_PROFILE_GROUPS 5

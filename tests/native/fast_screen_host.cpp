@@ -1,9 +1,11 @@
-// Host check of se2lam_b200/csrc/fast_screen.h — the source pass A of orb_fast_cells_tma8 is compiled from — with the
+// Host check of se2lam_b200/csrc/fast_screen.h — the source pass A of orb_fast_cells is compiled from — with the
 // packed-SIMD instructions emulated:
 //   1. screen4 == the scalar definition of the FAST-9-16 quick reject, per pixel, for random and extreme patches
 //   2. the screen never rejects a true FAST corner (scalar 9-contiguous-arc definition, cv::FAST [upstream OpenCV fast.cpp])
-//   3. a CTA's pass A simulated thread by thread (ItemWalk, inside_mask8, seg_offset, the kernel's word addressing): every
-//      interior pixel of a cell is screened exactly once, the warps' list segments neither overlap nor overflow
+//   3. a CTA's pass A simulated warp by warp (ItemWalk, group addressing, inside_mask8, warp scan + shared counter), for the TMA
+//      layout (pitch = box width, shift 0..15) and the plain-load layout (pitch rounded up to 4 B, shift 0..3): every interior
+//      pixel of a cell is screened exactly once, the candidate set equals the scalar screen, list entries stay below cw*ch
+//      slots and decode to their pixel, and no read leaves the patch
 // Prints "OK <checks>" and exits 0, or a diagnostic and exits 1.
 #include <cstdio>
 #include <cstdlib>
@@ -72,94 +74,100 @@ int main() {
             ++checks;
         }
     }
-    // ---- inside_mask8, exhaustively over the argument range the kernels produce (every alignment shift of the TMA box)
+    // ---- inside_mask8 and the group distribution, exhaustively over the argument range the kernel produces (every alignment shift)
     for (int shift = 0; shift < 16; ++shift)
         for (int cw = 1; cw <= 300; ++cw) {
             std::vector<int> seen(cw, 0);
-            for (int h = 0; h < fastpx::pairs_per_row(cw, shift); ++h) {
-                const int x0 = fastpx::pair_x0(h, shift);
-                if (x0 > cw - 1 || x0 < -7) FAIL("pair %d of a %d px row (shift %d) starts at %d", h, cw, shift, x0);
-                unsigned want = 0;
-                for (int j = 0; j < 8; ++j) if (x0 + j >= 0 && x0 + j < cw) { want |= 1u << j; seen[x0 + j]++; }
-                if (fastpx::inside_mask8(x0, cw) != want) FAIL("inside_mask8(%d, %d) = %x, want %x", x0, cw, fastpx::inside_mask8(x0, cw), want);
-                ++checks;
-            }
-            for (int x = 0; x < cw; ++x) if (seen[x] != 1) FAIL("pairs cover pixel %d of %d (shift %d) %d times", x, cw, shift, seen[x]);
-            std::fill(seen.begin(), seen.end(), 0);
             for (int g = 0; g < fastpx::groups_per_row(cw, shift); ++g) {
                 const int x0 = fastpx::group_x0(g, shift);
                 if (x0 > cw - 1 || x0 < -3) FAIL("group %d of a %d px row (shift %d) starts at %d", g, cw, shift, x0);
                 const unsigned m = fastpx::inside_mask8(x0, cw) & 0xFu;
                 for (int j = 0; j < 4; ++j) { const bool in = x0 + j >= 0 && x0 + j < cw; if ((((m >> j) & 1u) != 0) != in) FAIL("group mask"); if (in) seen[x0 + j]++; }
+                ++checks;
             }
             for (int x = 0; x < cw; ++x) if (seen[x] != 1) FAIL("groups cover pixel %d of %d (shift %d) %d times", x, cw, shift, seen[x]);
         }
-    // ---- 3: pass A of one CTA (256 threads = 8 warps), simulated thread by thread exactly as the kernel addresses the patch
+    // ---- 3: pass A of one CTA (256 threads = 8 warps), simulated warp by warp exactly as the kernel addresses the patch. Warps run
+    // their 32-item chunks in any interleaving; here chunk k of every warp runs before chunk k+1 of any.
     const int NT = 256, NW = 8;
-    const int sizes[][2] = {{122, 75}, {101, 62}, {103, 61}, {85, 50}, {93, 50}, {75, 41}, {61, 33}, {49, 26}, {1, 1}, {5, 3}, {6, 9}, {230, 225}, {250, 249}, {7, 200}, {13, 1}, {229, 17}};
-    int cell_no = 0;
+    const int sizes[][2] = {{122, 75}, {101, 62}, {103, 61}, {85, 50}, {93, 50}, {75, 41}, {61, 33}, {49, 26}, {1, 1}, {5, 3}, {6, 9},
+                            {230, 225}, {250, 249}, {7, 200}, {13, 1}, {229, 17}, {312, 99}, {300, 150}};
+    for (int tma = 0; tma < 2; ++tma)
     for (const auto& sz : sizes) {
-      for (int rep = 0; rep < 4; ++rep) {
+      for (int shift = 0; shift < (tma ? 16 : 4); ++shift) {   // alignment shift of the patch start
         const int cw = sz[0], ch = sz[1];
-        const int shift = (cell_no++ * 7 + rep * 5) % 16;                       // alignment shift of the TMA box start
-        const int pw = (shift + cw + 6 + 15) & ~15, pww = pw / 4, bh = ch + 6 + (int)(rng() % 3);
-        if ((size_t)pw * bh > 65535 || pw > 256 || bh > 256) continue;   // the library takes such cells to orb_fast_cells / _big (16-bit list entries, box <= 256 x 256)
-        std::vector<uint8_t> smem((size_t)pw * bh + 4096, 0xAB);   // bytes behind the patch = the kernel's score plane (garbage to pass A)
-        for (int y = 0; y < bh; ++y) for (int x = 0; x < pw; ++x) smem[(size_t)y * pw + x] = (uint8_t)((((x / 5) ^ (y / 4)) & 1) * 60 + 80 + (int)(rng() % 25));
-        const uint8_t* patch = smem.data();
-        const uint8_t* p0 = patch + 3 * pw + 3 + shift;
+        // patch pitch and rows as orb_fast_cells<TMA> derives them; the TMA box is the level's widest x tallest patch, so it may
+        // have more columns and rows than this cell needs
+        const int pw = tma ? ((shift + cw + 6 + 15) & ~15) + 16 * (int)(rng() % 2) : (shift + cw + 6 + 3) & ~3, pww = pw / 4;
+        const int ph = tma ? ch + 6 + (int)(rng() % 3) : ch + 6;
+        if ((size_t)pw * ph > 65535 || (tma && (pw > 256 || ph > 256))) continue;   // the library takes such cells to orb_fast_cells<false> / _big
+        std::vector<uint8_t> patch((size_t)pw * ph);
+        for (int y = 0; y < ph; ++y) for (int x = 0; x < pw; ++x) patch[(size_t)y * pw + x] = (uint8_t)((((x / 5) ^ (y / 4)) & 1) * 60 + 80 + (int)(rng() % 25));
+        const uint8_t* p0 = patch.data() + 3 * pw + 3 + shift;
         const int t = 20;
-        const int h0 = fastpx::first_pair(shift), G2 = fastpx::pairs_per_row(cw, shift), nitems = ch * G2;
+        const unsigned T1 = fastpx::screen_T1(t), U1 = fastpx::screen_U1(t);
+        const int g0 = fastpx::first_group(shift), G = fastpx::groups_per_row(cw, shift), nitems = ch * G;
+        const long nwords_patch = (long)pww * ph;
+        bool read_outside = false;
+        auto ld = [&](long word) { if (word < 0 || word >= nwords_patch) { read_outside = true; return 0u; } return ldw(patch.data(), word); };
         std::vector<int> visited((size_t)cw * ch, 0), cand((size_t)cw * ch, 0);
-        std::vector<int> owner((size_t)8 * nitems, -1);
-        std::vector<int> nseg(NW, 0);
-        for (int tid = 0; tid < NT; ++tid) {
-            const int wid = tid / 32, lane = tid % 32;
-            fastpx::ItemWalk it;
-            it.init(tid, NT, G2);
-            const int seg = fastpx::seg_offset(wid, nitems, NW);
-            for (int it0 = wid * 32; it0 < nitems; it0 += NW * 32) {
-                const bool active = it.y < ch;
-                if (active != (it0 + lane < nitems)) FAIL("activity test differs from the item bound (cw %d ch %d tid %d)", cw, ch, tid);
-                if (active) {
-                    if (it.y * G2 + it.h != it0 + lane) FAIL("ItemWalk left its item sequence (cw %d ch %d tid %d)", cw, ch, tid);
-                    const int x0 = fastpx::pair_x0(it.h, shift);
-                    const long cp = (long)(it.y + 3) * pww + 2 * (it.h + h0);
-                    if (cp & 1) FAIL("odd word index for a 64-bit load");
-                    const uint32_t n3x = ldw(patch, cp - 3 * pww), n3y = ldw(patch, cp - 3 * pww + 1), s3x = ldw(patch, cp + 3 * pww), s3y = ldw(patch, cp + 3 * pww + 1);
-                    const uint32_t n2x = ldw(patch, cp - 2 * pww), n2y = ldw(patch, cp - 2 * pww + 1), s2x = ldw(patch, cp + 2 * pww), s2y = ldw(patch, cp + 2 * pww + 1);
-                    const uint32_t zx = ldw(patch, cp), zy = ldw(patch, cp + 1);
-                    const uint32_t n2l = ldw(patch, cp - 2 * pww - 1), n2r = ldw(patch, cp - 2 * pww + 2), s2l = ldw(patch, cp + 2 * pww - 1), s2r = ldw(patch, cp + 2 * pww + 2);
-                    const uint32_t zl = ldw(patch, cp - 1), zr = ldw(patch, cp + 2);
-                    if (4 * (cp + 3 * pww + 1) + 4 > (long)smem.size() || cp - 3 * pww < 0) FAIL("pass A reads outside shared memory");
-                    unsigned m = fastpx::screen4(n3x, s3x, n2l, n2x, n2y, s2l, s2x, s2y, zl, zx, zy, fastpx::screen_T1(t), fastpx::screen_U1(t)) |
-                                 fastpx::screen4(n3y, s3y, n2x, n2y, n2r, s2x, s2y, s2r, zx, zy, zr, fastpx::screen_T1(t), fastpx::screen_U1(t)) << 4;
-                    const unsigned in = fastpx::inside_mask8(x0, cw);
-                    for (int j = 0; j < 8; ++j) if ((in >> j) & 1u) visited[(size_t)it.y * cw + x0 + j]++;
-                    m &= in;
-                    const int e0 = it.y * pw + x0;
-                    while (m) {
-                        const int j = __builtin_ffs((int)m) - 1;
-                        m &= m - 1;
+        std::vector<int> list((size_t)cw * ch, -1);
+        int ncand = 0;                                  // the kernel's shared counter s_ncand
+        std::vector<fastpx::ItemWalk> walk(NT);
+        for (int tid = 0; tid < NT; ++tid) walk[tid].init(tid, NT, G);
+        for (int it0c = 0; it0c < nitems; it0c += NW * 32)
+            for (int wid = 0; wid < NW; ++wid) {
+                const int it0 = it0c + wid * 32;
+                if (it0 >= nitems) break;               // the warp's loop has ended (it0 < nitems is warp-uniform)
+                unsigned m[32];
+                int col0[32], y[32];
+                for (int lane = 0; lane < 32; ++lane) {
+                    fastpx::ItemWalk& it = walk[wid * 32 + lane];
+                    m[lane] = 0;
+                    col0[lane] = fastpx::group_x0(it.g, shift);
+                    y[lane] = it.y;
+                    const bool active = it.y < ch;
+                    if (active != (it0 + lane < nitems)) FAIL("activity test differs from the item bound (cw %d ch %d tid %d)", cw, ch, wid * 32 + lane);
+                    if (active) {
+                        if (it.y * G + it.g != it0 + lane) FAIL("ItemWalk left its item sequence (cw %d ch %d tid %d)", cw, ch, wid * 32 + lane);
+                        const long c = (long)(it.y + 3) * pww + it.g + g0;
+                        m[lane] = fastpx::screen4(ld(c - 3 * pww), ld(c + 3 * pww), ld(c - 2 * pww - 1), ld(c - 2 * pww), ld(c - 2 * pww + 1),
+                                                  ld(c + 2 * pww - 1), ld(c + 2 * pww), ld(c + 2 * pww + 1), ld(c - 1), ld(c), ld(c + 1), T1, U1);
+                        if (read_outside) FAIL("pass A reads outside the patch (cw %d ch %d shift %d tma %d)", cw, ch, shift, tma);
+                        const unsigned in = fastpx::inside_mask8(col0[lane], cw) & 0xFu;
+                        for (int j = 0; j < 4; ++j) if ((in >> j) & 1u) visited[(size_t)it.y * cw + col0[lane] + j]++;
+                        m[lane] &= in;
+                    }
+                    it.next();
+                }
+                // warp scan of the survivor counts, one atomicAdd on the shared counter, then each lane writes its survivors
+                int inc[32], run = 0;
+                for (int lane = 0; lane < 32; ++lane) { run += __builtin_popcount(m[lane]); inc[lane] = run; }
+                if (run == 0) continue;
+                const int base0 = ncand;
+                ncand += run;
+                for (int lane = 0; lane < 32; ++lane) {
+                    int base = base0 + inc[lane] - __builtin_popcount(m[lane]);
+                    const int e0 = y[lane] * pw + col0[lane];
+                    for (unsigned mm = m[lane]; mm; mm &= mm - 1) {
+                        const int j = __builtin_ffs((int)mm) - 1;
                         const int off = e0 + j;
-                        if (off < 0 || off > 65535 || off % pw != x0 + j || off / pw != it.y) FAIL("bad list entry");
-                        cand[(size_t)it.y * cw + x0 + j] = 1;
-                        const int slot = seg + nseg[wid]++;
-                        if (slot >= 8 * nitems) FAIL("list overflow");
-                        if (owner[slot] != -1) FAIL("segments of warps %d and %d overlap", owner[slot], wid);
-                        owner[slot] = wid;
+                        if (off < 0 || off > 65535 || off % pw != col0[lane] + j ||off / pw != y[lane]) FAIL("bad list entry");
+                        if (base >= cw * ch) FAIL("list overflow: slot %d of %d (cw %d ch %d)", base, cw * ch, cw, ch);
+                        if (list[base] != -1) FAIL("list slot %d written twice", base);
+                        list[base++] = off;
+                        cand[(size_t)y[lane] * cw + col0[lane] + j] = 1;
                     }
                 }
-                it.next();
             }
-        }
-        for (int w = 0; w + 1 < NW; ++w)
-            if (fastpx::seg_offset(w, nitems, NW) + nseg[w] > fastpx::seg_offset(w + 1, nitems, NW)) FAIL("segment of warp %d overflows into the next one", w);
+        int nlisted = 0;
+        for (int v : list) nlisted += v >= 0;
+        if (nlisted != ncand) FAIL("%d list entries for a counter of %d", nlisted, ncand);
         for (int y = 0; y < ch; ++y)
             for (int x = 0; x < cw; ++x) {
                 if (visited[(size_t)y * cw + x] != 1) FAIL("pixel (%d,%d) of a %dx%d cell screened %d times", x, y, cw, ch, visited[(size_t)y * cw + x]);
                 const bool want = scalar_screen(p0 + y * pw + x, pw, t);
-                if ((cand[(size_t)y * cw + x] != 0) != want) FAIL("candidate set differs at (%d,%d) of a %dx%d cell", x, y, cw, ch);
+                if ((cand[(size_t)y * cw + x] != 0) != want) FAIL("candidate set differs at (%d,%d) of a %dx%d cell (tma %d)", x, y, cw, ch, tma);
                 ++checks;
             }
       }

@@ -153,13 +153,19 @@ def test_warp_nth_element_matches_std_nth_element():
 
 def test_hd_frame_big_cells():
     """1920x1080 with 1000 features has 470 x 150 px grid cells: too large for the compacting FAST kernel's shared-memory
-    candidate list, so the one-thread-per-pixel fallback kernel runs; results must still be bit-exact."""
+    candidate list, so the one-thread-per-pixel fallback kernel runs; results must still be bit-exact. 1280x720 with 1000
+    features (level-0 cells 312 x 99 px) exceeds the 256 px TMA box and takes the plain-load instantiation of the compacting
+    kernel; 1024x768 with 1500 features takes its TMA instantiation."""
     img = synth.orb_frame(4242, 1920, 1080)
     ext = ORBextractor(1000, 1.2, 8, fastTh=20, max_width=1920, max_height=1080, max_batch=1)
     kg, dg = ext(img)
     ko, do_ = pyoracle.OrbOracle(1000, 1.2, 8, 20).extract(img)
     assert_same(kg, dg, ko, do_, "1080p")
-    # and a frame size in between, which still takes the compacting kernel
+    img1 = synth.orb_frame(4244, 1280, 720)
+    ext1 = ORBextractor(1000, 1.2, 8, fastTh=20, max_width=1280, max_height=720, max_batch=1)
+    kg1, dg1 = ext1(img1)
+    ko1, do1 = pyoracle.OrbOracle(1000, 1.2, 8, 20).extract(img1)
+    assert_same(kg1, dg1, ko1, do1, "720p")
     img2 = synth.orb_frame(4243, 1024, 768)
     ext2 = ORBextractor(1500, 1.2, 8, fastTh=20, max_width=1024, max_height=768, max_batch=1)
     kg2, dg2 = ext2(img2)
