@@ -25,6 +25,7 @@
 #include <cstring>
 #include <vector>
 
+#include "blur_px.h"
 #include "common.h"
 #include "fast_screen.h"
 #include "introselect.h"
@@ -39,7 +40,8 @@ constexpr int PATCH = 31;          // PATCH_SIZE :81
 constexpr int MAX_LEVELS = 16;
 constexpr int FAST_THREADS = 256;
 constexpr int ORB_LANES = 4;
-constexpr int BLUR_TW = 128, BLUR_TH = 36;   // one warp per tile; BLUR_TH + 6 warm-up rows = 6 turns of the 7-row ring
+constexpr int BLUR_WARPS = 4;      // warps (tiles) per orb_blur CTA
+constexpr int BLUR_TH = 48;        // ROI rows per orb_blur strip, before rounding to the 7-row ring (build_geometry)
 
 __device__ const signed char d_pattern[1024] = {
 #include "orb_pattern_31.inc"
@@ -56,7 +58,8 @@ struct LevelGeo {
     int kp_off, kp_cap; // slot range in the per-frame level keypoint buffer
     float scale, kp_size;
     int tab_off;        // offset of this level's resize tables (xofs | yofs) in the int table
-    int tile_base, tiles_x, tiles_y;
+    int tile_base;      // first orb_blur tile of this level
+    int blur_th, blur_strips;   // orb_blur: ROI rows per strip, strips (the last one ends at the ROI's last row)
     int fbw, fbh;       // orb_fast_cells<true>: TMA box of this level's FAST cells (bytes per row: multiple of 16; rows)
 };
 
@@ -66,7 +69,7 @@ struct CellGeo {
     int cand_off, cand_cap;     // slot range in the per-frame candidate buffer
 };
 
-struct TileGeo { int level, x0, y0; };  // blur tile origin in bordered-plane coordinates
+struct TileGeo { int level, strip, cg; };  // orb_blur warp: its first (strip, column group of 8 bytes) item; lane j takes the j-th item after it
 
 struct CellHdr { int n_base, n_a, n_b, pad; };
 
@@ -818,79 +821,90 @@ __global__ void __launch_bounds__(128) orb_debug_nth(uint32_t* v, const int* __r
 
 // GaussianBlur 7x7 sigma 2 on the level ROI; the 16 px ring keeps its un-blurred reflect-101 copies.
 // cv::GaussianBlur's float arithmetic: row pass = sequential fmaf over the 7 taps, column pass = centre tap then the
-// three symmetric pairs, round-to-nearest-even, saturate. No shared memory: a tile is one warp = 128 columns x
-// BLUR_TH output rows; a thread owns 4 adjacent columns (one output word) and walks down its strip with the last 7
-// row-pass results in a register ring, so every source word is loaded once per row (3 coalesced words per thread:
-// its own and both neighbours, the latter L1 hits) and every output row costs one 32-bit store.
-__global__ void __launch_bounds__(256) orb_blur(OrbDev d, int tile0, int tile_end) {
-    const int tile = tile0 + blockIdx.x * 8 + (threadIdx.x >> 5);
+// three symmetric pairs, round-to-nearest-even, saturate. No shared memory, so the CTAs co-reside with the resize and FAST CTAs.
+// A thread owns 8 adjacent columns (one column group) of one strip of ROI rows and walks down it with the last 7 row-pass results
+// in a register ring: per source row one 8-byte load of its columns and two 4-byte loads of the neighbouring bytes (L1 hits), per
+// output row one 8-byte store. A level's strips have one height (the last one is moved up to end at the ROI's last row, so a few
+// rows are blurred twice, with the same result); a warp takes 32 consecutive (strip, column group) items of one level, so lanes
+// idle only in a level's last warp. Only ROI rows are blurred: their 7-row windows and the neighbour words stay inside the
+// bordered plane (beyond a row's ends the neighbour word is the adjacent row's, which only feeds ring columns), so no row index is
+// clamped and no load is tested; the lanes of the first and the last strip copy the 16 ring rows above and below.
+// The kernel is issue bound: bytes become floats and rounded sums become bytes through the float bit patterns (blur_px.h), which
+// keeps it off the conversion pipe; 8 columns per thread share the 6 neighbour conversions of a row.
+__global__ void __launch_bounds__(BLUR_WARPS * 32, 4) orb_blur(OrbDev d, int tile0, int tile_end) {
+    const int tile = tile0 + blockIdx.x * BLUR_WARPS + (threadIdx.x >> 5);
     if (tile >= tile_end) return;
-    const int lane = threadIdx.x & 31;
     const TileGeo t = d.tiles[tile];
-    const int f = blockIdx.y + d.frame0;
-    const int pitch = d.levels[t.level].pitch, Lw = d.levels[t.level].w, Lh = d.levels[t.level].h, H = Lh + 2 * EDGE;
-    const int x4 = t.x0 + 4 * lane;
-    if (x4 >= pitch) return;
-    const size_t plane_off = f * d.frame_plane_bytes + d.levels[t.level].plane_off + x4;
-    const uint8_t* __restrict__ src = d.plain + plane_off;
-    uint8_t* __restrict__ dst = d.blurred + plane_off;
-    const bool has_l = x4 >= 4, has_r = x4 + 8 <= pitch;
-    uint32_t colmask = 0;          // 0xFF in the byte lanes of ROI columns
+    const LevelGeo& L = d.levels[t.level];
+    const int pitch = L.pitch, Lw = L.w, Lh = L.h, th = L.blur_th, strips = L.blur_strips, ncg = pitch / 8;
+    int s = t.strip, cg = t.cg + (threadIdx.x & 31);   // lane j: item j after the tile's first one, strip by strip
+    while (cg >= ncg) { cg -= ncg; ++s; }
+    if (s >= strips) return;
+    const int x8 = 8 * cg;
+    const size_t off = (size_t)(blockIdx.y + d.frame0) * d.frame_plane_bytes + L.plane_off + x8;
+    const uint8_t* __restrict__ src = d.plain + off;
+    uint8_t* __restrict__ dst = d.blurred + off;
+    if (s == 0)
+        for (int y = 0; y < EDGE; ++y) *reinterpret_cast<uint2*>(dst + (size_t)y * pitch) = __ldg(reinterpret_cast<const uint2*>(src + (size_t)y * pitch));
+    if (s == strips - 1)
+        for (int y = EDGE + Lh; y < Lh + 2 * EDGE; ++y) *reinterpret_cast<uint2*>(dst + (size_t)y * pitch) = __ldg(reinterpret_cast<const uint2*>(src + (size_t)y * pitch));
+    uint32_t m0 = 0, m1 = 0;       // 0xFF in the byte lanes of ROI columns
 #pragma unroll
-    for (int q = 0; q < 4; ++q) colmask |= (x4 + q >= EDGE && x4 + q < EDGE + Lw) ? (0xFFu << (8 * q)) : 0u;
-    const float g0 = c_gauss[0], g1 = c_gauss[1], g2 = c_gauss[2], g3 = c_gauss[3], g4 = c_gauss[4], g5 = c_gauss[5], g6 = c_gauss[6];
-    float hr[7][4];      // row-pass results of the last 7 source rows
-    uint32_t cw[7];      // their centre words (ring pixels are copied through)
-    // rows outside the plane only feed ring outputs (copies), so the row index is clamped instead of tested
-    auto row_ptr = [&](int i) { return src + (size_t)min(max(t.y0 - 3 + i, 0), H - 1) * pitch; };
-    uint32_t n0, n1, n2;  // words of the next source row (software prefetch, one row ahead)
-    {
-        const uint8_t* rp = row_ptr(0);
-        n1 = __ldg(reinterpret_cast<const uint32_t*>(rp));
-        n0 = has_l ? __ldg(reinterpret_cast<const uint32_t*>(rp - 4)) : 0u;
-        n2 = has_r ? __ldg(reinterpret_cast<const uint32_t*>(rp + 4)) : 0u;
+    for (int q = 0; q < 4; ++q) {
+        m0 |= (x8 + q >= EDGE && x8 + q < EDGE + Lw) ? (0xFFu << (8 * q)) : 0u;
+        m1 |= (x8 + 4 + q >= EDGE && x8 + 4 + q < EDGE + Lw) ? (0xFFu << (8 * q)) : 0u;
     }
-    for (int i0 = 0; i0 < BLUR_TH + 6; i0 += 7) {
+    const int y0 = EDGE + min(s * th, Lh - th);   // first output row of the strip
+    const uint8_t* rp = src + (size_t)(y0 - 3) * pitch;
+    uint8_t* wp = dst + (size_t)y0 * pitch;
+    float hr[7][8];      // row-pass results of the last 7 source rows
+    uint2 cw[7];         // their own 8 bytes (ring columns are copied through)
+    uint2 nc = __ldg(reinterpret_cast<const uint2*>(rp));     // the next source row (software prefetch, one row ahead)
+    uint32_t nl = __ldg(reinterpret_cast<const uint32_t*>(rp - 4)), nr = __ldg(reinterpret_cast<const uint32_t*>(rp + 8));
+    auto row = [&](const int k) {      // row pass of the next source row into ring slot k
+        const uint2 c = nc;
+        const uint32_t l = nl, r = nr;
+        rp += pitch;
+        nc = __ldg(reinterpret_cast<const uint2*>(rp));
+        nl = __ldg(reinterpret_cast<const uint32_t*>(rp - 4));
+        nr = __ldg(reinterpret_cast<const uint32_t*>(rp + 8));
+        float b[14];                    // bytes x8-3 .. x8+10
 #pragma unroll
-        for (int k = 0; k < 7; ++k) {
-            const int i = i0 + k;                       // source row t.y0 - 3 + i, kept in ring slot k
-            const uint32_t w0 = n0, w1 = n1, w2 = n2;
-            {
-                const uint8_t* rp = row_ptr(i + 1);
-                n1 = __ldg(reinterpret_cast<const uint32_t*>(rp));
-                n0 = has_l ? __ldg(reinterpret_cast<const uint32_t*>(rp - 4)) : 0u;
-                n2 = has_r ? __ldg(reinterpret_cast<const uint32_t*>(rp + 4)) : 0u;
-            }
-            float b[10];                                // bytes x4-3 .. x4+6
+        for (int j = 0; j < 3; ++j) b[j] = blurpx::byte_to_float(l, j + 1);
 #pragma unroll
-            for (int j = 0; j < 3; ++j) b[j] = (float)((w0 >> (8 * (j + 1))) & 255u);
+        for (int j = 0; j < 4; ++j) { b[3 + j] = blurpx::byte_to_float(c.x, j); b[7 + j] = blurpx::byte_to_float(c.y, j); }
 #pragma unroll
-            for (int j = 0; j < 4; ++j) b[3 + j] = (float)((w1 >> (8 * j)) & 255u);
+        for (int j = 0; j < 3; ++j) b[11 + j] = blurpx::byte_to_float(r, j);
 #pragma unroll
-            for (int j = 0; j < 3; ++j) b[7 + j] = (float)((w2 >> (8 * j)) & 255u);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                float s = __fmul_rn(g0, b[q]);
-                s = __fmaf_rn(g1, b[q + 1], s); s = __fmaf_rn(g2, b[q + 2], s); s = __fmaf_rn(g3, b[q + 3], s);
-                s = __fmaf_rn(g4, b[q + 4], s); s = __fmaf_rn(g5, b[q + 5], s); s = __fmaf_rn(g6, b[q + 6], s);
-                hr[k][q] = s;
-            }
-            cw[k] = w1;
-            const int gy = t.y0 + i - 6;                // output row whose 7-row window ends at source row i
-            if (i >= 6 && gy < H && gy < t.y0 + BLUR_TH) {
-                uint32_t word = 0;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    float sacc = __fmul_rn(g3, hr[(k + 4) % 7][q]);
-                    sacc = __fmaf_rn(g4, __fadd_rn(hr[(k + 5) % 7][q], hr[(k + 3) % 7][q]), sacc);
-                    sacc = __fmaf_rn(g5, __fadd_rn(hr[(k + 6) % 7][q], hr[(k + 2) % 7][q]), sacc);
-                    sacc = __fmaf_rn(g6, __fadd_rn(hr[k][q], hr[(k + 1) % 7][q]), sacc);
-                    word |= (uint32_t)min(max(__float2int_rn(sacc), 0), 255) << (8 * q);
-                }
-                const uint32_t m = (gy >= EDGE && gy < EDGE + Lh) ? colmask : 0u;
-                *reinterpret_cast<uint32_t*>(dst + (size_t)gy * pitch) = (word & m) | (cw[(k + 4) % 7] & ~m);   // centre word = source row i-3
-            }
+        for (int q = 0; q < 8; ++q) {
+            float a = __fmul_rn(c_gauss[0], b[q]);
+            a = __fmaf_rn(c_gauss[1], b[q + 1], a); a = __fmaf_rn(c_gauss[2], b[q + 2], a); a = __fmaf_rn(c_gauss[3], b[q + 3], a);
+            a = __fmaf_rn(c_gauss[4], b[q + 4], a); a = __fmaf_rn(c_gauss[5], b[q + 5], a); a = __fmaf_rn(c_gauss[6], b[q + 6], a);
+            hr[k][q] = a;
         }
+        cw[k] = c;
+    };
+    auto out = [&](const int k) {      // column pass of the output row whose 7-row window ends in slot k; centre row in slot (k + 4) % 7
+        unsigned o[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            float a = __fmul_rn(c_gauss[3], hr[(k + 4) % 7][q]);
+            a = __fmaf_rn(c_gauss[4], __fadd_rn(hr[(k + 5) % 7][q], hr[(k + 3) % 7][q]), a);
+            a = __fmaf_rn(c_gauss[5], __fadd_rn(hr[(k + 6) % 7][q], hr[(k + 2) % 7][q]), a);
+            a = __fmaf_rn(c_gauss[6], __fadd_rn(hr[k][q], hr[(k + 1) % 7][q]), a);
+            o[q] = blurpx::round_sat_bits(a);
+        }
+        const uint2 ctr = cw[(k + 4) % 7];
+        const uint32_t v0 = blurpx::pack_low_bytes(o[0], o[1], o[2], o[3]), v1 = blurpx::pack_low_bytes(o[4], o[5], o[6], o[7]);
+        *reinterpret_cast<uint2*>(wp) = make_uint2((v0 & m0) | (ctr.x & ~m0), (v1 & m1) | (ctr.y & ~m1));
+        wp += pitch;
+    };
+#pragma unroll
+    for (int k = 0; k < 7; ++k) row(k);   // source rows y0-3 .. y0+3
+    out(6);                                // output row y0
+    for (int i = 1; i < th; i += 7) {      // th - 1 is a multiple of 7 (build_geometry)
+#pragma unroll
+        for (int k = 0; k < 7; ++k) { row(k); out(k); }
     }
 }
 
@@ -1150,9 +1164,17 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
             }
         }
         ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 4 + (size_t)g.nCells * 16 + (size_t)SEL_STAGE * 4);
+        // orb_blur: at least 2 strips of at most about BLUR_TH rows, of one height: with its 6 warm-up rows a strip is a whole number
+        // of turns of the kernel's 7-row ring, and at most the ROI's height (h >= 39). A tile = 32 consecutive (strip, column group)
+        // items. The tile count grows with w and h, so the table sized at create time holds every smaller frame's.
+        // Strip height measured on an H100 SXM (400 W), 64 frames of 640x480, kernel alone: 0.093 ms per batch at BLUR_TH = 48 (and
+        // at 32), 0.096 at 64, 0.103 at 96, 0.114 at 128. Shorter strips make more, shorter warps and a shorter tail, although more
+        // lane-steps go to warm-up rows: at 48, 79 % of the lane-steps produce new pixels, 10 % are warm-up rows, 6 % rows blurred
+        // twice and 4 % idle lanes.
         g.tile_base = (int)T.size();
-        g.tiles_x = (g.w + 2 * EDGE + BLUR_TW - 1) / BLUR_TW; g.tiles_y = (g.h + 2 * EDGE + BLUR_TH - 1) / BLUR_TH;
-        for (int ty = 0; ty < g.tiles_y; ++ty) for (int tx = 0; tx < g.tiles_x; ++tx) T.push_back(TileGeo{l, tx * BLUR_TW, ty * BLUR_TH});
+        g.blur_strips = std::max(2, (g.h + BLUR_TH - 1) / BLUR_TH);
+        g.blur_th = ((g.h + g.blur_strips - 1) / g.blur_strips + 12) / 7 * 7 - 6;
+        for (int it = 0; it < g.blur_strips * (g.pitch / 8); it += 32) T.push_back(TileGeo{l, it / (g.pitch / 8), it % (g.pitch / 8)});
     }
     *plane_bytes = poff; *cand_total = coff; *n_cells = C.size(); *n_tiles = T.size(); *tab_total = toff;
     if (fsm > 227 * 1024) fast_big = true;
@@ -1185,7 +1207,11 @@ EncodeTiledFn tensor_map_encoder() {
 // a TMA kernel with 8-pixel items and per-warp candidate lists (whole step 0.72 ms against 0.74 / 0.76 ms); batched loads in
 // orb_orient_describe take it from 0.1045 to 0.097 ms against one dependent load pair per loop trip. The plain-load
 // instantiation stays for geometries whose cell patch exceeds a 256 x 256 TMA box and for drivers without the tensor-map encoder.
-constexpr int BLUR_SPLIT = 2;          // blur group A = levels [0, BLUR_SPLIT), started behind the pyramid tail (run_device)
+// Blur group A = levels [0, BLUR_SPLIT) on the side stream once its last level exists, the rest behind FAST (run_device). Measured with
+// this orb_blur (same card, 64 frames of 640x480, range over 2 runs of 200 steps): 0.697-0.698 ms per step at 1, 0.709-0.711 at 2,
+// 0.709-0.710 at 3. The blur now costs less than the resize tail it would hide behind, and level 0 alone next to FAST finishes
+// before FAST does, so the levels left for the selection's idle SMs are the ones that shorten the step most.
+constexpr int BLUR_SPLIT = 1;
 // host-buffer pipeline shape (orb_enqueue): se2gpu_orb_extract splits a batch into PIPE_CHUNKS chunks round-robin over all
 // pipeline lanes, the first PIPE_FIRST_PCT percent of an even share so that less of the initial H2D copy is exposed;
 // se2gpu_orb_submit already overlaps a batch with its twin's, so chunking a submitted batch would only add launches
@@ -1400,14 +1426,14 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
     if (splitA - 1 <= 0 && side && !pr.on) SE2_CUDA(cudaEventRecord(h->ev_l1, s));   // level 0 alone is group A (or there is only one level)
     pr.end(s);
     nvtxRangePop();
-    // The blur of a level only needs that level's plane: on the side stream the blur of levels 0-1 (55 % of the pixels,
-    // no shared memory, so it co-resides with the resize CTAs) starts as soon as level 1 exists and hides behind the
-    // tail of the pyramid, a chain of small latency-bound launches; the remaining levels are blurred behind the FAST launch,
+    // The blur of a level only needs that level's plane: on the side stream the blur of group A (no shared memory, so it co-resides
+    // with the resize and FAST CTAs) starts once its last level exists - with BLUR_SPLIT = 1 that is level 0 alone (about a third of
+    // the pixels), behind the whole pyramid, next to FAST; the remaining levels are blurred behind the FAST launch,
     // next to the selection. The main stream joins before the descriptors are sampled. With the
     // profiler on everything stays on one stream so that the per-kernel event times are not polluted by the overlap.
     const bool overlap = !pr.on && side != nullptr;
     auto launch_blur = [&](cudaStream_t st, int t0, int t1) {
-        if (t1 > t0) SE2_LAUNCH(orb_blur, dim3((t1 - t0 + 7) / 8, n), 256, 0, st, d, t0, t1);
+        if (t1 > t0) SE2_LAUNCH(orb_blur, dim3((t1 - t0 + BLUR_WARPS - 1) / BLUR_WARPS, n), BLUR_WARPS * 32, 0, st, d, t0, t1);
     };
     const int tilesA = splitA < h->nlevels ? h->levels[splitA].tile_base : d.n_tiles;
     if (overlap) {
