@@ -3,7 +3,8 @@ import numpy as np
 import pytest
 
 from oracle import pyoracle
-from tests.matcher_cases import brute_candidates, make_frame_pair, make_projection_case, make_bow_case, GRID
+from tests.matcher_cases import (GRID, UNDIST_BOUNDS, UNDIST_GRID, brute_candidates, grid_pos, half_cell_coords, make_bow_case,
+                                 make_frame_pair, make_grid_edge_pair, make_projection_case, make_projection_edge_case)
 
 
 def test_descriptor_distance_is_popcount():
@@ -13,16 +14,13 @@ def test_descriptor_distance_is_popcount():
         assert pyoracle.descriptor_distance(a, b) == int(np.unpackbits(a ^ b).sum())
 
 
-def test_match_by_window_against_bruteforce():
-    f1, f2, prev = make_frame_pair(seed=1)
-    n, m, prev_out = pyoracle.match_by_window(f1["kp"], f1["desc"], f2["kp"], f2["desc"], prev, GRID, 20, 1, 0, 8, 0.9)
-    # brute-force greedy with the same semantics, candidates from an explicit grid walk
-    kp1, kp2, d1, d2 = f1["kp"], f2["kp"], f1["desc"], f2["desc"]
+def brute_match_by_window(kp1, d1, kp2, d2, prev, grid, win, ratio):
+    """Brute-force greedy MatchByWindow with the reference's semantics, candidates from an explicit grid walk."""
     vdist = np.full(len(kp2), np.iinfo(np.int32).max, np.int64); m21 = -np.ones(len(kp2), int); m12 = -np.ones(len(kp1), int)
     hist = [[] for _ in range(30)]
     for i1 in range(len(kp1)):
         lvl = int(kp1["octave"][i1])
-        cand = brute_candidates(kp2, prev[i1, 0], prev[i1, 1], 20.0, max(lvl - 1, 0), lvl + 1)
+        cand = brute_candidates(kp2, prev[i1, 0], prev[i1, 1], win, max(lvl - 1, 0), lvl + 1, grid)
         best = best2 = 1 << 31; bi = -1
         for i2 in cand:
             dist = int(np.unpackbits(d1[i1] ^ d2[i2]).sum())
@@ -32,7 +30,7 @@ def test_match_by_window_against_bruteforce():
                 best2, best, bi = best, dist, i2
             elif dist < best2:
                 best2 = dist
-        if best <= 75 and best < np.float32(best2) * np.float32(0.9):
+        if best <= 75 and best < np.float32(best2) * np.float32(ratio):
             if m21[bi] >= 0:
                 m12[m21[bi]] = -1
             m12[i1] = bi; m21[bi] = i1; vdist[bi] = best
@@ -52,10 +50,19 @@ def test_match_by_window_against_bruteforce():
         if b not in top:
             for i1 in hist[b]:
                 m12[i1] = -1
-    assert n == int((m12 >= 0).sum()) and n > 50
-    np.testing.assert_array_equal(m, m12)
+    prev_out = prev.copy()
     for i1 in np.flatnonzero(m12 >= 0):
-        assert prev_out[i1, 0] == kp2["x"][m12[i1]] and prev_out[i1, 1] == kp2["y"][m12[i1]]
+        prev_out[i1] = kp2["x"][m12[i1]], kp2["y"][m12[i1]]
+    return int((m12 >= 0).sum()), m12, prev_out
+
+
+def test_match_by_window_against_bruteforce():
+    f1, f2, prev = make_frame_pair(seed=1)
+    n, m, prev_out = pyoracle.match_by_window(f1["kp"], f1["desc"], f2["kp"], f2["desc"], prev, GRID, 20, 1, 0, 8, 0.9)
+    n_b, m12, prev_b = brute_match_by_window(f1["kp"], f1["desc"], f2["kp"], f2["desc"], prev, GRID, 20.0, 0.9)
+    assert n == n_b and n > 50
+    np.testing.assert_array_equal(m, m12)
+    np.testing.assert_array_equal(prev_out, prev_b)
 
 
 def _popcount(a, b):
@@ -74,12 +81,9 @@ def _keep_top3_bins(hist):
     return top
 
 
-@pytest.mark.parametrize("seed", [2, 7, 11])
-def test_match_by_projection_against_bruteforce(seed):
+def brute_match_by_projection(a):
     """Independent numpy restatement of ORBmatcher::MatchByProjection (ORBmatcher.cpp:383-454): explicit grid walk for
     GetFeaturesInArea, window = mMainOctave * winSize (0 px for octave 0), same-level ratio rule, TH_HIGH, steal."""
-    a = make_projection_case(seed=seed)["args"]
-    n, m = pyoracle.match_by_projection(**a)
     kp, desc = a["kfkp"], a["kfdesc"]
     ratio = np.float32(a["nnratio"])
     INT_MAX = np.iinfo(np.int32).max
@@ -91,7 +95,8 @@ def test_match_by_projection_against_bruteforce(seed):
             continue
         pl = int(a["mp_octave"][i])
         lo = a["level_offset"]
-        cand = brute_candidates(kp, a["mp_uv"][i, 0], a["mp_uv"][i, 1], float(pl * a["win_size"]), pl - lo if pl > lo else 0, pl + lo)
+        cand = brute_candidates(kp, a["mp_uv"][i, 0], a["mp_uv"][i, 1], float(pl * a["win_size"]), pl - lo if pl > lo else 0, pl + lo,
+                                a["grid"])
         if not cand:
             continue
         best = best2 = INT_MAX
@@ -113,9 +118,66 @@ def test_match_by_projection_against_bruteforce(seed):
             if out[bi] >= 0:
                 out[bi] = -1; nm -= 1
             out[bi] = i; vdist[bi] = best; nm += 1
+    return nm, out
+
+
+@pytest.mark.parametrize("seed", [2, 7, 11])
+def test_match_by_projection_against_bruteforce(seed):
+    a = make_projection_case(seed=seed)["args"]
+    n, m = pyoracle.match_by_projection(**a)
+    nm, out = brute_match_by_projection(a)
     assert n == nm and n > 20
     np.testing.assert_array_equal(m, out)
     assert not np.any(a["kf_observed"].astype(bool) & (m >= 0))
+
+
+def test_grid_pos_rounds_half_away_from_zero():
+    """PosInGrid uses C++ round() of the float32 product: -0.5 cells -> -1 (outside), 1.5 -> 2, 2.5 -> 3 (round-half-even would
+    give 2), 63.5 -> 64 and 47.5 -> 48 (outside)."""
+    minX, minY, invW, invH = UNDIST_GRID
+    hx = half_cell_coords(minX, invW, [-0.5, 1.5, 2.5, 63.5])
+    hy = half_cell_coords(minY, invH, [-0.5, 2.5, 47.5])
+    kp = np.zeros(len(hx) + len(hy), pyoracle.KP_DTYPE)
+    kp["x"][:len(hx)], kp["y"][:len(hx)] = list(hx.values()), minY + 100
+    kp["x"][len(hx):], kp["y"][len(hx):] = minX + 100, list(hy.values())
+    px, py, inside = grid_pos(kp, UNDIST_GRID)
+    np.testing.assert_array_equal(px[:len(hx)], [int(np.floor(h)) + 1 if h > 0 else -1 for h in hx])
+    np.testing.assert_array_equal(py[len(hx):], [int(np.floor(h)) + 1 if h > 0 else -1 for h in hy])
+    assert list(inside) == [h not in (-0.5, 63.5) for h in hx] + [h not in (-0.5, 47.5) for h in hy]
+    assert set(hx) == {-0.5, 1.5, 2.5, 63.5} and set(hy) == {-0.5, 2.5, 47.5}
+
+
+@pytest.mark.parametrize("seed", [21, 23])
+def test_match_by_window_against_bruteforce_on_grid_edges(seed):
+    """Non-zero origin, non-round cells (undistorted bounds), keypoints outside the grid and on half cells, windows outside."""
+    f1, f2, prev, q = make_grid_edge_pair(seed=seed)
+    kp2 = f2["kp"]
+    _, _, inside = grid_pos(kp2, UNDIST_GRID)
+    assert (kp2["x"] < 0).any() and (kp2["x"] >= UNDIST_BOUNDS[2]).any() and (kp2["y"] >= UNDIST_BOUNDS[3]).any() and (~inside).sum() > 50
+    for i in q["empty"]:
+        assert brute_candidates(kp2, prev[i, 0], prev[i, 1], 20.0, -1, -1, UNDIST_GRID) == []
+    n, m, prev_out = pyoracle.match_by_window(f1["kp"], f1["desc"], kp2, f2["desc"], prev, UNDIST_GRID, 20, 1, 0, 8, 0.9)
+    n_b, m12, prev_b = brute_match_by_window(f1["kp"], f1["desc"], kp2, f2["desc"], prev, UNDIST_GRID, 20.0, 0.9)
+    assert n == n_b and n > 300
+    np.testing.assert_array_equal(m, m12)
+    np.testing.assert_array_equal(prev_out, prev_b)
+    assert inside[m[m >= 0]].all()            # nothing outside the grid is ever matched
+    assert (m[q["empty"]] == -1).all()
+
+
+@pytest.mark.parametrize("seed", [22, 24])
+def test_match_by_projection_against_bruteforce_on_grid_edges(seed):
+    c = make_projection_edge_case(seed=seed)
+    a = c["args"]
+    n, m = pyoracle.match_by_projection(**a)
+    nm, out = brute_match_by_projection(a)
+    assert n == nm and n > 150
+    np.testing.assert_array_equal(m, out)
+    _, _, inside = grid_pos(a["kfkp"], a["grid"])
+    assert inside[m >= 0].all()
+    # the grid walk's order decides every tie: the lower index B, visited first, takes the map point
+    for (b, a_), mp in zip(c["ties"], c["tie_mps"]):
+        assert m[b] == mp and m[a_] == -1, (b, a_, mp)
 
 
 @pytest.mark.parametrize("seed,mp_only,ori", [(3, True, True), (8, False, True), (9, True, False), (12, False, False)])
