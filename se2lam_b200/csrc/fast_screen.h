@@ -135,4 +135,72 @@ struct ItemWalk {
     SE2_HD void next() { g += dG; y += dY; if (g >= G) { g -= G; ++y; } }
 };
 
+// ---- pass C (strict 3x3 non-maximum suppression) and pass E (emission) of orb_fast_cells
+// The u8 score plane has the patch's row pitch pw (a multiple of 4, at least cw + 6) and holds cell pixel (x, y) at byte
+// (y + 1) * pw + x + NMS_X0: a zero apron of 1 px around the cell, every other byte of a row zero too. Pixel x's word is then
+// word x/4 + 1 of its row, so the 32 pixels of bitmap word k are the whole plane words 8k+1 .. 8k+8.
+constexpr int NMS_X0 = 4;
+// nms32 on the last word of a row reads up to 32 bytes past the row's end (32 * words_per_row + 8 <= cw + 39 <= pw + 33), so
+// past the plane behind its last row: the plane's shared-memory block is this long
+SE2_HD int nms_plane_bytes(int pw, int ch) { return pw * (ch + 2) + 32; }
+// the bitmap has whole words per cell row: bit x & 31 of word y * nms_words_per_row(cw) + (x >> 5) is pixel (x, y)
+SE2_HD int nms_words_per_row(int cw) { return (cw + 31) >> 5; }
+// bits of bitmap word k that lie inside the cell
+SE2_HD unsigned nms_row_mask(int k, int cw) { const int n = cw - 32 * k; return n >= 32 ? 0xFFFFFFFFu : (1u << n) - 1u; }
+
+// Bitmap word k of cell row y: bit i set <=> score(32k+i, y) > all 8 neighbours (so it is nonzero). u, c, d point at plane word 8k
+// of the plane rows y, y+1, y+2 (the cell rows y-1, y, y+1); each supplies the 10 words of pixels 32k-4 .. 32k+35. Scores are
+// 0..255, so two pixels ride in the two 16-bit halves of a word: E = bytes (0, 2) and O = bytes (1, 3) of a plane word.
+SE2_HD unsigned nms32(const uint32_t* u, const uint32_t* c, const uint32_t* d) {
+    unsigned c3e[10], c3o[10];   // 3-row maxima; [0] only needs the odd bytes, [9] only the even ones
+    unsigned r[4];               // 8 result bits each at bits 24..31
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int j = 0; j < 10; ++j) {
+        const unsigned ua = u[j], ca = c[j], da = d[j];
+        if (j > 0) c3e[j] = max3s2(perm(ua, 0, 0x4240), perm(ca, 0, 0x4240), perm(da, 0, 0x4240));
+        if (j < 9) c3o[j] = max3s2(perm(ua, 0, 0x4341), perm(ca, 0, 0x4341), perm(da, 0, 0x4341));
+    }
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int g = 0; g < 8; ++g) {   // pixels 4g .. 4g+3 = plane word j = g + 1
+        const int j = g + 1;
+        const unsigned ua = u[j], ca = c[j], da = d[j];
+        const unsigned ce = perm(ca, 0, 0x4240), co = perm(ca, 0, 0x4341);                       // centres of pixels (0,2), (1,3)
+        const unsigned ve = maxs2(perm(ua, 0, 0x4240), perm(da, 0, 0x4240));                   // above / below
+        const unsigned vo = maxs2(perm(ua, 0, 0x4341), perm(da, 0, 0x4341));
+        // pixels (0,2): left = bytes (-1, 1) = halves (hi of O_j-1, lo of O_j), right = bytes (1, 3) = O_j
+        // pixels (1,3): left = bytes (0, 2) = E_j, right = bytes (2, 4) = halves (hi of E_j, lo of E_j+1)
+        const unsigned ne = max3s2(perm(c3o[j - 1], c3o[j], 0x5432), ve, c3o[j]);
+        const unsigned no = max3s2(c3e[j], vo, perm(c3e[j], c3e[j + 1], 0x5432));
+        // 255 + centre - max in [0, 510] per half (no borrow across halves): bit 8 of the half <=> centre > max
+        const unsigned te = ce + 0x00FF00FFu - ne, to = co + 0x00FF00FFu - no;
+        const unsigned bytes = perm(te, to, 0x7351);            // byte i = 1 <=> pixel 4g+i is kept
+        if (g & 1) {
+            // bytes of pixels 4g-4 .. 4g-1 in the low nibbles, 4g .. 4g+3 in the high ones; the product's byte 3 is the 8 bits
+            r[g >> 1] = (r[g >> 1] + (bytes << 4)) * 0x01020408u;
+        } else {
+            r[g >> 1] = bytes;
+        }
+    }
+    return perm(perm(r[0], r[1], 0x7373), perm(r[2], r[3], 0x7373), 0x5410);
+}
+
+// passes C and E: thread tid owns the consecutive bitmap words [w, w1) in raster order, so an exclusive scan of the threads'
+// keypoint counts gives every keypoint its raster-order slot; (y, k) of the word is walked, not divided per word
+struct WordRun {
+    int w, w1, y, k, wpr;
+    SE2_HD void init(int tid, int nthreads, int ch, int words_per_row) {
+        wpr = words_per_row;
+        const int nw = ch * wpr, q = (nw + nthreads - 1) / nthreads;
+        w = tid * q < nw ? tid * q : nw;
+        w1 = w + q < nw ? w + q : nw;
+        y = w / wpr; k = w - y * wpr;
+    }
+    SE2_HD bool more() const { return w < w1; }
+    SE2_HD void next() { ++w; if (++k == wpr) { k = 0; ++y; } }
+};
+
 }  // namespace fastpx

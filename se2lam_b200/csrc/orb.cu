@@ -415,8 +415,8 @@ __device__ __forceinline__ void orb_tma_box3(void* dst_smem, const CUtensorMap* 
 // one CTA per (cell, frame): cv::FAST(cell, fastTh, NMS) and, if that yields <= 3 keypoints, cv::FAST(cell, 7, NMS)
 // (ORBextractor.cpp:616-623). The cell and its 3 px apron are staged once in shared memory, by one of two means:
 //   TMA    ONE cp.async.bulk.tensor.3d per CTA pulls the patch (box fbw x fbh of the level's tensor map, origin at the 16 B aligned
-//          column left of the cell's first apron pixel, pitch = the level's constant fbw) while the CTA clears its score plane
-//          and bitmap; the threads issue no staging loads. Needs every level's patch to fit a 256 x 256 box and the driver's
+//          column left of the cell's first apron pixel, pitch = the level's constant fbw) while the CTA clears its score plane;
+//          the threads issue no staging loads. Needs every level's patch to fit a 256 x 256 box and the driver's
 //          tensor-map encoder.
 //   plain  aligned 32-bit loads from the 4 B aligned column left of the first apron pixel, pitch = the cell's patch width
 //          rounded up to 4 B. Takes any cell whose patch and candidate list fit shared memory with 16-bit list offsets.
@@ -424,18 +424,19 @@ __device__ __forceinline__ void orb_tma_box3(void* dst_smem, const CUtensorMap* 
 //   A  every pixel: necessary condition (fastpx::screen4: a 9-arc contains one pixel of each opposite pair (k, k+8), so for one
 //      polarity all 4 tested pairs need a member beyond t), branch-free on two pixels per s16x2 word; one thread = the 4 pixels
 //      of one patch word (group), (row, group) items walked without a division; survivors are compacted into a shared list
-//      (warp scan + one shared atomic per 128 pixels)
-//   B  list entries, full warps: arc score -> score plane (same pitch as the patch, 1 px apron)
-//   C  list entries: strict 3x3 maximum -> one bit per pixel in a raster-order bitmap
-//   D  one warp: exclusive scan of the bitmap words' popcounts = raster-order output slots
-//   E  one thread per bitmap word: emit (score | y | x)
+//      (4 ballots + one shared atomic per 128 pixels)
+//   B  list entries, full warps: arc score -> score plane (same pitch as the patch, zero apron and padding, fastpx::NMS_X0)
+//   C  every thread a run of consecutive bitmap words (whole words per cell row): fastpx::nms32, the strict 3x3 maximum of 32
+//      pixels from the dense score plane, branch-free on two pixels per u16x2 word
+//   D  CTA-wide exclusive scan of the threads' keypoint counts = raster-order output slots
+//   E  every thread its own bitmap words: emit (score | y | x), (y, x) from the word's row and column
 // Registers: the plain instantiation is capped at 48 (at least 5 CTAs of 256 threads per SM); uncapped it takes 64 where 40
 // suffice without spilling. The TMA instantiation has no minimum (0) and gets 64 registers (4 CTAs): a minimum of 4 CTAs keeps
 // 64 registers but schedules a kernel measured 0.8 % slower on an H100 SXM (400 W), a minimum of 1 lets it grow to 72 (3 CTAs).
 template <bool TMA>
 __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbDev d, const __grid_constant__ FastMaps maps) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
-    __shared__ int s_total, s_ncand;
+    __shared__ int s_ncand, s_wsum[FAST_THREADS / 32];
     __shared__ __align__(8) unsigned long long s_bar;
     const CellGeo c = d.cells[blockIdx.x];
     const int f = blockIdx.y + d.frame0;
@@ -452,13 +453,12 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
     const int pw = TMA ? L.fbw : (shift + cw + 6 + 3) & ~3, pww = pw >> 2;   // patch pitch
     const int ph = TMA ? L.fbh : ch + 6;                                      // patch rows
     uint8_t* smem = TMA ? smem_raw + ((128u - (orb_smem_u32(smem_raw) & 127u)) & 127u) : smem_raw;   // TMA destination: 128 B aligned
-    const int nbits = pw * ch, nwords = (nbits + 31) >> 5;
     const int g0 = fastpx::first_group(shift), G = fastpx::groups_per_row(cw, shift), nitems = ch * G;   // pass A work items
+    const int wpr = fastpx::nms_words_per_row(cw);                                        // bitmap words per cell row
     uint8_t* patch = smem;                                                                // [ph x pw], pixel (x,y) of the cell at (y+3)*pw + x+3+shift
-    uint8_t* score = smem + ((pw * ph + 15) & ~15);                                       // [(ch+2) x pw], pixel (x,y) at (y+1)*pw + x+1
-    uint32_t* bitmap = reinterpret_cast<uint32_t*>(score + ((pw * (ch + 2) + 15) & ~15)); // [nwords], bit y*pw + x
-    uint32_t* woff = bitmap + nwords;                                                     // [nwords] exclusive popcount scan
-    uint16_t* list = reinterpret_cast<uint16_t*>(woff + nwords);                          // [<= cw*ch] entries y*pw + x
+    uint8_t* score = smem + ((pw * ph + 15) & ~15);                                       // [(ch+2) x pw], pixel (x,y) at (y+1)*pw + x+NMS_X0
+    uint32_t* bitmap = reinterpret_cast<uint32_t*>(score + ((fastpx::nms_plane_bytes(pw, ch) + 15) & ~15));   // [ch x wpr]
+    uint16_t* list = reinterpret_cast<uint16_t*>(bitmap + ch * wpr);                      // [<= cw*ch] entries y*pw + x
     if (TMA) {
         if (threadIdx.x == 0) orb_mbar_init(&s_bar, 1);
         __syncthreads();
@@ -476,10 +476,12 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
     const uint8_t* p0 = patch + 3 * pw + 3 + shift;
     fastpx::ItemWalk first;      // pass A: item = y*G + g; this thread's items are threadIdx.x, +256, +512, ...
     first.init((int)threadIdx.x, FAST_THREADS, G);
+    fastpx::WordRun words;       // passes C and E: this thread's run of bitmap words
+    words.init((int)threadIdx.x, FAST_THREADS, ch, wpr);
     int thr = d.fast_th;
+    int total = 0, pos0 = 0;     // keypoints of the cell, and the raster-order slot of this thread's first one
     for (int pass = 0; pass < 2; ++pass) {
-        for (int i = threadIdx.x; i < (pw * (ch + 2) + 3) / 4; i += FAST_THREADS) reinterpret_cast<uint32_t*>(score)[i] = 0u;
-        for (int i = threadIdx.x; i < nwords; i += FAST_THREADS) bitmap[i] = 0u;
+        for (int i = threadIdx.x; i < pw * (ch + 2) / 4; i += FAST_THREADS) reinterpret_cast<uint32_t*>(score)[i] = 0u;
         if (threadIdx.x == 0) s_ncand = 0;
         if (TMA && pass == 0 && !orb_mbar_wait(&s_bar, 0)) { *d.err = 4; return; }   // the patch has landed (async-proxy writes are visible after the wait)
         __syncthreads();
@@ -500,21 +502,21 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
                     // necessary condition, then drop the group's pixels outside the cell interior
                     m = fastpx::screen4(n3, s3, n2a, n2b, n2c, s2a, s2b, s2c, za, zb, zc, T1, U1) & fastpx::inside_mask8(col0, cw) & 0xFu;
                 }
-                const int cnt = __popc(m);
-                int inc = cnt;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += u; }
-                const int tot = __shfl_sync(0xffffffffu, inc, 31);
+                // list slots: the list's order does not matter (B writes each entry's own plane byte, C and E are dense), so a
+                // survivor's slot is the warp's base + the survivors of lower group bits + those of lower lanes at its bit
+                const unsigned b0 = __ballot_sync(0xffffffffu, m & 1u), b1 = __ballot_sync(0xffffffffu, m & 2u);
+                const unsigned b2 = __ballot_sync(0xffffffffu, m & 4u), b3 = __ballot_sync(0xffffffffu, m & 8u);
+                const int n0 = __popc(b0), n01 = n0 + __popc(b1), n012 = n01 + __popc(b2), tot = n012 + __popc(b3);
                 if (tot) {
                     int base = 0;
-                    if (lane == 31) base = atomicAdd(&s_ncand, tot);
-                    base = __shfl_sync(0xffffffffu, base, 31) + inc - cnt;
+                    if (lane == 0) base = atomicAdd(&s_ncand, tot);
+                    base = __shfl_sync(0xffffffffu, base, 0);
+                    const unsigned lt = (1u << lane) - 1u;
                     const int e0 = it.y * pw + col0;
-                    while (m) {
-                        const int j = __ffs(m) - 1;
-                        m &= m - 1;
-                        list[base++] = (uint16_t)(e0 + j);
-                    }
+                    if (m & 1u) list[base + __popc(b0 & lt)] = (uint16_t)e0;
+                    if (m & 2u) list[base + n0 + __popc(b1 & lt)] = (uint16_t)(e0 + 1);
+                    if (m & 4u) list[base + n01 + __popc(b2 & lt)] = (uint16_t)(e0 + 2);
+                    if (m & 8u) list[base + n012 + __popc(b3 & lt)] = (uint16_t)(e0 + 3);
                 }
                 it.next();
             }
@@ -525,51 +527,44 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
         for (int i = threadIdx.x; i < ncand; i += FAST_THREADS) {
             const int off = list[i];
             const int m = fast_arc_score(p0 + off, pw);
-            if (m > thr) score[off + pw + 1] = (uint8_t)(m - 1);
+            if (m > thr) score[off + pw + fastpx::NMS_X0] = (uint8_t)(m - 1);
         }
         __syncthreads();
-        // C
-        for (int i = threadIdx.x; i < ncand; i += FAST_THREADS) {
-            const int off = list[i];
-            const uint8_t* q = score + off + pw + 1;
-            const int sc = q[0];
-            if (sc && sc > q[-pw - 1] && sc > q[-pw] && sc > q[-pw + 1] && sc > q[-1] && sc > q[1] && sc > q[pw - 1] && sc > q[pw] && sc > q[pw + 1])
-                atomicOr(&bitmap[off >> 5], 1u << (off & 31));
+        // C: whole bitmap words, dense over the score plane; D: CTA-wide exclusive scan of the threads' keypoint counts
+        int nkp = 0;
+        for (fastpx::WordRun r = words; r.more(); r.next()) {
+            const uint32_t* u = reinterpret_cast<const uint32_t*>(score) + r.y * pww + 8 * r.k;
+            const unsigned bits = fastpx::nms32(u, u + pww, u + 2 * pww) & fastpx::nms_row_mask(r.k, cw);
+            bitmap[r.w] = bits;
+            nkp += __popc(bits);
         }
-        __syncthreads();
-        // D
-        if (wid == 0) {
-            int run = 0;
-            for (int b0 = 0; b0 < nwords; b0 += 32) {
-                const int v = (b0 + lane < nwords) ? __popc(bitmap[b0 + lane]) : 0;
-                int inc = v;
+        int inc = nkp;
 #pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += u; }
-                if (b0 + lane < nwords) woff[b0 + lane] = run + inc - v;
-                run += __shfl_sync(0xffffffffu, inc, 31);
-            }
-            if (lane == 0) s_total = run;
-        }
+        for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += u; }
+        if (lane == 31) s_wsum[wid] = inc;
         __syncthreads();
-        if (s_total > 3 || thr == 7) break;
+        total = 0; pos0 = inc - nkp;
+#pragma unroll
+        for (int w = 0; w < NW; ++w) { const int v = s_wsum[w]; total += v; if (w < wid) pos0 += v; }
+        if (total > 3 || thr == 7) break;
         thr = 7;                 // cellKeyPoints.size() <= 3: clear and retry with the fixed fallback threshold
-        __syncthreads();
     }
-    // E
+    // E: this thread's bitmap words (it wrote them in C), in raster order from its slot pos0
     uint32_t* out = d.cand + (size_t)f * d.cand_total + c.cand_off;
-    for (int j = threadIdx.x; j < nwords; j += FAST_THREADS) {
-        uint32_t w = bitmap[j];
-        int pos = woff[j];
-        while (w) {
-            const int off = j * 32 + __ffs(w) - 1;
-            w &= w - 1;
-            const int y = off / pw, x = off - y * pw;
-            if (pos < c.cand_cap) out[pos] = ((uint32_t)score[off + pw + 1] << 24) | ((uint32_t)(c.y0 + y) << 12) | (uint32_t)(c.x0 + x);
+    int pos = pos0;
+    for (fastpx::WordRun r = words; r.more(); r.next()) {
+        uint32_t bits = bitmap[r.w];
+        const uint8_t* srow = score + (r.y + 1) * pw + fastpx::NMS_X0 + 32 * r.k;
+        const uint32_t yx = ((uint32_t)(c.y0 + r.y) << 12) | (uint32_t)(c.x0 + 32 * r.k);
+        while (bits) {
+            const int i = __ffs(bits) - 1;
+            bits &= bits - 1;
+            if (pos < c.cand_cap) out[pos] = ((uint32_t)srow[i] << 24) | (yx + i);
             else *d.err = 1;
             ++pos;
         }
     }
-    if (threadIdx.x == 0) { hdr->n_base = s_total; hdr->n_a = s_total; hdr->n_b = s_total; }
+    if (threadIdx.x == 0) { hdr->n_base = total; hdr->n_a = total; hdr->n_b = total; }
 }
 
 // FAST-9-16 arc score M = max over the 16 nine-pixel arcs of min(+-(v - ring)); corner at t <=> M > t,
@@ -1142,9 +1137,9 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
                 if (cw > 0 && chh > 0) {
                     max_cw = std::max(max_cw, ((c.x0 - 3 + EDGE) & 15) + cw); max_ch = std::max(max_ch, chh);   // incl. the TMA alignment shift
                     const size_t pwb = (size_t)((cw + 6 + 3 + 3) / 4 + 1) * 4;   // worst-case alignment shift
-                    const size_t nwords = (pwb * chh + 31) / 32;
+                    const size_t bitmap = (size_t)chh * fastpx::nms_words_per_row(cw) * 4;
                     if (pwb * (chh + 6) > 65535) fast_big = true;    // 16-bit patch offsets in the candidate list
-                    fsm = std::max(fsm, ((pwb * (chh + 6) + 15) & ~(size_t)15) + ((pwb * (chh + 2) + 15) & ~(size_t)15) + nwords * 8 + (size_t)cw * chh * 2 + 64);
+                    fsm = std::max(fsm, ((pwb * (chh + 6) + 15) & ~(size_t)15) + (((size_t)fastpx::nms_plane_bytes((int)pwb, chh) + 15) & ~(size_t)15) + bitmap + (size_t)cw * chh * 2 + 64);
                     const size_t nchunk = (size_t)chh * ((cw + 31) / 32);
                     fsm_big = std::max(fsm_big, ((pwb * (chh + 6) + 15) & ~(size_t)15) + (((size_t)(cw + 2) * (chh + 2) + 15) & ~(size_t)15) + nchunk * 4 + 64);
                 }
@@ -1158,9 +1153,9 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
             for (size_t ci = first_cell; ci < C.size(); ++ci) {
                 const int cw = C[ci].x1 - C[ci].x0, chh = C[ci].y1 - C[ci].y0;
                 if (C[ci].skipped || cw <= 0 || chh <= 0) continue;
-                const size_t pw = (size_t)g.fbw, nwords = (pw * chh + 31) / 32;
-                // 128 B of alignment slack, patch, score plane, bitmap + scan, candidate list (one 16-bit entry per interior pixel)
-                fsm_tma = std::max(fsm_tma, (size_t)128 + ((pw * g.fbh + 15) & ~(size_t)15) + ((pw * (chh + 2) + 15) & ~(size_t)15) + nwords * 8 + (size_t)cw * chh * 2 + 64);
+                const size_t pw = (size_t)g.fbw, bitmap = (size_t)chh * fastpx::nms_words_per_row(cw) * 4;
+                // 128 B of alignment slack, patch, score plane, bitmap, candidate list (one 16-bit entry per interior pixel)
+                fsm_tma = std::max(fsm_tma, (size_t)128 + ((pw * g.fbh + 15) & ~(size_t)15) + (((size_t)fastpx::nms_plane_bytes(g.fbw, chh) + 15) & ~(size_t)15) + bitmap + (size_t)cw * chh * 2 + 64);
             }
         }
         ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 4 + (size_t)g.nCells * 16 + (size_t)SEL_STAGE * 4);
