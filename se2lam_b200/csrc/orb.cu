@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(128) orb_pyr0_undistort(OrbDev d, LevelGeo L, 
 
 // level l>0: resize(level l-1 -> level l, INTER_LINEAR) + copyMakeBorder(REFLECT_101) in one pass, cv::resize's
 // fixed-point arithmetic (11-bit coefficients, horizontal pass kept at full precision, vertical pass >>4, >>16, +2 >>2).
-// One CTA = a 128 x RESIZE_TR tile of the bordered output plane, three stages in shared memory:
+// One CTA = a 128 x RESIZE_TR tile (32 or 64 rows, see below) of the bordered output plane, three stages in shared memory:
 //   0  the source rows/columns the tile touches (a contiguous box, also across the reflected border) as 16 B vectors
 //   1  horizontal pass h[s][x] = src[s][sx]*a0 + src[s][sx+1]*a1 for every staged source row s, ONCE per (row, column)
 //      (consecutive output rows share source rows; cv::resize does the same with its row buffers)
@@ -198,15 +198,27 @@ __global__ void __launch_bounds__(128) orb_pyr0_undistort(OrbDev d, LevelGeo L, 
 // the last wave of this launch frees and run their table set-up there; they read this level's plane only behind
 // griddepcontrol.wait, which returns when this whole grid has completed and its writes are visible. The pyramid is a chain of seven
 // dependent, short launches: this overlaps each launch's ramp-up with its predecessor's tail.
-constexpr int RESIZE_TR = 32;
+// Tile height: RESIZE_TR rows, or RESIZE_TR_TALL rows on levels whose grid of tall tiles still fills every resident CTA slot of the
+// GPU at least once (run_device). A CTA's fixed costs - table loads, two dependent L2 round trips, three barriers - are then spread
+// over twice the output rows, and more output rows share each staged source row; on the small levels tall tiles would leave SMs
+// idle in a single partial wave. Measured on an H100 SXM (400 W), 64 frames of 640x480, 8 levels: per-level kernel times in us
+// (levels 1..7, torch.profiler, tools/orb_pyramid_trace.py) and the pyramid profile group in ms:
+//   32 rows everywhere       39.6 32.6 27.2 20.9 18.9 15.8 11.7   0.153
+//   64 rows everywhere       32.0 29.6 25.5 20.6 19.4 15.7 21.4   0.135
+//   96 rows everywhere       31.3 28.5 27.2 21.9 19.0 17.6 22.9   0.135
+//  128 rows everywhere       32.5 29.3 27.6 24.3 19.0 22.4 21.6   0.136
+//   64 rows on levels 1-5    32.1 29.6 25.2 21.3 19.8 16.1 11.7   0.134-0.135 (this rule; step 0.623-0.627 ms against 0.644-0.649)
+constexpr int RESIZE_TR = 32, RESIZE_TR_TALL = 64;
 struct ResizeRow { int s0, s1, b0, b1; };
 struct ResizeCol { int sx0, sx1; short a0, a1; int valid; };   // 16 B
+template <int RESIZE_TR>
 __global__ void __launch_bounds__(256) orb_resize_w(OrbDev d, LevelGeo L, LevelGeo S, int max_rows, int raw_pitch) {
+    static_assert(RESIZE_TR % 32 == 0 && RESIZE_TR <= 128, "row terms take one thread per row in warps 4..7");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     extern __shared__ __align__(16) uint8_t rs_smem[];
     __shared__ ResizeRow rowinfo[RESIZE_TR];
     __shared__ __align__(16) ResizeCol colinfo[128];
-    __shared__ int s_lo[2], s_hi[2];     // [1] source rows
+    __shared__ int s_lo[RESIZE_TR / 32], s_hi[RESIZE_TR / 32];   // source row range per row warp
     __shared__ int s_cmin[4], s_cmax[4]; // source column range per column warp
     uint16_t* hbuf = reinterpret_cast<uint16_t*>(rs_smem);                  // [max_rows][128], 16 bit: (255 * 2048) >> 4 = 32 640
     uint8_t* raw = rs_smem + (size_t)max_rows * 128 * sizeof(uint16_t);     // [max_rows][raw_pitch] (+16 B of slack behind the last row)
@@ -219,7 +231,7 @@ __global__ void __launch_bounds__(256) orb_resize_w(OrbDev d, LevelGeo L, LevelG
     const short2* ialpha = reinterpret_cast<const short2*>(d.stab + 2 * (size_t)L.tab_off);
     const short2* ibeta = ialpha + L.w;
     // column terms of the tile's 128 output columns: warps 0..3, one column per thread (the 8 thread rows share them through
-    // shared memory instead of each recomputing its 4 columns); row terms: warp 4
+    // shared memory instead of each recomputing its 4 columns); row terms: warps 4.., one row per thread
     if (tid < 128) {
         const int x = blockIdx.x * 128 + tid;
         ResizeCol c{0, 0, 0, 0, 0};
@@ -236,25 +248,28 @@ __global__ void __launch_bounds__(256) orb_resize_w(OrbDev d, LevelGeo L, LevelG
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { cmin = min(cmin, __shfl_xor_sync(0xffffffffu, cmin, o)); cmax = max(cmax, __shfl_xor_sync(0xffffffffu, cmax, o)); }
         if (tx == 0) { s_cmin[ty] = cmin; s_cmax[ty] = cmax; }
-    } else if (ty == 4) {   // row terms of the tile's RESIZE_TR output rows and their source row range
-        const int y = y0 + tx;
+    } else if (ty < 4 + RESIZE_TR / 32) {   // row terms of the tile's RESIZE_TR output rows and their source row range
+        const int ry = tid - 128, y = y0 + ry;
         int rmin = 0x7fffffff, rmax = -1;
         if (y < H) {
             const int dy = reflect101(y - EDGE, L.h);
             const int sy = __ldg(yofs + dy);
             const short2 bb = __ldg(ibeta + dy);
             ResizeRow r{min(max(sy, 0), S.h - 1), min(max(sy + 1, 0), S.h - 1), bb.x, bb.y};
-            rowinfo[tx] = r;
+            rowinfo[ry] = r;
             rmin = r.s0; rmax = r.s1;
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { rmin = min(rmin, __shfl_xor_sync(0xffffffffu, rmin, o)); rmax = max(rmax, __shfl_xor_sync(0xffffffffu, rmax, o)); }
-        if (tx == 0) { s_lo[1] = rmin; s_hi[1] = rmax; }
+        if (tx == 0) { s_lo[ty - 4] = rmin; s_hi[ty - 4] = rmax; }
     }
     __syncthreads();
     const int c_min = min(min(s_cmin[0], s_cmin[1]), min(s_cmin[2], s_cmin[3])), c_max = max(max(s_cmax[0], s_cmax[1]), max(s_cmax[2], s_cmax[3]));
     const int c_lo = c_min & ~15, nvec = c_max < 0 ? 0 : (c_max - c_lo) / 16 + 1;
-    const int r_lo = s_lo[1], nsr = s_hi[1] - r_lo + 1;
+    int r_lo = s_lo[0], r_hi = s_hi[0];
+#pragma unroll
+    for (int k = 1; k < RESIZE_TR / 32; ++k) { r_lo = min(r_lo, s_lo[k]); r_hi = max(r_hi, s_hi[k]); }
+    const int nsr = r_hi - r_lo + 1;
     if (nsr > max_rows || nvec * 16 > raw_pitch) { if (tid == 0) *d.err = 3; return; }   // sized on the host from the scale factor
     const uint8_t* src = d.plain + f * d.frame_plane_bytes + S.plane_off + (size_t)EDGE * S.pitch + EDGE;
     asm volatile("griddepcontrol.wait;" ::: "memory");     // the source level is complete and visible from here on
@@ -1034,6 +1049,8 @@ struct se2gpu_orb {
     std::vector<TileGeo> tiles;
     size_t fast_smem = 0, select_smem = 0, resize_w_smem = 0;
     int resize_rows = 0, resize_raw_pitch = 0;   // shared-memory box of orb_resize_w, sized from the scale factor
+    int resize_tall_rows = 0; size_t resize_tall_smem = 0;   // the same for RESIZE_TR_TALL-row tiles
+    int resize_tall_ctas = 0;    // resident CTAs of orb_resize_w<RESIZE_TR_TALL> on the whole GPU; 0: tall tiles are not used
     bool fast_big = false;       // cells too large for the compacting FAST kernel: use orb_fast_cells_big
     bool fast_tma = false;       // cells staged by the TMA unit: orb_fast_cells<true>, else orb_fast_cells<false>
     size_t fast_tma_smem = 0;
@@ -1283,7 +1300,17 @@ int set_geometry(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
         h->resize_raw_pitch = (((int)ceil(128 * ratio) + 4 + 15 + 15) / 16) * 16;
         h->resize_w_smem = (size_t)h->resize_rows * (128 * sizeof(uint16_t) + h->resize_raw_pitch) + 16;   // 16-bit row-pass results, 16 B of slack behind the last staged row
         if (h->resize_w_smem > 200 * 1024) return fail(SE2GPU_ERR_CAPACITY, "scale factor %.3f needs %zu B of shared memory in orb_resize_w", ratio, h->resize_w_smem);
-        SE2_CUDA(cudaFuncSetAttribute(orb_resize_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->resize_w_smem));
+        SE2_CUDA(cudaFuncSetAttribute(orb_resize_w<RESIZE_TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->resize_w_smem));
+        h->resize_tall_rows = (int)ceil(RESIZE_TR_TALL * ratio) + 4;
+        h->resize_tall_smem = (size_t)h->resize_tall_rows * (128 * sizeof(uint16_t) + h->resize_raw_pitch) + 16;
+        h->resize_tall_ctas = 0;
+        if (h->resize_tall_smem <= 200 * 1024) {     // else every level keeps RESIZE_TR-row tiles
+            SE2_CUDA(cudaFuncSetAttribute(orb_resize_w<RESIZE_TR_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->resize_tall_smem));
+            int per_sm = 0, sms = 0;
+            SE2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, orb_resize_w<RESIZE_TR_TALL>, 256, h->resize_tall_smem));
+            SE2_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+            h->resize_tall_ctas = per_sm * sms;
+        }
     }
     SE2_CUDA(cudaFuncSetAttribute(orb_fast_cells_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(fsm, 1024)));
     SE2_CUDA(cudaFuncSetAttribute(orb_fast_cells<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(fsm, 1024)));
@@ -1408,13 +1435,19 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
     for (int l = 1; l < h->nlevels; ++l) {
         const LevelGeo& g = h->levels[l];
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3((g.pitch + 127) / 128, (g.h + 2 * EDGE + RESIZE_TR - 1) / RESIZE_TR, n);
-        cfg.blockDim = dim3(32, 8); cfg.dynamicSmemBytes = h->resize_w_smem; cfg.stream = s;
+        // tall tiles where their grid fills every resident CTA slot at least once (see RESIZE_TR_TALL)
+        const int ncx = (g.pitch + 127) / 128, H = g.h + 2 * EDGE;
+        const int tall_grid = ncx * ((H + RESIZE_TR_TALL - 1) / RESIZE_TR_TALL) * n;
+        const bool tall = h->resize_tall_ctas > 0 && tall_grid >= h->resize_tall_ctas;
+        const int tr = tall ? RESIZE_TR_TALL : RESIZE_TR;
+        cfg.gridDim = dim3(ncx, (H + tr - 1) / tr, n);
+        cfg.blockDim = dim3(32, 8); cfg.dynamicSmemBytes = tall ? h->resize_tall_smem : h->resize_w_smem; cfg.stream = s;
         cudaLaunchAttribute at[1];   // programmatic dependent launch along the resize chain (see orb_resize_w)
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        SE2_CUDA(cudaLaunchKernelEx(&cfg, orb_resize_w, d, g, h->levels[l - 1], h->resize_rows, h->resize_raw_pitch));
+        if (tall) SE2_CUDA(cudaLaunchKernelEx(&cfg, orb_resize_w<RESIZE_TR_TALL>, d, g, h->levels[l - 1], h->resize_tall_rows, h->resize_raw_pitch));
+        else SE2_CUDA(cudaLaunchKernelEx(&cfg, orb_resize_w<RESIZE_TR>, d, g, h->levels[l - 1], h->resize_rows, h->resize_raw_pitch));
         ::se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed);
         if (l == splitA - 1 && side && !pr.on) SE2_CUDA(cudaEventRecord(h->ev_l1, s));
     }
