@@ -30,6 +30,10 @@
  *   se2gpu_ba_build_information      per-edge Omega of Map::loadLocalGraph    src/Map.cpp:1024-1049
  *   se2gpu_voc_create / _transform   DBoW2 TemplatedVocabulary::transform     Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1220-1262
  *   se2gpu_median_descriptor         MapPoint::updateMainKFandDescriptor      src/MapPoint.cpp:228-272
+ *   se2gpu_triangulate[_device]      cvu::triangulate                         src/cvutil.cpp:46-59
+ *   se2gpu_track_triangulate[_device]  Track::doTriangulate                   src/Track.cpp:389-416
+ *   se2gpu_xyz_info[_device]         Track::calcSE3toXYZInfo                  src/Track.cpp:259-306
+ *   se2gpu_projection_observations[_device]  LocalMapper::findCorrespd, MatchByProjection branch  src/LocalMapper.cpp:119-141
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -240,6 +244,71 @@ int se2gpu_voc_transform_device(se2gpu_voc* v, const uint8_t* d_desc, int n, int
  * with the least median Hamming distance to the others - median = element int(0.5*(N-1)) of the sorted distances incl. the
  * zero self-distance, first index wins ties - and best_median [m] (may be NULL) that median. HOST buffers. */
 int se2gpu_median_descriptor(const uint8_t* desc, const int* ptr, int M, int* best_idx, int* best_median, int device);
+
+/* ------------------------------------------------------------------------------------------ two-view geometry */
+/* Reproduces the reference's float arithmetic and OpenCV's primitives on an x86-64 AVX2 host with glibc 2.39 bit for bit, with
+ * two steps matched by restatement rather than proven against cv2 (DESIGN.md section 8): the double hypot inside the SVD
+ * (OpenCV's lapack.cpp template, which cv2 does not expose) and the last bits of sin/cos inside Rodrigues (the device's
+ * sincos is not glibc's; a difference survives the rounding to float only at a float rounding boundary). NaN results
+ * are NaN on both sides with possibly different payloads.
+ * Projection matrices are 3x4 row-major floats (Config::Kcam * Tcw.rowRange(0,3)); poses are 4x4 row-major floats.
+ * The _device forms take DEVICE buffers and are asynchronous on `stream` (cudaStream_t as void*, NULL = default stream);
+ * the others take HOST buffers, run on `device` and return when the results are in place. */
+
+/* cvu::triangulate (src/cvutil.cpp:46-59) for n pairs: xyz[3i..] = triangulate(pt1[i], pt2[i], P[idx1[i]], P[idx2[i]]),
+ * pt1/pt2 [n*2], P [n_proj*12]. NaN / inf results (w = 0) are returned as computed. */
+int se2gpu_triangulate(int n, const float* pt1, const float* pt2, const float* P, int n_proj, const int* idx1, const int* idx2,
+                       float* xyz, int device);
+int se2gpu_triangulate_device(int n, const float* d_pt1, const float* d_pt2, const float* d_P, const int* d_idx1,
+                              const int* d_idx2, float* d_xyz, void* stream);
+
+/* Track::doTriangulate (src/Track.cpp:389-416) after its nMinFrames early return, which stays with the caller. kp_kf [n_kf]
+ * are the reference keyframe's keyPointsUn, kp_frame the current frame's, matches12 [n_kf] the result of MatchByWindow
+ * (updated in place: -1 where the depth test fails), kf_observed [n_kf] mpKF->hasObservation(i), kf_view_mp [n_kf*3]
+ * mpKF->mViewMPs, Tcr [16] mFrame.Tcr, K [9] Config::Kcam, lower/upper_depth Config::LOWER/UPPER_DEPTH,
+ * min_parallax_deg the checkParallax degree (1..4; the reference uses 2). local_mps [n_kf*3] is updated in place: unmatched
+ * entries and those failing the depth test keep their previous value. good_prl [n_kf] = mvbGoodPrl,
+ * counts [2] = {nTrackedOld, nGoodPrl}. The _device form takes d_n_kf (may be NULL) with the keyframe's keypoint count
+ * (<= n_kf) as the extractor wrote it; entries at or past it are not touched. */
+int se2gpu_track_triangulate(const se2gpu_keypoint* kp_kf, int n_kf, const se2gpu_keypoint* kp_frame, int n_frame, int* matches12,
+                             const uint8_t* kf_observed, const float* kf_view_mp, const float* Tcr, const float* K,
+                             float lower_depth, float upper_depth, int min_parallax_deg, float* local_mps, uint8_t* good_prl,
+                             int* counts, int device);
+int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, const int* d_n_kf, const se2gpu_keypoint* d_kp_frame,
+                                    int* d_matches12, const uint8_t* d_kf_observed, const float* d_kf_view_mp, const float* d_Tcr,
+                                    const float* d_K, float lower_depth, float upper_depth, int min_parallax_deg,
+                                    float* d_local_mps, uint8_t* d_good_prl, int* d_counts, void* stream);
+
+/* Track::calcSE3toXYZInfo (src/Track.cpp:259-306) for n points: calcSE3toXYZInfo(xyz1[i], Tcw[pose1[i]], Tcw[pose2[i]]),
+ * Tcw [n_pose*16], fx = Config::fxCam. info1/info2 [n*9] are the float matrices widened to double (toMatrix3d). */
+int se2gpu_xyz_info(int n, const float* xyz1, const int* pose1, const int* pose2, const float* Tcw, int n_pose, float fx,
+                    double* info1, double* info2, int device);
+int se2gpu_xyz_info_device(int n, const float* d_xyz1, const int* d_pose1, const int* d_pose2, const float* d_Tcw, float fx,
+                           double* d_info1, double* d_info2, void* stream);
+
+/* Body of LocalMapper::findCorrespd's MatchByProjection loop (src/LocalMapper.cpp:119-141) without the object-graph updates.
+ * kf_kp [n_kf] are mNewKF->keyPointsUn: their x, y feed the triangulation (keyPointsUn[i].pt) and their octave stands for
+ * keyPoints[i].octave, which the undistortion leaves unchanged. matches_idx_mp [n_kf] is the result of MatchByProjection,
+ * Tcw_new [16] mNewKF->Tcw.
+ * Map point m: mp_main_measure [2m..] getMainMeasure(), mp_main_pose [m] index of mMainKF->Tcw in Tcw_table [n_pose*16],
+ * mp_main_octave [m] the main keyframe's octave of the point, mp_normal [3m..] mNormalVector, mp_min_dist / mp_max_dist [m].
+ * accept [i] = 1 where the reference adds the observation (acceptNewObserve and the depth window pass); there
+ * pos_new_kf [3i..] = posNewKF and info_new [9i..] = infoNew. Rows with accept[i] = 0 are not written. */
+int se2gpu_projection_observations(const se2gpu_keypoint* kf_kp, int n_kf, const int* matches_idx_mp, const float* Tcw_new,
+                                   const float* mp_main_measure, const int* mp_main_pose, const int* mp_main_octave,
+                                   const float* mp_normal, const float* mp_min_dist, const float* mp_max_dist, int n_mp,
+                                   const float* Tcw_table, int n_pose, const float* K, float lower_depth, float upper_depth,
+                                   float fx, uint8_t* accept, float* pos_new_kf, double* info_new, int device);
+int se2gpu_projection_observations_device(const se2gpu_keypoint* d_kf_kp, int n_kf, const int* d_n_kf, const int* d_matches_idx_mp,
+                                          const float* d_Tcw_new, const float* d_mp_main_measure, const int* d_mp_main_pose,
+                                          const int* d_mp_main_octave, const float* d_mp_normal, const float* d_mp_min_dist,
+                                          const float* d_mp_max_dist, const float* d_Tcw_table, const float* d_K, float lower_depth,
+                                          float upper_depth, float fx, uint8_t* d_accept, float* d_pos_new_kf, double* d_info_new,
+                                          void* stream);
+
+/* Test hook: the 4x4 Jacobi SVD behind cvu::triangulate (cv::SVD::compute, MODIFY_A|FULL_UV) on n row-major matrices
+ * A [n*16]; w [n*4] singular values (descending), vt [n*16]. HOST buffers. */
+int se2gpu_debug_svd4(int n, const float* A, float* w, float* vt, int device);
 
 /* ------------------------------------------------------------------------------------------ local BA */
 typedef struct se2gpu_ba se2gpu_ba;

@@ -51,6 +51,9 @@ SYMBOLS = [
     "se2gpu_ba_set_shard", "se2gpu_ba_peer_export", "se2gpu_ba_peer_import", "se2gpu_ba_set_stream", "se2gpu_ba_debug_system", "se2gpu_ba_reset", "se2gpu_ba_profile",
     "se2gpu_ba_profile_read", "se2gpu_ba_set_mode", "se2gpu_ba_get_f32", "se2gpu_ba_build_information", "se2gpu_ba_optimize_from", "se2gpu_ba_peer_attach_local",
     "se2gpu_voc_create", "se2gpu_voc_destroy", "se2gpu_voc_transform", "se2gpu_voc_transform_device", "se2gpu_median_descriptor",
+    "se2gpu_triangulate", "se2gpu_triangulate_device", "se2gpu_track_triangulate", "se2gpu_track_triangulate_device",
+    "se2gpu_xyz_info", "se2gpu_xyz_info_device", "se2gpu_projection_observations", "se2gpu_projection_observations_device",
+    "se2gpu_debug_svd4",
 ]
 
 
@@ -127,6 +130,15 @@ def lib():
     L.se2gpu_voc_transform.argtypes = [vp, vp, i, i, vp, vp, vp]
     L.se2gpu_voc_transform_device.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
     L.se2gpu_median_descriptor.argtypes = [vp, vp, i, vp, vp, i]
+    L.se2gpu_triangulate.argtypes = [i, vp, vp, vp, i, vp, vp, vp, i]
+    L.se2gpu_triangulate_device.argtypes = [i] + [vp] * 7
+    L.se2gpu_track_triangulate.argtypes = [vp, i, vp, i, vp, vp, vp, vp, vp, f, f, i, vp, vp, vp, i]
+    L.se2gpu_track_triangulate_device.argtypes = [vp, i, vp, vp, vp, vp, vp, vp, vp, f, f, i, vp, vp, vp, vp]
+    L.se2gpu_xyz_info.argtypes = [i, vp, vp, vp, vp, i, f, vp, vp, i]
+    L.se2gpu_xyz_info_device.argtypes = [i, vp, vp, vp, vp, f, vp, vp, vp]
+    L.se2gpu_projection_observations.argtypes = [vp, i] + [vp] * 8 + [i, vp, i, vp, f, f, f, vp, vp, vp, i]
+    L.se2gpu_projection_observations_device.argtypes = [vp, i] + [vp] * 11 + [f, f, f, vp, vp, vp, vp]
+    L.se2gpu_debug_svd4.argtypes = [i, vp, vp, vp, i]
     _lib = L
     return L
 

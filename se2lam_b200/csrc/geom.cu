@@ -1,0 +1,676 @@
+// Two-view geometry over matches: cvu::triangulate, Track::doTriangulate, Track::calcSE3toXYZInfo and the MatchByProjection
+// branch of LocalMapper::findCorrespd (DESIGN.md section 8). One thread per match; counts are reduced with warp ballots and
+// one atomic per warp.
+//
+// Every floating-point operation is written with an explicitly rounded intrinsic, in the order the reference and OpenCV
+// evaluate it on the host, so that the compiler cannot contract a multiply and an add the host keeps apart. The only fused
+// multiply-adds of the reference's arithmetic are the rows of A (cv::addWeighted's dispatched SIMD kernel on an AVX2 host).
+#include <cfloat>
+#include <cstdint>
+
+#include "common.h"
+
+using namespace se2gpu;
+
+namespace {
+
+constexpr int kBlock = 128;
+
+struct F3 { float x, y, z; };
+
+__device__ __forceinline__ float fm(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float fa(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float fs(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ float fd(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double ds(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ double dd(double a, double b) { return __ddiv_rn(a, b); }
+
+__device__ __forceinline__ F3 sub3(F3 a, F3 b) { return {fs(a.x, b.x), fs(a.y, b.y), fs(a.z, b.z)}; }
+__device__ __forceinline__ float dot3(F3 a, F3 b) { return fa(fa(fm(a.x, b.x), fm(a.y, b.y)), fm(a.z, b.z)); }
+__device__ __forceinline__ F3 cross3(F3 a, F3 b) {
+    return {fs(fm(a.y, b.z), fm(a.z, b.y)), fs(fm(a.z, b.x), fm(a.x, b.z)), fs(fm(a.x, b.y), fm(a.y, b.x))};
+}
+// cv::norm(Point3_): sqrt of the double sum of squares
+__device__ __forceinline__ double norm3(F3 p) {
+    const double x = p.x, y = p.y, z = p.z;
+    return __dsqrt_rn(da(da(dm(x, x), dm(y, y)), dm(z, z)));
+}
+
+// The double hypot of OpenCV's JacobiSVDImpl_: lapack.cpp's inline template (not libm's hypot), the larger magnitude times
+// sqrt(1 + ratio^2), evaluated unfused as on the host.
+__device__ __forceinline__ double cv_hypot(double a, double b) {
+    a = fabs(a);
+    b = fabs(b);
+    if (a > b) return dm(a, __dsqrt_rn(da(1.0, dm(dd(b, a), dd(b, a)))));
+    if (b > 0) return dm(b, __dsqrt_rn(da(1.0, dm(dd(a, b), dd(a, b)))));
+    return 0.0;
+}
+
+// std::asin(float) of the host: glibc's __ieee754_asinf (sysdeps/ieee754/flt-32/e_asinf.c, glibc 2.39; it is not correctly
+// rounded, so the device restates it operation by operation). Arguments here are >= 0 or NaN.
+__device__ __forceinline__ float asinf_host(float x) {
+    const float p0 = 1.666675248e-1f, p1 = 7.495297643e-2f, p2 = 4.547037598e-2f, p3 = 2.417951451e-2f, p4 = 4.216630880e-2f;
+    const float pio2_hi = 1.57079637050628662109375f, pio2_lo = -4.37113900018624283e-8f, pio4_hi = 0.785398185253143310546875f;
+    const int hx = __float_as_int(x), ix = hx & 0x7fffffff;
+    if (ix == 0x3f800000) return fa(fm(x, pio2_hi), fm(x, pio2_lo));
+    if (ix > 0x3f800000) return __fdiv_rn(fs(x, x), fs(x, x));
+    if (ix < 0x3f000000) {
+        if (ix < 0x32000000) return x;
+        const float t = fm(x, x);
+        const float w = fm(t, fa(p0, fm(t, fa(p1, fm(t, fa(p2, fm(t, fa(p3, fm(t, p4)))))))));
+        return fa(x, fm(x, w));
+    }
+    const float t = fm(fs(1.f, fabsf(x)), 0.5f);
+    float p = fm(t, fa(p0, fm(t, fa(p1, fm(t, fa(p2, fm(t, fa(p3, fm(t, p4)))))))));
+    const float s = __fsqrt_rn(t);
+    float r;
+    if (ix >= 0x3F79999A) {
+        r = fs(pio2_hi, fs(fm(2.f, fa(s, fm(s, p))), pio2_lo));
+    } else {
+        const float w = __int_as_float(__float_as_int(s) & 0xfffff000);
+        const float c = fd(fs(t, fm(w, w)), fa(s, w));
+        p = fs(fm(fm(2.f, s), p), fs(pio2_lo, fm(2.f, c)));
+        const float q = fs(pio4_hi, fm(2.f, w));
+        r = fs(pio4_hi, fs(p, q));
+    }
+    return hx > 0 ? r : -r;
+}
+
+// cv::gemm(A[3x3], B[3x ncols], alpha) through OpenCV's small-matrix path: float sums left to right, then (float)(t*alpha + 0)
+__device__ __forceinline__ float gemm3_elem(const float* A, int lda, int i, const float* B, int ldb, int j, double alpha) {
+    const float t = fa(fa(fm(A[i * lda], B[j]), fm(A[i * lda + 1], B[ldb + j])), fm(A[i * lda + 2], B[2 * ldb + j]));
+    return __double2float_rn(da(dm((double)t, alpha), 0.0));
+}
+
+// Kcam * T.rowRange(0,3)
+__device__ __forceinline__ void projection(const float* K, const float* T, float* P) {
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) P[i * 4 + j] = gemm3_elem(K, 3, i, T, 4, j, 1.0);
+}
+
+// cvu::inv: [R^T | -R^T t]
+__device__ __forceinline__ void inv4(const float* T, float* Ti) {
+    float RT[9];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) RT[i * 3 + j] = T[j * 4 + i];
+    const float t[3] = {T[3], T[7], T[11]};
+#pragma unroll
+    for (int i = 0; i < 16; i++) Ti[i] = (i % 5 == 0) ? 1.f : 0.f;
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+#pragma unroll
+        for (int j = 0; j < 3; j++) Ti[i * 4 + j] = RT[i * 3 + j];
+        Ti[i * 4 + 3] = gemm3_elem(RT, 3, i, t, 1, 0, -1.0);
+    }
+}
+
+// cvu::se3map: Matx33f * Point3f (float sums from 0) + t
+__device__ __forceinline__ F3 se3map(const float* T, F3 p) {
+    float r[3];
+#pragma unroll
+    for (int i = 0; i < 3; i++) r[i] = fa(fa(fa(0.f, fm(T[i * 4], p.x)), fm(T[i * 4 + 1], p.y)), fm(T[i * 4 + 2], p.z));
+    return {fa(r[0], T[3]), fa(r[1], T[7]), fa(r[2], T[11])};
+}
+
+// cv::SVD::compute(A, w, u, vt, MODIFY_A|FULL_UV) on a 4x4 float matrix: OpenCV's one-sided Jacobi (JacobiSVDImpl_<float>)
+// on A^T, in registers. w and vt only.
+__device__ __forceinline__ void svd4(const float* A, float* w_out, float (&Vt)[4][4]) {
+    float At[4][4];
+    double W[4];
+    const float eps = FLT_EPSILON * 2;
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int k = 0; k < 4; k++) At[i][k] = A[k * 4 + i];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        double sd = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) sd = da(sd, dm((double)At[i][k], (double)At[i][k]));
+        W[i] = sd;
+#pragma unroll
+        for (int k = 0; k < 4; k++) Vt[i][k] = (i == k) ? 1.f : 0.f;
+    }
+    for (int iter = 0; iter < 30; iter++) {
+        bool changed = false;
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+#pragma unroll
+            for (int j = i + 1; j < 4; j++) {
+                double a = W[i], p = 0, b = W[j];
+#pragma unroll
+                for (int k = 0; k < 4; k++) p = da(p, dm((double)At[i][k], (double)At[j][k]));
+                if (fabs(p) <= dm((double)eps, __dsqrt_rn(dm(a, b)))) continue;
+                p = dm(p, 2.0);
+                const double beta = ds(a, b), gamma = cv_hypot(p, beta);
+                float c, s;
+                if (beta < 0) {
+                    const double delta = dm(ds(gamma, beta), 0.5);
+                    s = __double2float_rn(__dsqrt_rn(dd(delta, gamma)));
+                    c = __double2float_rn(dd(p, dm(dm(gamma, (double)s), 2.0)));
+                } else {
+                    c = __double2float_rn(__dsqrt_rn(dd(da(gamma, beta), dm(gamma, 2.0))));
+                    s = __double2float_rn(dd(p, dm(dm(gamma, (double)c), 2.0)));
+                }
+                a = 0; b = 0;
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const float t0 = fa(fm(c, At[i][k]), fm(s, At[j][k]));
+                    const float t1 = fa(fm(-s, At[i][k]), fm(c, At[j][k]));
+                    At[i][k] = t0; At[j][k] = t1;
+                    a = da(a, dm((double)t0, (double)t0));
+                    b = da(b, dm((double)t1, (double)t1));
+                }
+                W[i] = a; W[j] = b;
+                changed = true;
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const float t0 = fa(fm(Vt[i][k], c), fm(Vt[j][k], s));
+                    const float t1 = fs(fm(Vt[j][k], c), fm(Vt[i][k], s));
+                    Vt[i][k] = t0; Vt[j][k] = t1;
+                }
+            }
+        if (!changed) break;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        double sd = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) sd = da(sd, dm((double)At[i][k], (double)At[i][k]));
+        W[i] = __dsqrt_rn(sd);
+    }
+    // descending selection sort; swaps are register moves by predicate so the arrays stay in registers
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        int j = i;
+        double wj = W[i];
+#pragma unroll
+        for (int k = i + 1; k < 4; k++)
+            if (wj < W[k]) { j = k; wj = W[k]; }
+#pragma unroll
+        for (int k = i + 1; k < 4; k++)
+            if (j == k) {
+                const double tw = W[i]; W[i] = W[k]; W[k] = tw;
+#pragma unroll
+                for (int q = 0; q < 4; q++) { const float tv = Vt[i][q]; Vt[i][q] = Vt[k][q]; Vt[k][q] = tv; }
+            }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) w_out[i] = __double2float_rn(W[i]);
+}
+
+// cvu::triangulate: A rows = fma(x, P.row(2), -P.row(0)) (cv::addWeighted), SVD, vt.row(3), then x3D / w as
+// convertTo(scale = 1./w): x * (float)(1.0 / w) + 0.
+__device__ __forceinline__ F3 triangulate(float x1, float y1, float x2, float y2, const float* P1, const float* P2) {
+    float A[16], w[4], Vt[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        A[k] = __fmaf_rn(x1, P1[8 + k], -P1[k]);
+        A[4 + k] = __fmaf_rn(y1, P1[8 + k], -P1[4 + k]);
+        A[8 + k] = __fmaf_rn(x2, P2[8 + k], -P2[k]);
+        A[12 + k] = __fmaf_rn(y2, P2[8 + k], -P2[4 + k]);
+    }
+    svd4(A, w, Vt);
+    const double inv = dd(1.0, (double)Vt[3][3]);
+    float r[3];
+    if (fabs(inv) == 1.0) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) r[k] = fa(__double2float_rn(dm((double)Vt[3][k], inv)), 0.f);
+    } else {
+        const float a = __double2float_rn(inv);
+#pragma unroll
+        for (int k = 0; k < 3; k++) r[k] = fa(fm(Vt[3][k], a), 0.f);
+    }
+    return {r[0], r[1], r[2]};
+}
+
+// cv::Rodrigues of a float rotation vector: double arithmetic, rounded to float
+__device__ __forceinline__ void rodrigues(const float* rv, float* R) {
+    double rx = rv[0], ry = rv[1], rz = rv[2];
+    const double theta = __dsqrt_rn(da(da(dm(rx, rx), dm(ry, ry)), dm(rz, rz)));
+    if (theta < DBL_EPSILON) {
+#pragma unroll
+        for (int i = 0; i < 9; i++) R[i] = (i % 4 == 0) ? 1.f : 0.f;
+        return;
+    }
+    double s, c;
+    sincos(theta, &s, &c);
+    const double c1 = ds(1.0, c);
+    const double itheta = theta != 0.0 ? dd(1.0, theta) : 0.0;
+    rx = dm(rx, itheta); ry = dm(ry, itheta); rz = dm(rz, itheta);
+    const double rrt[9] = {dm(rx, rx), dm(rx, ry), dm(rx, rz), dm(rx, ry), dm(ry, ry), dm(ry, rz), dm(rx, rz), dm(ry, rz), dm(rz, rz)};
+    const double r_x[9] = {0, -rz, ry, rz, 0, -rx, -ry, rx, 0};
+#pragma unroll
+    for (int i = 0; i < 9; i++) {
+        const double e = (i % 4 == 0) ? 1.0 : 0.0;
+        R[i] = __double2float_rn(da(da(dm(c, e), dm(c1, rrt[i])), dm(s, r_x[i])));
+    }
+}
+
+// Track::calcSE3toXYZInfo (Track.cpp:259-306); a null info1 / info2 skips that half
+__device__ __forceinline__ void xyz_info(F3 xyz1, const float* Tcw1, const float* Tcw2, float fx, double* info1, double* info2) {
+    float T1i[16], T2i[16];
+    inv4(Tcw1, T1i);
+    inv4(Tcw2, T2i);
+    const F3 O1 = {T1i[3], T1i[7], T1i[11]}, O2 = {T2i[3], T2i[7], T2i[11]};
+    const F3 xyz = se3map(T1i, xyz1);
+    const F3 vO1 = sub3(xyz, O1), vO2 = sub3(xyz, O2);
+    const float sinParallax = __double2float_rn(dd(norm3(cross3(vO1, vO2)), dm(norm3(vO1), norm3(vO2))));
+    const F3 xyz2 = se3map(Tcw2, xyz);
+    const float length1 = __double2float_rn(norm3(xyz1)), length2 = __double2float_rn(norm3(xyz2));
+    const float dxy1 = fd(fm(2.f, length1), fx), dxy2 = fd(fm(2.f, length2), fx);
+    const float dz1 = fd(dxy2, sinParallax), dz2 = fd(dxy1, sinParallax);
+    const float d1[3] = {fd(1.f, fm(dxy1, dxy1)), fd(1.f, fm(dxy1, dxy1)), fd(1.f, fm(dz1, dz1))};
+    const float d2[3] = {fd(1.f, fm(dxy2, dxy2)), fd(1.f, fm(dxy2, dxy2)), fd(1.f, fm(dz2, dz2))};
+    const F3 xx[2] = {xyz1, xyz2};
+    const float len[2] = {length1, length2};
+    const float* dg[2] = {d1, d2};
+    double* out[2] = {info1, info2};
+#pragma unroll
+    for (int v = 0; v < 2; v++) {
+        if (!out[v]) continue;
+        const F3 z = {0.f, 0.f, len[v]};
+        const F3 k = cross3(xx[v], z);
+        const float normk = __double2float_rn(norm3(k));
+        const float sinv = __double2float_rn(dd((double)normk, dm(norm3(z), norm3(xx[v]))));
+        const float f = fd(asinf_host(sinv), normk);
+        const float kv[3] = {fm(k.x, f), fm(k.y, f), fm(k.z, f)};
+        float R[9];
+        rodrigues(kv, R);
+        // R.t() * info (generic gemm, double sums; info is diagonal with +0 off the diagonal), then (...) * R (small path)
+        float I[9] = {dg[v][0], 0.f, 0.f, 0.f, dg[v][1], 0.f, 0.f, 0.f, dg[v][2]};
+        float tmp[9];
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                double s = 0;
+#pragma unroll
+                for (int q = 0; q < 3; q++) s = da(s, dm((double)R[q * 3 + i], (double)I[q * 3 + j]));
+                tmp[i * 3 + j] = __double2float_rn(dm(s, 1.0));
+            }
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+#pragma unroll
+            for (int j = 0; j < 3; j++) out[v][i * 3 + j] = (double)gemm3_elem(tmp, 3, i, R, 3, j, 1.0);
+    }
+}
+
+__device__ __forceinline__ int count_of(const int* d_n, int cap) { return d_n ? min(max(*d_n, 0), cap) : cap; }
+
+// warp-aggregated counter: one atomic per warp
+__device__ __forceinline__ void warp_count(int* counter, bool pred) {
+    const unsigned b = __ballot_sync(0xffffffffu, pred);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(counter, __popc(b));
+}
+
+__global__ void __launch_bounds__(kBlock) k_triangulate(int n, const float* __restrict__ pt1, const float* __restrict__ pt2,
+                                                        const float* __restrict__ P, const int* __restrict__ idx1,
+                                                        const int* __restrict__ idx2, float* __restrict__ xyz) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float P1[12], P2[12];
+    const float* p1 = P + 12 * idx1[i];
+    const float* p2 = P + 12 * idx2[i];
+#pragma unroll
+    for (int k = 0; k < 12; k++) { P1[k] = p1[k]; P2[k] = p2[k]; }
+    const F3 r = triangulate(pt1[2 * i], pt1[2 * i + 1], pt2[2 * i], pt2[2 * i + 1], P1, P2);
+    xyz[3 * i] = r.x; xyz[3 * i + 1] = r.y; xyz[3 * i + 2] = r.z;
+}
+
+__global__ void __launch_bounds__(kBlock) k_track_triangulate(
+    const se2gpu_keypoint* __restrict__ kp_kf, int cap, const int* __restrict__ d_n, const se2gpu_keypoint* __restrict__ kp_fr,
+    int* __restrict__ matches, const uint8_t* __restrict__ observed, const float* __restrict__ view_mp,
+    const float* __restrict__ Tcr_g, const float* __restrict__ K_g, float lower, float upper, float min_cos,
+    float* __restrict__ local_mps, uint8_t* __restrict__ good_prl, int* __restrict__ counts) {
+    // P_KF = Config::PrjMtrxEye, P = Kcam * Tcr.rowRange(0,3) and Ocam = inv(Tcr).col(3) are the same for the whole launch:
+    // one thread per block builds them in shared memory
+    __shared__ float sP[24], sO[3];
+    if (threadIdx.x == 0) {
+        float Tcr[16], K[9], Ti[16];
+#pragma unroll
+        for (int k = 0; k < 16; k++) Tcr[k] = Tcr_g[k];
+#pragma unroll
+        for (int k = 0; k < 9; k++) K[k] = K_g[k];
+        const float eye34[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+        projection(K, eye34, sP);
+        projection(K, Tcr, sP + 12);
+        inv4(Tcr, Ti);
+        sO[0] = Ti[3]; sO[1] = Ti[7]; sO[2] = Ti[11];
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n = count_of(d_n, cap);
+    bool tracked = false, good = false;
+    if (i < n) {
+        good_prl[i] = 0;
+        const int m = matches[i];
+        if (m >= 0) {
+            if (observed[i]) {
+                local_mps[3 * i] = view_mp[3 * i]; local_mps[3 * i + 1] = view_mp[3 * i + 1]; local_mps[3 * i + 2] = view_mp[3 * i + 2];
+                tracked = true;
+            } else {
+                float P_KF[12], P[12];
+#pragma unroll
+                for (int k = 0; k < 12; k++) { P_KF[k] = sP[k]; P[k] = sP[12 + k]; }
+                const se2gpu_keypoint a = kp_kf[i], b = kp_fr[m];
+                const F3 pos = triangulate(a.x, a.y, b.x, b.y, P_KF, P);
+                if (pos.z >= lower && pos.z <= upper) {
+                    local_mps[3 * i] = pos.x; local_mps[3 * i + 1] = pos.y; local_mps[3 * i + 2] = pos.z;
+                    // cvu::checkParallax(0, Ocam, pos, deg)
+                    const F3 p1 = sub3(pos, {0.f, 0.f, 0.f}), p2 = sub3(pos, {sO[0], sO[1], sO[2]});
+                    const float cosp = __double2float_rn(dd(fabs((double)dot3(p1, p2)), dm(norm3(p1), norm3(p2))));
+                    if (cosp < min_cos) { good = true; good_prl[i] = 1; }
+                } else {
+                    matches[i] = -1;
+                }
+            }
+        }
+    }
+    warp_count(counts, tracked);
+    warp_count(counts + 1, good);
+}
+
+__global__ void __launch_bounds__(kBlock) k_xyz_info(int n, const float* __restrict__ xyz1, const int* __restrict__ pose1,
+                                                     const int* __restrict__ pose2, const float* __restrict__ Tcw, float fx,
+                                                     double* __restrict__ info1, double* __restrict__ info2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float T1[16], T2[16];
+    const float* a = Tcw + 16 * pose1[i];
+    const float* b = Tcw + 16 * pose2[i];
+#pragma unroll
+    for (int k = 0; k < 16; k++) { T1[k] = a[k]; T2[k] = b[k]; }
+    double o1[9], o2[9];
+    xyz_info({xyz1[3 * i], xyz1[3 * i + 1], xyz1[3 * i + 2]}, T1, T2, fx, o1, o2);
+#pragma unroll
+    for (int k = 0; k < 9; k++) { info1[9 * i + k] = o1[k]; info2[9 * i + k] = o2[k]; }
+}
+
+struct MpTable {
+    const float* main_measure; const int* main_pose; const int* main_octave; const float* normal;
+    const float* min_dist; const float* max_dist;
+};
+
+__global__ void __launch_bounds__(kBlock) k_projection_observations(
+    const se2gpu_keypoint* __restrict__ kf_kp, int cap, const int* __restrict__ d_n, const int* __restrict__ match_mp,
+    const float* __restrict__ Tnew_g, MpTable mp, const float* __restrict__ Tcw_table, const float* __restrict__ K_g,
+    float lower, float upper, float fx, uint8_t* __restrict__ accept, float* __restrict__ pos_out, double* __restrict__ info_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count_of(d_n, cap)) return;
+    accept[i] = 0;
+    const int m = match_mp[i];
+    if (m < 0) return;
+    float Tn[16], Tm[16], K[9], P1[12], P2[12];
+    const float* tm = Tcw_table + 16 * mp.main_pose[m];
+#pragma unroll
+    for (int k = 0; k < 16; k++) { Tn[k] = Tnew_g[k]; Tm[k] = tm[k]; }
+#pragma unroll
+    for (int k = 0; k < 9; k++) K[k] = K_g[k];
+    projection(K, Tm, P1);
+    projection(K, Tn, P2);
+    const se2gpu_keypoint kp = kf_kp[i];
+    const F3 x3d = triangulate(mp.main_measure[2 * m], mp.main_measure[2 * m + 1], kp.x, kp.y, P1, P2);
+    const F3 pos = se3map(Tn, x3d);
+    // MapPoint::acceptNewObserve
+    const F3 nv = {mp.normal[3 * m], mp.normal[3 * m + 1], mp.normal[3 * m + 2]};
+    const float dist = __double2float_rn(norm3(pos));
+    const float cosAngle = __double2float_rn(dd(fabs((double)dot3(pos, nv)), dm((double)dist, norm3(nv))));
+    const bool c1 = abs(mp.main_octave[m] - kp.octave) <= 2;
+    const bool c2 = cosAngle >= 0.866f;
+    const bool c3 = dist >= mp.min_dist[m] && dist <= mp.max_dist[m];
+    if (!(c1 && c2 && c3)) return;
+    if (pos.z > upper || pos.z < lower) return;
+    double info[9];
+    xyz_info(pos, Tn, Tm, fx, info, nullptr);
+    pos_out[3 * i] = pos.x; pos_out[3 * i + 1] = pos.y; pos_out[3 * i + 2] = pos.z;
+#pragma unroll
+    for (int k = 0; k < 9; k++) info_out[9 * i + k] = info[k];
+    accept[i] = 1;
+}
+
+__global__ void k_debug_svd4(int n, const float* __restrict__ A, float* __restrict__ w, float* __restrict__ vt) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float a[16], ww[4], V[4][4];
+#pragma unroll
+    for (int k = 0; k < 16; k++) a[k] = A[16 * i + k];
+    svd4(a, ww, V);
+#pragma unroll
+    for (int k = 0; k < 4; k++) w[4 * i + k] = ww[k];
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+#pragma unroll
+        for (int k = 0; k < 4; k++) vt[16 * i + 4 * r + k] = V[r][k];
+}
+
+inline int blocks(int n) { return (n + kBlock - 1) / kBlock; }
+
+const float kMinCos[4] = {0.9998f, 0.9994f, 0.9986f, 0.9976f};   // cvu::checkParallax
+
+int need_device() {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available");
+    return SE2GPU_OK;
+}
+
+// scoped device buffers of the host-buffer entry points
+struct DevBufs {
+    void* p[16];
+    int n = 0;
+    ~DevBufs() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
+    template <class T>
+    T* get(size_t count) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, count ? count * sizeof(T) : 1) != cudaSuccess) return nullptr;
+        p[n++] = q;
+        return static_cast<T*>(q);
+    }
+    template <class T>
+    T* upload(const T* h, size_t count) {
+        T* d = get<T>(count);
+        if (d && count && cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+        return d;
+    }
+};
+
+}  // namespace
+
+// ------------------------------------------------------------------------------------------ device-buffer entries
+int se2gpu_triangulate_device(int n, const float* d_pt1, const float* d_pt2, const float* d_P, const int* d_idx1,
+                              const int* d_idx2, float* d_xyz, void* stream) {
+    if (n < 0 || (n && (!d_pt1 || !d_pt2 || !d_P || !d_idx1 || !d_idx2 || !d_xyz))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = need_device(); if (rc) return rc; }
+    if (n == 0) return SE2GPU_OK;
+    SE2_LAUNCH(k_triangulate, blocks(n), kBlock, 0, (cudaStream_t)stream, n, d_pt1, d_pt2, d_P, d_idx1, d_idx2, d_xyz);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, const int* d_n_kf, const se2gpu_keypoint* d_kp_frame,
+                                    int* d_matches12, const uint8_t* d_kf_observed, const float* d_kf_view_mp, const float* d_Tcr,
+                                    const float* d_K, float lower_depth, float upper_depth, int min_parallax_deg,
+                                    float* d_local_mps, uint8_t* d_good_prl, int* d_counts, void* stream) {
+    if (n_kf < 0 || !d_counts || min_parallax_deg < 1 || min_parallax_deg > 4 || !d_Tcr || !d_K) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (n_kf && (!d_kp_kf || !d_kp_frame || !d_matches12 || !d_kf_observed || !d_kf_view_mp || !d_local_mps || !d_good_prl))
+        return fail(SE2GPU_ERR_INVALID, "null argument");
+    { const int rc = need_device(); if (rc) return rc; }
+    cudaStream_t s = (cudaStream_t)stream;
+    SE2_CUDA(cudaMemsetAsync(d_counts, 0, 2 * sizeof(int), s));
+    if (n_kf == 0) return SE2GPU_OK;
+    SE2_LAUNCH(k_track_triangulate, blocks(n_kf), kBlock, 0, s, d_kp_kf, n_kf, d_n_kf, d_kp_frame, d_matches12, d_kf_observed,
+               d_kf_view_mp, d_Tcr, d_K, lower_depth, upper_depth, kMinCos[min_parallax_deg - 1], d_local_mps, d_good_prl, d_counts);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+int se2gpu_xyz_info_device(int n, const float* d_xyz1, const int* d_pose1, const int* d_pose2, const float* d_Tcw, float fx,
+                           double* d_info1, double* d_info2, void* stream) {
+    if (n < 0 || (n && (!d_xyz1 || !d_pose1 || !d_pose2 || !d_Tcw || !d_info1 || !d_info2))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = need_device(); if (rc) return rc; }
+    if (n == 0) return SE2GPU_OK;
+    SE2_LAUNCH(k_xyz_info, blocks(n), kBlock, 0, (cudaStream_t)stream, n, d_xyz1, d_pose1, d_pose2, d_Tcw, fx, d_info1, d_info2);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+int se2gpu_projection_observations_device(const se2gpu_keypoint* d_kf_kp, int n_kf, const int* d_n_kf, const int* d_matches_idx_mp,
+                                          const float* d_Tcw_new, const float* d_mp_main_measure, const int* d_mp_main_pose,
+                                          const int* d_mp_main_octave, const float* d_mp_normal, const float* d_mp_min_dist,
+                                          const float* d_mp_max_dist, const float* d_Tcw_table, const float* d_K, float lower_depth,
+                                          float upper_depth, float fx, uint8_t* d_accept, float* d_pos_new_kf, double* d_info_new,
+                                          void* stream) {
+    if (n_kf < 0) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (n_kf && (!d_kf_kp || !d_matches_idx_mp || !d_Tcw_new || !d_mp_main_measure || !d_mp_main_pose || !d_mp_main_octave ||
+                 !d_mp_normal || !d_mp_min_dist || !d_mp_max_dist || !d_Tcw_table || !d_K || !d_accept || !d_pos_new_kf || !d_info_new))
+        return fail(SE2GPU_ERR_INVALID, "null argument");
+    { const int rc = need_device(); if (rc) return rc; }
+    if (n_kf == 0) return SE2GPU_OK;
+    const MpTable mp{d_mp_main_measure, d_mp_main_pose, d_mp_main_octave, d_mp_normal, d_mp_min_dist, d_mp_max_dist};
+    SE2_LAUNCH(k_projection_observations, blocks(n_kf), kBlock, 0, (cudaStream_t)stream, d_kf_kp, n_kf, d_n_kf, d_matches_idx_mp,
+               d_Tcw_new, mp, d_Tcw_table, d_K, lower_depth, upper_depth, fx, d_accept, d_pos_new_kf, d_info_new);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------ host-buffer entries
+namespace {
+bool indices_ok(const int* idx, int n, int hi) {
+    for (int i = 0; i < n; i++)
+        if (idx[i] < 0 || idx[i] >= hi) return false;
+    return true;
+}
+}  // namespace
+
+#define GEOM_ALLOC(ptr) \
+    if (!(ptr)) return fail(SE2GPU_ERR_CUDA, "device allocation or copy failed")
+
+int se2gpu_triangulate(int n, const float* pt1, const float* pt2, const float* P, int n_proj, const int* idx1, const int* idx2,
+                       float* xyz, int device) {
+    if (n < 0 || n_proj < 0 || (n && (!pt1 || !pt2 || !P || !idx1 || !idx2 || !xyz))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (!indices_ok(idx1, n, n_proj) || !indices_ok(idx2, n, n_proj)) return fail(SE2GPU_ERR_INVALID, "projection index out of range");
+    { const int rc = select_device(device); if (rc) return rc; }
+    if (n == 0) return SE2GPU_OK;
+    DevBufs b;
+    const float* d1 = b.upload(pt1, 2 * (size_t)n); GEOM_ALLOC(d1);
+    const float* d2 = b.upload(pt2, 2 * (size_t)n); GEOM_ALLOC(d2);
+    const float* dP = b.upload(P, 12 * (size_t)n_proj); GEOM_ALLOC(dP);
+    const int* i1 = b.upload(idx1, n); GEOM_ALLOC(i1);
+    const int* i2 = b.upload(idx2, n); GEOM_ALLOC(i2);
+    float* dx = b.get<float>(3 * (size_t)n); GEOM_ALLOC(dx);
+    { const int rc = se2gpu_triangulate_device(n, d1, d2, dP, i1, i2, dx, nullptr); if (rc) return rc; }
+    SE2_CUDA(cudaMemcpy(xyz, dx, 3 * sizeof(float) * n, cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
+
+int se2gpu_track_triangulate(const se2gpu_keypoint* kp_kf, int n_kf, const se2gpu_keypoint* kp_frame, int n_frame, int* matches12,
+                             const uint8_t* kf_observed, const float* kf_view_mp, const float* Tcr, const float* K,
+                             float lower_depth, float upper_depth, int min_parallax_deg, float* local_mps, uint8_t* good_prl,
+                             int* counts, int device) {
+    if (n_kf < 0 || n_frame < 0 || !counts || !Tcr || !K || min_parallax_deg < 1 || min_parallax_deg > 4)
+        return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (n_kf && (!kp_kf || !matches12 || !kf_observed || !kf_view_mp || !local_mps || !good_prl)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    for (int i = 0; i < n_kf; i++)
+        if (matches12[i] >= n_frame) return fail(SE2GPU_ERR_INVALID, "matches12[%d] = %d is not a frame keypoint", i, matches12[i]);
+    if (n_frame && !kp_frame) return fail(SE2GPU_ERR_INVALID, "null argument");
+    { const int rc = select_device(device); if (rc) return rc; }
+    counts[0] = counts[1] = 0;
+    if (n_kf == 0) return SE2GPU_OK;
+    DevBufs b;
+    const se2gpu_keypoint* dk = b.upload(kp_kf, n_kf); GEOM_ALLOC(dk);
+    const se2gpu_keypoint* df = b.upload(kp_frame, n_frame); GEOM_ALLOC(df);
+    int* dm12 = b.upload(matches12, n_kf); GEOM_ALLOC(dm12);
+    const uint8_t* dobs = b.upload(kf_observed, n_kf); GEOM_ALLOC(dobs);
+    const float* dvm = b.upload(kf_view_mp, 3 * (size_t)n_kf); GEOM_ALLOC(dvm);
+    const float* dT = b.upload(Tcr, 16); GEOM_ALLOC(dT);
+    const float* dK = b.upload(K, 9); GEOM_ALLOC(dK);
+    float* dl = b.upload(local_mps, 3 * (size_t)n_kf); GEOM_ALLOC(dl);
+    uint8_t* dg = b.get<uint8_t>(n_kf); GEOM_ALLOC(dg);
+    int* dc = b.get<int>(2); GEOM_ALLOC(dc);
+    { const int rc = se2gpu_track_triangulate_device(dk, n_kf, nullptr, df, dm12, dobs, dvm, dT, dK, lower_depth, upper_depth,
+                                                     min_parallax_deg, dl, dg, dc, nullptr); if (rc) return rc; }
+    SE2_CUDA(cudaMemcpy(matches12, dm12, sizeof(int) * n_kf, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(local_mps, dl, 3 * sizeof(float) * n_kf, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(good_prl, dg, n_kf, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(counts, dc, 2 * sizeof(int), cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
+
+int se2gpu_xyz_info(int n, const float* xyz1, const int* pose1, const int* pose2, const float* Tcw, int n_pose, float fx,
+                    double* info1, double* info2, int device) {
+    if (n < 0 || n_pose < 0 || (n && (!xyz1 || !pose1 || !pose2 || !Tcw || !info1 || !info2))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (!indices_ok(pose1, n, n_pose) || !indices_ok(pose2, n, n_pose)) return fail(SE2GPU_ERR_INVALID, "pose index out of range");
+    { const int rc = select_device(device); if (rc) return rc; }
+    if (n == 0) return SE2GPU_OK;
+    DevBufs b;
+    const float* dx = b.upload(xyz1, 3 * (size_t)n); GEOM_ALLOC(dx);
+    const int* p1 = b.upload(pose1, n); GEOM_ALLOC(p1);
+    const int* p2 = b.upload(pose2, n); GEOM_ALLOC(p2);
+    const float* dT = b.upload(Tcw, 16 * (size_t)n_pose); GEOM_ALLOC(dT);
+    double* i1 = b.get<double>(9 * (size_t)n); GEOM_ALLOC(i1);
+    double* i2 = b.get<double>(9 * (size_t)n); GEOM_ALLOC(i2);
+    { const int rc = se2gpu_xyz_info_device(n, dx, p1, p2, dT, fx, i1, i2, nullptr); if (rc) return rc; }
+    SE2_CUDA(cudaMemcpy(info1, i1, 9 * sizeof(double) * n, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(info2, i2, 9 * sizeof(double) * n, cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
+
+int se2gpu_projection_observations(const se2gpu_keypoint* kf_kp, int n_kf, const int* matches_idx_mp, const float* Tcw_new,
+                                   const float* mp_main_measure, const int* mp_main_pose, const int* mp_main_octave,
+                                   const float* mp_normal, const float* mp_min_dist, const float* mp_max_dist, int n_mp,
+                                   const float* Tcw_table, int n_pose, const float* K, float lower_depth, float upper_depth,
+                                   float fx, uint8_t* accept, float* pos_new_kf, double* info_new, int device) {
+    if (n_kf < 0 || n_mp < 0 || n_pose < 0) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (n_kf && (!kf_kp || !matches_idx_mp || !Tcw_new || !K || !accept || !pos_new_kf || !info_new)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (n_mp && (!mp_main_measure || !mp_main_pose || !mp_main_octave || !mp_normal || !mp_min_dist || !mp_max_dist || !Tcw_table))
+        return fail(SE2GPU_ERR_INVALID, "null argument");
+    for (int i = 0; i < n_kf; i++)
+        if (matches_idx_mp[i] >= n_mp) return fail(SE2GPU_ERR_INVALID, "matches_idx_mp[%d] = %d is not a map point", i, matches_idx_mp[i]);
+    if (!indices_ok(mp_main_pose, n_mp, n_pose)) return fail(SE2GPU_ERR_INVALID, "main keyframe index out of range");
+    { const int rc = select_device(device); if (rc) return rc; }
+    if (n_kf == 0) return SE2GPU_OK;
+    DevBufs b;
+    const size_t m = n_mp ? n_mp : 1;
+    const float zero16[16] = {0};
+    const se2gpu_keypoint* dk = b.upload(kf_kp, n_kf); GEOM_ALLOC(dk);
+    const int* dmi = b.upload(matches_idx_mp, n_kf); GEOM_ALLOC(dmi);
+    const float* dTn = b.upload(Tcw_new, 16); GEOM_ALLOC(dTn);
+    const float* dmm = n_mp ? b.upload(mp_main_measure, 2 * m) : b.upload(zero16, 2); GEOM_ALLOC(dmm);
+    const int* dmp = n_mp ? b.upload(mp_main_pose, m) : b.get<int>(1); GEOM_ALLOC(dmp);
+    const int* dmo = n_mp ? b.upload(mp_main_octave, m) : b.get<int>(1); GEOM_ALLOC(dmo);
+    const float* dnv = n_mp ? b.upload(mp_normal, 3 * m) : b.upload(zero16, 3); GEOM_ALLOC(dnv);
+    const float* dmin = n_mp ? b.upload(mp_min_dist, m) : b.upload(zero16, 1); GEOM_ALLOC(dmin);
+    const float* dmax = n_mp ? b.upload(mp_max_dist, m) : b.upload(zero16, 1); GEOM_ALLOC(dmax);
+    const float* dtab = n_pose ? b.upload(Tcw_table, 16 * (size_t)n_pose) : b.upload(zero16, 16); GEOM_ALLOC(dtab);
+    const float* dK = b.upload(K, 9); GEOM_ALLOC(dK);
+    uint8_t* dacc = b.get<uint8_t>(n_kf); GEOM_ALLOC(dacc);
+    float* dpos = b.upload(pos_new_kf, 3 * (size_t)n_kf); GEOM_ALLOC(dpos);
+    double* dinfo = b.upload(info_new, 9 * (size_t)n_kf); GEOM_ALLOC(dinfo);
+    { const int rc = se2gpu_projection_observations_device(dk, n_kf, nullptr, dmi, dTn, dmm, dmp, dmo, dnv, dmin, dmax, dtab, dK,
+                                                           lower_depth, upper_depth, fx, dacc, dpos, dinfo, nullptr); if (rc) return rc; }
+    SE2_CUDA(cudaMemcpy(accept, dacc, n_kf, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(pos_new_kf, dpos, 3 * sizeof(float) * n_kf, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(info_new, dinfo, 9 * sizeof(double) * n_kf, cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
+
+int se2gpu_debug_svd4(int n, const float* A, float* w, float* vt, int device) {
+    if (n < 0 || (n && (!A || !w || !vt))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = select_device(device); if (rc) return rc; }
+    if (n == 0) return SE2GPU_OK;
+    DevBufs b;
+    const float* dA = b.upload(A, 16 * (size_t)n); GEOM_ALLOC(dA);
+    float* dw = b.get<float>(4 * (size_t)n); GEOM_ALLOC(dw);
+    float* dv = b.get<float>(16 * (size_t)n); GEOM_ALLOC(dv);
+    SE2_LAUNCH(k_debug_svd4, blocks(n), kBlock, 0, (cudaStream_t)0, n, dA, dw, dv);
+    SE2_CUDA(cudaGetLastError());
+    SE2_CUDA(cudaMemcpy(w, dw, 4 * sizeof(float) * n, cudaMemcpyDeviceToHost));
+    SE2_CUDA(cudaMemcpy(vt, dv, 16 * sizeof(float) * n, cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
