@@ -40,9 +40,9 @@ PEER_HANDLE_BYTES = 128   # SE2GPU_BA_PEER_HANDLE_BYTES
 
 SYMBOLS = [
     "se2gpu_device_count", "se2gpu_last_error", "se2gpu_launch_count",
-    "se2gpu_orb_create", "se2gpu_orb_destroy", "se2gpu_orb_extract", "se2gpu_orb_extract_device", "se2gpu_orb_submit", "se2gpu_orb_wait",
+    "se2gpu_orb_create", "se2gpu_orb_create_scored", "se2gpu_orb_destroy", "se2gpu_orb_extract", "se2gpu_orb_extract_device", "se2gpu_orb_submit", "se2gpu_orb_wait",
     "se2gpu_orb_level_dims", "se2gpu_orb_get_level", "se2gpu_orb_profile", "se2gpu_orb_profile_read",
-    "se2gpu_orb_debug_nth_element", "se2gpu_orb_set_undistort", "se2gpu_orb_debug_undistort_map",
+    "se2gpu_orb_debug_nth_element", "se2gpu_orb_debug_nth_element_f32", "se2gpu_orb_set_undistort", "se2gpu_orb_debug_undistort_map",
     "se2gpu_hamming_distance", "se2gpu_match_by_window", "se2gpu_match_by_projection", "se2gpu_search_by_bow",
     "se2gpu_matcher_create", "se2gpu_matcher_destroy", "se2gpu_match_by_window_device", "se2gpu_keypoints_to_points_device",
     "se2gpu_match_by_projection_device", "se2gpu_matcher_match_by_window", "se2gpu_matcher_match_by_projection",
@@ -77,6 +77,8 @@ def lib():
     L.se2gpu_launch_count.restype = C.c_ulonglong
     L.se2gpu_orb_create.restype = vp
     L.se2gpu_orb_create.argtypes = [i, f, i, i, i, i, i, i]
+    L.se2gpu_orb_create_scored.restype = vp
+    L.se2gpu_orb_create_scored.argtypes = [i, f, i, i, i, i, i, i, i]
     L.se2gpu_orb_destroy.argtypes = [vp]
     L.se2gpu_orb_extract.argtypes = [vp, vp, i, i, i, i, sz, vp, vp, vp]
     L.se2gpu_orb_submit.argtypes = [vp, vp, i, i, i, i, sz, vp, vp, vp]
@@ -87,6 +89,7 @@ def lib():
     L.se2gpu_orb_profile.argtypes = [vp, i]
     L.se2gpu_orb_profile_read.argtypes = [vp, vp, vp]
     L.se2gpu_orb_debug_nth_element.argtypes = [vp, vp, vp, i, i]
+    L.se2gpu_orb_debug_nth_element_f32.argtypes = [vp, vp, vp, i, vp, i]
     L.se2gpu_orb_set_undistort.argtypes = [vp, vp, vp, i]
     L.se2gpu_orb_debug_undistort_map.argtypes = [vp, vp, i, i, i, vp, vp]
     L.se2gpu_ba_reset.argtypes = [vp]

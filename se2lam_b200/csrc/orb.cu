@@ -11,8 +11,11 @@
 //                           M = max over the 16 nine-pixel arcs of min(+-diff) (corner at t <=> M > t, score = M-1)
 //                           at full lane occupancy, cell-local 3x3 strict NMS into a bitmap, raster-ordered emission
 //   orb_fast_cells_big      the same result for cells too large for the shared-memory candidate list
-//   orb_select              quota redistribution :631-679 + KeyPointsFilter::retainBest twice :687-710 — the
-//                           libstdc++ introselect permutation is reproduced exactly, warp-cooperatively (introselect.h)
+//   orb_harris              HARRIS_SCORE handles only: HarrisResponses(cell, kps, 7, 0.04f) :85-126, :625-629 on the un-blurred
+//                           level, one 64-bit record (order key of the response, FAST record) per candidate
+//   orb_select<HARRIS>      quota redistribution :631-679 + KeyPointsFilter::retainBest twice :687-710 — the
+//                           libstdc++ introselect permutation is reproduced exactly, warp-cooperatively (introselect.h);
+//                           keyed by the FAST score, or by the Harris response on 64-bit records
 //   orb_blur                GaussianBlur 7x7 sigma 2 :769 (float32 separable, fused multiply-add, RNE to u8)
 //   orb_orient_describe     IC_Angle :130-157 + computeOrbDescriptor :160-200, one warp per keypoint; keypoint
 //                           records are written as 28-byte cv::KeyPoint and 32-byte descriptors
@@ -23,12 +26,14 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "blur_px.h"
 #include "common.h"
 #include "fast_screen.h"
 #include "introselect.h"
+#include "resp_key.h"
 
 namespace {
 
@@ -731,14 +736,76 @@ __global__ void __launch_bounds__(FAST_THREADS) orb_fast_cells_big(OrbDev d) {
     if (threadIdx.x == 0) { hdr->n_base = s_total; hdr->n_a = s_total; hdr->n_b = s_total; }
 }
 
+// HARRIS_SCORE: HarrisResponses(cellImage, cellKeyPoints, 7, HARRIS_K = 0.04f) (ORBextractor.cpp:85-126, called at :625-629 after
+// the FAST / FAST(7) fallback of every cell). One CTA per (cell, frame), threads striding over the cell's candidate list in the
+// raster order the FAST kernel left it (any of the three FAST kernels). A candidate's 7x7 block of 3x3 Sobel-like gradients
+// reads the 9x9 footprint around it on the un-blurred level (4 px beyond the keypoint: one pixel past the cell's FAST apron,
+// always inside the level ROI), as three aligned 32-bit words per row funnel-shifted to the footprint's first column.
+// a = sum Ix^2, b = sum Iy^2, c = sum Ix*Iy in int32 (|Ix|, |Iy| <= 1020, 49 * 1020^2 < 2^31), then the reference's float
+// expression in C++ evaluation order with every operation rounded on its own (no contraction):
+//   ((float)a*b - (float)c*c - k*((float)a+b)*((float)a+b)) * scale_sq_sq,   scale_sq_sq = ((s*s)*s)*s,  s = 1/(4*7*255.f).
+// Output: cand64[i] = resp_key(response) << 32 | cand[i], the FAST record kept in the low word.
+constexpr int HARRIS_THREADS = 128;
+constexpr float HARRIS_SCALE = 1.0f / ((1 << 2) * 7 * 255.0f);   // float arithmetic, folded by the compiler
+constexpr float HARRIS_SCALE_SQ_SQ = HARRIS_SCALE * HARRIS_SCALE * HARRIS_SCALE * HARRIS_SCALE;
+__global__ void __launch_bounds__(HARRIS_THREADS) orb_harris(OrbDev d, uint64_t* __restrict__ cand64) {
+    const CellGeo c = d.cells[blockIdx.x];
+    const int f = blockIdx.y + d.frame0;
+    if (c.skipped) return;
+    const int n = min(d.hdr[(size_t)f * d.n_cells + blockIdx.x].n_base, c.cand_cap);
+    if (n <= 0) return;
+    const LevelGeo& L = d.levels[c.level];
+    const uint8_t* plane = d.plain + f * d.frame_plane_bytes + L.plane_off;
+    const size_t co = (size_t)f * d.cand_total + c.cand_off;
+    const uint32_t* cand = d.cand + co;
+    for (int i = threadIdx.x; i < n; i += HARRIS_THREADS) {
+        const uint32_t rec = cand[i];
+        const int x = rec & 0xFFF, y = (rec >> 12) & 0xFFF;
+        const int bx = EDGE + x - 4, ax = bx & ~3;
+        const unsigned sh = 8u * (unsigned)(bx - ax);
+        const uint8_t* row0 = plane + (size_t)(EDGE + y - 4) * L.pitch + ax;
+        int p[9][9];
+#pragma unroll
+        for (int r = 0; r < 9; ++r) {
+            const uint32_t* w = reinterpret_cast<const uint32_t*>(row0 + (size_t)r * L.pitch);
+            const uint32_t w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2);
+            const uint32_t lo = __funnelshift_r(w0, w1, sh), mid = __funnelshift_r(w1, w2, sh), hi = __funnelshift_r(w2, 0u, sh);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) { p[r][k] = __byte_perm(lo, 0u, 0x4440 + k); p[r][4 + k] = __byte_perm(mid, 0u, 0x4440 + k); }
+            p[r][8] = hi & 0xFF;
+        }
+        int a = 0, b = 0, cc = 0;
+#pragma unroll
+        for (int r = 1; r < 8; ++r)
+#pragma unroll
+            for (int k = 1; k < 8; ++k) {
+                const int Ix = (p[r][k + 1] - p[r][k - 1]) * 2 + (p[r - 1][k + 1] - p[r - 1][k - 1]) + (p[r + 1][k + 1] - p[r + 1][k - 1]);
+                const int Iy = (p[r + 1][k] - p[r - 1][k]) * 2 + (p[r + 1][k - 1] - p[r - 1][k - 1]) + (p[r + 1][k + 1] - p[r - 1][k + 1]);
+                a += Ix * Ix; b += Iy * Iy; cc += Ix * Iy;
+            }
+        const float fa = __int2float_rn(a), fb = __int2float_rn(b), fc = __int2float_rn(cc);
+        const float apb = __fadd_rn(fa, fb);
+        const float t = __fsub_rn(__fsub_rn(__fmul_rn(fa, fb), __fmul_rn(fc, fc)), __fmul_rn(__fmul_rn(0.04f, apb), apb));
+        const float resp = __fmul_rn(t, HARRIS_SCALE_SQ_SQ);
+        cand64[co + i] = ((uint64_t)se2gpu::resp_key(resp) << 32) | rec;
+    }
+}
+
 // one CTA per (level, frame): quota redistribution, retainBest per cell and per level. The cells' candidate lists
 // are staged in shared memory when the level's total fits (SEL_STAGE entries), otherwise they are processed in place
 // in global memory. retainBest is std::nth_element; one warp per cell runs the warp-cooperative introselect of
 // introselect.h (same permutation as libstdc++'s, 32 elements per step), cells round-robin over the CTA's warps.
+// HARRIS: the records are orb_harris' 64-bit ones (cand64, selected by their upper word), the stage holds half as many of
+// them (the same bytes), and the level lists are written as the 32-bit FAST records plus the float responses in lresp.
 constexpr int SEL_STAGE = 12288;
 constexpr int SEL_THREADS = 512;
-__global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d) {
-    extern __shared__ uint32_t sbuf[];   // [cap] level list | [4*nCells] ints | [SEL_STAGE] staged candidates
+struct HarrisBufs { uint64_t* cand64; float* lresp; };   // orb_select<true> / orb_orient_describe<true> only
+template <bool HARRIS>
+__global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d, HarrisBufs hb) {
+    typedef typename std::conditional<HARRIS, se2gpu::KpKey64, se2gpu::KpScore32>::type K;
+    typedef typename K::rec R;
+    constexpr int STAGE = HARRIS ? SEL_STAGE / 2 : SEL_STAGE;
+    extern __shared__ uint32_t sbuf[];   // [cap] level list | [4*nCells] ints | [STAGE] staged candidates (records of type R)
     __shared__ int wq[SEL_THREADS / 32][128];
     constexpr int NW = SEL_THREADS / 32;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -746,15 +813,17 @@ __global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d) {
     const LevelGeo& L = d.levels[level];
     const int nCells = L.nCells;
     const int cap = 2 * L.nDesired + 4 * nCells + 64;
-    uint32_t* lbuf = sbuf;
-    int* nTotal = (int*)(sbuf + cap);
+    R* lbuf = reinterpret_cast<R*>(sbuf);
+    int* nTotal = (int*)(lbuf + cap);
     int* nToRetain = nTotal + nCells;
     int* kept = nToRetain + nCells;
     int* koff = kept + nCells;
-    uint32_t* stage = (uint32_t*)(koff + nCells);
+    R* stage = (R*)(koff + nCells);
     __shared__ int s_total, s_staged;
     const CellHdr* hdr = d.hdr + (size_t)f * d.n_cells + L.cell_base;
-    uint32_t* cand = d.cand + (size_t)f * d.cand_total;
+    R* cand;
+    if constexpr (HARRIS) cand = hb.cand64 + (size_t)f * d.cand_total;
+    else cand = d.cand + (size_t)f * d.cand_total;
     for (int c = threadIdx.x; c < nCells; c += SEL_THREADS) nTotal[c] = d.cells[L.cell_base + c].skipped ? 0 : hdr[c].n_base;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -778,7 +847,7 @@ __global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d) {
                     else { nToRetain[c] = nTotal[c]; nToDistribute += nNew - nTotal[c]; koff[c] = 1; nNoMore++; }
                 }
         }
-        s_staged = tot <= SEL_STAGE;
+        s_staged = tot <= STAGE;
         int o = 0;
         for (int c = 0; c < nCells; ++c) { kept[c] = o; o += nTotal[c]; }   // staging offsets (reused below)
     }
@@ -786,15 +855,15 @@ __global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d) {
     const bool staged = s_staged;
     for (int c = wid; c < nCells; c += NW) {
         const int n = nToRetain[c], tot = nTotal[c];
-        uint32_t* g = cand + d.cells[L.cell_base + c].cand_off;
-        uint32_t* v = g;
+        R* g = cand + d.cells[L.cell_base + c].cand_off;
+        R* v = g;
         if (staged) {
             v = stage + kept[c];
             for (int i = lane; i < tot; i += 32) v[i] = g[i];
             __syncwarp();
         }
         if (lane == 0) koff[c] = (int)(v - (staged ? stage : cand));   // remember where the list lives
-        if (tot > n && n > 0) se2gpu::kp_nth_element_warp(v, tot, n - 1, wq[wid]);   // KeyPointsFilter::retainBest + resize (:692-694)
+        if (tot > n && n > 0) se2gpu::kp_nth_element_warp<K>(v, tot, n - 1, wq[wid]);   // KeyPointsFilter::retainBest + resize (:692-694)
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -805,21 +874,30 @@ __global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d) {
     }
     __syncthreads();
     for (int c = wid; c < nCells; c += NW) {
-        const uint32_t* v = (staged ? stage : cand) + koff[c];
+        const R* v = (staged ? stage : cand) + koff[c];
         const int o = kept[c];
         for (int i = lane; i < nTotal[c] && o + i < cap; i += 32) lbuf[o + i] = v[i];
     }
     __syncthreads();
     int total = s_total;
     if (total > L.nDesired) {  // :706-710
-        if (wid == 0) se2gpu::kp_nth_element_warp(lbuf, total, L.nDesired - 1, wq[0]);
+        if (wid == 0) se2gpu::kp_nth_element_warp<K>(lbuf, total, L.nDesired - 1, wq[0]);
         total = L.nDesired;
         __syncthreads();
     }
     uint32_t* out = d.lkp + (size_t)f * d.lkp_total + L.kp_off;
-    for (int i = threadIdx.x; i < total; i += SEL_THREADS) out[i] = lbuf[i];
+    if constexpr (HARRIS) {
+        float* resp = hb.lresp + (size_t)f * d.lkp_total + L.kp_off;
+        for (int i = threadIdx.x; i < total; i += SEL_THREADS) { const R r = lbuf[i]; out[i] = (uint32_t)r; resp[i] = se2gpu::resp_from_key((uint32_t)(r >> 32)); }
+    } else {
+        for (int i = threadIdx.x; i < total; i += SEL_THREADS) out[i] = lbuf[i];
+    }
     if (threadIdx.x == 0) d.lcount[f * d.nlevels + level] = total;
 }
+// instantiated here, ahead of the templates used later in the file: the module's dynamic shared-memory declarations then keep
+// the order in which ptxas places the dynamic buffer of orb_select<false> right behind its static arrays
+template __global__ void orb_select<false>(OrbDev, HarrisBufs);
+template __global__ void orb_select<true>(OrbDev, HarrisBufs);
 
 // test hook: one warp per list, lists in global memory
 __global__ void __launch_bounds__(128) orb_debug_nth(uint32_t* v, const int* __restrict__ offs, const int* __restrict__ nth, int count) {
@@ -827,6 +905,14 @@ __global__ void __launch_bounds__(128) orb_debug_nth(uint32_t* v, const int* __r
     const int k = blockIdx.x * 4 + (threadIdx.x >> 5);
     if (k >= count) return;
     se2gpu::kp_nth_element_warp(v + offs[k], offs[k + 1] - offs[k], nth[k], wq[threadIdx.x >> 5]);
+}
+
+// test hook: the same on 64-bit records keyed by their upper word (the Harris-score selection)
+__global__ void __launch_bounds__(128) orb_debug_nth64(uint64_t* v, const int* __restrict__ offs, const int* __restrict__ nth, int count) {
+    __shared__ int wq[4][128];
+    const int k = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (k >= count) return;
+    se2gpu::kp_nth_element_warp<se2gpu::KpKey64>(v + offs[k], offs[k + 1] - offs[k], nth[k], wq[threadIdx.x >> 5]);
 }
 
 // GaussianBlur 7x7 sigma 2 on the level ROI; the 16 px ring keeps its un-blurred reflect-101 copies.
@@ -945,8 +1031,10 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {
 // (predicated off beyond the column's half-height) instead of one dependent +-v pair per loop trip, and the 16 descriptor taps of
 // a lane are loaded back to back: the kernel is bound by the latency of first-touch sectors (every plane byte comes from DRAM
 // once), so the loads in flight per warp set its speed. Integer moments: any summation order gives the reference's m10, m01.
+// HARRIS: the keypoint's response is the Harris response orb_select<true> left in lresp, else the FAST score of the record.
+template <bool HARRIS>
 __global__ void __launch_bounds__(256) orb_orient_describe(OrbDev d, se2gpu_keypoint* __restrict__ kps, uint8_t* __restrict__ desc,
-                                                           int* __restrict__ counts) {
+                                                           int* __restrict__ counts, const float* __restrict__ lresp) {
     __shared__ float4 patf[256];     // the 256 point pairs of the rBRIEF pattern as floats (x0, y0, x1, y1); test 8*lane+k at [k][lane]
     for (int i = threadIdx.x; i < 256; i += blockDim.x) patf[(i & 7) * 32 + (i >> 3)] = make_float4((float)d_pattern[4 * i], (float)d_pattern[4 * i + 1], (float)d_pattern[4 * i + 2], (float)d_pattern[4 * i + 3]);
     __syncthreads();
@@ -963,7 +1051,8 @@ __global__ void __launch_bounds__(256) orb_orient_describe(OrbDev d, se2gpu_keyp
     if (slot == 0 && lane == 0) counts[f] = total;
     if (level < 0) return;
     const LevelGeo& L = d.levels[level];
-    const uint32_t rec = d.lkp[(size_t)f * d.lkp_total + L.kp_off + (slot - off)];
+    const size_t kslot = (size_t)f * d.lkp_total + L.kp_off + (slot - off);
+    const uint32_t rec = d.lkp[kslot];
     const int x = rec & 0xFFF, y = (rec >> 12) & 0xFFF, score = rec >> 24;
     const size_t base = f * d.frame_plane_bytes + L.plane_off + (size_t)(EDGE + y) * L.pitch + (EDGE + x);
     const uint8_t* center = d.plain + base;
@@ -1027,7 +1116,7 @@ __global__ void __launch_bounds__(256) orb_orient_describe(OrbDev d, se2gpu_keyp
         se2gpu_keypoint kp;
         kp.x = level ? __fmul_rn((float)x, L.scale) : (float)x;
         kp.y = level ? __fmul_rn((float)y, L.scale) : (float)y;
-        kp.size = L.kp_size; kp.angle = angle; kp.response = (float)score; kp.octave = level; kp.class_id = -1;
+        kp.size = L.kp_size; kp.angle = angle; kp.response = HARRIS ? lresp[kslot] : (float)score; kp.octave = level; kp.class_id = -1;
         kps[oslot] = kp;
     }
 }
@@ -1039,6 +1128,7 @@ inline int cv_round_f(float v) { return (int)lrintf(v); }
 // =================================================================================================
 struct se2gpu_orb {
     int device = 0, nfeatures = 0, nlevels = 0, fast_th = 20, max_w = 0, max_h = 0, max_batch = 0;
+    bool harris = false;         // scoreType == HARRIS_SCORE: orb_harris + the 64-bit selection
     double scaleFactor = 1.2;
     std::vector<float> mvScaleFactor, mvInvScaleFactor;
     std::vector<int> mnFeaturesPerLevel;
@@ -1066,6 +1156,7 @@ struct se2gpu_orb {
     LevelGeo* d_levels = nullptr; CellGeo* d_cells = nullptr; TileGeo* d_tiles = nullptr; int* d_itab = nullptr; short* d_stab = nullptr;
 
     uint8_t* d_in = nullptr; se2gpu_keypoint* d_kps = nullptr; uint8_t* d_desc = nullptr; int* d_counts = nullptr;
+    HarrisBufs hb{};             // HARRIS_SCORE handles only: [B][cand_total] 64-bit records, [B][lkp_total] level-list responses
     std::vector<void*> bufs;
     int last_n = 0;
     se2gpu::Profiler prof;
@@ -1084,7 +1175,7 @@ struct se2gpu_orb {
     // batch k+1 in and batch k-1 out while the SMs work on batch k)
     se2gpu_orb* twin = nullptr;
     int submit_next = 0, wait_next = 0, in_flight = 0;
-    int create_args[8] = {};
+    int create_args[9] = {};
 };
 
 namespace {
@@ -1175,7 +1266,8 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
                 fsm_tma = std::max(fsm_tma, (size_t)128 + ((pw * g.fbh + 15) & ~(size_t)15) + (((size_t)fastpx::nms_plane_bytes(g.fbw, chh) + 15) & ~(size_t)15) + bitmap + (size_t)cw * chh * 2 + 64);
             }
         }
-        ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 4 + (size_t)g.nCells * 16 + (size_t)SEL_STAGE * 4);
+        if (h->harris) ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 8 + (size_t)g.nCells * 16 + (size_t)(SEL_STAGE / 2) * 8);
+        else ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 4 + (size_t)g.nCells * 16 + (size_t)SEL_STAGE * 4);
         // orb_blur: at least 2 strips of at most about BLUR_TH rows, of one height: with its 6 warm-up rows a strip is a whole number
         // of turns of the kernel's 7-row ring, and at most the ROI's height (h >= 39). A tile = 32 consecutive (strip, column group)
         // items. The tile count grows with w and h, so the table sized at create time holds every smaller frame's.
@@ -1318,7 +1410,9 @@ int set_geometry(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
     h->fast_tma = fsm_tma > 0 && encode_fast_maps(h, pb);
     h->fast_tma_smem = fsm_tma;
     if (h->fast_tma) SE2_CUDA(cudaFuncSetAttribute(orb_fast_cells<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(fsm_tma, 1024)));
-    SE2_CUDA(cudaFuncSetAttribute(orb_select, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(ssm, 1024)));
+    if (h->harris && ssm > 227 * 1024) return fail(SE2GPU_ERR_CAPACITY, "the Harris-score selection of a %dx%d frame needs %zu B of shared memory", w, hgt, ssm);
+    if (h->harris) SE2_CUDA(cudaFuncSetAttribute(orb_select<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(ssm, 1024)));
+    else SE2_CUDA(cudaFuncSetAttribute(orb_select<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(ssm, 1024)));
     OrbDev& d = h->d;
     d.n_cells = (int)h->cells.size(); d.n_tiles = (int)h->tiles.size();
     d.frame_plane_bytes = pb; d.cand_total = ct;
@@ -1473,6 +1567,7 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
     if (h->fast_big) SE2_LAUNCH(orb_fast_cells_big, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d);
     else if (h->fast_tma) SE2_LAUNCH(orb_fast_cells<true>, dim3(d.n_cells, n), FAST_THREADS, h->fast_tma_smem, s, d, h->fast_maps);
     else SE2_LAUNCH(orb_fast_cells<false>, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d, h->fast_maps);
+    if (h->harris) SE2_LAUNCH(orb_harris, dim3(d.n_cells, n), HARRIS_THREADS, 0, s, d, h->hb.cand64);   // timed with FAST (group 1)
     pr.end(s);
     if (overlap) {      // group B behind FAST in stream order, concurrent with the selection
         SE2_CUDA(cudaEventRecord(ev_pyr, s));
@@ -1481,7 +1576,8 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
         SE2_CUDA(cudaEventRecord(ev_blur, side));
     }
     pr.begin(2, s);
-    SE2_LAUNCH(orb_select, dim3(h->nlevels, n), SEL_THREADS, h->select_smem, s, d);
+    if (h->harris) SE2_LAUNCH(orb_select<true>, dim3(h->nlevels, n), SEL_THREADS, h->select_smem, s, d, h->hb);
+    else SE2_LAUNCH(orb_select<false>, dim3(h->nlevels, n), SEL_THREADS, h->select_smem, s, d, h->hb);
     pr.end(s);
     if (overlap) {
         SE2_CUDA(cudaStreamWaitEvent(s, ev_blur, 0));
@@ -1492,7 +1588,8 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
     }
     const int warps = 8;
     pr.begin(4, s);
-    SE2_LAUNCH(orb_orient_describe, dim3((h->nfeatures + warps - 1) / warps, n), warps * 32, 0, s, d, d_kps, d_desc, d_counts);
+    if (h->harris) SE2_LAUNCH(orb_orient_describe<true>, dim3((h->nfeatures + warps - 1) / warps, n), warps * 32, 0, s, d, d_kps, d_desc, d_counts, h->hb.lresp);
+    else SE2_LAUNCH(orb_orient_describe<false>, dim3((h->nfeatures + warps - 1) / warps, n), warps * 32, 0, s, d, d_kps, d_desc, d_counts, h->hb.lresp);
     pr.end(s);
     h->last_n = std::max(h->last_n * (frame0 > 0), frame0 + n);
     return SE2GPU_OK;
@@ -1502,15 +1599,19 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
 
 extern "C" {
 
-se2gpu_orb* se2gpu_orb_create(int nfeatures, float scale_factor, int nlevels, int fast_th, int max_w, int max_h,
-                              int max_batch, int device) {
+se2gpu_orb* se2gpu_orb_create_scored(int nfeatures, float scale_factor, int nlevels, int score_type, int fast_th, int max_w, int max_h,
+                                     int max_batch, int device) {
+    if (score_type != SE2GPU_ORB_HARRIS_SCORE && score_type != SE2GPU_ORB_FAST_SCORE) {
+        fail(SE2GPU_ERR_INVALID, "unknown ORB score type %d (HARRIS_SCORE = 0, FAST_SCORE = 1)", score_type); return nullptr;
+    }
     if (nfeatures <= 0 || nlevels <= 0 || nlevels > MAX_LEVELS || !(scale_factor > 1.0f) || fast_th < 1 || fast_th > 254 ||
         max_w <= 0 || max_h <= 0 || max_batch <= 0) { fail(SE2GPU_ERR_INVALID, "bad ORB parameters"); return nullptr; }
     if (se2gpu::select_device(device) != SE2GPU_OK) return nullptr;
     se2gpu_orb* h = new se2gpu_orb;
     h->device = device; h->nfeatures = nfeatures; h->nlevels = nlevels; h->fast_th = fast_th;
+    h->harris = score_type == SE2GPU_ORB_HARRIS_SCORE;
     h->max_w = max_w; h->max_h = max_h; h->max_batch = max_batch;
-    { int* a = h->create_args; a[0] = nfeatures; memcpy(&a[1], &scale_factor, sizeof(float)); a[2] = nlevels; a[3] = fast_th; a[4] = max_w; a[5] = max_h; a[6] = max_batch; a[7] = device; }
+    { int* a = h->create_args; a[0] = nfeatures; memcpy(&a[1], &scale_factor, sizeof(float)); a[2] = nlevels; a[3] = fast_th; a[4] = max_w; a[5] = max_h; a[6] = max_batch; a[7] = device; a[8] = score_type; }
     h->scaleFactor = scale_factor;   // the reference keeps it in a double member (ORBextractor.h:67)
     // ORBextractor::ORBextractor, ORBextractor.cpp:463-520
     h->mvScaleFactor.resize(nlevels); h->mvInvScaleFactor.resize(nlevels); h->mnFeaturesPerLevel.resize(nlevels);
@@ -1548,6 +1649,7 @@ se2gpu_orb* se2gpu_orb_create(int nfeatures, float scale_factor, int nlevels, in
     A(&d.plain, B * h->cap_plane); A(&d.blurred, B * h->cap_plane);
     A(&d.cand, B * h->cap_cand); A(&d.hdr, B * h->cap_cells); A(&d.lkp, B * h->cap_lkp); A(&d.lcount, B * nlevels); A(&d.err, 1);
     A(&h->d_in, B * (size_t)max_w * max_h); A(&h->d_kps, B * nfeatures); A(&h->d_desc, B * nfeatures * 32); A(&h->d_counts, B);
+    if (h->harris) { A(&h->hb.cand64, B * h->cap_cand); A(&h->hb.lresp, B * h->cap_lkp); }
     if (!ok) { fail(SE2GPU_ERR_CUDA, "device allocation failed (%s)", cudaGetErrorString(cudaGetLastError())); se2gpu_orb_destroy(h); return nullptr; }
     cudaMemset(d.err, 0, sizeof(int));
     if (cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_pyr, cudaEventDisableTiming) != cudaSuccess ||
@@ -1565,6 +1667,11 @@ se2gpu_orb* se2gpu_orb_create(int nfeatures, float scale_factor, int nlevels, in
     d.levels = h->d_levels; d.cells = h->d_cells; d.tiles = h->d_tiles; d.itab = h->d_itab; d.stab = h->d_stab;
     if (cudaDeviceSynchronize() != cudaSuccess) { fail(SE2GPU_ERR_CUDA, "init failed"); se2gpu_orb_destroy(h); return nullptr; }
     return h;
+}
+
+se2gpu_orb* se2gpu_orb_create(int nfeatures, float scale_factor, int nlevels, int fast_th, int max_w, int max_h,
+                              int max_batch, int device) {
+    return se2gpu_orb_create_scored(nfeatures, scale_factor, nlevels, SE2GPU_ORB_FAST_SCORE, fast_th, max_w, max_h, max_batch, device);
 }
 
 void se2gpu_orb_destroy(se2gpu_orb* h) {
@@ -1698,7 +1805,7 @@ int se2gpu_orb_submit(se2gpu_orb* h, const uint8_t* imgs, int n, int w, int hgt,
     if (!h->twin) {
         const int* a = h->create_args;
         float sf; memcpy(&sf, &a[1], sizeof sf);
-        h->twin = se2gpu_orb_create(a[0], sf, a[2], a[3], a[4], a[5], a[6], a[7]);
+        h->twin = se2gpu_orb_create_scored(a[0], sf, a[2], a[8], a[3], a[4], a[5], a[6], a[7]);
         if (!h->twin) return SE2GPU_ERR_CUDA;
         if (h->und_on && se2gpu_orb_set_undistort(h->twin, h->und_K, h->und_nd ? h->und_D : nullptr, h->und_nd) != SE2GPU_OK) return SE2GPU_ERR_CUDA;
     }
@@ -1738,6 +1845,29 @@ int se2gpu_orb_debug_nth_element(uint32_t* values, const int* offsets, const int
     SE2_CUDA(cudaGetLastError());
     SE2_CUDA(cudaMemcpy(values, dv, total * 4, cudaMemcpyDeviceToHost));
     cudaFree(dv); cudaFree(dofs); cudaFree(dn);
+    return SE2GPU_OK;
+}
+
+int se2gpu_orb_debug_nth_element_f32(const float* values, const int* offsets, const int* nth, int count, int* perm, int device) {
+    if (count <= 0) return SE2GPU_OK;
+    if (!values || !offsets || !nth || !perm) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (se2gpu::select_device(device) != SE2GPU_OK) return SE2GPU_ERR_CUDA;
+    const size_t total = (size_t)offsets[count];
+    std::vector<uint64_t> rec(total);
+    for (int k = 0; k < count; ++k)
+        for (int i = offsets[k]; i < offsets[k + 1]; ++i) rec[i] = ((uint64_t)se2gpu::resp_key(values[i]) << 32) | (uint32_t)(i - offsets[k]);
+    uint64_t* dv = nullptr; int* dofs = nullptr; int* dn = nullptr;
+    SE2_CUDA(cudaMalloc((void**)&dv, std::max<size_t>(total, 1) * 8));
+    SE2_CUDA(cudaMalloc((void**)&dofs, sizeof(int) * (count + 1)));
+    SE2_CUDA(cudaMalloc((void**)&dn, sizeof(int) * count));
+    SE2_CUDA(cudaMemcpy(dv, rec.data(), total * 8, cudaMemcpyHostToDevice));
+    SE2_CUDA(cudaMemcpy(dofs, offsets, sizeof(int) * (count + 1), cudaMemcpyHostToDevice));
+    SE2_CUDA(cudaMemcpy(dn, nth, sizeof(int) * count, cudaMemcpyHostToDevice));
+    SE2_LAUNCH(orb_debug_nth64, (count + 3) / 4, 128, 0, nullptr, dv, dofs, dn, count);
+    SE2_CUDA(cudaGetLastError());
+    SE2_CUDA(cudaMemcpy(rec.data(), dv, total * 8, cudaMemcpyDeviceToHost));
+    cudaFree(dv); cudaFree(dofs); cudaFree(dn);
+    for (size_t i = 0; i < total; ++i) perm[i] = (int)(uint32_t)rec[i];
     return SE2GPU_OK;
 }
 
