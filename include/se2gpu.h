@@ -440,6 +440,22 @@ int se2gpu_ba_profile_read(se2gpu_ba* h, double* ms, int* launches);
 int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hpp, double* bp, double* Hll, double* bl,
                            double* Hpl, double* S, double* bs, double* dx_p, double* dx_l);
 
+/* test hook: the host-side plan of the last set_problem that rebuilt the structure (a same-topology reload keeps it).
+ * Writes min(n_out, SE2GPU_BA_PLAN_FIELDS) ints to `out` and returns SE2GPU_BA_PLAN_FIELDS; changes nothing.
+ *   [0] nf (free poses)    [1] n = 3 nf
+ *   [2] structure build: 0 dense nf x nf counting table, 1 comparison sort (nf * nf > 2^22)
+ *   [3] envelope half-width w in pose blocks (max over block columns a of the last coupled block row - a)
+ *   [4] reduced solve: 0 single-CTA shared-memory LDL^T, 1 two-CTA twisted solve (persistent kernel; one kernel per phase
+ *       still uses 0), 2 partitioned band solver, 3 global-memory envelope factorisation
+ *   [5] twisted split m0   [6] twisted separator width (0 when [4] != 1)
+ *   [7] band half-width w  [8] band partition count p (0 when [4] != 2)
+ *   [9] persistent grid (0 = no cooperative launch)   [10] Schur workers W of the persistent kernel
+ *   [11] blocks of S       [12] most blocks one worker owns
+ *   [13] workers whose blocks do not all fit the shared-memory cache (more than 16 blocks, or pair and edge lists beyond the
+ *        arena): they run the sequential Schur sweep over lists in global memory */
+#define SE2GPU_BA_PLAN_FIELDS 14
+int se2gpu_ba_debug_plan(se2gpu_ba* h, int* out, int n_out);
+
 #ifdef __cplusplus
 }
 #endif

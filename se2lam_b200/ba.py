@@ -144,6 +144,23 @@ class LocalBA:
         out["n"] = n
         return out
 
+    PLAN_FIELDS = ("nf", "n", "structure", "env_w", "solver", "tw_m0", "tw_w", "band_w", "band_p", "pk_grid", "workers",
+                   "nblk", "max_own", "uncached")
+    STRUCTURES = ("dense", "sorted")
+    SOLVERS = ("smem", "twisted", "band", "envelope")
+
+    def debug_plan(self):
+        """Host-side decisions of the last set_problem (se2gpu_ba_debug_plan): structure build, reduced solver and the
+        persistent kernel's Schur work split. `structure` and `solver` are returned as names."""
+        buf = np.zeros(len(self.PLAN_FIELDS), np.int32)
+        nf = check(lib().se2gpu_ba_debug_plan(self.h, ptr(buf), len(buf)), "se2gpu_ba_debug_plan")
+        if nf != len(buf):
+            raise _capi.Se2GpuError(f"se2gpu_ba_debug_plan reports {nf} fields, the binding knows {len(buf)}")
+        out = {k: int(v) for k, v in zip(self.PLAN_FIELDS, buf)}
+        out["structure"] = self.STRUCTURES[out["structure"]]
+        out["solver"] = self.SOLVERS[out["solver"]]
+        return out
+
 
 # ------------------------------------------------------------------------------------------------
 # g2o-graph-style facade (the calls Map::loadLocalGraph / LocalMapper::localBA make)

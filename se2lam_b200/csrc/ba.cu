@@ -1336,6 +1336,9 @@ __device__ void pk_phase_linearize(const Dev& d, const Cam& cam, int xi, double*
 // the dependent L2 round trips for index data from every Schur / pose-gather phase (only the payload is gathered).
 constexpr int PK_MAXOWN = 16;
 struct PKOwn { int blk, a, b, p0, np, e0, ne; };
+constexpr int PK_RED_SCRATCH_BYTES = (PK_THREADS / 32) * 21 * 33 * 8;   // per-warp reduction scratch at the top of a worker's arena
+// dynamic shared memory of the persistent launch: CTA 0's reduced solve, and on worker CTAs pair lists + reduction scratch
+inline size_t pk_dyn_smem_bytes(int n) { return std::max(ldlt_smem_bytes(n), (size_t)160 * 1024); }
 
 // pose a: Hpp diagonal block (6 unique) + bp from its edges (list in `edges`, shared or global) and odometry edges
 __device__ void pk_pose_item(const Dev& d, int a, const int* edges, int ne, double* sh9 /*[8][9]*/) {
@@ -1722,7 +1725,7 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
     __shared__ PKOwn own[PK_MAXOWN];
     __shared__ int s_nown, s_plan_ok;
     __shared__ unsigned char plan_w0[PK_MAXOWN], plan_nw[PK_MAXOWN];   // warp groups of the concurrent Schur phase
-    constexpr int RED_SCRATCH_BYTES = (PK_THREADS / 32) * 21 * 33 * 8;
+    constexpr int RED_SCRATCH_BYTES = PK_RED_SCRATCH_BYTES;
     double* red_scratch = sm + (pa.dyn_smem_bytes - RED_SCRATCH_BYTES) / 8;      // worker CTAs only (CTA 0 keeps its arena for the solve)
     PKWork work;
     {
@@ -2081,6 +2084,7 @@ struct se2gpu_ba {
     std::vector<int> t_edge_pose, t_edge_point, t_odo_i, t_odo_j; std::vector<uint8_t> t_fixed; int t_rank = -1, t_world = -1;
     se2band::Plan band;        // partitioned band solver for reduced systems beyond one CTA's shared memory
     int smem_optin = 0;
+    int plan[SE2GPU_BA_PLAN_FIELDS] = {};   // host-side decisions of the last full set_problem (se2gpu_ba_debug_plan)
 };
 
 namespace {
@@ -2564,6 +2568,25 @@ int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double
         for (auto& l : lists) maxlen = std::max(maxlen, l.size());
         blk_order.assign((size_t)W * maxlen, -1);
         for (int w2 = 0; w2 < W; ++w2) for (size_t i = 0; i < lists[w2].size(); ++i) blk_order[i * W + w2] = lists[w2][i];
+        // workers whose blocks do not all fit the shared-memory cache (the rule of ba_persistent's prologue): they run the
+        // sequential Schur sweep over pair lists in global memory
+        const int arena_ints = (int)(pk_dyn_smem_bytes(n) - PK_RED_SCRATCH_BYTES) / 4;
+        int uncached = 0;
+        for (auto& l : lists) {
+            int off = 0, no = 0;
+            for (int b : l) {
+                const int np = blk_pair_ptr[b + 1] - blk_pair_ptr[b], ne = blk_a[b] == blk_b[b] ? pose_ptr[blk_a[b] + 1] - pose_ptr[blk_a[b]] : 0;
+                if (no >= PK_MAXOWN || off + 2 * np + ne > arena_ints) break;
+                off += 2 * np + ne; ++no;
+            }
+            if (no < (int)l.size()) ++uncached;
+        }
+        int* pl = h->plan;
+        pl[0] = nf; pl[1] = n; pl[2] = (size_t)nf * nf <= ((size_t)1 << 22) ? 0 : 1;
+        pl[3] = 0; for (int a = 0; a < nf; ++a) pl[3] = std::max(pl[3], bmax[a] - a);
+        pl[4] = n <= SMEM_CHOL_MAX_N ? (tw_m0 > 0 ? 1 : 0) : (h->band.active ? 2 : 3);
+        pl[5] = tw_m0; pl[6] = tw_w; pl[7] = h->band.active ? h->band.w : 0; pl[8] = h->band.active ? h->band.p : 0;
+        pl[9] = h->pk_grid; pl[10] = W; pl[11] = nblk; pl[12] = (int)maxlen; pl[13] = uncached;
     }
     int rc = ensure_cap(h, npairs, std::max<size_t>(std::max<size_t>(nblk, blk_order.size()), odob.size()), odob.size());
     if (rc != SE2GPU_OK) return rc;
@@ -2733,7 +2756,7 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
         PKArgs pa{max_iters, first_iteration, h->stats_dev, trace_poses ? h->trace_p : nullptr, trace_points ? h->trace_l : nullptr,
                   h->abort_host_dev, h->abort_dev, h->pk_part_chi, h->pk_part_scale, h->pk_part_max, h->prof.on ? h->phase_cycles : nullptr, 0, getenv("SE2GPU_BA_DEBUG_SYSFENCE") ? 1 : 0, getenv("SE2GPU_BA_DEBUG") ? h->cta_work : nullptr};
         if (h->prof.on) h->pk_launches++;
-        const size_t smem = std::max(ldlt_smem_bytes(d.n), (size_t)160 * 1024);      // worker CTAs: pair lists + 87 KB of reduction scratch
+        const size_t smem = pk_dyn_smem_bytes(d.n);      // worker CTAs: pair lists + 87 KB of reduction scratch
         pa.dyn_smem_bytes = (int)smem;
         void* args[] = {(void*)&d, (void*)&h->cam, (void*)&pa, (void*)&shd};
         h->prof.begin(7, s);
@@ -2996,6 +3019,13 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
     SE2_CUDA(cudaMemcpyAsync(d.st, h->st_host, sizeof(LMState), cudaMemcpyHostToDevice, s));
     SE2_CUDA(cudaStreamSynchronize(s));
     return n;
+}
+
+int se2gpu_ba_debug_plan(se2gpu_ba* h, int* out, int n_out) {
+    if (!h || !h->loaded) return fail(SE2GPU_ERR_INVALID, "no problem loaded");
+    if (n_out < 0 || (n_out > 0 && !out)) return fail(SE2GPU_ERR_INVALID, "bad output buffer");
+    for (int k = 0; k < std::min(n_out, SE2GPU_BA_PLAN_FIELDS); ++k) out[k] = h->plan[k];
+    return SE2GPU_BA_PLAN_FIELDS;
 }
 
 }  // extern "C"
