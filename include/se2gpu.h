@@ -34,6 +34,7 @@
  *   se2gpu_track_triangulate[_device]  Track::doTriangulate                   src/Track.cpp:389-416
  *   se2gpu_xyz_info[_device]         Track::calcSE3toXYZInfo                  src/Track.cpp:259-306
  *   se2gpu_projection_observations[_device]  LocalMapper::findCorrespd, MatchByProjection branch  src/LocalMapper.cpp:119-141
+ *   se2gpu_remove_outliers[_device]  Track::removeOutliers (cv::findFundamentalMat)  src/Track.cpp:308-344
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -324,6 +325,30 @@ int se2gpu_projection_observations_device(const se2gpu_keypoint* d_kf_kp, int n_
 /* Test hook: the 4x4 Jacobi SVD behind cvu::triangulate (cv::SVD::compute, MODIFY_A|FULL_UV) on n row-major matrices
  * A [n*16]; w [n*4] singular values (descending), vt [n*16]. HOST buffers. */
 int se2gpu_debug_svd4(int n, const float* A, float* w, float* vt, int device);
+
+/* Track::removeOutliers (src/Track.cpp:308-344) for `batch` frame pairs: pt1 / pt2 are the pairs (kp1[i].pt,
+ * kp2[matches12[i]].pt) of the matched i in ascending order, mask = cv::findFundamentalMat(pt1, pt2, mask) with OpenCV
+ * 4.13's defaults (FM_RANSAC, 3 px, confidence 0.99, 1000 iterations; below 15 pairs OpenCV's LMedS, 7 pairs the 7-point
+ * kernel alone, fewer no estimate), matches12[i] = -1 where the mask is 0, then every match -1 when fewer than 10 inliers
+ * remain. The RNG, subset draws, epipolar error, acceptance rule and iteration update are OpenCV's bit for bit; the
+ * 7-point kernel is this project's own (DESIGN.md section 8).
+ * Pair b: kp1 [b*cap1 ..] with n1[b] keypoints (n1 NULL: cap1), kp2 [b*cap2 ..] with n2[b] keypoints, matches12 [b*cap1 ..]
+ * updated in place (entries at or past n1[b] untouched), ninliers [b] = the returned nInlier, F [9b ..] (may be NULL) the
+ * 3x3 row-major F cv::findFundamentalMat returns (for 7 pairs the first root's), zeros when it returns none, iters [b] (may be
+ * NULL) the number of hypotheses the estimator ran. cap1 <= 8192. Host form: matches12 entries must be < n2[b]. */
+int se2gpu_remove_outliers(int batch, const se2gpu_keypoint* kp1, const int* n1, int cap1, const se2gpu_keypoint* kp2, const int* n2,
+                           int cap2, int* matches12, int* ninliers, double* F, int* iters, int device);
+/* Track::removeOutliers (src/Track.cpp:308-344) on DEVICE buffers, asynchronous on `stream`: the extractor's d_kps / d_counts and
+ * MatchByWindow's d_matches12 (updated in place), laid out as above; d_n1 / d_n2 may be NULL. A match index at or past
+ * the frame-2 count counts as unmatched. */
+int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const int* d_n1, int cap1, const se2gpu_keypoint* d_kp2,
+                                  const int* d_n2, int cap2, int* d_matches12, int* d_ninliers, double* d_F, int* d_iters,
+                                  void* stream);
+/* Test hooks of RANSACUpdateNumIters(0.99, ep, 7, max_iters), which the device evaluates through a table built on the host
+ * with glibc's log / pow: thresholds [1000] receives the table (the least ep reaching k + 1 iterations; no device needed),
+ * and se2gpu_fundam_debug_niters evaluates the device lookup for ep = (n[i] - good[i]) / n[i] (HOST buffers). */
+void se2gpu_fundam_niters_table(double* thresholds);
+int se2gpu_fundam_debug_niters(int count, const int* n, const int* good, const int* max_iters, int* out, int device);
 
 /* ------------------------------------------------------------------------------------------ local BA */
 typedef struct se2gpu_ba se2gpu_ba;

@@ -54,7 +54,8 @@ SYMBOLS = [
     "se2gpu_voc_create", "se2gpu_voc_destroy", "se2gpu_voc_transform", "se2gpu_voc_transform_device", "se2gpu_median_descriptor",
     "se2gpu_triangulate", "se2gpu_triangulate_device", "se2gpu_track_triangulate", "se2gpu_track_triangulate_device",
     "se2gpu_xyz_info", "se2gpu_xyz_info_device", "se2gpu_projection_observations", "se2gpu_projection_observations_device",
-    "se2gpu_debug_svd4",
+    "se2gpu_debug_svd4", "se2gpu_remove_outliers", "se2gpu_remove_outliers_device", "se2gpu_fundam_niters_table",
+    "se2gpu_fundam_debug_niters",
 ]
 
 
@@ -144,6 +145,11 @@ def lib():
     L.se2gpu_projection_observations.argtypes = [vp, i] + [vp] * 8 + [i, vp, i, vp, f, f, f, vp, vp, vp, i]
     L.se2gpu_projection_observations_device.argtypes = [vp, i] + [vp] * 11 + [f, f, f, vp, vp, vp, vp]
     L.se2gpu_debug_svd4.argtypes = [i, vp, vp, vp, i]
+    L.se2gpu_remove_outliers.argtypes = [i, vp, vp, i, vp, vp, i, vp, vp, vp, vp, i]
+    L.se2gpu_remove_outliers_device.argtypes = [i, vp, vp, i, vp, vp, i, vp, vp, vp, vp, vp]
+    L.se2gpu_fundam_niters_table.restype = None
+    L.se2gpu_fundam_niters_table.argtypes = [vp]
+    L.se2gpu_fundam_debug_niters.argtypes = [i, vp, vp, vp, vp, i]
     _lib = L
     return L
 

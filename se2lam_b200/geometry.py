@@ -51,6 +51,31 @@ def doTriangulate(kp_kf, kp_frame, matches12, kf_observed, kf_view_mp, Tcr, K, l
     return int(counts[0]), m, lm, good.astype(bool), int(counts[1])
 
 
+def removeOutliers(kp1, kp2, matches12, device=0, return_details=False):
+    """Track::removeOutliers (Track.cpp:308-344): cv::findFundamentalMat's RANSAC / LMedS mask applied to matches12, then
+    every match dropped below 10 inliers. kp1 / kp2 are KP_DTYPE arrays, or lists of them for a batch of frame pairs (one
+    call). Returns (nInlier, matches12) - lists for a batch - and with return_details also F [3,3] (zeros when
+    cv::findFundamentalMat returns none) and the number of hypotheses run. The inputs are not modified."""
+    batch = isinstance(kp1, (list, tuple))
+    K1 = [_kp(k) for k in (kp1 if batch else [kp1])]
+    K2 = [_kp(k) for k in (kp2 if batch else [kp2])]
+    M = [_c(m, np.int32) for m in (matches12 if batch else [matches12])]
+    B = len(K1)
+    if len(K2) != B or len(M) != B or any(len(m) != len(k) for m, k in zip(M, K1)):
+        raise ValueError("kp1, kp2 and matches12 must describe the same frame pairs")
+    cap1 = max([len(k) for k in K1] + [0]); cap2 = max([len(k) for k in K2] + [0])
+    k1 = np.zeros((B, cap1), KP_DTYPE); k2 = np.zeros((B, cap2), KP_DTYPE); m = np.full((B, cap1), -1, np.int32)
+    for b in range(B):
+        k1[b, :len(K1[b])] = K1[b]; k2[b, :len(K2[b])] = K2[b]; m[b, :len(M[b])] = M[b]
+    n1 = np.array([len(k) for k in K1], np.int32); n2 = np.array([len(k) for k in K2], np.int32)
+    nin = np.zeros(B, np.int32); F = np.zeros((B, 3, 3)); it = np.zeros(B, np.int32)
+    check(lib().se2gpu_remove_outliers(B, ptr(k1), ptr(n1), cap1, ptr(k2), ptr(n2), cap2, ptr(m), ptr(nin), ptr(F), ptr(it),
+                                       device), "se2gpu_remove_outliers")
+    out = [(int(nin[b]), m[b, :n1[b]].copy(), F[b], int(it[b])) for b in range(B)]
+    out = [o if return_details else o[:2] for o in out]
+    return out if batch else out[0]
+
+
 def calcSE3toXYZInfo(xyz1, pose1, pose2, Tcw, fxCam, device=0):
     """Track::calcSE3toXYZInfo for n points: xyz1 [n,3], Tcw [n_pose,4,4], pose1/pose2 [n] indices into Tcw.
     Returns (info1, info2), each [n,3,3] float64."""
