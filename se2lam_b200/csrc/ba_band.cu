@@ -24,6 +24,7 @@
 
 #include "ba_band.h"
 #include "common.h"
+#include "sym3.h"
 
 namespace se2band {
 
@@ -47,17 +48,14 @@ __device__ void band_factor(double* __restrict__ Ab, int BW1, int nrows, int npi
         const int r = 3 * j;
         const double a = A_(r, r), b = A_(r + 1, r), c = A_(r + 2, r), e = A_(r + 1, r + 1), f = A_(r + 2, r + 1), i2 = A_(r + 2, r + 2);
         const double u0 = y[r], u1 = y[r + 1], u2 = y[r + 2];
-        const double c00 = e * i2 - f * f, c01 = c * f - b * i2, c02 = b * f - c * e;
-        const double det = a * c00 + b * c01 + c * c02, m2 = a * e - b * b;
-        const bool pd = (a > 0.0) && (m2 > 0.0) && (det > 0.0) && isfinite(det);
-        const double id = 1.0 / det;
-        const double w00 = c00 * id, w01 = c01 * id, w02 = c02 * id, w11 = (a * i2 - c * c) * id, w12 = (b * c - a * f) * id, w22 = m2 * id;
+        const Sym3Inv inv = sym3_inverse(a, b, c, e, f, i2);
+        const double w00 = inv.i00, w01 = inv.i01, w02 = inv.i02, w11 = inv.i11, w12 = inv.i12, w22 = inv.i22;
         if (lane == 0) {
             double* Wj = W + 9 * j;
             Wj[0] = w00; Wj[1] = w01; Wj[2] = w02; Wj[3] = w01; Wj[4] = w11; Wj[5] = w12; Wj[6] = w02; Wj[7] = w12; Wj[8] = w22;
             double* t = tb + 3 * (j & 1);
             t[0] = w00 * u0 + w01 * u1 + w02 * u2; t[1] = w01 * u0 + w11 * u1 + w12 * u2; t[2] = w02 * u0 + w12 * u1 + w22 * u2;
-            if (!pd) *ok = 0;
+            if (!inv.pd) *ok = 0;
         }
     };
     if (wid == 0 && npiv > 0) invert_and_publish(0);
