@@ -7,10 +7,11 @@
 //
 // A 9-pixel arc of the 16-pixel Bresenham ring always contains one pixel of each opposite pair (k, k+8). For a pixel to be a
 // corner at threshold t with a DARKER arc (all 9 ring pixels < v - t) every one of the 4 tested pairs (0,8) (4,12) (2,10) (6,14)
-// therefore needs a member with v - p > t; for a BRIGHTER arc a member with p - v > t. With e_k = 256 + v - p_k (in [1, 511]):
-//   darker possible   <=>  min over pairs of max(e_k, e_k+8) > 256 + t
-//   brighter possible <=>  max over pairs of min(e_k, e_k+8) < 256 - t
-// Two pixels ride in the two s16 halves of a word, so one VIMNMX(3).S16x2 evaluates two pixels at once.
+// therefore needs a member with v - p > t; for a BRIGHTER arc a member with p - v > t. On the ring pixels themselves:
+//   darker possible   <=>  lo = max over pairs of min(p_k, p_k+8) < v - t
+//   brighter possible <=>  hi = min over pairs of max(p_k, p_k+8) > v + t
+// Two pixels ride in the two s16 halves of a word, so one VIMNMX(3).S16x2 evaluates two pixels at once, and no ring difference
+// is formed: the two comparisons are one 3-input add each against the bias 511 - t.
 #pragma once
 #include <cstdint>
 
@@ -80,38 +81,46 @@ SE2_HD unsigned add2(unsigned a, unsigned b) {
 
 namespace fastpx {
 
-// threshold constants of screen4 (per halfword): D + T1 >= 0 (s16) <=> D > 256 + t ;  U1 + ~B >= 0 <=> B < 256 - t
-SE2_HD unsigned screen_T1(int t) { return (unsigned)(0x10000 - (257 + t)) * 0x10001u; }
-SE2_HD unsigned screen_U1(int t) { return (unsigned)(256 - t) * 0x10001u; }
+// threshold constant of screen4: the bias 511 - t in both halfwords, the same for either polarity:
+//   v + bias - lo >= 512  <=>  lo < v - t ;   hi + bias - v >= 512  <=>  hi > v + t
+// Every sum lies in [256 - t, 766 - t], inside a halfword and positive, so the plain 32-bit adds never carry across halves.
+SE2_HD unsigned screen_bias(int t) { return (unsigned)(511 - t) * 0x10001u; }
 
 // The 4 pixels of patch word `zc` (row y, bytes x..x+3). Neighbouring words: zl / zr = the words left / right of zc on row y,
 // n3 / s3 = the word above / below at rows y-3 / y+3, n2l n2c n2r / s2l s2c s2r = the three words at rows y-2 / y+2.
-// Returns bit j set <=> pixel j may be a FAST corner at the threshold encoded in T1/U1 (necessary condition).
+// Returns bit j set <=> pixel j may be a FAST corner at the threshold encoded in bias = screen_bias(t) (necessary condition).
 SE2_HD unsigned screen4(unsigned n3, unsigned s3, unsigned n2l, unsigned n2c, unsigned n2r, unsigned s2l, unsigned s2c, unsigned s2r,
-                        unsigned zl, unsigned zc, unsigned zr, unsigned T1, unsigned U1) {
+                        unsigned zl, unsigned zc, unsigned zr, unsigned bias) {
     // 4-byte spans starting at dx = -3, +3 (row y) and dx = -2, +2 (rows y-2, y+2) of the word's first pixel
     const unsigned w_m3 = perm(zl, zc, 0x4321), w_p3 = perm(zc, zr, 0x6543);
     const unsigned nw_ = perm(n2l, n2c, 0x5432), ne_ = perm(n2c, n2r, 0x5432);
     const unsigned sw_ = perm(s2l, s2c, 0x5432), se_ = perm(s2c, s2r, 0x5432);
-    unsigned m = 0;
+    unsigned ok[2];
 #if defined(__CUDA_ARCH__)
 #pragma unroll
 #endif
     for (int hlf = 0; hlf < 2; ++hlf) {
-        const unsigned sel = hlf ? 0x4342u : 0x4140u;      // pixels (0,1) or (2,3) -> the two s16 halves
-        const unsigned cb = perm(zc, 0, sel) + 0x01000100u;                                  // 256 + v
-        // e = 256 + v - ring (both halves stay in [1,511], so the plain subtraction never borrows)
-        const unsigned e0 = cb - perm(s3, 0, sel), e8 = cb - perm(n3, 0, sel);               // (0,+3) (0,-3)
-        const unsigned e4 = cb - perm(w_p3, 0, sel), e12 = cb - perm(w_m3, 0, sel);          // (+3,0) (-3,0)
-        const unsigned e2 = cb - perm(se_, 0, sel), e10 = cb - perm(nw_, 0, sel);            // (+2,+2) (-2,-2)
-        const unsigned e6 = cb - perm(ne_, 0, sel), e14 = cb - perm(sw_, 0, sel);            // (+2,-2) (-2,+2)
-        const unsigned D = mins2(min3s2(maxs2(e0, e8), maxs2(e4, e12), maxs2(e2, e10)), maxs2(e6, e14));
-        const unsigned B = maxs2(max3s2(mins2(e0, e8), mins2(e4, e12), mins2(e2, e10)), mins2(e6, e14));
-        const unsigned r = maxs2(add2(D, T1), add2(~B, U1));                                 // >= 0 per half <=> may be a corner
-        const unsigned ok = ~r & 0x80008000u;
-        m |= ((ok >> 15) & 1u) << (2 * hlf) | ((ok >> 31) & 1u) << (2 * hlf + 1);
+        const unsigned sel = hlf ? 0x4341u : 0x4240u;      // pixels (0,2) or (1,3) -> the two s16 halves
+        const unsigned v = perm(zc, 0, sel);
+        const unsigned p0 = perm(s3, 0, sel), p8 = perm(n3, 0, sel);          // (0,+3) (0,-3)
+        const unsigned p4 = perm(w_p3, 0, sel), p12 = perm(w_m3, 0, sel);     // (+3,0) (-3,0)
+        const unsigned p2 = perm(se_, 0, sel), p10 = perm(nw_, 0, sel);       // (+2,+2) (-2,-2)
+        const unsigned p6 = perm(ne_, 0, sel), p14 = perm(sw_, 0, sel);       // (+2,-2) (-2,+2)
+        const unsigned lo = maxs2(max3s2(mins2(p0, p8), mins2(p4, p12), mins2(p2, p10)), mins2(p6, p14));
+        const unsigned hi = mins2(min3s2(maxs2(p0, p8), maxs2(p4, p12), maxs2(p2, p10)), maxs2(p6, p14));
+        ok[hlf] = ((v + bias - lo) | (hi + bias - v)) & 0x02000200u;         // bit 9 of a half <=> that pixel may be a corner
     }
-    return m;
+    // bits 9, 10, 25, 26 = pixels 0, 1, 2, 3
+    const unsigned b = ok[0] + (ok[1] << 1);
+    return ((b >> 9) | (b >> 23)) & 0xFu;
+}
+// the form with one constant per polarity (darker T1, brighter U1) that tests/native/fast_screen_host.cpp is written against;
+// both constants are the bias, so U1 == T1
+SE2_HD unsigned screen_T1(int t) { return screen_bias(t); }
+SE2_HD unsigned screen_U1(int t) { return screen_bias(t); }
+SE2_HD unsigned screen4(unsigned n3, unsigned s3, unsigned n2l, unsigned n2c, unsigned n2r, unsigned s2l, unsigned s2c, unsigned s2r,
+                        unsigned zl, unsigned zc, unsigned zr, unsigned T1, unsigned /*U1*/) {
+    return screen4(n3, s3, n2l, n2c, n2r, s2l, s2c, s2r, zl, zc, zr, T1);
 }
 
 // bits j of an item of up to 8 pixels (interior x = x0 + j) that lie inside the cell interior [0, cw); needs x0 <= cw - 1 and x0 >= -7
@@ -121,13 +130,20 @@ SE2_HD unsigned inside_mask8(int x0, int cw) {
     return (0xFFu << lo) & (0xFFu >> (8 - hi)) & 0xFFu;
 }
 
-// ---- pass A work distribution of orb_fast_cells (shared with the host test, which simulates the CTA's threads)
+// ---- pass A work distribution of orb_fast_cells (shared with the host tests, which simulate the CTA's threads:
+// tests/native/fast_pass_a8_host.cpp the kernel's 8-pixel items, section 3 of tests/native/fast_screen_host.cpp the earlier
+// split of one 4-pixel group per item, which the kernel no longer uses)
 // The patch row starts `shift` bytes left of the cell's first apron pixel (0..15 with the 16 B aligned TMA box, 0..3 with the
 // 4 B aligned plain loads), so interior pixel x sits at patch byte x + 3 + shift. An item = row y of the cell x one 4-pixel group
 // g = 0 .. groups_per_row - 1, i.e. patch word first_group + g, interior x = group_x0(g) .. +3.
 SE2_HD int first_group(int shift) { return (shift + 3) >> 2; }
 SE2_HD int groups_per_row(int cw, int shift) { return ((shift + 2 + cw) >> 2) - first_group(shift) + 1; }
 SE2_HD int group_x0(int g, int shift) { return 4 * (g + first_group(shift)) - 3 - shift; }   // -3 .. cw-1
+// A pass A item is 8 pixels: the groups 2i and 2i+1 of row y (patch words first_group + 2i, +1; interior x = group_x0(2i) .. +7),
+// so the two screens share the 16 patch words they read. When groups_per_row is odd, the last item of a row has a second group
+// past the cell: inside_mask8 drops its pixels, and its reads end at most one word past the patch's last row, inside the score
+// plane that follows the patch in shared memory (its right-hand words on rows y-2 .. y+2 fall on the next patch row).
+SE2_HD int items_per_row(int cw, int shift) { return (groups_per_row(cw, shift) + 1) >> 1; }
 // thread tid visits items tid, tid + nthreads, tid + 2 nthreads, ... (item = y * G + g) without a division per item
 struct ItemWalk {
     int y, g, dY, dG, G;

@@ -442,19 +442,23 @@ __device__ __forceinline__ void orb_tma_box3(void* dst_smem, const CUtensorMap* 
 //          rounded up to 4 B. Takes any cell whose patch and candidate list fit shared memory with 16-bit list offsets.
 // Then, at either pitch:
 //   A  every pixel: necessary condition (fastpx::screen4: a 9-arc contains one pixel of each opposite pair (k, k+8), so for one
-//      polarity all 4 tested pairs need a member beyond t), branch-free on two pixels per s16x2 word; one thread = the 4 pixels
-//      of one patch word (group), (row, group) items walked without a division; survivors are compacted into a shared list
-//      (4 ballots + one shared atomic per 128 pixels)
+//      polarity all 4 tested pairs need a member beyond t), branch-free on two pixels per s16x2 word; one thread = the 8 pixels
+//      of two neighbouring patch words, whose screens share the 16 words they read; (row, item) items walked without a division;
+//      survivors are compacted into a shared list by one atomicAdd per lane, which the compiler turns into a warp scan and one
+//      shared atomic per warp (280 SASS per 8-pixel item in <true> at 48 registers, 35 per pixel, FAST group 0.237-0.239 ms
+//      per 64-frame batch on an H100 SXM at 700 W; the 4-pixel items with 4 ballots and a shared atomic per warp took 207 per
+//      4 pixels, 52 per pixel, at 64 registers and 4 CTAs per SM, and 0.275 ms)
 //   B  list entries, full warps: arc score -> score plane (same pitch as the patch, zero apron and padding, fastpx::NMS_X0)
 //   C  every thread a run of consecutive bitmap words (whole words per cell row): fastpx::nms32, the strict 3x3 maximum of 32
 //      pixels from the dense score plane, branch-free on two pixels per u16x2 word
 //   D  CTA-wide exclusive scan of the threads' keypoint counts = raster-order output slots
 //   E  every thread its own bitmap words: emit (score | y | x), (y, x) from the word's row and column
-// Registers: the plain instantiation is capped at 48 (at least 5 CTAs of 256 threads per SM); uncapped it takes 64 where 40
-// suffice without spilling. The TMA instantiation has no minimum (0) and gets 64 registers (4 CTAs): a minimum of 4 CTAs keeps
-// 64 registers but schedules a kernel measured 0.8 % slower on an H100 SXM (400 W), a minimum of 1 lets it grow to 72 (3 CTAs).
+// Registers: both instantiations are bounded for at least 5 CTAs of 256 threads per SM, so they get 48 (<true>) and 47
+// (<false>), without spilling. Unbounded, the 8-pixel pass A takes <true> to 74 registers (80 allocated, 3 CTAs per SM): on an
+// H100 SXM (700 W, 1980 MHz) its FAST group measured 0.2507-0.2523 ms per 64-frame batch against 0.2366-0.2385 ms with the
+// bound, although the bound costs pass A 280 SASS per item instead of 234 (address arithmetic recomputed per item).
 template <bool TMA>
-__global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbDev d, const __grid_constant__ FastMaps maps) {
+__global__ void __launch_bounds__(FAST_THREADS, 5) orb_fast_cells(OrbDev d, const __grid_constant__ FastMaps maps) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ int s_ncand, s_wsum[FAST_THREADS / 32];
     __shared__ __align__(8) unsigned long long s_bar;
@@ -473,7 +477,7 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
     const int pw = TMA ? L.fbw : (shift + cw + 6 + 3) & ~3, pww = pw >> 2;   // patch pitch
     const int ph = TMA ? L.fbh : ch + 6;                                      // patch rows
     uint8_t* smem = TMA ? smem_raw + ((128u - (orb_smem_u32(smem_raw) & 127u)) & 127u) : smem_raw;   // TMA destination: 128 B aligned
-    const int g0 = fastpx::first_group(shift), G = fastpx::groups_per_row(cw, shift), nitems = ch * G;   // pass A work items
+    const int g0 = fastpx::first_group(shift), G = fastpx::items_per_row(cw, shift), nitems = ch * G;   // pass A work items
     const int wpr = fastpx::nms_words_per_row(cw);                                        // bitmap words per cell row
     uint8_t* patch = smem;                                                                // [ph x pw], pixel (x,y) of the cell at (y+3)*pw + x+3+shift
     uint8_t* score = smem + ((pw * ph + 15) & ~15);                                       // [(ch+2) x pw], pixel (x,y) at (y+1)*pw + x+NMS_X0
@@ -505,52 +509,44 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
         if (threadIdx.x == 0) s_ncand = 0;
         if (TMA && pass == 0 && !orb_mbar_wait(&s_bar, 0)) { *d.err = 4; return; }   // the patch has landed (async-proxy writes are visible after the wait)
         __syncthreads();
-        // A
+        // pass A
         {
             const uint32_t* pwords = reinterpret_cast<const uint32_t*>(patch);
-            const unsigned T1 = fastpx::screen_T1(thr), U1 = fastpx::screen_U1(thr);
+            const unsigned bias = fastpx::screen_bias(thr);
             fastpx::ItemWalk it = first;
             for (int it0 = wid * 32; it0 < nitems; it0 += NW * 32) {
                 unsigned m = 0;
-                const int col0 = fastpx::group_x0(it.g, shift);    // interior x of the group's first pixel
-                if (it.y < ch) {                                   // <=> it0 + lane < nitems
-                    const uint32_t* c = pwords + (it.y + 3) * pww + it.g + g0;
-                    const uint32_t n3 = c[-3 * pww], s3 = c[3 * pww];
-                    const uint32_t n2a = c[-2 * pww - 1], n2b = c[-2 * pww], n2c = c[-2 * pww + 1];
-                    const uint32_t s2a = c[2 * pww - 1], s2b = c[2 * pww], s2c = c[2 * pww + 1];
-                    const uint32_t za = c[-1], zb = c[0], zc = c[1];
-                    // necessary condition, then drop the group's pixels outside the cell interior
-                    m = fastpx::screen4(n3, s3, n2a, n2b, n2c, s2a, s2b, s2c, za, zb, zc, T1, U1) & fastpx::inside_mask8(col0, cw) & 0xFu;
+                const int col0 = fastpx::group_x0(2 * it.g, shift);   // interior x of the item's first pixel
+                if (it.y < ch) {                                      // <=> it0 + lane < nitems
+                    const uint32_t* c = pwords + (it.y + 3) * pww + 2 * it.g + g0;
+                    const uint32_t n3a = c[-3 * pww], n3b = c[-3 * pww + 1], s3a = c[3 * pww], s3b = c[3 * pww + 1];
+                    const uint32_t n2a = c[-2 * pww - 1], n2b = c[-2 * pww], n2c = c[-2 * pww + 1], n2d = c[-2 * pww + 2];
+                    const uint32_t s2a = c[2 * pww - 1], s2b = c[2 * pww], s2c = c[2 * pww + 1], s2d = c[2 * pww + 2];
+                    const uint32_t za = c[-1], zb = c[0], zc = c[1], zd = c[2];
+                    // necessary condition on both words, then drop the item's pixels outside the cell interior
+                    m = (fastpx::screen4(n3a, s3a, n2a, n2b, n2c, s2a, s2b, s2c, za, zb, zc, bias) |
+                         fastpx::screen4(n3b, s3b, n2b, n2c, n2d, s2b, s2c, s2d, zb, zc, zd, bias) << 4) & fastpx::inside_mask8(col0, cw);
                 }
                 // list slots: the list's order does not matter (B writes each entry's own plane byte, C and E are dense), so a
-                // survivor's slot is the warp's base + the survivors of lower group bits + those of lower lanes at its bit
-                const unsigned b0 = __ballot_sync(0xffffffffu, m & 1u), b1 = __ballot_sync(0xffffffffu, m & 2u);
-                const unsigned b2 = __ballot_sync(0xffffffffu, m & 4u), b3 = __ballot_sync(0xffffffffu, m & 8u);
-                const int n0 = __popc(b0), n01 = n0 + __popc(b1), n012 = n01 + __popc(b2), tot = n012 + __popc(b3);
-                if (tot) {
-                    int base = 0;
-                    if (lane == 0) base = atomicAdd(&s_ncand, tot);
-                    base = __shfl_sync(0xffffffffu, base, 0);
-                    const unsigned lt = (1u << lane) - 1u;
-                    const int e0 = it.y * pw + col0;
-                    if (m & 1u) list[base + __popc(b0 & lt)] = (uint16_t)e0;
-                    if (m & 2u) list[base + n0 + __popc(b1 & lt)] = (uint16_t)(e0 + 1);
-                    if (m & 4u) list[base + n01 + __popc(b2 & lt)] = (uint16_t)(e0 + 2);
-                    if (m & 8u) list[base + n012 + __popc(b3 & lt)] = (uint16_t)(e0 + 3);
-                }
+                // lane's survivors take consecutive slots from its own atomicAdd
+                uint16_t* dst = list + atomicAdd(&s_ncand, __popc(m));
+                const int e0 = it.y * pw + col0;
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+                    if (m & (1u << j)) *dst++ = (uint16_t)(e0 + j);
                 it.next();
             }
         }
         __syncthreads();
         const int ncand = s_ncand;
-        // B
+        // pass B
         for (int i = threadIdx.x; i < ncand; i += FAST_THREADS) {
             const int off = list[i];
             const int m = fast_arc_score(p0 + off, pw);
             if (m > thr) score[off + pw + fastpx::NMS_X0] = (uint8_t)(m - 1);
         }
         __syncthreads();
-        // C: whole bitmap words, dense over the score plane; D: CTA-wide exclusive scan of the threads' keypoint counts
+        // pass C: whole bitmap words, dense over the score plane; D: CTA-wide exclusive scan of the threads' keypoint counts
         int nkp = 0;
         for (fastpx::WordRun r = words; r.more(); r.next()) {
             const uint32_t* u = reinterpret_cast<const uint32_t*>(score) + r.y * pww + 8 * r.k;
@@ -569,7 +565,7 @@ __global__ void __launch_bounds__(FAST_THREADS, TMA ? 0 : 5) orb_fast_cells(OrbD
         if (total > 3 || thr == 7) break;
         thr = 7;                 // cellKeyPoints.size() <= 3: clear and retry with the fixed fallback threshold
     }
-    // E: this thread's bitmap words (it wrote them in C), in raster order from its slot pos0
+    // pass E: this thread's bitmap words (it wrote them in C), in raster order from its slot pos0
     uint32_t* out = d.cand + (size_t)f * d.cand_total + c.cand_off;
     int pos = pos0;
     for (fastpx::WordRun r = words; r.more(); r.next()) {
