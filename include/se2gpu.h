@@ -35,6 +35,9 @@
  *   se2gpu_xyz_info[_device]         Track::calcSE3toXYZInfo                  src/Track.cpp:259-306
  *   se2gpu_projection_observations[_device]  LocalMapper::findCorrespd, MatchByProjection branch  src/LocalMapper.cpp:119-141
  *   se2gpu_remove_outliers[_device]  Track::removeOutliers (cv::findFundamentalMat)  src/Track.cpp:308-344
+ *   se2gpu_pose_ba[_device]          Localizer::DoLocalBA (pose-only SE(3) BA, g2o LM)  src/Localizer.cpp:233-302,
+ *                                    (addPlaneMotionSE3Expmap src/optimizer.cpp:236-314, EdgeSE3ExpmapPrior :159-189)
+ *   se2gpu_localizer_ba_device       Localizer::MatchLocalMap's observations + DoLocalBA  src/Localizer.cpp:211-302
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -480,6 +483,64 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
  *        arena): they run the sequential Schur sweep over lists in global memory */
 #define SE2GPU_BA_PLAN_FIELDS 14
 int se2gpu_ba_debug_plan(se2gpu_ba* h, int* out, int n_out);
+
+/* ------------------------------------------------------------------------------------------ pose-only BA */
+/* Localizer::DoLocalBA (src/Localizer.cpp:233-302) for B independent problems, one CTA each, every LM iteration on the
+ * device: one VertexSE3Expmap (estimate toSE3Quat(Tcw)), the plane-motion EdgeSE3ExpmapPrior of addPlaneMotionSE3Expmap
+ * (src/optimizer.cpp:236-314) and one EdgeProjectXYZ2UV per edge (error uv - cam_map(T.map(xyz)), information info[e] * I,
+ * RobustKernelHuber(huber_delta)), then g2o's optimize(iterations) with OptimizationAlgorithmLevenberg, in double precision
+ * (DESIGN.md section 9). */
+typedef struct se2gpu_pose_ba_params {
+    float fx, cx, cy;       /* CamPara: Config::Kcam (0,0), (0,2), (1,2) */
+    float Tbc[16];          /* Config::bTc, row-major 4x4 */
+    float huber_delta;      /* Config::TH_HUBER */
+    float xrot_info, yrot_info, z_info; /* Config::PLANEMOTION_XROT_INFO, _YROT_INFO, _Z_INFO (1e6, 1e6, 1) */
+    int iterations;         /* optimize(iterations): 30 in DoLocalBA */
+} se2gpu_pose_ba_params;
+
+/* per-problem status */
+#define SE2GPU_POSE_BA_OK 0
+#define SE2GPU_POSE_BA_NO_EDGES 1  /* no projection edge: Tcw left as it is, 0 iterations */
+#define SE2GPU_POSE_BA_NOT_PD 2    /* LM terminated because all 10 trials of its last iteration failed the Cholesky */
+#define SE2GPU_POSE_BA_GATED 3     /* se2gpu_localizer_ba_device: no more edges than min_edges, Tcw left as it is */
+
+/* HOST buffers, synchronous. Problem b owns edges edge_ptr[b] .. edge_ptr[b+1]-1 (edge_ptr [B+1], edge_ptr[0] = 0) of
+ * xyz [E*3] (MapPoint::getPos), uv [E*2] (keyPointsUn[idx].pt) and info [E] (the scalar of the edge's information w*I).
+ * Tcw [B*16] float row-major: in, the start estimate; out, toCvMat of the result (left as it is for NO_EDGES).
+ * Optional (may be NULL): stats [B*iterations] (row b*iterations + k is iteration k; rows past iterations[b] are zero),
+ * iterations [B] LM iterations done, status [B], pose [B*7] the double estimate (qx, qy, qz, qw, tx, ty, tz).
+ * Device buffers are a per-device workspace that only grows. */
+int se2gpu_pose_ba(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
+                   const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status, double* pose,
+                   int device);
+/* The same on DEVICE buffers, asynchronous on `stream` (params is a host pointer, read during the call). d_stats rows past
+ * an iteration count are not written. */
+int se2gpu_pose_ba_device(int B, float* d_Tcw, const int* d_edge_ptr, const float* d_xyz, const float* d_uv, const float* d_info,
+                          const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
+                          double* d_pose, void* stream);
+/* parity hook: se2gpu_pose_ba plus trace [B*iterations*7], the estimate after every iteration (rows past the count zero) */
+int se2gpu_pose_ba_debug_trace(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
+                               const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status,
+                               double* pose, double* trace, int device);
+
+/* Localizer context: the device workspace for up to max_map_points local map points. One per calling thread. */
+typedef struct se2gpu_localizer se2gpu_localizer;
+se2gpu_localizer* se2gpu_localizer_create(int max_map_points, int device);
+void se2gpu_localizer_destroy(se2gpu_localizer* h);
+/* MatchLocalMap's observations + DoLocalBA on DEVICE buffers, asynchronous on `stream`, fed straight from
+ * se2gpu_match_by_projection_device: d_kf_kp [n_kf] (*d_n_kf of them valid when d_n_kf is not NULL), d_matches_idx_mp [n_kf]
+ * (-1 = unmatched), d_mp_xyz [n_mp*3] (getPos), d_mp_use [n_mp] (!isNull && isGoodPrl), d_inv_sigma2 [nlevels]
+ * (mvInvLevelSigma2). The edges are the map points j with d_mp_use[j] that some keypoint matched, in ascending j; uv is
+ * the keypoint of the highest index that matched j (repeated KeyFrame::addObservation keeps the last); every edge's
+ * information is d_inv_sigma2[d_kf_kp[0].octave], which is what MapPoint::getOctave returns for the Localizer's new
+ * keyframe (see DESIGN.md section 9). d_n_edges (may be NULL) receives the edge count; the optimisation runs only when it
+ * exceeds min_edges (DoLocalBA's caller runs it above 30 observations), otherwise the status is GATED. d_Tcw [16] is
+ * updated in place. d_stats [iterations], d_iterations, d_status [1], d_pose [7] may be NULL. */
+int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_kp, int n_kf, const int* d_n_kf,
+                               const int* d_matches_idx_mp, int n_mp, const float* d_mp_xyz, const uint8_t* d_mp_use,
+                               const float* d_inv_sigma2, int nlevels, float* d_Tcw, const se2gpu_pose_ba_params* params,
+                               int min_edges, int* d_n_edges, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
+                               double* d_pose, void* stream);
 
 #ifdef __cplusplus
 }

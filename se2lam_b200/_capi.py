@@ -29,6 +29,11 @@ class BowKF(C.Structure):
                 ("node", C.c_void_p), ("n_node", C.c_int), ("ptr", C.c_void_p), ("feat", C.c_void_p)]
 
 
+class PoseBAParams(C.Structure):
+    _fields_ = [("fx", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("Tbc", C.c_float * 16), ("huber_delta", C.c_float),
+                ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float), ("iterations", C.c_int)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -56,6 +61,8 @@ SYMBOLS = [
     "se2gpu_xyz_info", "se2gpu_xyz_info_device", "se2gpu_projection_observations", "se2gpu_projection_observations_device",
     "se2gpu_debug_svd4", "se2gpu_remove_outliers", "se2gpu_remove_outliers_device", "se2gpu_fundam_niters_table",
     "se2gpu_fundam_debug_niters",
+    "se2gpu_pose_ba", "se2gpu_pose_ba_device", "se2gpu_pose_ba_debug_trace", "se2gpu_localizer_create", "se2gpu_localizer_destroy",
+    "se2gpu_localizer_ba_device",
 ]
 
 
@@ -150,6 +157,13 @@ def lib():
     L.se2gpu_fundam_niters_table.restype = None
     L.se2gpu_fundam_niters_table.argtypes = [vp]
     L.se2gpu_fundam_debug_niters.argtypes = [i, vp, vp, vp, vp, i]
+    L.se2gpu_pose_ba.argtypes = [i] + [vp] * 10 + [i]
+    L.se2gpu_pose_ba_device.argtypes = [i] + [vp] * 11
+    L.se2gpu_pose_ba_debug_trace.argtypes = [i] + [vp] * 11 + [i]
+    L.se2gpu_localizer_create.restype = vp
+    L.se2gpu_localizer_create.argtypes = [i, i]
+    L.se2gpu_localizer_destroy.argtypes = [vp]
+    L.se2gpu_localizer_ba_device.argtypes = [vp, vp, i, vp, vp, i, vp, vp, vp, i, vp, vp, i, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

@@ -1,0 +1,705 @@
+// Pose-only SE(3) bundle adjustment: Localizer::DoLocalBA (reference src/Localizer.cpp:233-302) for B independent problems,
+// one CTA each, all LM iterations inside the kernel.
+//
+// What a problem is (DESIGN.md section 9): one g2o VertexSE3Expmap (estimate toSE3Quat(Tcw)), one EdgeSE3ExpmapPrior from
+// addPlaneMotionSE3Expmap (src/optimizer.cpp:236-314) and one EdgeProjectXYZ2UV with a Huber kernel per observed map point
+// (fixed points, information w_e I), optimised by g2o's OptimizationAlgorithmLevenberg. Everything is double precision.
+//
+// Per CTA: thread 0 builds the prior and holds the LM scalars in shared memory; the edges are staged in shared memory when
+// they fit (kStageMax), otherwise read from global memory. Each linearisation has every thread accumulate the 21 upper
+// entries of H, the 6 of b and the robust chi2 of the edges e = tid, tid + 256, ... in registers; a warp xor-shuffle tree
+// and then the 8 warp sums in index order combine them (no atomics: bit-reproducible, independent of the CTA's position in
+// the batch). Thread 0 adds the prior, damps, factorises the 6 x 6 system (LL^T), applies SE3Quat::exp and the compose,
+// and a second reduction gives the trial chi2.
+#include <cuda_runtime.h>
+
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+#include <mutex>
+
+#include "common.h"
+
+using namespace se2gpu;
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kStageMax = 1536;  // edges staged in shared memory: 24 B each, 36 KB
+constexpr int kAcc = 28;         // 21 upper entries of H, 6 of b, chi2
+
+struct Params {
+    double fx, cx, cy, delta;
+    float Tbc[16];
+    float xrot, yrot, zinfo;
+    int iterations;
+};
+
+struct Quat { double x, y, z, w; };
+struct SE3 { Quat q; double t[3]; };
+
+__device__ inline void cross(const double* a, const double* b, double* c) {
+    c[0] = a[1] * b[2] - a[2] * b[1];
+    c[1] = a[2] * b[0] - a[0] * b[2];
+    c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// Eigen Quaterniond(const Matrix3d&)
+__device__ Quat quat_from_R(const double* m) {
+    Quat q;
+    double t = m[0] + m[4] + m[8];
+    if (t > 0) {
+        t = sqrt(t + 1.0);
+        q.w = 0.5 * t;
+        t = 0.5 / t;
+        q.x = (m[7] - m[5]) * t;
+        q.y = (m[2] - m[6]) * t;
+        q.z = (m[3] - m[1]) * t;
+    } else {
+        int i = 0;
+        if (m[4] > m[0]) i = 1;
+        if (m[8] > m[i * 4]) i = 2;
+        const int j = (i + 1) % 3, k = (j + 1) % 3;
+        double c[3];
+        t = sqrt(m[i * 4] - m[j * 4] - m[k * 4] + 1.0);
+        c[i] = 0.5 * t;
+        t = 0.5 / t;
+        q.w = (m[k * 3 + j] - m[j * 3 + k]) * t;
+        c[j] = (m[j * 3 + i] + m[i * 3 + j]) * t;
+        c[k] = (m[k * 3 + i] + m[i * 3 + k]) * t;
+        q.x = c[0]; q.y = c[1]; q.z = c[2];
+    }
+    return q;
+}
+
+// Eigen QuaternionBase::toRotationMatrix
+__device__ void quat_to_R(const Quat& q, double* R) {
+    const double tx = 2 * q.x, ty = 2 * q.y, tz = 2 * q.z;
+    const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w;
+    const double txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
+    const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
+    R[0] = 1 - (tyy + tzz); R[1] = txy - twz;       R[2] = txz + twy;
+    R[3] = txy + twz;       R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
+    R[6] = txz - twy;       R[7] = tyz + twx;       R[8] = 1 - (txx + tyy);
+}
+
+__device__ inline Quat qmul(const Quat& a, const Quat& b) {
+    return {a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
+            a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z,
+            a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x,
+            a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z};
+}
+
+// Eigen q * v (_transformVector)
+__device__ inline void qrot(const Quat& q, const double* v, double* out) {
+    const double qv[3] = {q.x, q.y, q.z};
+    double uv[3], c[3];
+    cross(qv, v, uv);
+    uv[0] += uv[0]; uv[1] += uv[1]; uv[2] += uv[2];
+    cross(qv, uv, c);
+    for (int i = 0; i < 3; ++i) out[i] = v[i] + q.w * uv[i] + c[i];
+}
+
+// g2o SE3Quat::normalizeRotation
+__device__ inline void normalize_rotation(Quat& q) {
+    if (q.w < 0) { q.x = -q.x; q.y = -q.y; q.z = -q.z; q.w = -q.w; }
+    const double n2 = q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w;
+    if (n2 > 0) {
+        const double n = sqrt(n2);
+        q.x /= n; q.y /= n; q.z /= n; q.w /= n;
+    }
+}
+
+// converter.cpp toSE3Quat(cv::Mat) on a float 4x4 row-major
+__device__ SE3 se3_from_f32(const float* T) {
+    const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+    SE3 r;
+    r.q = quat_from_R(R);
+    r.t[0] = T[3]; r.t[1] = T[7]; r.t[2] = T[11];
+    normalize_rotation(r.q);
+    return r;
+}
+
+__device__ SE3 se3_mul(const SE3& a, const SE3& b) {
+    SE3 r = a;
+    double rt[3];
+    qrot(a.q, b.t, rt);
+    for (int i = 0; i < 3; ++i) r.t[i] += rt[i];
+    r.q = qmul(a.q, b.q);
+    normalize_rotation(r.q);
+    return r;
+}
+
+__device__ SE3 se3_inv(const SE3& a) {
+    SE3 r;
+    r.q = {-a.q.x, -a.q.y, -a.q.z, a.q.w};
+    const double mt[3] = {a.t[0] * -1., a.t[1] * -1., a.t[2] * -1.};
+    qrot(r.q, mt, r.t);
+    return r;
+}
+
+__device__ inline void skew(const double* v, double* S) {
+    S[0] = 0;     S[1] = -v[2]; S[2] = v[1];
+    S[3] = v[2];  S[4] = 0;     S[5] = -v[0];
+    S[6] = -v[1]; S[7] = v[0];  S[8] = 0;
+}
+
+__device__ inline void mul3(const double* A, const double* B, double* C) {
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) C[r * 3 + c] = A[r * 3] * B[c] + A[r * 3 + 1] * B[3 + c] + A[r * 3 + 2] * B[6 + c];
+}
+
+// g2o SE3Quat::exp, update [omega, upsilon], small-angle branch below theta = 1e-5
+__device__ SE3 se3_exp(const double* u) {
+    const double* omega = u;
+    const double* upsilon = u + 3;
+    const double theta = sqrt(omega[0] * omega[0] + omega[1] * omega[1] + omega[2] * omega[2]);
+    double O[9], O2[9], R[9], V[9];
+    skew(omega, O);
+    mul3(O, O, O2);
+    if (theta < 0.00001) {
+        for (int k = 0; k < 9; ++k) { R[k] = (k % 4 == 0 ? 1.0 : 0.0) + O[k] + O2[k]; V[k] = R[k]; }
+    } else {
+        double s, c;
+        sincos(theta, &s, &c);
+        const double a = s / theta, b = (1 - c) / (theta * theta), d = (theta - s) / (theta * theta * theta);
+        for (int k = 0; k < 9; ++k) {
+            const double I = (k % 4 == 0 ? 1.0 : 0.0);
+            R[k] = I + a * O[k] + b * O2[k];
+            V[k] = I + b * O[k] + d * O2[k];
+        }
+    }
+    SE3 T;
+    for (int r = 0; r < 3; ++r) T.t[r] = V[r * 3] * upsilon[0] + V[r * 3 + 1] * upsilon[1] + V[r * 3 + 2] * upsilon[2];
+    T.q = quat_from_R(R);
+    normalize_rotation(T.q);
+    return T;
+}
+
+// g2o SE3Quat::log, small-rotation branch above d = 0.99999
+__device__ void se3_log(const SE3& T, double* res) {
+    double R[9];
+    quat_to_R(T.q, R);
+    const double d = 0.5 * (R[0] + R[4] + R[8] - 1);
+    const double dR[3] = {R[7] - R[5], R[2] - R[6], R[3] - R[1]};
+    double omega[3], O[9], O2[9], f;
+    if (d > 0.99999) {
+        for (int i = 0; i < 3; ++i) omega[i] = 0.5 * dR[i];
+        f = 1. / 12.;
+    } else {
+        const double theta = acos(d);
+        const double s = theta / (2 * sqrt(1 - d * d));
+        for (int i = 0; i < 3; ++i) omega[i] = s * dR[i];
+        f = (1 - theta / (2 * tan(theta / 2))) / (theta * theta);
+    }
+    skew(omega, O);
+    mul3(O, O, O2);
+    for (int i = 0; i < 3; ++i) res[i] = omega[i];
+    for (int r = 0; r < 3; ++r) {
+        double acc = 0;
+        for (int c = 0; c < 3; ++c) acc += ((r == c ? 1.0 : 0.0) - 0.5 * O[r * 3 + c] + f * O2[r * 3 + c]) * T.t[c];
+        res[3 + r] = acc;
+    }
+}
+
+// addPlaneMotionSE3Expmap (src/optimizer.cpp:236-314, non-USE_EULER branch)
+__device__ void plane_motion_prior(const SE3& pose, const Params& p, SE3* meas, double* info) {
+    const SE3 Tbc = se3_from_f32(p.Tbc);
+    SE3 Tbw = se3_mul(Tbc, pose);
+    const Quat& q = Tbw.q;  // Eigen 3.3 AngleAxisd(Quaterniond): angle = 2 atan2(|vec|, |w|), axis = vec / (+-|vec|)
+    double n = sqrt(q.x * q.x + q.y * q.y + q.z * q.z), angle = 0, axis_z = 0;
+    if (n != 0) {
+        angle = 2 * atan2(n, fabs(q.w));
+        if (q.w < 0) n = -n;
+        axis_z = q.z / n;
+    }
+    const double ha = 0.5 * (angle * axis_z);
+    double s, c;
+    sincos(ha, &s, &c);
+    Tbw.q = {s * 0.0, s * 0.0, s * 1.0, c};  // Quaterniond(AngleAxisd(yaw, UnitZ)); setRotation does not normalise
+    Tbw.t[2] = 0;
+    *meas = se3_mul(se3_inv(Tbc), Tbw);
+    // Info_cw = Adj(Tbc)^T diag(xrot, yrot, 1e-4, 1e-4, 1e-4, z) Adj(Tbc), Adj = [[R, 0], [skew(t) R, R]]
+    double R[9], S[9], SR[9], J[36];
+    quat_to_R(Tbc.q, R);
+    skew(Tbc.t, S);
+    mul3(S, R, SR);
+    for (int k = 0; k < 36; ++k) J[k] = 0;
+    for (int r = 0; r < 3; ++r)
+        for (int cc = 0; cc < 3; ++cc) {
+            J[r * 6 + cc] = R[r * 3 + cc];
+            J[(r + 3) * 6 + cc + 3] = R[r * 3 + cc];
+            J[(r + 3) * 6 + cc] = SR[r * 3 + cc];
+        }
+    const double dg[6] = {(double)p.xrot, (double)p.yrot, 1e-4, 1e-4, 1e-4, (double)p.zinfo};
+    for (int r = 0; r < 6; ++r)
+        for (int cc = r; cc < 6; ++cc) {
+            double acc = 0;
+            for (int k = 0; k < 6; ++k) acc += (J[k * 6 + r] * dg[k]) * J[k * 6 + cc];
+            info[r * 6 + cc] = acc;
+            info[cc * 6 + r] = acc;  // symmetric from the upper triangle
+        }
+}
+
+// log(meas * est^-1) and its chi2 under the prior's information
+__device__ double prior_error(const SE3& meas, const double* info, const SE3& T, double* e) {
+    se3_log(se3_mul(meas, se3_inv(T)), e);
+    double chi = 0;
+    for (int r = 0; r < 6; ++r) {
+        double we = 0;
+        for (int c = 0; c < 6; ++c) we += info[r * 6 + c] * e[c];
+        chi += e[r] * we;
+    }
+    return chi;
+}
+
+// one EdgeProjectXYZ2UV: robust chi2 into chi; with LIN also rho' J^T w J (upper triangle) into hb[0..20] and
+// -rho' J^T w e into hb[21..26]
+template <bool LIN>
+__device__ inline void edge_terms(const SE3& T, const float* xyz, const float* uv, float wf, const Params& p, double& chi,
+                                  double* hb) {
+    const double X[3] = {xyz[0], xyz[1], xyz[2]};
+    double pc[3];
+    qrot(T.q, X, pc);
+    for (int i = 0; i < 3; ++i) pc[i] += T.t[i];
+    const double w = wf;
+    const double e0 = (double)uv[0] - ((pc[0] / pc[2]) * p.fx + p.cx);
+    const double e1 = (double)uv[1] - ((pc[1] / pc[2]) * p.fx + p.cy);
+    const double c2 = e0 * (w * e0) + e1 * (w * e1);
+    const double dsqr = p.delta * p.delta;
+    const bool inlier = c2 <= dsqr;
+    const double sq = inlier ? 0.0 : sqrt(c2);
+    chi += inlier ? c2 : 2 * sq * p.delta - dsqr;
+    if (!LIN) return;
+    const double rho1 = inlier ? 1.0 : p.delta / sq;
+    const double x = pc[0], y = pc[1], z = pc[2], z2 = z * z, fx = p.fx;
+    const double J[12] = {x * y / z2 * fx,       -(1 + (x * x / z2)) * fx, y / z * fx,  -1. / z * fx, 0,            x / z2 * fx,
+                          (1 + y * y / z2) * fx, -x * y / z2 * fx,         -x / z * fx, 0,            -1. / z * fx, y / z2 * fx};
+    const double W = rho1 * w;
+    const double r0 = -(w * e0) * rho1, r1 = -(w * e1) * rho1;
+    int k = 0;
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+        hb[21 + r] += J[r] * r0 + J[6 + r] * r1;
+#pragma unroll
+        for (int c = r; c < 6; ++c) hb[k++] += (J[r] * W) * J[c] + (J[6 + r] * W) * J[6 + c];
+    }
+}
+
+// fixed-order block sum of N per-thread values: xor-shuffle tree, then the warps in index order by thread 0
+template <int N>
+__device__ inline void block_sum(double* a, double (*red)[kAcc], double* out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) a[k] += __shfl_xor_sync(0xffffffffu, a[k], off);
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) red[warp][k] = a[k];
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int k = 0; k < N; ++k) {
+            double s = red[0][k];
+            for (int w = 1; w < kWarps; ++w) s += red[w][k];
+            out[k] = s;
+        }
+}
+
+// dense LL^T of H + lam I (H full symmetric 6 x 6) and x = (H + lam I)^-1 b; false when not positive definite
+__device__ bool chol_solve6(const double* H, const double* b, double lam, double* x) {
+    double L[36];
+    for (int r = 0; r < 6; ++r)
+        for (int c = 0; c <= r; ++c) {
+            double s = H[r * 6 + c] + (r == c ? lam : 0.0);
+            for (int k = 0; k < c; ++k) s -= L[r * 6 + k] * L[c * 6 + k];
+            if (c == r) {
+                if (!(s > 0.0) || !isfinite(s)) return false;
+                L[r * 6 + r] = sqrt(s);
+            } else {
+                L[r * 6 + c] = s / L[c * 6 + c];
+            }
+        }
+    for (int r = 0; r < 6; ++r) {
+        double s = b[r];
+        for (int k = 0; k < r; ++k) s -= L[r * 6 + k] * x[k];
+        x[r] = s / L[r * 6 + r];
+    }
+    for (int r = 5; r >= 0; --r) {
+        double s = x[r];
+        for (int k = r + 1; k < 6; ++k) s -= L[k * 6 + r] * x[k];
+        x[r] = s / L[r * 6 + r];
+    }
+    return true;
+}
+
+__device__ inline void store_pose(const SE3& T, double* p7) {
+    p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
+    p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
+}
+
+__global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, const int* __restrict__ edge_ptr,
+                                                      const float* __restrict__ xyz, const float* __restrict__ uv,
+                                                      const float* __restrict__ info, Params p, int min_edges,
+                                                      se2gpu_ba_iter_stats* __restrict__ stats, int* __restrict__ iters,
+                                                      int* __restrict__ status, double* __restrict__ pose_out,
+                                                      double* __restrict__ trace) {
+    extern __shared__ float s_stage[];  // [kStageMax*3] xyz, [kStageMax*2] uv, [kStageMax] info
+    __shared__ double s_red[kWarps][kAcc];
+    __shared__ double s_H[36], s_b[6], s_info[36], s_sum[kAcc];
+    __shared__ SE3 s_est, s_trial, s_meas;
+    __shared__ double s_cur, s_lambda, s_ni;
+    __shared__ int s_ok2, s_more, s_stop;
+
+    const int pb = blockIdx.x, tid = threadIdx.x;
+    const int e0 = edge_ptr[pb], E = edge_ptr[pb + 1] - e0;
+    float* T16 = Tcw + 16 * (size_t)pb;
+    if (E <= 0 || E <= min_edges) {  // nothing to refine against: the pose is left as it is
+        if (tid == 0) {
+            if (iters) iters[pb] = 0;
+            if (status) status[pb] = E <= 0 ? SE2GPU_POSE_BA_NO_EDGES : SE2GPU_POSE_BA_GATED;
+            if (pose_out) store_pose(se3_from_f32(T16), pose_out + 7 * (size_t)pb);
+        }
+        return;
+    }
+    if (tid == 0) {
+        s_est = se3_from_f32(T16);
+        plane_motion_prior(s_est, p, &s_meas, s_info);
+        s_stop = 0;
+    }
+    const float* gx = xyz + 3 * (size_t)e0;
+    const float* gu = uv + 2 * (size_t)e0;
+    const float* gw = info + e0;
+    const bool staged = E <= kStageMax;
+    const float* px = gx;
+    const float* pu = gu;
+    const float* pw = gw;
+    if (staged) {
+        for (int k = tid; k < 3 * E; k += kThreads) s_stage[k] = gx[k];
+        for (int k = tid; k < 2 * E; k += kThreads) s_stage[3 * kStageMax + k] = gu[k];
+        for (int k = tid; k < E; k += kThreads) s_stage[5 * kStageMax + k] = gw[k];
+        px = s_stage; pu = s_stage + 3 * kStageMax; pw = s_stage + 5 * kStageMax;
+    }
+    __syncthreads();
+
+    int it = 0, last_failed = 0;
+    for (; it < p.iterations; ++it) {
+        // linearise at the current estimate: chi2, H, b
+        {
+            double acc[kAcc];
+#pragma unroll
+            for (int k = 0; k < kAcc; ++k) acc[k] = 0;
+            const SE3 T = s_est;
+            for (int e = tid; e < E; e += kThreads) edge_terms<true>(T, px + 3 * e, pu + 2 * e, pw[e], p, acc[27], acc);
+            block_sum<kAcc>(acc, s_red, s_sum);
+        }
+        se2gpu_ba_iter_stats st{};
+        if (tid == 0) {
+            double ep[6];
+            const double pchi = prior_error(s_meas, s_info, s_est, ep);
+            int k = 0;
+            for (int r = 0; r < 6; ++r)
+                for (int c = r; c < 6; ++c, ++k) s_H[r * 6 + c] = s_H[c * 6 + r] = s_sum[k] + s_info[r * 6 + c];
+            for (int r = 0; r < 6; ++r) {  // EdgeSE3ExpmapPrior, J = -I: b += Omega e
+                double we = 0;
+                for (int c = 0; c < 6; ++c) we += s_info[r * 6 + c] * ep[c];
+                s_b[r] = s_sum[21 + r] + we;
+            }
+            s_cur = s_sum[27] + pchi;
+            if (it == 0) {  // OptimizationAlgorithmLevenberg::computeLambdaInit, tau = 1e-5
+                double m = 0;
+                for (int r = 0; r < 6; ++r) m = fmax(m, fabs(s_H[r * 7]));
+                s_lambda = 1e-5 * m;
+                s_ni = 2;
+            }
+            st.chi2_before = s_cur;
+        }
+        int qmax = 0, failed = 0;
+        double rho = 0;
+        for (;;) {
+            double x[6], scale = 0;
+            if (tid == 0) {
+                const bool ok2 = chol_solve6(s_H, s_b, s_lambda, x);
+                s_ok2 = ok2;
+                if (ok2) {
+                    s_trial = se3_mul(se3_exp(x), s_est);
+                    for (int r = 0; r < 6; ++r) scale += x[r] * (s_lambda * x[r] + s_b[r]);
+                }
+            }
+            __syncthreads();
+            double temp = DBL_MAX;
+            if (s_ok2) {
+                double a[1] = {0};
+                const SE3 T = s_trial;
+                for (int e = tid; e < E; e += kThreads) edge_terms<false>(T, px + 3 * e, pu + 2 * e, pw[e], p, a[0], nullptr);
+                double tot[1];
+                block_sum<1>(a, s_red, tot);
+                if (tid == 0) {
+                    double ep[6];
+                    temp = tot[0] + prior_error(s_meas, s_info, s_trial, ep);
+                }
+            }
+            if (tid == 0) {
+                if (!s_ok2) ++failed;
+                rho = (s_cur - temp) / (scale + 1e-3);
+                if (rho > 0 && isfinite(temp)) {
+                    double alpha = 1. - pow((2 * rho - 1), 3);
+                    alpha = fmin(alpha, 2. / 3.);
+                    s_lambda *= fmax(1. / 3., alpha);
+                    s_ni = 2;
+                    s_cur = temp;
+                    s_est = s_trial;
+                    st.accepted = 1;
+                } else {
+                    s_lambda *= s_ni;
+                    s_ni *= 2;
+                }
+                ++qmax;
+                s_more = rho < 0 && qmax < 10;
+            }
+            __syncthreads();
+            if (!s_more) break;
+        }
+        if (tid == 0) {
+            st.chi2_after = s_cur; st.lambda = s_lambda; st.rho = rho; st.trials = qmax;
+            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
+            last_failed = st.terminate && failed == qmax;
+            if (stats) stats[(size_t)pb * p.iterations + it] = st;
+            if (trace) store_pose(s_est, trace + ((size_t)pb * p.iterations + it) * 7);
+            s_stop = st.terminate;
+        }
+        __syncthreads();
+        if (s_stop) { ++it; break; }
+    }
+    if (tid == 0) {
+        if (iters) iters[pb] = it;
+        if (status) status[pb] = last_failed ? SE2GPU_POSE_BA_NOT_PD : SE2GPU_POSE_BA_OK;
+        if (pose_out) store_pose(s_est, pose_out + 7 * (size_t)pb);
+        double R[9];  // converter.cpp toCvMat(SE3Quat): to_homogeneous_matrix narrowed to float
+        quat_to_R(s_est.q, R);
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) T16[r * 4 + c] = (float)R[r * 3 + c];
+            T16[r * 4 + 3] = (float)s_est.t[r];
+        }
+        T16[12] = 0.f; T16[13] = 0.f; T16[14] = 0.f; T16[15] = 1.f;
+    }
+}
+
+// Localizer::DoLocalBA's edge list from MatchByProjection's device output, in ascending map-point index: map point j is an
+// edge when some keypoint i < n matched it (the highest such i, as repeated KeyFrame::addObservation leaves it) and use[j];
+// every edge's information is inv_sigma2[kp[0].octave] (MapPoint::getOctave on a keyframe it never observed). One CTA.
+__global__ void __launch_bounds__(1024) k_localizer_edges(const se2gpu_keypoint* __restrict__ kp, int n_kf, const int* __restrict__ d_n_kf,
+                                                          const int* __restrict__ matches, int n_mp, const float* __restrict__ mp_xyz,
+                                                          const uint8_t* __restrict__ mp_use, const float* __restrict__ inv_sigma2,
+                                                          int nlevels, int* __restrict__ best, float* __restrict__ xyz,
+                                                          float* __restrict__ uv, float* __restrict__ w, int* __restrict__ edge_ptr,
+                                                          int* __restrict__ n_edges) {
+    __shared__ int s_wcount[32];
+    __shared__ int s_base;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n = d_n_kf ? min(max(*d_n_kf, 0), n_kf) : n_kf;
+    for (int j = tid; j < n_mp; j += blockDim.x) best[j] = -1;
+    if (tid == 0) s_base = 0;
+    __syncthreads();
+    for (int i = tid; i < n; i += blockDim.x) {
+        const int m = matches[i];
+        if (m >= 0 && m < n_mp) atomicMax(&best[m], i);
+    }
+    __syncthreads();
+    const float w0 = n > 0 ? inv_sigma2[min(max(kp[0].octave, 0), nlevels - 1)] : 0.f;
+    for (int j0 = 0; j0 < n_mp; j0 += blockDim.x) {
+        const int j = j0 + tid;
+        const int k = j < n_mp ? best[j] : -1;
+        const bool take = k >= 0 && mp_use[j];
+        const unsigned bal = __ballot_sync(0xffffffffu, take);
+        if (lane == 0) s_wcount[warp] = __popc(bal);
+        __syncthreads();
+        int off = s_base;
+        for (int v = 0; v < warp; ++v) off += s_wcount[v];
+        off += __popc(bal & ((1u << lane) - 1));
+        if (take) {
+            xyz[3 * off] = mp_xyz[3 * (size_t)j]; xyz[3 * off + 1] = mp_xyz[3 * (size_t)j + 1]; xyz[3 * off + 2] = mp_xyz[3 * (size_t)j + 2];
+            uv[2 * off] = kp[k].x; uv[2 * off + 1] = kp[k].y;
+            w[off] = w0;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int tot = 0;
+            for (int v = 0; v < (int)(blockDim.x >> 5); ++v) tot += s_wcount[v];
+            s_base += tot;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        edge_ptr[0] = 0;
+        edge_ptr[1] = s_base;
+        if (n_edges) *n_edges = s_base;
+    }
+}
+
+int check_params(const se2gpu_pose_ba_params* prm, Params* p) {
+    if (!prm) return fail(SE2GPU_ERR_INVALID, "null parameters");
+    if (prm->iterations < 0) return fail(SE2GPU_ERR_INVALID, "iterations = %d", prm->iterations);
+    p->fx = prm->fx; p->cx = prm->cx; p->cy = prm->cy; p->delta = prm->huber_delta;
+    std::memcpy(p->Tbc, prm->Tbc, sizeof p->Tbc);
+    p->xrot = prm->xrot_info; p->yrot = prm->yrot_info; p->zinfo = prm->z_info;
+    p->iterations = prm->iterations;
+    return SE2GPU_OK;
+}
+
+constexpr size_t kStageBytes = sizeof(float) * 6 * kStageMax;
+
+int launch(int B, float* d_Tcw, const int* d_edge_ptr, const float* d_xyz, const float* d_uv, const float* d_info, const Params& p,
+           int min_edges, se2gpu_ba_iter_stats* d_stats, int* d_iters, int* d_status, double* d_pose, double* d_trace,
+           cudaStream_t stream) {
+    SE2_NVTX("se2gpu_pose_ba");
+    SE2_LAUNCH(k_pose_ba, B, kThreads, kStageBytes, stream, d_Tcw, d_edge_ptr, d_xyz, d_uv, d_info, p, min_edges, d_stats, d_iters,
+               d_status, d_pose, d_trace);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+// grow-only device buffers of the host entry points, one set per device
+struct HostWorkspace {
+    std::mutex mu;
+    char* base = nullptr;
+    size_t cap = 0;
+};
+HostWorkspace g_ws[64];
+
+size_t align_up(size_t v) { return (v + 255) & ~size_t(255); }
+
+int host_run(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
+             const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status, double* pose,
+             double* trace, int device) {
+    Params p;
+    { const int rc = check_params(params, &p); if (rc) return rc; }
+    if (B < 0 || (B && (!Tcw || !edge_ptr))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (B && edge_ptr[0] != 0) return fail(SE2GPU_ERR_INVALID, "edge_ptr[0] must be 0");
+    for (int b = 0; b < B; ++b)
+        if (edge_ptr[b + 1] < edge_ptr[b]) return fail(SE2GPU_ERR_INVALID, "edge_ptr not ascending at %d", b);
+    const size_t E = B ? (size_t)edge_ptr[B] : 0;
+    if (E && (!xyz || !uv || !info)) return fail(SE2GPU_ERR_INVALID, "null edge arrays");
+    { const int rc = select_device(device); if (rc) return rc; }
+    if (B == 0) return SE2GPU_OK;
+    if (device >= 64) return fail(SE2GPU_ERR_INVALID, "device %d", device);
+    const size_t it = (size_t)p.iterations;
+    const size_t sizes[] = {sizeof(float) * 16 * B, sizeof(int) * (B + 1), sizeof(float) * 3 * E, sizeof(float) * 2 * E, sizeof(float) * E,
+                            stats ? sizeof(se2gpu_ba_iter_stats) * B * it : 0, sizeof(int) * B, sizeof(int) * B,
+                            pose ? sizeof(double) * 7 * B : 0, trace ? sizeof(double) * 7 * B * it : 0};
+    constexpr int NB = sizeof sizes / sizeof sizes[0];
+    size_t off[NB], total = 0;
+    for (int k = 0; k < NB; ++k) { off[k] = total; total += align_up(sizes[k]); }
+    HostWorkspace& ws = g_ws[device];
+    std::lock_guard<std::mutex> lock(ws.mu);
+    if (total > ws.cap) {
+        if (ws.base) cudaFree(ws.base);
+        ws.base = nullptr; ws.cap = 0;
+        SE2_CUDA(cudaMalloc((void**)&ws.base, total));
+        ws.cap = total;
+    }
+    char* d = ws.base;
+    float* dT = (float*)(d + off[0]);
+    int* dptr = (int*)(d + off[1]);
+    float* dx = (float*)(d + off[2]);
+    float* du = (float*)(d + off[3]);
+    float* dw = (float*)(d + off[4]);
+    auto* dst = stats ? (se2gpu_ba_iter_stats*)(d + off[5]) : nullptr;
+    int* dit = (int*)(d + off[6]);
+    int* dsts = (int*)(d + off[7]);
+    double* dpose = pose ? (double*)(d + off[8]) : nullptr;
+    double* dtr = trace ? (double*)(d + off[9]) : nullptr;
+    SE2_CUDA(cudaMemcpy(dT, Tcw, sizes[0], cudaMemcpyHostToDevice));
+    SE2_CUDA(cudaMemcpy(dptr, edge_ptr, sizes[1], cudaMemcpyHostToDevice));
+    if (E) {
+        SE2_CUDA(cudaMemcpy(dx, xyz, sizes[2], cudaMemcpyHostToDevice));
+        SE2_CUDA(cudaMemcpy(du, uv, sizes[3], cudaMemcpyHostToDevice));
+        SE2_CUDA(cudaMemcpy(dw, info, sizes[4], cudaMemcpyHostToDevice));
+    }
+    if (dst) SE2_CUDA(cudaMemset(dst, 0, sizes[5]));
+    if (dtr) SE2_CUDA(cudaMemset(dtr, 0, sizes[9]));
+    { const int rc = launch(B, dT, dptr, dx, du, dw, p, 0, dst, dit, dsts, dpose, dtr, nullptr); if (rc) return rc; }
+    SE2_CUDA(cudaMemcpy(Tcw, dT, sizes[0], cudaMemcpyDeviceToHost));
+    if (stats) SE2_CUDA(cudaMemcpy(stats, dst, sizes[5], cudaMemcpyDeviceToHost));
+    if (iterations) SE2_CUDA(cudaMemcpy(iterations, dit, sizes[6], cudaMemcpyDeviceToHost));
+    if (status) SE2_CUDA(cudaMemcpy(status, dsts, sizes[7], cudaMemcpyDeviceToHost));
+    if (pose) SE2_CUDA(cudaMemcpy(pose, dpose, sizes[8], cudaMemcpyDeviceToHost));
+    if (trace) SE2_CUDA(cudaMemcpy(trace, dtr, sizes[9], cudaMemcpyDeviceToHost));
+    return SE2GPU_OK;
+}
+
+}  // namespace
+
+struct se2gpu_localizer {
+    int device = 0, max_mp = 0;
+    int* best = nullptr;
+    float* xyz = nullptr;
+    float* uv = nullptr;
+    float* w = nullptr;
+    int* edge_ptr = nullptr;
+};
+
+se2gpu_localizer* se2gpu_localizer_create(int max_map_points, int device) {
+    if (max_map_points < 0) { fail(SE2GPU_ERR_INVALID, "max_map_points = %d", max_map_points); return nullptr; }
+    if (select_device(device)) return nullptr;
+    auto* h = new se2gpu_localizer;
+    h->device = device; h->max_mp = max_map_points;
+    const size_t m = (size_t)(max_map_points ? max_map_points : 1);
+    if (dev_alloc(&h->best, m) != cudaSuccess || dev_alloc(&h->xyz, 3 * m) != cudaSuccess || dev_alloc(&h->uv, 2 * m) != cudaSuccess ||
+        dev_alloc(&h->w, m) != cudaSuccess || dev_alloc(&h->edge_ptr, 2) != cudaSuccess) {
+        fail(SE2GPU_ERR_CUDA, "device allocation failed");
+        se2gpu_localizer_destroy(h);
+        return nullptr;
+    }
+    return h;
+}
+
+void se2gpu_localizer_destroy(se2gpu_localizer* h) {
+    if (!h) return;
+    cudaSetDevice(h->device);
+    cudaFree(h->best); cudaFree(h->xyz); cudaFree(h->uv); cudaFree(h->w); cudaFree(h->edge_ptr);
+    delete h;
+}
+
+int se2gpu_pose_ba(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
+                   const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status, double* pose,
+                   int device) {
+    return host_run(B, Tcw, edge_ptr, xyz, uv, info, params, stats, iterations, status, pose, nullptr, device);
+}
+
+int se2gpu_pose_ba_debug_trace(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
+                               const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status,
+                               double* pose, double* trace, int device) {
+    return host_run(B, Tcw, edge_ptr, xyz, uv, info, params, stats, iterations, status, pose, trace, device);
+}
+
+int se2gpu_pose_ba_device(int B, float* d_Tcw, const int* d_edge_ptr, const float* d_xyz, const float* d_uv, const float* d_info,
+                          const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
+                          double* d_pose, void* stream) {
+    Params p;
+    { const int rc = check_params(params, &p); if (rc) return rc; }
+    if (B < 0 || (B && (!d_Tcw || !d_edge_ptr))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { int nd = 0; if (cudaGetDeviceCount(&nd) != cudaSuccess || nd <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available"); }
+    if (B == 0) return SE2GPU_OK;
+    return launch(B, d_Tcw, d_edge_ptr, d_xyz, d_uv, d_info, p, 0, d_stats, d_iterations, d_status, d_pose, nullptr, (cudaStream_t)stream);
+}
+
+int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_kp, int n_kf, const int* d_n_kf,
+                               const int* d_matches_idx_mp, int n_mp, const float* d_mp_xyz, const uint8_t* d_mp_use,
+                               const float* d_inv_sigma2, int nlevels, float* d_Tcw, const se2gpu_pose_ba_params* params,
+                               int min_edges, int* d_n_edges, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
+                               double* d_pose, void* stream) {
+    Params p;
+    { const int rc = check_params(params, &p); if (rc) return rc; }
+    if (!h || n_kf < 0 || n_mp < 0 || nlevels <= 0 || !d_Tcw || !d_inv_sigma2 || (n_kf && (!d_kf_kp || !d_matches_idx_mp)) ||
+        (n_mp && (!d_mp_xyz || !d_mp_use)))
+        return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (n_mp > h->max_mp) return fail(SE2GPU_ERR_CAPACITY, "n_mp = %d exceeds the context's %d map points", n_mp, h->max_mp);
+    SE2_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    SE2_LAUNCH(k_localizer_edges, 1, 1024, 0, s, d_kf_kp, n_kf, d_n_kf, d_matches_idx_mp, n_mp, d_mp_xyz, d_mp_use, d_inv_sigma2,
+               nlevels, h->best, h->xyz, h->uv, h->w, h->edge_ptr, d_n_edges);
+    SE2_CUDA(cudaGetLastError());
+    return launch(1, d_Tcw, h->edge_ptr, h->xyz, h->uv, h->w, p, min_edges, d_stats, d_iterations, d_status, d_pose, nullptr, s);
+}
