@@ -1841,39 +1841,7 @@ __global__ void __launch_bounds__(256) ba_writeback_f32(const double* __restrict
 }  // namespace
 
 // =================================================================================================
-// page-locked bump arena: uploads staged through it are real asynchronous DMA transfers (a cudaMemcpyAsync from a
-// pageable std::vector is staged by the driver and returns only after the host-side copy)
-struct PinnedArena {
-    uint8_t* base = nullptr; size_t cap = 0, used = 0;
-    ~PinnedArena() { if (base) cudaFreeHost(base); }
-    bool reserve(size_t bytes) {
-        used = 0;
-        if (bytes <= cap) return true;
-        if (base) cudaFreeHost(base);
-        base = nullptr; cap = 0;
-        if (cudaMallocHost((void**)&base, bytes + bytes / 4) != cudaSuccess) { cudaGetLastError(); return false; }
-        cap = bytes + bytes / 4;
-        return true;
-    }
-    template <typename T>
-    T* alloc(size_t count) {       // page-locked array built in place (nullptr when the arena is exhausted / unavailable)
-        const size_t bytes = (count * sizeof(T) + 63) & ~(size_t)63;
-        if (!base || used + bytes > cap) return nullptr;
-        T* p = reinterpret_cast<T*>(base + used);
-        used += bytes;
-        return p;
-    }
-    bool owns(const void* p) const { return base && p >= (const void*)base && p < (const void*)(base + cap); }
-    template <typename T>
-    int up(T* dst, const T* src, size_t count, cudaStream_t s) {
-        if (!count) return SE2GPU_OK;
-        const size_t bytes = count * sizeof(T);
-        const void* from = src;
-        if (base && used + bytes <= cap) { memcpy(base + used, src, bytes); from = base + used; used += (bytes + 63) & ~(size_t)63; }
-        SE2_CUDA(cudaMemcpyAsync(dst, from, bytes, cudaMemcpyHostToDevice, s));
-        return SE2GPU_OK;
-    }
-};
+using se2gpu::PinnedArena;
 
 struct se2gpu_ba {
     PinnedArena* arena = nullptr;   // page-locked staging of set_problem's uploads
@@ -1899,8 +1867,7 @@ struct se2gpu_ba {
     void* ar_user = nullptr;
     Dev d{};
     Cam cam{};
-    // owned device buffers
-    std::vector<void*> bufs;
+    se2gpu::DeviceBuffers bufs;   // owned device buffers
     int *e_pose = nullptr, *e_hidx = nullptr, *lm_ptr = nullptr, *hidx = nullptr, *o_i = nullptr, *o_j = nullptr;
     double *e_u = nullptr, *e_v = nullptr, *e_w00 = nullptr, *e_w01 = nullptr, *e_w11 = nullptr, *o_m = nullptr, *o_w = nullptr;
     int *pose_ptr = nullptr, *pose_edges = nullptr, *pose_odo_ptr = nullptr, *pose_odo = nullptr;
@@ -1938,13 +1905,6 @@ struct se2gpu_ba {
 namespace {
 
 template <class T>
-int alloc(se2gpu_ba* h, T** p, size_t count) {
-    if (se2gpu::dev_alloc(p, count) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "cudaMalloc of %zu bytes failed", count * sizeof(T));
-    h->bufs.push_back(*p);
-    return SE2GPU_OK;
-}
-
-template <class T>
 int upload(T* dst, const std::vector<T>& src, cudaStream_t s) {
     if (src.empty()) return SE2GPU_OK;
     SE2_CUDA(cudaMemcpyAsync(dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, s));
@@ -1956,14 +1916,13 @@ int ensure_cap(se2gpu_ba* h, size_t npairs, size_t nblk, size_t nblk_odo) {
     if (npairs > h->cap_pairs) {
         size_t cap = npairs + npairs / 4 + 1024;
         int *a, *b;
-        if (se2gpu::dev_alloc(&a, cap) != cudaSuccess || se2gpu::dev_alloc(&b, cap) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "pair list alloc failed");
-        h->bufs.push_back(a); h->bufs.push_back(b);
+        if (h->bufs.alloc(&a, cap) != cudaSuccess || h->bufs.alloc(&b, cap) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "pair list alloc failed");
         h->pair_e1 = a; h->pair_e2 = b; h->cap_pairs = cap;
     }
     if (nblk + 1 > h->cap_blk) {
         size_t cap = nblk + nblk / 4 + 1024;
         int* p[6];
-        for (int i = 0; i < 6; ++i) { if (se2gpu::dev_alloc(&p[i], cap + 1) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "block list alloc failed"); h->bufs.push_back(p[i]); }
+        for (int i = 0; i < 6; ++i) if (h->bufs.alloc(&p[i], cap + 1) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "block list alloc failed");
         h->blk_a = p[0]; h->blk_b = p[1]; h->blk_pair_ptr = p[2]; h->blk_odo_ptr = p[3]; h->blk_odo = p[4]; h->blk_order = p[5];
         h->cap_blk = cap;
     }
@@ -1985,7 +1944,9 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
     const size_t P = max_poses, L = max_points, E = max_edges, O = max_odo ? max_odo : 1;
     int rc = SE2GPU_OK;
     Dev& d = h->d;
-    auto A = [&](auto** p, size_t c) { if (rc == SE2GPU_OK) rc = alloc(h, p, c); };
+    auto A = [&](auto** p, size_t c) {
+        if (rc == SE2GPU_OK && h->bufs.alloc(p, c) != cudaSuccess) rc = fail(SE2GPU_ERR_CUDA, "cudaMalloc of %zu bytes failed", c * sizeof **p);
+    };
     A(&d.xp[0], 3 * P); A(&d.xp[1], 3 * P); A(&d.xl[0], 3 * L); A(&d.xl[1], 3 * L); A(&d.st, 1);
     A(&h->e_pose, E); A(&h->e_hidx, E); A(&h->lm_ptr, L + 1); A(&h->hidx, P);
     A(&h->e_u, E); A(&h->e_v, E); A(&h->e_w00, E); A(&h->e_w01, E); A(&h->e_w11, E);
@@ -2030,7 +1991,6 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
 void se2gpu_ba_destroy(se2gpu_ba* h) {
     if (!h) return;
     cudaSetDevice(h->device);
-    for (void* p : h->bufs) cudaFree(p);
     if (h->trace_p) cudaFree(h->trace_p);
     if (h->trace_l) cudaFree(h->trace_l);
     if (h->abort_host) cudaFreeHost(h->abort_host);

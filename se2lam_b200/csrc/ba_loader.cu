@@ -82,35 +82,20 @@ int se2gpu_ba_build_information(int P, int L, int E, const float* view_mp, const
         return fail(SE2GPU_ERR_INVALID, "null argument");
     for (int e = 0; e < E; ++e)
         if (edge_pose[e] < 0 || edge_pose[e] >= P || edge_point[e] < 0 || edge_point[e] >= L) return fail(SE2GPU_ERR_INVALID, "edge %d references a missing vertex", e);
-    int rc = se2gpu::select_device(device);
-    if (rc != SE2GPU_OK) return rc;
-    // one device block for all inputs + the output
-    const size_t b_lc = sizeof(float) * 3 * (size_t)E, b_i = sizeof(int) * (size_t)E, b_R = sizeof(float) * 9 * (size_t)P,
-                 b_t = sizeof(float) * 2 * (size_t)P, b_lw = sizeof(float) * 3 * (size_t)L, b_s = sizeof(float) * (size_t)nlevels,
-                 b_out = sizeof(double) * 3 * (size_t)E;
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    const size_t total = al(b_out) + al(b_lc) + 3 * al(b_i) + al(b_R) + al(b_t) + al(b_lw) + al(b_s);
-    uint8_t* dev = nullptr;
-    if (cudaMalloc((void**)&dev, total) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "cudaMalloc of %zu bytes failed", total);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { uint8_t* p = dev + off; off += al(bytes); return p; };
+    se2gpu::HostStage st(device);
+    if (const int rc = st.status()) return rc;
     InfoArgs a{};
     a.E = E; a.nlevels = nlevels; a.fx = fx;
     a.sigma_rotxy = 1.f / xrot_info;       // float Sigma_rotxy = 1./Config::PLANEMOTION_XROT_INFO   (Map.cpp:1043)
     a.sigma_z = 1.f / z_info;              // float Sigma_z = 1./Config::PLANEMOTION_Z_INFO          (Map.cpp:1044)
-    a.info = (double*)take(b_out);
-    cudaError_t err = cudaSuccess;
-    auto up = [&](const void* src, size_t bytes) { void* d = take(bytes); if (err == cudaSuccess) err = cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice); return d; };
-    a.lc = (const float*)up(view_mp, b_lc); a.edge_pose = (const int*)up(edge_pose, b_i); a.edge_point = (const int*)up(edge_point, b_i);
-    a.octave = (const int*)up(octave, b_i); a.Rcw = (const float*)up(kf_Rcw, b_R); a.twb = (const float*)up(kf_twb_xy, b_t);
-    a.lw = (const float*)up(mp_pos, b_lw); a.level_sigma2 = (const float*)up(level_sigma2, b_s);
-    if (err == cudaSuccess) {
-        SE2_LAUNCH(k_edge_information, (E + 255) / 256, 256, 0, 0, a);
-        err = cudaMemcpy(info, a.info, b_out, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(dev);
-    if (err != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "se2gpu_ba_build_information: %s", cudaGetErrorString(err));
-    return SE2GPU_OK;
+    a.info = st.output(info, 3 * (size_t)E);
+    a.lc = st.upload(view_mp, 3 * (size_t)E); a.edge_pose = st.upload(edge_pose, E); a.edge_point = st.upload(edge_point, E);
+    a.octave = st.upload(octave, E); a.Rcw = st.upload(kf_Rcw, 9 * (size_t)P); a.twb = st.upload(kf_twb_xy, 2 * (size_t)P);
+    a.lw = st.upload(mp_pos, 3 * (size_t)L); a.level_sigma2 = st.upload(level_sigma2, nlevels);
+    if (const int rc = st.status()) return rc;
+    SE2_LAUNCH(k_edge_information, (E + 255) / 256, 256, 0, 0, a);
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }
 
 }  // extern "C"

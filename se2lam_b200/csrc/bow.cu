@@ -23,20 +23,13 @@ struct se2gpu_voc {
     int* children = nullptr;      // [child_ptr[n_nodes]]
     int* word_id = nullptr;       // [n_nodes]  (-1 = inner node)
     double* weight = nullptr;     // [n_nodes]
-    // per-call staging (grown on demand)
-    uint8_t* d_in = nullptr; int* d_word = nullptr; int* d_node = nullptr; double* d_w = nullptr; int cap = 0;
+    se2gpu::DeviceBuffers bufs;
 };
 
 namespace {
 
 using se2gpu::fail;
-
-__device__ __forceinline__ int hamming256(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
-    const uint4 a0 = *reinterpret_cast<const uint4*>(a), a1 = *reinterpret_cast<const uint4*>(a + 4);
-    const uint4 b0 = *reinterpret_cast<const uint4*>(b), b1 = *reinterpret_cast<const uint4*>(b + 4);
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
+using se2gpu::hamming256;
 
 // one warp per feature; root = node 0
 __global__ void __launch_bounds__(256) k_voc_transform(const uint32_t* __restrict__ feat, int n, const uint32_t* __restrict__ ndesc,
@@ -127,9 +120,9 @@ se2gpu_voc* se2gpu_voc_create(int n_nodes, const uint8_t* node_desc, const int* 
     if (se2gpu::select_device(device) != SE2GPU_OK) return nullptr;
     se2gpu_voc* v = new se2gpu_voc;
     v->device = device; v->n_nodes = n_nodes; v->levels = levels; v->max_children = max_children;
-    bool ok = cudaMalloc((void**)&v->desc, (size_t)n_nodes * 32) == cudaSuccess && cudaMalloc((void**)&v->child_ptr, sizeof(int) * ((size_t)n_nodes + 1)) == cudaSuccess &&
-              cudaMalloc((void**)&v->children, sizeof(int) * (size_t)std::max(nc, 1)) == cudaSuccess && cudaMalloc((void**)&v->word_id, sizeof(int) * (size_t)n_nodes) == cudaSuccess &&
-              cudaMalloc((void**)&v->weight, sizeof(double) * (size_t)n_nodes) == cudaSuccess;
+    bool ok = v->bufs.alloc(&v->desc, (size_t)n_nodes * 8) == cudaSuccess && v->bufs.alloc(&v->child_ptr, (size_t)n_nodes + 1) == cudaSuccess &&
+              v->bufs.alloc(&v->children, (size_t)nc) == cudaSuccess && v->bufs.alloc(&v->word_id, (size_t)n_nodes) == cudaSuccess &&
+              v->bufs.alloc(&v->weight, (size_t)n_nodes) == cudaSuccess;
     ok = ok && cudaMemcpy(v->desc, node_desc, (size_t)n_nodes * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(v->child_ptr, child_ptr, sizeof(int) * ((size_t)n_nodes + 1), cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(v->children, children, sizeof(int) * (size_t)nc, cudaMemcpyHostToDevice) == cudaSuccess &&
@@ -142,8 +135,6 @@ se2gpu_voc* se2gpu_voc_create(int n_nodes, const uint8_t* node_desc, const int* 
 void se2gpu_voc_destroy(se2gpu_voc* v) {
     if (!v) return;
     cudaSetDevice(v->device);
-    cudaFree(v->desc); cudaFree(v->child_ptr); cudaFree(v->children); cudaFree(v->word_id); cudaFree(v->weight);
-    cudaFree(v->d_in); cudaFree(v->d_word); cudaFree(v->d_node); cudaFree(v->d_w);
     delete v;
 }
 
@@ -156,6 +147,7 @@ int se2gpu_voc_transform_device(se2gpu_voc* v, const uint8_t* d_desc, int n, int
     SE2_CUDA(cudaSetDevice(v->device));
     SE2_LAUNCH(k_voc_transform, (n * 32 + 255) / 256, 256, 0, (cudaStream_t)stream, reinterpret_cast<const uint32_t*>(d_desc), n, v->desc, v->child_ptr,
                v->children, v->word_id, v->weight, v->levels, levelsup, d_word_id, d_weight, d_node_id);
+    SE2_CUDA(cudaGetLastError());
     return SE2GPU_OK;
 }
 
@@ -163,22 +155,14 @@ int se2gpu_voc_transform(se2gpu_voc* v, const uint8_t* desc, int n, int levelsup
     if (!v) return fail(SE2GPU_ERR_INVALID, "null vocabulary");
     if (n < 0 || (n && (!desc || !word_id || !weight))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     if (n == 0) return SE2GPU_OK;
-    SE2_CUDA(cudaSetDevice(v->device));
-    if (n > v->cap) {
-        cudaFree(v->d_in); cudaFree(v->d_word); cudaFree(v->d_node); cudaFree(v->d_w);
-        v->d_in = nullptr; v->d_word = v->d_node = nullptr; v->d_w = nullptr; v->cap = 0;
-        const size_t c = (size_t)n + n / 4 + 256;
-        SE2_CUDA(cudaMalloc((void**)&v->d_in, c * 32)); SE2_CUDA(cudaMalloc((void**)&v->d_word, c * sizeof(int)));
-        SE2_CUDA(cudaMalloc((void**)&v->d_node, c * sizeof(int))); SE2_CUDA(cudaMalloc((void**)&v->d_w, c * sizeof(double)));
-        v->cap = (int)c;
-    }
-    SE2_CUDA(cudaMemcpy(v->d_in, desc, (size_t)n * 32, cudaMemcpyHostToDevice));
-    int rc = se2gpu_voc_transform_device(v, v->d_in, n, levelsup, v->d_word, v->d_w, v->d_node, nullptr);
-    if (rc != SE2GPU_OK) return rc;
-    SE2_CUDA(cudaMemcpy(word_id, v->d_word, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(weight, v->d_w, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
-    if (node_id) SE2_CUDA(cudaMemcpy(node_id, v->d_node, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    se2gpu::HostStage st(v->device);
+    const uint8_t* d_in = st.upload(desc, (size_t)n * 32);
+    int* d_word = st.output(word_id, n);
+    double* d_w = st.output(weight, n);
+    int* d_node = node_id ? st.output(node_id, n) : st.scratch<int>(n);
+    if (const int rc = st.status()) return rc;
+    { const int rc = se2gpu_voc_transform_device(v, d_in, n, levelsup, d_word, d_w, d_node, nullptr); if (rc) return rc; }
+    return st.finish();
 }
 
 int se2gpu_median_descriptor(const uint8_t* desc, const int* ptr, int M, int* best_idx, int* best_median, int device) {
@@ -188,26 +172,18 @@ int se2gpu_median_descriptor(const uint8_t* desc, const int* ptr, int M, int* be
     for (int m = 0; m < M; ++m) { if (ptr[m + 1] < ptr[m]) return fail(SE2GPU_ERR_INVALID, "ptr must be non-decreasing"); maxN = std::max(maxN, ptr[m + 1] - ptr[m]); }
     const size_t smem = (size_t)maxN * maxN * sizeof(unsigned short);
     if (maxN > 320) return fail(SE2GPU_ERR_CAPACITY, "a map point with %d observations exceeds this build's limit of 320", maxN);
-    int rc = se2gpu::select_device(device);
-    if (rc != SE2GPU_OK) return rc;
+    se2gpu::HostStage st(device);
+    if (const int rc = st.status()) return rc;
     const size_t total = (size_t)ptr[M];
-    uint32_t* d_desc = nullptr; int *d_ptr = nullptr, *d_idx = nullptr, *d_med = nullptr;
-    cudaError_t e = cudaSuccess;
-    auto chk = [&](cudaError_t x) { if (e == cudaSuccess) e = x; };
-    chk(cudaMalloc((void**)&d_desc, std::max<size_t>(total, 1) * 32)); chk(cudaMalloc((void**)&d_ptr, sizeof(int) * ((size_t)M + 1)));
-    chk(cudaMalloc((void**)&d_idx, sizeof(int) * (size_t)M)); chk(cudaMalloc((void**)&d_med, sizeof(int) * (size_t)M));
-    if (e == cudaSuccess) {
-        chk(cudaMemcpy(d_desc, desc, total * 32, cudaMemcpyHostToDevice)); chk(cudaMemcpy(d_ptr, ptr, sizeof(int) * ((size_t)M + 1), cudaMemcpyHostToDevice));
-        if (smem > 48 * 1024) chk(cudaFuncSetAttribute(k_median_descriptor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    if (e == cudaSuccess) {
-        SE2_LAUNCH(k_median_descriptor, M, 128, smem, 0, d_desc, d_ptr, M, d_idx, d_med);
-        chk(cudaMemcpy(best_idx, d_idx, sizeof(int) * (size_t)M, cudaMemcpyDeviceToHost));
-        if (best_median) chk(cudaMemcpy(best_median, d_med, sizeof(int) * (size_t)M, cudaMemcpyDeviceToHost));
-    }
-    cudaFree(d_desc); cudaFree(d_ptr); cudaFree(d_idx); cudaFree(d_med);
-    if (e != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "se2gpu_median_descriptor: %s", cudaGetErrorString(e));
-    return SE2GPU_OK;
+    const uint32_t* d_desc = st.upload(reinterpret_cast<const uint32_t*>(desc), total * 8);
+    const int* d_ptr = st.upload(ptr, (size_t)M + 1);
+    int* d_idx = st.output(best_idx, M);
+    int* d_med = best_median ? st.output(best_median, M) : st.scratch<int>(M);
+    if (smem > 48 * 1024) st.check(cudaFuncSetAttribute(k_median_descriptor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute");
+    if (const int rc = st.status()) return rc;
+    SE2_LAUNCH(k_median_descriptor, M, 128, smem, 0, d_desc, d_ptr, M, d_idx, d_med);
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }
 
 }  // extern "C"

@@ -1,12 +1,16 @@
-// Shared host-side helpers of libse2gpu (error reporting, launch accounting).
+// Shared host-side helpers of libse2gpu (error reporting, launch accounting, device selection, memory ownership).
 #pragma once
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
 
 #include <atomic>
 #include <cstdarg>
+#include <cstdint>
 #include <cstdio>
+#include <cstring>
+#include <mutex>
 #include <string>
+#include <vector>
 
 #include "../../include/se2gpu.h"
 
@@ -40,10 +44,26 @@ inline int fail(int code, const char* fmt, ...) {
         ::se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed); \
     } while (0)
 
+// size of the library's per-device tables (host workspaces, default matchers, prepared kernels)
+constexpr int kMaxDevices = 64;
+
+// the number of devices; a machine without one is SE2GPU_ERR_NO_DEVICE
+inline int count_devices(int* n) {
+    *n = 0;
+    const cudaError_t e = cudaGetDeviceCount(n);
+    if (e != cudaSuccess || *n <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available (%s)", cudaGetErrorString(e));
+    return SE2GPU_OK;
+}
+
+// the device check of the handle-less _device entry points (they run on the caller's current device)
+inline int require_device() {
+    int n;
+    return count_devices(&n);
+}
+
 inline int select_device(int device) {
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available (%s)", cudaGetErrorString(e));
+    int n;
+    { const int rc = count_devices(&n); if (rc) return rc; }
     if (device < 0 || device >= n) return fail(SE2GPU_ERR_INVALID, "device %d out of range (%d devices)", device, n);
     SE2_CUDA(cudaSetDevice(device));
     return SE2GPU_OK;
@@ -90,6 +110,121 @@ struct NvtxRange {
 template <class T>
 inline cudaError_t dev_alloc(T** p, size_t count) {
     return cudaMalloc((void**)p, (count ? count : 1) * sizeof(T));
+}
+
+// The device buffers of a handle: everything alloc() hands out is freed when the list is destroyed.
+class DeviceBuffers {
+  public:
+    DeviceBuffers() = default;
+    DeviceBuffers(const DeviceBuffers&) = delete;
+    DeviceBuffers& operator=(const DeviceBuffers&) = delete;
+    ~DeviceBuffers() { for (void* p : bufs_) cudaFree(p); }
+    template <class T>
+    cudaError_t alloc(T** p, size_t count) {
+        const cudaError_t e = dev_alloc(p, count);
+        if (e == cudaSuccess) bufs_.push_back(*p);
+        return e;
+    }
+
+  private:
+    std::vector<void*> bufs_;
+};
+
+// Device memory of one call of a host-buffer entry point. The constructor selects the device and takes that device's
+// grow-only workspace, under its mutex, for the whole call. upload / output / inout / scratch hand out 256-byte aligned
+// pieces of it; a piece that does not fit takes a temporary block, freed with the stage, and the workspace then grows to
+// the call's high-water mark, so a later call of the same size allocates nothing. Copies are synchronous on the legacy
+// default stream. The first CUDA error is kept: status() reports it as SE2GPU_ERR_CUDA (or select_device's failure), and
+// once it is set no further piece, copy or launch check does anything.
+struct Workspace;
+class HostStage {
+  public:
+    explicit HostStage(int device);
+    ~HostStage();
+    HostStage(const HostStage&) = delete;
+    HostStage& operator=(const HostStage&) = delete;
+
+    int status() const;
+    void check(cudaError_t e, const char* what);       // e.g. check(cudaGetLastError(), "kernel launch")
+    template <class T>
+    T* scratch(size_t count) { return static_cast<T*>(take(count * sizeof(T))); }
+    template <class T>
+    T* upload(const T* h, size_t count) {
+        T* d = scratch<T>(count);
+        if (d && count) check(cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice), "cudaMemcpy to the device");
+        return d;
+    }
+    template <class T>
+    T* output(T* h, size_t count) {             // copied back to h by finish()
+        T* d = scratch<T>(count);
+        if (d) outs_.push_back({h, d, count * sizeof(T)});
+        return d;
+    }
+    template <class T>
+    T* inout(T* h, size_t count) {
+        T* d = upload<T>(h, count);
+        if (d) outs_.push_back({h, d, count * sizeof(T)});
+        return d;
+    }
+    int finish();                               // copies the outputs back; status()
+
+  private:
+    struct Out { void* host; const void* dev; size_t bytes; };
+    void* take(size_t bytes);
+    Workspace* ws_ = nullptr;
+    std::unique_lock<std::mutex> lock_;
+    int rc_ = SE2GPU_OK;
+    cudaError_t err_ = cudaSuccess;
+    const char* what_ = "";
+    size_t used_ = 0, high_ = 0;
+    std::vector<void*> temps_;
+    std::vector<Out> outs_;
+};
+
+// page-locked bump arena: uploads staged through it are real asynchronous DMA transfers (a cudaMemcpyAsync from a
+// pageable std::vector is staged by the driver and returns only after the host-side copy)
+struct PinnedArena {
+    uint8_t* base = nullptr; size_t cap = 0, used = 0;
+    ~PinnedArena() { if (base) cudaFreeHost(base); }
+    bool reserve(size_t bytes) {
+        used = 0;
+        if (bytes <= cap) return true;
+        if (base) cudaFreeHost(base);
+        base = nullptr; cap = 0;
+        if (cudaMallocHost((void**)&base, bytes + bytes / 4) != cudaSuccess) { cudaGetLastError(); return false; }
+        cap = bytes + bytes / 4;
+        return true;
+    }
+    template <typename T>
+    T* alloc(size_t count) {       // page-locked array built in place (nullptr when the arena is exhausted / unavailable)
+        const size_t bytes = (count * sizeof(T) + 63) & ~(size_t)63;
+        if (!base || used + bytes > cap) return nullptr;
+        T* p = reinterpret_cast<T*>(base + used);
+        used += bytes;
+        return p;
+    }
+    bool owns(const void* p) const { return base && p >= (const void*)base && p < (const void*)(base + cap); }
+    template <typename T>
+    int up(T* dst, const T* src, size_t count, cudaStream_t s) {
+        if (!count) return SE2GPU_OK;
+        const size_t bytes = count * sizeof(T);
+        const void* from = src;
+        if (base && used + bytes <= cap) { memcpy(base + used, src, bytes); from = base + used; used += (bytes + 63) & ~(size_t)63; }
+        SE2_CUDA(cudaMemcpyAsync(dst, from, bytes, cudaMemcpyHostToDevice, s));
+        return SE2GPU_OK;
+    }
+};
+
+// ---------------------------------------------------------------------------------------------- shared device helpers
+// number of valid entries: *d_n clamped to [0, cap], or cap when there is no device-side count
+__device__ __forceinline__ int count_of(const int* d_n, int cap) { return d_n ? min(max(*d_n, 0), cap) : cap; }
+
+// Hamming distance of two 256-bit ORB descriptors (8 x 32 bit, 16-byte aligned)
+__device__ __forceinline__ int hamming256(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
+    const uint4 a0 = *reinterpret_cast<const uint4*>(a), a1 = *reinterpret_cast<const uint4*>(a + 4);
+    const uint4 b0 = *reinterpret_cast<const uint4*>(b), b1 = *reinterpret_cast<const uint4*>(b + 4);
+    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
+           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
 }
 
 }  // namespace se2gpu

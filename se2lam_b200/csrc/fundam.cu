@@ -521,35 +521,16 @@ const double* niters_table() {
 // per device: the table uploaded and the kernel's shared-memory limit raised
 int prepare_device() {
     static std::mutex mu;
-    static bool ready[64] = {};
+    static bool ready[kMaxDevices] = {};
     int dev = 0;
     SE2_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lk(mu);
-    if (dev < 64 && ready[dev]) return SE2GPU_OK;
+    if (dev < kMaxDevices && ready[dev]) return SE2GPU_OK;
     SE2_CUDA(cudaMemcpyToSymbol(c_niters, niters_table(), sizeof(double) * kNitersTable));
     SE2_CUDA(cudaFuncSetAttribute(k_remove_outliers, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * kMaxPairs));
-    if (dev < 64) ready[dev] = true;
+    if (dev < kMaxDevices) ready[dev] = true;
     return SE2GPU_OK;
 }
-
-struct DevBufs {
-    void* p[16];
-    int n = 0;
-    ~DevBufs() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
-    template <class T>
-    T* get(size_t count) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, count ? count * sizeof(T) : 1) != cudaSuccess) return nullptr;
-        p[n++] = q;
-        return static_cast<T*>(q);
-    }
-    template <class T>
-    T* upload(const T* h, size_t count) {
-        T* d = get<T>(count);
-        if (d && count && cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-        return d;
-    }
-};
 
 }  // namespace
 
@@ -560,7 +541,7 @@ int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const
     if (cap1 > kMaxPairs) return fail(SE2GPU_ERR_CAPACITY, "cap1 = %d exceeds %d keypoints", cap1, kMaxPairs);
     if (batch && (!d_ninliers || (cap1 && (!d_kp1 || !d_matches12)) || (cap2 && !d_kp2)))
         return fail(SE2GPU_ERR_INVALID, "null argument");
-    { int nd = 0; if (cudaGetDeviceCount(&nd) != cudaSuccess || nd <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available"); }
+    { const int rc = require_device(); if (rc) return rc; }
     if (batch == 0) return SE2GPU_OK;
     { const int rc = prepare_device(); if (rc) return rc; }
     static const int lmeds_niters = [] { const int v = update_num_iters_host(0.99, 0.45, kModelPoints, 1000); return v < 3 ? 3 : v; }();
@@ -570,9 +551,6 @@ int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const
     SE2_CUDA(cudaGetLastError());
     return SE2GPU_OK;
 }
-
-#define FUNDAM_ALLOC(ptr) \
-    if (!(ptr)) return fail(SE2GPU_ERR_CUDA, "device allocation or copy failed")
 
 int se2gpu_remove_outliers(int batch, const se2gpu_keypoint* kp1, const int* n1, int cap1, const se2gpu_keypoint* kp2, const int* n2,
                            int cap2, int* matches12, int* ninliers, double* F, int* iters, int device) {
@@ -586,23 +564,20 @@ int se2gpu_remove_outliers(int batch, const se2gpu_keypoint* kp1, const int* n1,
             if (matches12[(size_t)b * cap1 + i] >= c2)
                 return fail(SE2GPU_ERR_INVALID, "pair %d: matches12[%d] = %d is not a frame-2 keypoint", b, i, matches12[(size_t)b * cap1 + i]);
     }
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (batch == 0) return SE2GPU_OK;
-    DevBufs d;
-    const se2gpu_keypoint* dk1 = d.upload(kp1, (size_t)batch * cap1); FUNDAM_ALLOC(dk1);
-    const se2gpu_keypoint* dk2 = d.upload(kp2, (size_t)batch * cap2); FUNDAM_ALLOC(dk2);
-    const int* dn1 = n1 ? d.upload(n1, batch) : nullptr; if (n1) FUNDAM_ALLOC(dn1);
-    const int* dn2 = n2 ? d.upload(n2, batch) : nullptr; if (n2) FUNDAM_ALLOC(dn2);
-    int* dm = d.upload(matches12, (size_t)batch * cap1); FUNDAM_ALLOC(dm);
-    int* dnin = d.get<int>(batch); FUNDAM_ALLOC(dnin);
-    double* dF = F ? d.get<double>(9 * (size_t)batch) : nullptr; if (F) FUNDAM_ALLOC(dF);
-    int* dit = iters ? d.get<int>(batch) : nullptr; if (iters) FUNDAM_ALLOC(dit);
+    const se2gpu_keypoint* dk1 = st.upload(kp1, (size_t)batch * cap1);
+    const se2gpu_keypoint* dk2 = st.upload(kp2, (size_t)batch * cap2);
+    const int* dn1 = n1 ? st.upload(n1, batch) : nullptr;
+    const int* dn2 = n2 ? st.upload(n2, batch) : nullptr;
+    int* dm = st.inout(matches12, (size_t)batch * cap1);
+    int* dnin = st.output(ninliers, batch);
+    double* dF = F ? st.output(F, 9 * (size_t)batch) : nullptr;
+    int* dit = iters ? st.output(iters, batch) : nullptr;
+    if (const int rc = st.status()) return rc;
     { const int rc = se2gpu_remove_outliers_device(batch, dk1, dn1, cap1, dk2, dn2, cap2, dm, dnin, dF, dit, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(matches12, dm, sizeof(int) * (size_t)batch * cap1, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(ninliers, dnin, sizeof(int) * batch, cudaMemcpyDeviceToHost));
-    if (F) SE2_CUDA(cudaMemcpy(F, dF, sizeof(double) * 9 * batch, cudaMemcpyDeviceToHost));
-    if (iters) SE2_CUDA(cudaMemcpy(iters, dit, sizeof(int) * batch, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 void se2gpu_fundam_niters_table(double* thresholds) { std::memcpy(thresholds, niters_table(), sizeof(double) * kNitersTable); }
@@ -612,16 +587,16 @@ int se2gpu_fundam_debug_niters(int count, const int* n, const int* good, const i
     for (int i = 0; i < count; i++)
         if (n[i] <= 0 || good[i] < 0 || good[i] > n[i] || max_iters[i] < 0 || max_iters[i] > kNitersTable)
             return fail(SE2GPU_ERR_INVALID, "entry %d out of range", i);
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (count == 0) return SE2GPU_OK;
     { const int rc = prepare_device(); if (rc) return rc; }
-    DevBufs d;
-    const int* dn = d.upload(n, count); FUNDAM_ALLOC(dn);
-    const int* dg = d.upload(good, count); FUNDAM_ALLOC(dg);
-    const int* dm = d.upload(max_iters, count); FUNDAM_ALLOC(dm);
-    int* dout = d.get<int>(count); FUNDAM_ALLOC(dout);
+    const int* dn = st.upload(n, count);
+    const int* dg = st.upload(good, count);
+    const int* dm = st.upload(max_iters, count);
+    int* dout = st.output(out, count);
+    if (const int rc = st.status()) return rc;
     SE2_LAUNCH(k_debug_niters, (count + 255) / 256, 256, 0, nullptr, count, dn, dg, dm, dout);
-    SE2_CUDA(cudaGetLastError());
-    SE2_CUDA(cudaMemcpy(out, dout, sizeof(int) * count, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }

@@ -302,8 +302,6 @@ __device__ __forceinline__ void xyz_info(F3 xyz1, const float* Tcw1, const float
     }
 }
 
-__device__ __forceinline__ int count_of(const int* d_n, int cap) { return d_n ? min(max(*d_n, 0), cap) : cap; }
-
 // warp-aggregated counter: one atomic per warp
 __device__ __forceinline__ void warp_count(int* counter, bool pred) {
     const unsigned b = __ballot_sync(0xffffffffu, pred);
@@ -454,39 +452,13 @@ inline int blocks(int n) { return (n + kBlock - 1) / kBlock; }
 
 const float kMinCos[4] = {0.9998f, 0.9994f, 0.9986f, 0.9976f};   // cvu::checkParallax
 
-int need_device() {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available");
-    return SE2GPU_OK;
-}
-
-// scoped device buffers of the host-buffer entry points
-struct DevBufs {
-    void* p[16];
-    int n = 0;
-    ~DevBufs() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
-    template <class T>
-    T* get(size_t count) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, count ? count * sizeof(T) : 1) != cudaSuccess) return nullptr;
-        p[n++] = q;
-        return static_cast<T*>(q);
-    }
-    template <class T>
-    T* upload(const T* h, size_t count) {
-        T* d = get<T>(count);
-        if (d && count && cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-        return d;
-    }
-};
-
 }  // namespace
 
 // ------------------------------------------------------------------------------------------ device-buffer entries
 int se2gpu_triangulate_device(int n, const float* d_pt1, const float* d_pt2, const float* d_P, const int* d_idx1,
                               const int* d_idx2, float* d_xyz, void* stream) {
     if (n < 0 || (n && (!d_pt1 || !d_pt2 || !d_P || !d_idx1 || !d_idx2 || !d_xyz))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    { const int rc = need_device(); if (rc) return rc; }
+    { const int rc = require_device(); if (rc) return rc; }
     if (n == 0) return SE2GPU_OK;
     SE2_LAUNCH(k_triangulate, blocks(n), kBlock, 0, (cudaStream_t)stream, n, d_pt1, d_pt2, d_P, d_idx1, d_idx2, d_xyz);
     SE2_CUDA(cudaGetLastError());
@@ -500,7 +472,7 @@ int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, co
     if (n_kf < 0 || !d_counts || min_parallax_deg < 1 || min_parallax_deg > 4 || !d_Tcr || !d_K) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     if (n_kf && (!d_kp_kf || !d_kp_frame || !d_matches12 || !d_kf_observed || !d_kf_view_mp || !d_local_mps || !d_good_prl))
         return fail(SE2GPU_ERR_INVALID, "null argument");
-    { const int rc = need_device(); if (rc) return rc; }
+    { const int rc = require_device(); if (rc) return rc; }
     cudaStream_t s = (cudaStream_t)stream;
     SE2_CUDA(cudaMemsetAsync(d_counts, 0, 2 * sizeof(int), s));
     if (n_kf == 0) return SE2GPU_OK;
@@ -513,7 +485,7 @@ int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, co
 int se2gpu_xyz_info_device(int n, const float* d_xyz1, const int* d_pose1, const int* d_pose2, const float* d_Tcw, float fx,
                            double* d_info1, double* d_info2, void* stream) {
     if (n < 0 || (n && (!d_xyz1 || !d_pose1 || !d_pose2 || !d_Tcw || !d_info1 || !d_info2))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    { const int rc = need_device(); if (rc) return rc; }
+    { const int rc = require_device(); if (rc) return rc; }
     if (n == 0) return SE2GPU_OK;
     SE2_LAUNCH(k_xyz_info, blocks(n), kBlock, 0, (cudaStream_t)stream, n, d_xyz1, d_pose1, d_pose2, d_Tcw, fx, d_info1, d_info2);
     SE2_CUDA(cudaGetLastError());
@@ -530,7 +502,7 @@ int se2gpu_projection_observations_device(const se2gpu_keypoint* d_kf_kp, int n_
     if (n_kf && (!d_kf_kp || !d_matches_idx_mp || !d_Tcw_new || !d_mp_main_measure || !d_mp_main_pose || !d_mp_main_octave ||
                  !d_mp_normal || !d_mp_min_dist || !d_mp_max_dist || !d_Tcw_table || !d_K || !d_accept || !d_pos_new_kf || !d_info_new))
         return fail(SE2GPU_ERR_INVALID, "null argument");
-    { const int rc = need_device(); if (rc) return rc; }
+    { const int rc = require_device(); if (rc) return rc; }
     if (n_kf == 0) return SE2GPU_OK;
     const MpTable mp{d_mp_main_measure, d_mp_main_pose, d_mp_main_octave, d_mp_normal, d_mp_min_dist, d_mp_max_dist};
     SE2_LAUNCH(k_projection_observations, blocks(n_kf), kBlock, 0, (cudaStream_t)stream, d_kf_kp, n_kf, d_n_kf, d_matches_idx_mp,
@@ -548,25 +520,22 @@ bool indices_ok(const int* idx, int n, int hi) {
 }
 }  // namespace
 
-#define GEOM_ALLOC(ptr) \
-    if (!(ptr)) return fail(SE2GPU_ERR_CUDA, "device allocation or copy failed")
-
 int se2gpu_triangulate(int n, const float* pt1, const float* pt2, const float* P, int n_proj, const int* idx1, const int* idx2,
                        float* xyz, int device) {
     if (n < 0 || n_proj < 0 || (n && (!pt1 || !pt2 || !P || !idx1 || !idx2 || !xyz))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     if (!indices_ok(idx1, n, n_proj) || !indices_ok(idx2, n, n_proj)) return fail(SE2GPU_ERR_INVALID, "projection index out of range");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (n == 0) return SE2GPU_OK;
-    DevBufs b;
-    const float* d1 = b.upload(pt1, 2 * (size_t)n); GEOM_ALLOC(d1);
-    const float* d2 = b.upload(pt2, 2 * (size_t)n); GEOM_ALLOC(d2);
-    const float* dP = b.upload(P, 12 * (size_t)n_proj); GEOM_ALLOC(dP);
-    const int* i1 = b.upload(idx1, n); GEOM_ALLOC(i1);
-    const int* i2 = b.upload(idx2, n); GEOM_ALLOC(i2);
-    float* dx = b.get<float>(3 * (size_t)n); GEOM_ALLOC(dx);
+    const float* d1 = st.upload(pt1, 2 * (size_t)n);
+    const float* d2 = st.upload(pt2, 2 * (size_t)n);
+    const float* dP = st.upload(P, 12 * (size_t)n_proj);
+    const int* i1 = st.upload(idx1, n);
+    const int* i2 = st.upload(idx2, n);
+    float* dx = st.output(xyz, 3 * (size_t)n);
+    if (const int rc = st.status()) return rc;
     { const int rc = se2gpu_triangulate_device(n, d1, d2, dP, i1, i2, dx, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(xyz, dx, 3 * sizeof(float) * n, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 int se2gpu_track_triangulate(const se2gpu_keypoint* kp_kf, int n_kf, const se2gpu_keypoint* kp_frame, int n_frame, int* matches12,
@@ -579,46 +548,42 @@ int se2gpu_track_triangulate(const se2gpu_keypoint* kp_kf, int n_kf, const se2gp
     for (int i = 0; i < n_kf; i++)
         if (matches12[i] >= n_frame) return fail(SE2GPU_ERR_INVALID, "matches12[%d] = %d is not a frame keypoint", i, matches12[i]);
     if (n_frame && !kp_frame) return fail(SE2GPU_ERR_INVALID, "null argument");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     counts[0] = counts[1] = 0;
     if (n_kf == 0) return SE2GPU_OK;
-    DevBufs b;
-    const se2gpu_keypoint* dk = b.upload(kp_kf, n_kf); GEOM_ALLOC(dk);
-    const se2gpu_keypoint* df = b.upload(kp_frame, n_frame); GEOM_ALLOC(df);
-    int* dm12 = b.upload(matches12, n_kf); GEOM_ALLOC(dm12);
-    const uint8_t* dobs = b.upload(kf_observed, n_kf); GEOM_ALLOC(dobs);
-    const float* dvm = b.upload(kf_view_mp, 3 * (size_t)n_kf); GEOM_ALLOC(dvm);
-    const float* dT = b.upload(Tcr, 16); GEOM_ALLOC(dT);
-    const float* dK = b.upload(K, 9); GEOM_ALLOC(dK);
-    float* dl = b.upload(local_mps, 3 * (size_t)n_kf); GEOM_ALLOC(dl);
-    uint8_t* dg = b.get<uint8_t>(n_kf); GEOM_ALLOC(dg);
-    int* dc = b.get<int>(2); GEOM_ALLOC(dc);
+    const se2gpu_keypoint* dk = st.upload(kp_kf, n_kf);
+    const se2gpu_keypoint* df = st.upload(kp_frame, n_frame);
+    int* dm12 = st.inout(matches12, n_kf);
+    const uint8_t* dobs = st.upload(kf_observed, n_kf);
+    const float* dvm = st.upload(kf_view_mp, 3 * (size_t)n_kf);
+    const float* dT = st.upload(Tcr, 16);
+    const float* dK = st.upload(K, 9);
+    float* dl = st.inout(local_mps, 3 * (size_t)n_kf);
+    uint8_t* dg = st.output(good_prl, n_kf);
+    int* dc = st.output(counts, 2);
+    if (const int rc = st.status()) return rc;
     { const int rc = se2gpu_track_triangulate_device(dk, n_kf, nullptr, df, dm12, dobs, dvm, dT, dK, lower_depth, upper_depth,
                                                      min_parallax_deg, dl, dg, dc, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(matches12, dm12, sizeof(int) * n_kf, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(local_mps, dl, 3 * sizeof(float) * n_kf, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(good_prl, dg, n_kf, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(counts, dc, 2 * sizeof(int), cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 int se2gpu_xyz_info(int n, const float* xyz1, const int* pose1, const int* pose2, const float* Tcw, int n_pose, float fx,
                     double* info1, double* info2, int device) {
     if (n < 0 || n_pose < 0 || (n && (!xyz1 || !pose1 || !pose2 || !Tcw || !info1 || !info2))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     if (!indices_ok(pose1, n, n_pose) || !indices_ok(pose2, n, n_pose)) return fail(SE2GPU_ERR_INVALID, "pose index out of range");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (n == 0) return SE2GPU_OK;
-    DevBufs b;
-    const float* dx = b.upload(xyz1, 3 * (size_t)n); GEOM_ALLOC(dx);
-    const int* p1 = b.upload(pose1, n); GEOM_ALLOC(p1);
-    const int* p2 = b.upload(pose2, n); GEOM_ALLOC(p2);
-    const float* dT = b.upload(Tcw, 16 * (size_t)n_pose); GEOM_ALLOC(dT);
-    double* i1 = b.get<double>(9 * (size_t)n); GEOM_ALLOC(i1);
-    double* i2 = b.get<double>(9 * (size_t)n); GEOM_ALLOC(i2);
+    const float* dx = st.upload(xyz1, 3 * (size_t)n);
+    const int* p1 = st.upload(pose1, n);
+    const int* p2 = st.upload(pose2, n);
+    const float* dT = st.upload(Tcw, 16 * (size_t)n_pose);
+    double* i1 = st.output(info1, 9 * (size_t)n);
+    double* i2 = st.output(info2, 9 * (size_t)n);
+    if (const int rc = st.status()) return rc;
     { const int rc = se2gpu_xyz_info_device(n, dx, p1, p2, dT, fx, i1, i2, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(info1, i1, 9 * sizeof(double) * n, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(info2, i2, 9 * sizeof(double) * n, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 int se2gpu_projection_observations(const se2gpu_keypoint* kf_kp, int n_kf, const int* matches_idx_mp, const float* Tcw_new,
@@ -633,44 +598,41 @@ int se2gpu_projection_observations(const se2gpu_keypoint* kf_kp, int n_kf, const
     for (int i = 0; i < n_kf; i++)
         if (matches_idx_mp[i] >= n_mp) return fail(SE2GPU_ERR_INVALID, "matches_idx_mp[%d] = %d is not a map point", i, matches_idx_mp[i]);
     if (!indices_ok(mp_main_pose, n_mp, n_pose)) return fail(SE2GPU_ERR_INVALID, "main keyframe index out of range");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (n_kf == 0) return SE2GPU_OK;
-    DevBufs b;
     const size_t m = n_mp ? n_mp : 1;
     const float zero16[16] = {0};
-    const se2gpu_keypoint* dk = b.upload(kf_kp, n_kf); GEOM_ALLOC(dk);
-    const int* dmi = b.upload(matches_idx_mp, n_kf); GEOM_ALLOC(dmi);
-    const float* dTn = b.upload(Tcw_new, 16); GEOM_ALLOC(dTn);
-    const float* dmm = n_mp ? b.upload(mp_main_measure, 2 * m) : b.upload(zero16, 2); GEOM_ALLOC(dmm);
-    const int* dmp = n_mp ? b.upload(mp_main_pose, m) : b.get<int>(1); GEOM_ALLOC(dmp);
-    const int* dmo = n_mp ? b.upload(mp_main_octave, m) : b.get<int>(1); GEOM_ALLOC(dmo);
-    const float* dnv = n_mp ? b.upload(mp_normal, 3 * m) : b.upload(zero16, 3); GEOM_ALLOC(dnv);
-    const float* dmin = n_mp ? b.upload(mp_min_dist, m) : b.upload(zero16, 1); GEOM_ALLOC(dmin);
-    const float* dmax = n_mp ? b.upload(mp_max_dist, m) : b.upload(zero16, 1); GEOM_ALLOC(dmax);
-    const float* dtab = n_pose ? b.upload(Tcw_table, 16 * (size_t)n_pose) : b.upload(zero16, 16); GEOM_ALLOC(dtab);
-    const float* dK = b.upload(K, 9); GEOM_ALLOC(dK);
-    uint8_t* dacc = b.get<uint8_t>(n_kf); GEOM_ALLOC(dacc);
-    float* dpos = b.upload(pos_new_kf, 3 * (size_t)n_kf); GEOM_ALLOC(dpos);
-    double* dinfo = b.upload(info_new, 9 * (size_t)n_kf); GEOM_ALLOC(dinfo);
+    const se2gpu_keypoint* dk = st.upload(kf_kp, n_kf);
+    const int* dmi = st.upload(matches_idx_mp, n_kf);
+    const float* dTn = st.upload(Tcw_new, 16);
+    const float* dmm = n_mp ? st.upload(mp_main_measure, 2 * m) : st.upload(zero16, 2);
+    const int* dmp = n_mp ? st.upload(mp_main_pose, m) : st.scratch<int>(1);
+    const int* dmo = n_mp ? st.upload(mp_main_octave, m) : st.scratch<int>(1);
+    const float* dnv = n_mp ? st.upload(mp_normal, 3 * m) : st.upload(zero16, 3);
+    const float* dmin = n_mp ? st.upload(mp_min_dist, m) : st.upload(zero16, 1);
+    const float* dmax = n_mp ? st.upload(mp_max_dist, m) : st.upload(zero16, 1);
+    const float* dtab = n_pose ? st.upload(Tcw_table, 16 * (size_t)n_pose) : st.upload(zero16, 16);
+    const float* dK = st.upload(K, 9);
+    uint8_t* dacc = st.output(accept, n_kf);
+    float* dpos = st.inout(pos_new_kf, 3 * (size_t)n_kf);
+    double* dinfo = st.inout(info_new, 9 * (size_t)n_kf);
+    if (const int rc = st.status()) return rc;
     { const int rc = se2gpu_projection_observations_device(dk, n_kf, nullptr, dmi, dTn, dmm, dmp, dmo, dnv, dmin, dmax, dtab, dK,
                                                            lower_depth, upper_depth, fx, dacc, dpos, dinfo, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(accept, dacc, n_kf, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(pos_new_kf, dpos, 3 * sizeof(float) * n_kf, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(info_new, dinfo, 9 * sizeof(double) * n_kf, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 int se2gpu_debug_svd4(int n, const float* A, float* w, float* vt, int device) {
     if (n < 0 || (n && (!A || !w || !vt))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (n == 0) return SE2GPU_OK;
-    DevBufs b;
-    const float* dA = b.upload(A, 16 * (size_t)n); GEOM_ALLOC(dA);
-    float* dw = b.get<float>(4 * (size_t)n); GEOM_ALLOC(dw);
-    float* dv = b.get<float>(16 * (size_t)n); GEOM_ALLOC(dv);
+    const float* dA = st.upload(A, 16 * (size_t)n);
+    float* dw = st.output(w, 4 * (size_t)n);
+    float* dv = st.output(vt, 16 * (size_t)n);
+    if (const int rc = st.status()) return rc;
     SE2_LAUNCH(k_debug_svd4, blocks(n), kBlock, 0, (cudaStream_t)0, n, dA, dw, dv);
-    SE2_CUDA(cudaGetLastError());
-    SE2_CUDA(cudaMemcpy(w, dw, 4 * sizeof(float) * n, cudaMemcpyDeviceToHost));
-    SE2_CUDA(cudaMemcpy(vt, dv, 16 * sizeof(float) * n, cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }

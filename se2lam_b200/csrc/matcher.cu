@@ -43,33 +43,26 @@ struct se2gpu_matcher {
     uint8_t *d_desc1 = nullptr, *d_desc2 = nullptr, *d_u8a = nullptr, *d_u8b = nullptr;
     float *d_f1 = nullptr, *d_f2 = nullptr;
     int *d_i1 = nullptr, *d_i2 = nullptr, *d_i3 = nullptr, *d_i4 = nullptr, *d_out = nullptr;
-    uint8_t* pin = nullptr; size_t pin_bytes = 0;
-    std::vector<void*> bufs;
+    se2gpu::PinnedArena pin; size_t pin_bytes = 0;
+    se2gpu::DeviceBuffers bufs;
     se2gpu::Profiler prof;
     int resolve_smem_max = 0;
 };
 
 namespace {
 
+using se2gpu::count_of;
 using se2gpu::fail;
+using se2gpu::hamming256;
 
 constexpr int TH_HIGH = 100, TH_LOW = 75, HISTO_LENGTH = 30;   // ORBmatcher.cpp:45-47
 constexpr int GRID_ROWS = 48, GRID_COLS = 64;                  // Frame.h:26-27
 constexpr int MODE_WINDOW = 0, MODE_PROJ = 1, MODE_BOW = 2;
 
-__device__ __forceinline__ int hamming256(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
-    const uint4 a0 = *reinterpret_cast<const uint4*>(a), a1 = *reinterpret_cast<const uint4*>(a + 4);
-    const uint4 b0 = *reinterpret_cast<const uint4*>(b), b1 = *reinterpret_cast<const uint4*>(b + 4);
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
-
 __global__ void k_hamming_pairs(const uint32_t* a, const uint32_t* b, int n, int* out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = hamming256(a + 8 * (size_t)i, b + 8 * (size_t)i);
 }
-
-__device__ __forceinline__ int count_of(const int* d_n, int cap) { return d_n ? min(max(*d_n, 0), cap) : cap; }
 
 // Frame::PosInGrid (Frame.cpp:209-220) for every database keypoint and the grid-walk order (cell column, cell row,
 // insertion index) of the valid ones by rank counting. Every CTA computes ALL sort keys (cell << 13 | index, INT_MAX for
@@ -543,13 +536,6 @@ __global__ void k_kp_to_xy(const se2gpu_keypoint* __restrict__ kp, int n_cap, co
     if (i < count_of(d_n, n_cap)) { xy[2 * i] = kp[i].x; xy[2 * i + 1] = kp[i].y; }
 }
 
-template <class T>
-bool dalloc(se2gpu_matcher* m, T** p, size_t count) {
-    if (se2gpu::dev_alloc(p, count) != cudaSuccess) return false;
-    m->bufs.push_back(*p);
-    return true;
-}
-
 int launch_grid(se2gpu_matcher* m, const se2gpu_keypoint* d_kp, int n, const int* d_n, se2gpu_grid_params grid, cudaStream_t s) {
     m->prof.begin(0, s);
     if (n <= GRID_SMEM_KEYS) {
@@ -594,7 +580,7 @@ int launch_resolve(se2gpu_matcher* m, ResolveArgs ra, const se2gpu_keypoint* kp1
 }
 
 std::mutex g_default_mutex;
-se2gpu_matcher* g_default[64] = {};
+se2gpu_matcher* g_default[se2gpu::kMaxDevices] = {};
 
 }  // namespace
 
@@ -608,14 +594,15 @@ se2gpu_matcher* se2gpu_matcher_create(int max_queries, int max_db, int device) {
     m->device = device; m->max_q = max_queries; m->max_db = max_db;
     const size_t Q = max_queries, D = max_db, N = std::max(Q, D);
     bool ok = true;
-    ok = ok && dalloc(m, &m->cell, D) && dalloc(m, &m->order, D) && dalloc(m, &m->nvalid, 1);
-    ok = ok && dalloc(m, &m->cand, Q * D) && dalloc(m, &m->ncand, Q) && dalloc(m, &m->work, 2 * D + Q) && dalloc(m, &m->flags, 2) && dalloc(m, &m->nm, 1);
-    ok = ok && dalloc(m, &m->d_kp1, N) && dalloc(m, &m->d_kp2, N) && dalloc(m, &m->d_desc1, N * 32) && dalloc(m, &m->d_desc2, N * 32);
-    ok = ok && dalloc(m, &m->d_u8a, N) && dalloc(m, &m->d_u8b, N) && dalloc(m, &m->d_f1, 2 * N) && dalloc(m, &m->d_f2, 2 * N);
-    ok = ok && dalloc(m, &m->d_i1, N + 1) && dalloc(m, &m->d_i2, N + 1) && dalloc(m, &m->d_i3, N + 1) && dalloc(m, &m->d_i4, N + 1) && dalloc(m, &m->d_out, N);
+    auto A = [&](auto** p, size_t count) { ok = ok && m->bufs.alloc(p, count) == cudaSuccess; };
+    A(&m->cell, D); A(&m->order, D); A(&m->nvalid, 1);
+    A(&m->cand, Q * D); A(&m->ncand, Q); A(&m->work, 2 * D + Q); A(&m->flags, 2); A(&m->nm, 1);
+    A(&m->d_kp1, N); A(&m->d_kp2, N); A(&m->d_desc1, N * 32); A(&m->d_desc2, N * 32);
+    A(&m->d_u8a, N); A(&m->d_u8b, N); A(&m->d_f1, 2 * N); A(&m->d_f2, 2 * N);
+    A(&m->d_i1, N + 1); A(&m->d_i2, N + 1); A(&m->d_i3, N + 1); A(&m->d_i4, N + 1); A(&m->d_out, N);
     // pinned staging: both keypoint sets + descriptors + per-item side arrays + outputs
     m->pin_bytes = N * (2 * (sizeof(se2gpu_keypoint) + 32) + 2 + 16 + 5 * sizeof(int) + 8) + 4096;
-    ok = ok && cudaMallocHost((void**)&m->pin, m->pin_bytes) == cudaSuccess;
+    ok = ok && m->pin.reserve(m->pin_bytes);
     ok = ok && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) == cudaSuccess;
     if (ok) {
         int optin = 0;
@@ -632,8 +619,6 @@ se2gpu_matcher* se2gpu_matcher_create(int max_queries, int max_db, int device) {
 void se2gpu_matcher_destroy(se2gpu_matcher* m) {
     if (!m) return;
     cudaSetDevice(m->device);
-    for (void* p : m->bufs) cudaFree(p);
-    if (m->pin) cudaFreeHost(m->pin);
     if (m->stream) cudaStreamDestroy(m->stream);
     delete m;
 }
@@ -665,8 +650,10 @@ int se2gpu_matcher_last_rounds(se2gpu_matcher* m, int* rounds, int* used_fallbac
 
 int se2gpu_keypoints_to_points_device(const se2gpu_keypoint* d_kp, int n, const int* d_n, float* d_xy, void* stream) {
     if (n < 0 || (n && (!d_kp || !d_xy))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = se2gpu::require_device(); if (rc) return rc; }
     if (n == 0) return SE2GPU_OK;
     SE2_LAUNCH(k_kp_to_xy, (n + 255) / 256, 256, 0, (cudaStream_t)stream, d_kp, n, d_n, d_xy);
+    SE2_CUDA(cudaGetLastError());
     return SE2GPU_OK;
 }
 
@@ -741,25 +728,8 @@ int se2gpu_match_by_projection_device(se2gpu_matcher* m, const se2gpu_keypoint* 
 
 namespace {
 
-// bump allocator over the handle's pinned staging block
-struct Stage {
-    se2gpu_matcher* m; size_t used = 0;
-    template <class T> T* get(size_t n) {
-        const size_t bytes = (n * sizeof(T) + 63) & ~(size_t)63;
-        if (used + bytes > m->pin_bytes) return nullptr;
-        T* p = reinterpret_cast<T*>(m->pin + used); used += bytes; return p;
-    }
-    template <class T> bool up(T* dst, const T* src, size_t n, cudaStream_t s) {
-        if (!n) return true;
-        T* p = get<T>(n);
-        if (!p) return false;
-        memcpy(p, src, n * sizeof(T));
-        return cudaMemcpyAsync(dst, p, n * sizeof(T), cudaMemcpyHostToDevice, s) == cudaSuccess;
-    }
-};
-
 se2gpu_matcher* default_matcher(int device, int nq, int ndb) {
-    if (device < 0 || device >= 64) { fail(SE2GPU_ERR_INVALID, "device %d out of range", device); return nullptr; }
+    if (device < 0 || device >= se2gpu::kMaxDevices) { fail(SE2GPU_ERR_INVALID, "device %d out of range", device); return nullptr; }
     se2gpu_matcher*& m = g_default[device];
     if (m && (m->max_q < nq || m->max_db < ndb)) { se2gpu_matcher_destroy(m); m = nullptr; }
     if (!m) m = se2gpu_matcher_create(std::max(nq, 2048), std::max(ndb, 2048), device);
@@ -772,23 +742,16 @@ extern "C" {
 
 int se2gpu_hamming_distance(const uint8_t* a, const uint8_t* b, int n, int* out, int device) {
     if (n < 0 || (n && (!a || !b || !out))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    int rc = se2gpu::select_device(device);
-    if (rc != SE2GPU_OK) return rc;
+    se2gpu::HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (n == 0) return SE2GPU_OK;
-    uint32_t *da = nullptr, *db = nullptr; int* dout = nullptr;
-    const bool ok = cudaMalloc((void**)&da, (size_t)n * 32) == cudaSuccess && cudaMalloc((void**)&db, (size_t)n * 32) == cudaSuccess &&
-                    cudaMalloc((void**)&dout, (size_t)n * 4) == cudaSuccess;
-    cudaError_t e = cudaSuccess;
-    if (ok) {
-        cudaMemcpy(da, a, (size_t)n * 32, cudaMemcpyHostToDevice); cudaMemcpy(db, b, (size_t)n * 32, cudaMemcpyHostToDevice);
-        k_hamming_pairs<<<(n + 255) / 256, 256>>>(da, db, n, dout);
-        se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaMemcpy(out, dout, sizeof(int) * n, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(da); cudaFree(db); cudaFree(dout);
-    if (!ok) return fail(SE2GPU_ERR_CUDA, "alloc failed");
-    if (e != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "hamming kernel failed: %s", cudaGetErrorString(e));
-    return SE2GPU_OK;
+    const uint32_t* da = st.upload(reinterpret_cast<const uint32_t*>(a), (size_t)n * 8);
+    const uint32_t* db = st.upload(reinterpret_cast<const uint32_t*>(b), (size_t)n * 8);
+    int* dout = st.output(out, n);
+    if (const int rc = st.status()) return rc;
+    SE2_LAUNCH(k_hamming_pairs, (n + 255) / 256, 256, 0, nullptr, da, db, n, dout);
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }
 
 int se2gpu_matcher_match_by_window(se2gpu_matcher* m, const se2gpu_keypoint* kp1, const uint8_t* desc1, int n1, const se2gpu_keypoint* kp2,
@@ -803,14 +766,15 @@ int se2gpu_matcher_match_by_window(se2gpu_matcher* m, const se2gpu_keypoint* kp1
     if (n1 > m->max_q || n2 > m->max_db) return fail(SE2GPU_ERR_CAPACITY, "%d x %d exceeds the matcher's capacity %d x %d", n1, n2, m->max_q, m->max_db);
     SE2_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = m->stream;
-    Stage st{m};
-    if (!st.up(m->d_kp1, kp1, n1, s) || !st.up(m->d_kp2, kp2, n2, s) || !st.up(m->d_desc1, desc1, (size_t)n1 * 32, s) ||
-        !st.up(m->d_desc2, desc2, (size_t)n2 * 32, s) || !st.up(m->d_f1, prev, (size_t)2 * n1, s))
-        return fail(SE2GPU_ERR_CUDA, "upload failed");
+    se2gpu::PinnedArena& st = m->pin;
+    st.reserve(m->pin_bytes);
+    if (st.up(m->d_kp1, kp1, n1, s) || st.up(m->d_kp2, kp2, n2, s) || st.up(m->d_desc1, desc1, (size_t)n1 * 32, s) ||
+        st.up(m->d_desc2, desc2, (size_t)n2 * 32, s) || st.up(m->d_f1, prev, (size_t)2 * n1, s))
+        return SE2GPU_ERR_CUDA;
     int rc = se2gpu_match_by_window_device(m, m->d_kp1, m->d_desc1, n1, nullptr, m->d_kp2, m->d_desc2, n2, nullptr, m->d_f1, grid, win_size,
                                            level_offset, min_level, max_level, nnratio, m->d_out, m->nm, s);
     if (rc != SE2GPU_OK) return rc;
-    int* h_m = st.get<int>(n1); float* h_prev = st.get<float>((size_t)2 * n1); int* h_nm = st.get<int>(1);
+    int* h_m = st.alloc<int>(n1); float* h_prev = st.alloc<float>((size_t)2 * n1); int* h_nm = st.alloc<int>(1);
     if (!h_m || !h_prev || !h_nm) return fail(SE2GPU_ERR_CAPACITY, "staging exhausted");
     SE2_CUDA(cudaMemcpyAsync(h_m, m->d_out, sizeof(int) * n1, cudaMemcpyDeviceToHost, s));
     SE2_CUDA(cudaMemcpyAsync(h_prev, m->d_f1, sizeof(float) * 2 * n1, cudaMemcpyDeviceToHost, s));
@@ -833,15 +797,16 @@ int se2gpu_matcher_match_by_projection(se2gpu_matcher* m, const se2gpu_keypoint*
     if (n_mp > m->max_q || n_kf > m->max_db) return fail(SE2GPU_ERR_CAPACITY, "%d x %d exceeds the matcher's capacity %d x %d", n_mp, n_kf, m->max_q, m->max_db);
     SE2_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = m->stream;
-    Stage st{m};
-    if (!st.up(m->d_kp2, kf_kp, n_kf, s) || !st.up(m->d_desc2, kf_desc, (size_t)n_kf * 32, s) || !st.up(m->d_desc1, mp_desc, (size_t)n_mp * 32, s) ||
-        !st.up(m->d_u8a, kf_observed, n_kf, s) || !st.up(m->d_u8b, mp_valid, n_mp, s) || !st.up(m->d_f1, mp_uv, (size_t)2 * n_mp, s) ||
-        !st.up(m->d_i1, mp_octave, n_mp, s))
-        return fail(SE2GPU_ERR_CUDA, "upload failed");
+    se2gpu::PinnedArena& st = m->pin;
+    st.reserve(m->pin_bytes);
+    if (st.up(m->d_kp2, kf_kp, n_kf, s) || st.up(m->d_desc2, kf_desc, (size_t)n_kf * 32, s) || st.up(m->d_desc1, mp_desc, (size_t)n_mp * 32, s) ||
+        st.up(m->d_u8a, kf_observed, n_kf, s) || st.up(m->d_u8b, mp_valid, n_mp, s) || st.up(m->d_f1, mp_uv, (size_t)2 * n_mp, s) ||
+        st.up(m->d_i1, mp_octave, n_mp, s))
+        return SE2GPU_ERR_CUDA;
     int rc = se2gpu_match_by_projection_device(m, m->d_kp2, m->d_desc2, n_kf, nullptr, m->d_u8a, m->d_u8b, m->d_f1, n_mp, m->d_i1, m->d_desc1, grid,
                                                win_size, level_offset, nnratio, m->d_out, m->nm, s);
     if (rc != SE2GPU_OK) return rc;
-    int* h_m = st.get<int>(n_kf); int* h_nm = st.get<int>(1);
+    int* h_m = st.alloc<int>(n_kf); int* h_nm = st.alloc<int>(1);
     if (!h_m || !h_nm) return fail(SE2GPU_ERR_CAPACITY, "staging exhausted");
     SE2_CUDA(cudaMemcpyAsync(h_m, m->d_out, sizeof(int) * n_kf, cudaMemcpyDeviceToHost, s));
     SE2_CUDA(cudaMemcpyAsync(h_nm, m->nm, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -877,12 +842,13 @@ int se2gpu_matcher_search_by_bow(se2gpu_matcher* m, const se2gpu_bow_kf* k1, con
         return fail(SE2GPU_ERR_CAPACITY, "BoW problem (%d queries, %d x %d features) exceeds the matcher's capacity %d x %d", nq, k1->n, k2->n, m->max_q, m->max_db);
     SE2_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = m->stream;
-    Stage st{m};
-    if (!st.up(m->d_desc1, k1->desc, (size_t)k1->n * 32, s) || !st.up(m->d_desc2, k2->desc, (size_t)k2->n * 32, s) ||
-        !st.up(m->d_u8a, k1->has_mp, k1->n, s) || !st.up(m->d_u8b, k2->has_mp, k2->n, s) || !st.up(m->d_f1, k1->angle, k1->n, s) ||
-        !st.up(m->d_f2, k2->angle, k2->n, s) || !st.up(m->d_i1, qidx.data(), nq, s) || !st.up(m->d_i2, qb0.data(), nq, s) ||
-        !st.up(m->d_i3, qb1.data(), nq, s) || !st.up(m->d_i4, k2->feat, nf2, s))
-        return fail(SE2GPU_ERR_CUDA, "upload failed");
+    se2gpu::PinnedArena& st = m->pin;
+    st.reserve(m->pin_bytes);
+    if (st.up(m->d_desc1, k1->desc, (size_t)k1->n * 32, s) || st.up(m->d_desc2, k2->desc, (size_t)k2->n * 32, s) ||
+        st.up(m->d_u8a, k1->has_mp, k1->n, s) || st.up(m->d_u8b, k2->has_mp, k2->n, s) || st.up(m->d_f1, k1->angle, k1->n, s) ||
+        st.up(m->d_f2, k2->angle, k2->n, s) || st.up(m->d_i1, qidx.data(), nq, s) || st.up(m->d_i2, qb0.data(), nq, s) ||
+        st.up(m->d_i3, qb1.data(), nq, s) || st.up(m->d_i4, k2->feat, nf2, s))
+        return SE2GPU_ERR_CUDA;
     m->prof.begin(1, s);
     SE2_LAUNCH(k_candidates_bow, (nq * 32 + 255) / 256, 256, 0, s, nq, m->d_i1, m->d_i2, m->d_i3, reinterpret_cast<const uint32_t*>(m->d_desc1), m->d_u8a,
                m->d_i4, reinterpret_cast<const uint32_t*>(m->d_desc2), m->d_u8b, mp_only, m->max_db, m->cand, m->ncand);
@@ -893,7 +859,7 @@ int se2gpu_matcher_search_by_bow(se2gpu_matcher* m, const se2gpu_bow_kf* k1, con
     ra.qid = m->d_i1; ra.out = m->d_out; ra.n_out = k1->n; ra.nmatches = m->nm; ra.flags = m->flags;
     int rc = launch_resolve<MODE_BOW>(m, ra, nullptr, s);
     if (rc != SE2GPU_OK) return rc;
-    int* h_m = st.get<int>(k1->n); int* h_nm = st.get<int>(1);
+    int* h_m = st.alloc<int>(k1->n); int* h_nm = st.alloc<int>(1);
     if (!h_m || !h_nm) return fail(SE2GPU_ERR_CAPACITY, "staging exhausted");
     SE2_CUDA(cudaMemcpyAsync(h_m, m->d_out, sizeof(int) * k1->n, cudaMemcpyDeviceToHost, s));
     SE2_CUDA(cudaMemcpyAsync(h_nm, m->nm, sizeof(int), cudaMemcpyDeviceToHost, s));

@@ -1153,7 +1153,7 @@ struct se2gpu_orb {
 
     uint8_t* d_in = nullptr; se2gpu_keypoint* d_kps = nullptr; uint8_t* d_desc = nullptr; int* d_counts = nullptr;
     HarrisBufs hb{};             // HARRIS_SCORE handles only: [B][cand_total] 64-bit records, [B][lkp_total] level-list responses
-    std::vector<void*> bufs;
+    se2gpu::DeviceBuffers bufs;
     int last_n = 0;
     se2gpu::Profiler prof;
     cudaStream_t side = nullptr;          // blur runs here, concurrently with FAST + selection
@@ -1639,7 +1639,7 @@ se2gpu_orb* se2gpu_orb_create_scored(int nfeatures, float scale_factor, int nlev
     h->cap_lkp = nfeatures + 64;
     const size_t B = max_batch;
     bool ok = true;
-    auto A = [&](auto** p, size_t c) { if (ok && se2gpu::dev_alloc(p, c) == cudaSuccess) h->bufs.push_back(*p); else ok = false; };
+    auto A = [&](auto** p, size_t c) { ok = ok && h->bufs.alloc(p, c) == cudaSuccess; };
     OrbDev& d = h->d;
     A(&h->d_levels, (size_t)nlevels); A(&h->d_cells, h->cap_cells); A(&h->d_tiles, h->cap_tiles); A(&h->d_itab, h->cap_tab); A(&h->d_stab, 2 * h->cap_tab);
     A(&d.plain, B * h->cap_plane); A(&d.blurred, B * h->cap_plane);
@@ -1674,7 +1674,6 @@ void se2gpu_orb_destroy(se2gpu_orb* h) {
     if (!h) return;
     if (h->twin) { se2gpu_orb_destroy(h->twin); h->twin = nullptr; }
     cudaSetDevice(h->device);
-    for (void* p : h->bufs) cudaFree(p);
     if (h->side) cudaStreamDestroy(h->side);
     if (h->ev_pyr) cudaEventDestroy(h->ev_pyr);
     if (h->d_und_m1) cudaFree(h->d_und_m1);
@@ -1828,41 +1827,33 @@ int se2gpu_orb_wait(se2gpu_orb* h) {
 int se2gpu_orb_debug_nth_element(uint32_t* values, const int* offsets, const int* nth, int count, int device) {
     if (count <= 0) return SE2GPU_OK;
     if (!values || !offsets || !nth) return fail(SE2GPU_ERR_INVALID, "null argument");
-    if (se2gpu::select_device(device) != SE2GPU_OK) return SE2GPU_ERR_CUDA;
-    const size_t total = (size_t)offsets[count];
-    uint32_t* dv = nullptr; int* dofs = nullptr; int* dn = nullptr;
-    SE2_CUDA(cudaMalloc((void**)&dv, std::max<size_t>(total, 1) * 4));
-    SE2_CUDA(cudaMalloc((void**)&dofs, sizeof(int) * (count + 1)));
-    SE2_CUDA(cudaMalloc((void**)&dn, sizeof(int) * count));
-    SE2_CUDA(cudaMemcpy(dv, values, total * 4, cudaMemcpyHostToDevice));
-    SE2_CUDA(cudaMemcpy(dofs, offsets, sizeof(int) * (count + 1), cudaMemcpyHostToDevice));
-    SE2_CUDA(cudaMemcpy(dn, nth, sizeof(int) * count, cudaMemcpyHostToDevice));
+    se2gpu::HostStage st(device);
+    if (const int rc = st.status()) return rc;
+    uint32_t* dv = st.inout(values, (size_t)offsets[count]);
+    const int* dofs = st.upload(offsets, (size_t)count + 1);
+    const int* dn = st.upload(nth, count);
+    if (const int rc = st.status()) return rc;
     SE2_LAUNCH(orb_debug_nth, (count + 3) / 4, 128, 0, nullptr, dv, dofs, dn, count);
-    SE2_CUDA(cudaGetLastError());
-    SE2_CUDA(cudaMemcpy(values, dv, total * 4, cudaMemcpyDeviceToHost));
-    cudaFree(dv); cudaFree(dofs); cudaFree(dn);
-    return SE2GPU_OK;
+    st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
 }
 
 int se2gpu_orb_debug_nth_element_f32(const float* values, const int* offsets, const int* nth, int count, int* perm, int device) {
     if (count <= 0) return SE2GPU_OK;
     if (!values || !offsets || !nth || !perm) return fail(SE2GPU_ERR_INVALID, "null argument");
-    if (se2gpu::select_device(device) != SE2GPU_OK) return SE2GPU_ERR_CUDA;
+    se2gpu::HostStage st(device);
+    if (const int rc = st.status()) return rc;
     const size_t total = (size_t)offsets[count];
     std::vector<uint64_t> rec(total);
     for (int k = 0; k < count; ++k)
         for (int i = offsets[k]; i < offsets[k + 1]; ++i) rec[i] = ((uint64_t)se2gpu::resp_key(values[i]) << 32) | (uint32_t)(i - offsets[k]);
-    uint64_t* dv = nullptr; int* dofs = nullptr; int* dn = nullptr;
-    SE2_CUDA(cudaMalloc((void**)&dv, std::max<size_t>(total, 1) * 8));
-    SE2_CUDA(cudaMalloc((void**)&dofs, sizeof(int) * (count + 1)));
-    SE2_CUDA(cudaMalloc((void**)&dn, sizeof(int) * count));
-    SE2_CUDA(cudaMemcpy(dv, rec.data(), total * 8, cudaMemcpyHostToDevice));
-    SE2_CUDA(cudaMemcpy(dofs, offsets, sizeof(int) * (count + 1), cudaMemcpyHostToDevice));
-    SE2_CUDA(cudaMemcpy(dn, nth, sizeof(int) * count, cudaMemcpyHostToDevice));
+    uint64_t* dv = st.inout(rec.data(), total);
+    const int* dofs = st.upload(offsets, (size_t)count + 1);
+    const int* dn = st.upload(nth, count);
+    if (const int rc = st.status()) return rc;
     SE2_LAUNCH(orb_debug_nth64, (count + 3) / 4, 128, 0, nullptr, dv, dofs, dn, count);
-    SE2_CUDA(cudaGetLastError());
-    SE2_CUDA(cudaMemcpy(rec.data(), dv, total * 8, cudaMemcpyDeviceToHost));
-    cudaFree(dv); cudaFree(dofs); cudaFree(dn);
+    st.check(cudaGetLastError(), "kernel launch");
+    if (const int rc = st.finish()) return rc;
     for (size_t i = 0; i < total; ++i) perm[i] = (int)(uint32_t)rec[i];
     return SE2GPU_OK;
 }

@@ -16,7 +16,6 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
-#include <mutex>
 
 #include "common.h"
 
@@ -560,16 +559,6 @@ int launch(int B, float* d_Tcw, const int* d_edge_ptr, const float* d_xyz, const
     return SE2GPU_OK;
 }
 
-// grow-only device buffers of the host entry points, one set per device
-struct HostWorkspace {
-    std::mutex mu;
-    char* base = nullptr;
-    size_t cap = 0;
-};
-HostWorkspace g_ws[64];
-
-size_t align_up(size_t v) { return (v + 255) & ~size_t(255); }
-
 int host_run(int B, float* Tcw, const int* edge_ptr, const float* xyz, const float* uv, const float* info,
              const se2gpu_pose_ba_params* params, se2gpu_ba_iter_stats* stats, int* iterations, int* status, double* pose,
              double* trace, int device) {
@@ -581,52 +570,25 @@ int host_run(int B, float* Tcw, const int* edge_ptr, const float* xyz, const flo
         if (edge_ptr[b + 1] < edge_ptr[b]) return fail(SE2GPU_ERR_INVALID, "edge_ptr not ascending at %d", b);
     const size_t E = B ? (size_t)edge_ptr[B] : 0;
     if (E && (!xyz || !uv || !info)) return fail(SE2GPU_ERR_INVALID, "null edge arrays");
-    { const int rc = select_device(device); if (rc) return rc; }
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
     if (B == 0) return SE2GPU_OK;
-    if (device >= 64) return fail(SE2GPU_ERR_INVALID, "device %d", device);
     const size_t it = (size_t)p.iterations;
-    const size_t sizes[] = {sizeof(float) * 16 * B, sizeof(int) * (B + 1), sizeof(float) * 3 * E, sizeof(float) * 2 * E, sizeof(float) * E,
-                            stats ? sizeof(se2gpu_ba_iter_stats) * B * it : 0, sizeof(int) * B, sizeof(int) * B,
-                            pose ? sizeof(double) * 7 * B : 0, trace ? sizeof(double) * 7 * B * it : 0};
-    constexpr int NB = sizeof sizes / sizeof sizes[0];
-    size_t off[NB], total = 0;
-    for (int k = 0; k < NB; ++k) { off[k] = total; total += align_up(sizes[k]); }
-    HostWorkspace& ws = g_ws[device];
-    std::lock_guard<std::mutex> lock(ws.mu);
-    if (total > ws.cap) {
-        if (ws.base) cudaFree(ws.base);
-        ws.base = nullptr; ws.cap = 0;
-        SE2_CUDA(cudaMalloc((void**)&ws.base, total));
-        ws.cap = total;
-    }
-    char* d = ws.base;
-    float* dT = (float*)(d + off[0]);
-    int* dptr = (int*)(d + off[1]);
-    float* dx = (float*)(d + off[2]);
-    float* du = (float*)(d + off[3]);
-    float* dw = (float*)(d + off[4]);
-    auto* dst = stats ? (se2gpu_ba_iter_stats*)(d + off[5]) : nullptr;
-    int* dit = (int*)(d + off[6]);
-    int* dsts = (int*)(d + off[7]);
-    double* dpose = pose ? (double*)(d + off[8]) : nullptr;
-    double* dtr = trace ? (double*)(d + off[9]) : nullptr;
-    SE2_CUDA(cudaMemcpy(dT, Tcw, sizes[0], cudaMemcpyHostToDevice));
-    SE2_CUDA(cudaMemcpy(dptr, edge_ptr, sizes[1], cudaMemcpyHostToDevice));
-    if (E) {
-        SE2_CUDA(cudaMemcpy(dx, xyz, sizes[2], cudaMemcpyHostToDevice));
-        SE2_CUDA(cudaMemcpy(du, uv, sizes[3], cudaMemcpyHostToDevice));
-        SE2_CUDA(cudaMemcpy(dw, info, sizes[4], cudaMemcpyHostToDevice));
-    }
-    if (dst) SE2_CUDA(cudaMemset(dst, 0, sizes[5]));
-    if (dtr) SE2_CUDA(cudaMemset(dtr, 0, sizes[9]));
+    float* dT = st.inout(Tcw, 16 * (size_t)B);
+    const int* dptr = st.upload(edge_ptr, (size_t)B + 1);
+    const float* dx = st.upload(xyz, 3 * E);
+    const float* du = st.upload(uv, 2 * E);
+    const float* dw = st.upload(info, E);
+    se2gpu_ba_iter_stats* dst = stats ? st.output(stats, B * it) : nullptr;
+    int* dit = iterations ? st.output(iterations, B) : st.scratch<int>(B);
+    int* dsts = status ? st.output(status, B) : st.scratch<int>(B);
+    double* dpose = pose ? st.output(pose, 7 * (size_t)B) : nullptr;
+    double* dtr = trace ? st.output(trace, 7 * B * it) : nullptr;
+    if (dst) st.check(cudaMemset(dst, 0, sizeof(se2gpu_ba_iter_stats) * B * it), "cudaMemset");
+    if (dtr) st.check(cudaMemset(dtr, 0, sizeof(double) * 7 * B * it), "cudaMemset");
+    if (const int rc = st.status()) return rc;
     { const int rc = launch(B, dT, dptr, dx, du, dw, p, 0, dst, dit, dsts, dpose, dtr, nullptr); if (rc) return rc; }
-    SE2_CUDA(cudaMemcpy(Tcw, dT, sizes[0], cudaMemcpyDeviceToHost));
-    if (stats) SE2_CUDA(cudaMemcpy(stats, dst, sizes[5], cudaMemcpyDeviceToHost));
-    if (iterations) SE2_CUDA(cudaMemcpy(iterations, dit, sizes[6], cudaMemcpyDeviceToHost));
-    if (status) SE2_CUDA(cudaMemcpy(status, dsts, sizes[7], cudaMemcpyDeviceToHost));
-    if (pose) SE2_CUDA(cudaMemcpy(pose, dpose, sizes[8], cudaMemcpyDeviceToHost));
-    if (trace) SE2_CUDA(cudaMemcpy(trace, dtr, sizes[9], cudaMemcpyDeviceToHost));
-    return SE2GPU_OK;
+    return st.finish();
 }
 
 }  // namespace
@@ -638,6 +600,7 @@ struct se2gpu_localizer {
     float* uv = nullptr;
     float* w = nullptr;
     int* edge_ptr = nullptr;
+    se2gpu::DeviceBuffers bufs;
 };
 
 se2gpu_localizer* se2gpu_localizer_create(int max_map_points, int device) {
@@ -646,8 +609,8 @@ se2gpu_localizer* se2gpu_localizer_create(int max_map_points, int device) {
     auto* h = new se2gpu_localizer;
     h->device = device; h->max_mp = max_map_points;
     const size_t m = (size_t)(max_map_points ? max_map_points : 1);
-    if (dev_alloc(&h->best, m) != cudaSuccess || dev_alloc(&h->xyz, 3 * m) != cudaSuccess || dev_alloc(&h->uv, 2 * m) != cudaSuccess ||
-        dev_alloc(&h->w, m) != cudaSuccess || dev_alloc(&h->edge_ptr, 2) != cudaSuccess) {
+    if (h->bufs.alloc(&h->best, m) != cudaSuccess || h->bufs.alloc(&h->xyz, 3 * m) != cudaSuccess || h->bufs.alloc(&h->uv, 2 * m) != cudaSuccess ||
+        h->bufs.alloc(&h->w, m) != cudaSuccess || h->bufs.alloc(&h->edge_ptr, 2) != cudaSuccess) {
         fail(SE2GPU_ERR_CUDA, "device allocation failed");
         se2gpu_localizer_destroy(h);
         return nullptr;
@@ -658,7 +621,6 @@ se2gpu_localizer* se2gpu_localizer_create(int max_map_points, int device) {
 void se2gpu_localizer_destroy(se2gpu_localizer* h) {
     if (!h) return;
     cudaSetDevice(h->device);
-    cudaFree(h->best); cudaFree(h->xyz); cudaFree(h->uv); cudaFree(h->w); cudaFree(h->edge_ptr);
     delete h;
 }
 
@@ -680,7 +642,7 @@ int se2gpu_pose_ba_device(int B, float* d_Tcw, const int* d_edge_ptr, const floa
     Params p;
     { const int rc = check_params(params, &p); if (rc) return rc; }
     if (B < 0 || (B && (!d_Tcw || !d_edge_ptr))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    { int nd = 0; if (cudaGetDeviceCount(&nd) != cudaSuccess || nd <= 0) return fail(SE2GPU_ERR_NO_DEVICE, "no CUDA device available"); }
+    { const int rc = require_device(); if (rc) return rc; }
     if (B == 0) return SE2GPU_OK;
     return launch(B, d_Tcw, d_edge_ptr, d_xyz, d_uv, d_info, p, 0, d_stats, d_iterations, d_status, d_pose, nullptr, (cudaStream_t)stream);
 }
