@@ -13,9 +13,10 @@
 //   orb_fast_cells_big      the same result for cells too large for the shared-memory candidate list
 //   orb_harris              HARRIS_SCORE handles only: HarrisResponses(cell, kps, 7, 0.04f) :85-126, :625-629 on the un-blurred
 //                           level, one 64-bit record (order key of the response, FAST record) per candidate
-//   orb_select<HARRIS>      quota redistribution :631-679 + KeyPointsFilter::retainBest twice :687-710 — the
-//                           libstdc++ introselect permutation is reproduced exactly, warp-cooperatively (introselect.h);
-//                           keyed by the FAST score, or by the Harris response on 64-bit records
+//   orb_select_cells<HARRIS> quota redistribution :631-679 + KeyPointsFilter::retainBest per cell :687-694, one warp per cell;
+//   orb_select_levels<HARRIS> retainBest per level :706-710, one warp per level — the libstdc++ introselect permutation is
+//                           reproduced exactly, warp-cooperatively (introselect.h); keyed by the FAST score, or by the Harris
+//                           response on 64-bit records
 //   orb_blur                GaussianBlur 7x7 sigma 2 :769 (float32 separable, fused multiply-add, RNE to u8)
 //   orb_orient_describe     IC_Angle :130-157 + computeOrbDescriptor :160-200, one warp per keypoint; keypoint
 //                           records are written as 28-byte cv::KeyPoint and 32-byte descriptors
@@ -66,6 +67,7 @@ struct LevelGeo {
     int tile_base;      // first orb_blur tile of this level
     int blur_th, blur_strips;   // orb_blur: ROI rows per strip, strips (the last one ends at the ROI's last row)
     int fbw, fbh;       // orb_fast_cells<true>: TMA box of this level's FAST cells (bytes per row: multiple of 16; rows)
+    int sel_off, sel_cap;   // slot range of the level list (the cells' survivors) in the per-frame selection buffer
 };
 
 struct CellGeo {
@@ -95,6 +97,8 @@ struct OrbDev {  // passed by value to kernels
     uint32_t* lkp;              // [B][lkp_total]
     int lkp_total;
     int* lcount;                // [B][nlevels]
+    uint64_t* sel;              // [B][sel_total] level lists between orb_select_cells and orb_select_levels (32- or 64-bit records)
+    int sel_total;
     int* err;                   // device error flag
     int frame0;                 // first frame of this launch group (pipelined host path processes the batch in chunks)
 };
@@ -483,8 +487,9 @@ __global__ void __launch_bounds__(FAST_THREADS, 5) orb_fast_cells(OrbDev d, cons
     uint8_t* score = smem + ((pw * ph + 15) & ~15);                                       // [(ch+2) x pw], pixel (x,y) at (y+1)*pw + x+NMS_X0
     uint32_t* bitmap = reinterpret_cast<uint32_t*>(score + ((fastpx::nms_plane_bytes(pw, ch) + 15) & ~15));   // [ch x wpr]
     uint16_t* list = reinterpret_cast<uint16_t*>(bitmap + ch * wpr);                      // [<= cw*ch] entries y*pw + x
+    if (TMA && threadIdx.x == 0) orb_mbar_init(&s_bar, 1);
+    asm volatile("griddepcontrol.wait;" ::: "memory");     // programmatic dependent of the last resize: the pyramid is complete from here on
     if (TMA) {
-        if (threadIdx.x == 0) orb_mbar_init(&s_bar, 1);
         __syncthreads();
         if (threadIdx.x == 0) orb_tma_box3(patch, &maps.m[c.level], ax0, c.y0 - 3 + EDGE, f, (unsigned)(pw * ph), &s_bar);
     } else {
@@ -787,113 +792,138 @@ __global__ void __launch_bounds__(HARRIS_THREADS) orb_harris(OrbDev d, uint64_t*
     }
 }
 
-// one CTA per (level, frame): quota redistribution, retainBest per cell and per level. The cells' candidate lists
-// are staged in shared memory when the level's total fits (SEL_STAGE entries), otherwise they are processed in place
-// in global memory. retainBest is std::nth_element; one warp per cell runs the warp-cooperative introselect of
-// introselect.h (same permutation as libstdc++'s, 32 elements per step), cells round-robin over the CTA's warps.
-// HARRIS: the records are orb_harris' 64-bit ones (cand64, selected by their upper word), the stage holds half as many of
-// them (the same bytes), and the level lists are written as the 32-bit FAST records plus the float responses in lresp.
-constexpr int SEL_STAGE = 12288;
-constexpr int SEL_THREADS = 512;
-struct HarrisBufs { uint64_t* cand64; float* lresp; };   // orb_select<true> / orb_orient_describe<true> only
+// Selection (:625-710) in two launches, neither of which leaves one CTA to carry a pyramid level:
+//   orb_select_cells   one warp per (cell, frame): the level's quota redistribution :631-679, computed warp-cooperatively by
+//                      every warp of the level (integer sums, so any summation order gives the reference's numbers), then
+//                      KeyPointsFilter::retainBest of its own cell (:687-694) and the survivors copied to the cell's slot range
+//                      in the level list (d.sel, cells in order); the level's cell 0 also writes the list length to d.lcount
+//   orb_select_levels  one warp per (level, frame): retainBest of the level list (:706-710) into the keypoint buffer
+// retainBest is std::nth_element: the warp-cooperative introselect of introselect.h reproduces libstdc++'s permutation. A cell
+// list that fits the warp's SEL_STAGE_BYTES of shared memory is selected in the warp's shared memory, a longer one in place in global memory.
+// Level 0, which has by far the most candidates, is then as many warps as it has cells, spread over the GPU, and its level-wide
+// nth_element runs on at most about 2 * nDesired survivors.
+// HARRIS: the records are orb_harris' 64-bit ones (cand64, selected by their upper word), and the level lists are written as the
+// 32-bit FAST records plus the float responses in lresp.
+// PDL: both launch as programmatic dependents; each releases its dependent at once, and reads what its predecessor wrote only
+// behind griddepcontrol.wait.
+constexpr int SEL_WARPS = 4;            // warps (cells) per orb_select_cells CTA
+// shared memory per warp for its cell list. Measured on an H100 SXM (700 W), 64 frames of 640x480, ms per step: 0.5550 at
+// 2 KB, 0.5545 at 4 KB, 0.5632 at 8 KB, 0.568-0.571 at 12 and 16 KB (fewer resident warps for a latency-bound kernel)
+constexpr int SEL_STAGE_BYTES = 4096;
+constexpr int SEL_NOMORE = 1 << 30;     // bNoMore flag next to a cell's nToRetain
+struct HarrisBufs { uint64_t* cand64; float* lresp; };   // orb_select_*<true> / orb_orient_describe<true> only
+
+__device__ __forceinline__ int warp_sum(int v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
 template <bool HARRIS>
-__global__ void __launch_bounds__(SEL_THREADS) orb_select(OrbDev d, HarrisBufs hb) {
+__global__ void __launch_bounds__(SEL_WARPS * 32) orb_select_cells(OrbDev d, HarrisBufs hb, int max_cells, int stage_n) {
     typedef typename std::conditional<HARRIS, se2gpu::KpKey64, se2gpu::KpScore32>::type K;
     typedef typename K::rec R;
-    constexpr int STAGE = HARRIS ? SEL_STAGE / 2 : SEL_STAGE;
-    extern __shared__ uint32_t sbuf[];   // [cap] level list | [4*nCells] ints | [STAGE] staged candidates (records of type R)
-    __shared__ int wq[SEL_THREADS / 32][128];
-    constexpr int NW = SEL_THREADS / 32;
+    extern __shared__ __align__(16) uint8_t selc_smem[];   // [SEL_WARPS][stage_n] records | [SEL_WARPS][2][max_cells] ints
+    __shared__ int wq[SEL_WARPS][128];
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int level = blockIdx.x, f = blockIdx.y + d.frame0;
+    const int cell = blockIdx.y * SEL_WARPS + wid, f = blockIdx.x + d.frame0;   // frames fastest: see run_device
+    if (cell >= d.n_cells) return;
+    const CellGeo c = d.cells[cell];
+    const int level = c.level;
     const LevelGeo& L = d.levels[level];
-    const int nCells = L.nCells;
-    const int cap = 2 * L.nDesired + 4 * nCells + 64;
-    R* lbuf = reinterpret_cast<R*>(sbuf);
-    int* nTotal = (int*)(lbuf + cap);
-    int* nToRetain = nTotal + nCells;
-    int* kept = nToRetain + nCells;
-    int* koff = kept + nCells;
-    R* stage = (R*)(koff + nCells);
-    __shared__ int s_total, s_staged;
-    const CellHdr* hdr = d.hdr + (size_t)f * d.n_cells + L.cell_base;
-    R* cand;
-    if constexpr (HARRIS) cand = hb.cand64 + (size_t)f * d.cand_total;
-    else cand = d.cand + (size_t)f * d.cand_total;
-    for (int c = threadIdx.x; c < nCells; c += SEL_THREADS) nTotal[c] = d.cells[L.cell_base + c].skipped ? 0 : hdr[c].n_base;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        // :625-679 (skipped cells never enter the first pass: nToRetain/nTotal stay 0, bNoMore stays false)
-        const int nfeaturesCell = L.nfeaturesCell;
-        int nNoMore = 0, nToDistribute = 0, tot = 0;
-        for (int c = 0; c < nCells; ++c) {
-            const bool skipped = d.cells[L.cell_base + c].skipped;
-            koff[c] = 0;  // bNoMore
-            tot += nTotal[c];
-            if (skipped) { nToRetain[c] = 0; continue; }
-            if (nTotal[c] > nfeaturesCell) nToRetain[c] = nfeaturesCell;
-            else { nToRetain[c] = nTotal[c]; nToDistribute += nfeaturesCell - nTotal[c]; koff[c] = 1; nNoMore++; }
+    const int nCells = L.nCells, cb = L.cell_base, nfc = L.nfeaturesCell, me = cell - cb;
+    R* stage = reinterpret_cast<R*>(selc_smem) + wid * stage_n;
+    int* nTotal = reinterpret_cast<int*>(reinterpret_cast<R*>(selc_smem) + SEL_WARPS * stage_n) + wid * 2 * max_cells;
+    int* nToRetain = nTotal + max_cells;     // | SEL_NOMORE once bNoMore
+    asm volatile("griddepcontrol.wait;" ::: "memory");     // the FAST (Harris) candidates are complete and visible from here on
+    const CellHdr* hdr = d.hdr + (size_t)f * d.n_cells + cb;
+    // :631-679; skipped cells never enter the first pass (nToRetain/nTotal stay 0, bNoMore stays false)
+    int nToDistribute = 0, nNoMore = 0;
+    for (int k = lane; k < nCells; k += 32) {
+        const bool skipped = d.cells[cb + k].skipped;
+        const int t = skipped ? 0 : hdr[k].n_base;
+        int r = 0;
+        if (!skipped) {
+            if (t > nfc) r = nfc;
+            else { r = t | SEL_NOMORE; nToDistribute += nfc - t; ++nNoMore; }
         }
-        while (nToDistribute > 0 && nNoMore < nCells) {
-            const int nNew = (int)((float)nfeaturesCell + ceilf((float)nToDistribute / (float)(nCells - nNoMore)));
-            nToDistribute = 0;
-            for (int c = 0; c < nCells; ++c)
-                if (!koff[c]) {
-                    if (nTotal[c] > nNew) nToRetain[c] = nNew;
-                    else { nToRetain[c] = nTotal[c]; nToDistribute += nNew - nTotal[c]; koff[c] = 1; nNoMore++; }
-                }
-        }
-        s_staged = tot <= STAGE;
-        int o = 0;
-        for (int c = 0; c < nCells; ++c) { kept[c] = o; o += nTotal[c]; }   // staging offsets (reused below)
+        nTotal[k] = t; nToRetain[k] = r;
     }
-    __syncthreads();
-    const bool staged = s_staged;
-    for (int c = wid; c < nCells; c += NW) {
-        const int n = nToRetain[c], tot = nTotal[c];
-        R* g = cand + d.cells[L.cell_base + c].cand_off;
-        R* v = g;
-        if (staged) {
-            v = stage + kept[c];
+    nToDistribute = warp_sum(nToDistribute); nNoMore = warp_sum(nNoMore);
+    while (nToDistribute > 0 && nNoMore < nCells) {
+        const int nNew = (int)((float)nfc + ceilf((float)nToDistribute / (float)(nCells - nNoMore)));
+        int dist = 0, more = 0;
+        for (int k = lane; k < nCells; k += 32) {
+            if (nToRetain[k] & SEL_NOMORE) continue;
+            const int t = nTotal[k];
+            if (t > nNew) nToRetain[k] = nNew;
+            else { nToRetain[k] = t | SEL_NOMORE; dist += nNew - t; ++more; }
+        }
+        nToDistribute = warp_sum(dist); nNoMore += warp_sum(more);
+    }
+    // the cell's slot in the level list: the survivors min(nTotal, nToRetain) of the cells before it
+    int before = 0, all = 0;
+    for (int k = lane; k < nCells; k += 32) {
+        const int kept = min(nTotal[k], nToRetain[k] & ~SEL_NOMORE);
+        all += kept;
+        if (k < me) before += kept;
+    }
+    before = warp_sum(before); all = warp_sum(all);
+    __syncwarp();
+    const int cap = L.sel_cap;
+    if (me == 0 && lane == 0) {
+        if (all > cap) *d.err = 2;
+        d.lcount[f * d.nlevels + level] = min(all, cap);
+    }
+    const int tot = nTotal[me], n = nToRetain[me] & ~SEL_NOMORE, kept = min(tot, n);
+    if (kept <= 0 || before >= cap) return;
+    R* g;
+    if constexpr (HARRIS) g = hb.cand64 + (size_t)f * d.cand_total + c.cand_off;
+    else g = d.cand + (size_t)f * d.cand_total + c.cand_off;
+    R* v = g;
+    if (tot > n) {   // KeyPointsFilter::retainBest + resize (:692-694)
+        if (tot <= stage_n) {
+            v = stage;
             for (int i = lane; i < tot; i += 32) v[i] = g[i];
             __syncwarp();
         }
-        if (lane == 0) koff[c] = (int)(v - (staged ? stage : cand));   // remember where the list lives
-        if (tot > n && n > 0) se2gpu::kp_nth_element_warp<K>(v, tot, n - 1, wq[wid]);   // KeyPointsFilter::retainBest + resize (:692-694)
+        se2gpu::kp_nth_element_warp<K>(v, tot, n - 1, wq[wid]);
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int o = 0;
-        for (int c = 0; c < nCells; ++c) { const int k = min(nTotal[c], nToRetain[c]); nTotal[c] = k; kept[c] = o; o += k; }
-        if (o > cap) { *d.err = 2; o = cap; }
-        s_total = o;
-    }
-    __syncthreads();
-    for (int c = wid; c < nCells; c += NW) {
-        const R* v = (staged ? stage : cand) + koff[c];
-        const int o = kept[c];
-        for (int i = lane; i < nTotal[c] && o + i < cap; i += 32) lbuf[o + i] = v[i];
-    }
-    __syncthreads();
-    int total = s_total;
+    R* out = reinterpret_cast<R*>(d.sel) + (size_t)f * d.sel_total + L.sel_off + before;
+    for (int i = lane; i < kept && before + i < cap; i += 32) out[i] = v[i];
+}
+
+template <bool HARRIS>
+__global__ void __launch_bounds__(32) orb_select_levels(OrbDev d, HarrisBufs hb) {
+    typedef typename std::conditional<HARRIS, se2gpu::KpKey64, se2gpu::KpScore32>::type K;
+    typedef typename K::rec R;
+    extern __shared__ __align__(16) uint8_t sell_smem[];   // [sel_cap] records of the level list
+    __shared__ int wq[128];
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    const int lane = threadIdx.x, level = blockIdx.x, f = blockIdx.y + d.frame0;
+    const LevelGeo& L = d.levels[level];
+    R* v = reinterpret_cast<R*>(sell_smem);
+    const R* g = reinterpret_cast<const R*>(d.sel) + (size_t)f * d.sel_total + L.sel_off;
+    int* lc = d.lcount + f * d.nlevels + level;
+    asm volatile("griddepcontrol.wait;" ::: "memory");     // the level list is complete and visible from here on
+    int total = *lc;
+    for (int i = lane; i < total; i += 32) v[i] = g[i];
+    __syncwarp();
     if (total > L.nDesired) {  // :706-710
-        if (wid == 0) se2gpu::kp_nth_element_warp<K>(lbuf, total, L.nDesired - 1, wq[0]);
+        se2gpu::kp_nth_element_warp<K>(v, total, L.nDesired - 1, wq);
         total = L.nDesired;
-        __syncthreads();
     }
     uint32_t* out = d.lkp + (size_t)f * d.lkp_total + L.kp_off;
     if constexpr (HARRIS) {
         float* resp = hb.lresp + (size_t)f * d.lkp_total + L.kp_off;
-        for (int i = threadIdx.x; i < total; i += SEL_THREADS) { const R r = lbuf[i]; out[i] = (uint32_t)r; resp[i] = se2gpu::resp_from_key((uint32_t)(r >> 32)); }
+        for (int i = lane; i < total; i += 32) { const R r = v[i]; out[i] = (uint32_t)r; resp[i] = se2gpu::resp_from_key((uint32_t)(r >> 32)); }
     } else {
-        for (int i = threadIdx.x; i < total; i += SEL_THREADS) out[i] = lbuf[i];
+        for (int i = lane; i < total; i += 32) out[i] = v[i];
     }
-    if (threadIdx.x == 0) d.lcount[f * d.nlevels + level] = total;
+    __syncwarp();
+    if (lane == 0) *lc = total;
 }
-// instantiated here, ahead of the templates used later in the file: the module's dynamic shared-memory declarations then keep
-// the order in which ptxas places the dynamic buffer of orb_select<false> right behind its static arrays
-template __global__ void orb_select<false>(OrbDev, HarrisBufs);
-template __global__ void orb_select<true>(OrbDev, HarrisBufs);
 
 // test hook: one warp per list, lists in global memory
 __global__ void __launch_bounds__(128) orb_debug_nth(uint32_t* v, const int* __restrict__ offs, const int* __restrict__ nth, int count) {
@@ -1027,13 +1057,14 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {
 // (predicated off beyond the column's half-height) instead of one dependent +-v pair per loop trip, and the 16 descriptor taps of
 // a lane are loaded back to back: the kernel is bound by the latency of first-touch sectors (every plane byte comes from DRAM
 // once), so the loads in flight per warp set its speed. Integer moments: any summation order gives the reference's m10, m01.
-// HARRIS: the keypoint's response is the Harris response orb_select<true> left in lresp, else the FAST score of the record.
+// HARRIS: the keypoint's response is the Harris response orb_select_levels<true> left in lresp, else the FAST score of the record.
 template <bool HARRIS>
 __global__ void __launch_bounds__(256) orb_orient_describe(OrbDev d, se2gpu_keypoint* __restrict__ kps, uint8_t* __restrict__ desc,
                                                            int* __restrict__ counts, const float* __restrict__ lresp) {
     __shared__ float4 patf[256];     // the 256 point pairs of the rBRIEF pattern as floats (x0, y0, x1, y1); test 8*lane+k at [k][lane]
     for (int i = threadIdx.x; i < 256; i += blockDim.x) patf[(i & 7) * 32 + (i >> 3)] = make_float4((float)d_pattern[4 * i], (float)d_pattern[4 * i + 1], (float)d_pattern[4 * i + 2], (float)d_pattern[4 * i + 3]);
     __syncthreads();
+    asm volatile("griddepcontrol.wait;" ::: "memory");     // programmatic dependent of the selection: the level lists are complete from here on
     const int f = blockIdx.y + d.frame0;
     const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
@@ -1133,7 +1164,9 @@ struct se2gpu_orb {
     std::vector<LevelGeo> levels;
     std::vector<CellGeo> cells;
     std::vector<TileGeo> tiles;
-    size_t fast_smem = 0, select_smem = 0, resize_w_smem = 0;
+    size_t fast_smem = 0, select_smem = 0, select_levels_smem = 0, resize_w_smem = 0;
+    int sel_max_cells = 0;       // most cells of a level: orb_select_cells' per-warp quota arrays
+    int sel_stage_n = 0;         // records of a cell list orb_select_cells stages per warp
     int resize_rows = 0, resize_raw_pitch = 0;   // shared-memory box of orb_resize_w, sized from the scale factor
     int resize_tall_rows = 0; size_t resize_tall_smem = 0;   // the same for RESIZE_TR_TALL-row tiles
     int resize_tall_ctas = 0;    // resident CTAs of orb_resize_w<RESIZE_TR_TALL> on the whole GPU; 0: tall tiles are not used
@@ -1147,7 +1180,7 @@ struct se2gpu_orb {
     int und_nd = 0, und_w = 0, und_h = 0;
     short2* d_und_m1 = nullptr; uint16_t* d_und_m2 = nullptr; size_t und_cap = 0;
     // capacities (computed for max_w x max_h)
-    size_t cap_plane = 0, cap_cand = 0, cap_cells = 0, cap_tiles = 0, cap_tab = 0, cap_lkp = 0;
+    size_t cap_plane = 0, cap_cand = 0, cap_cells = 0, cap_tiles = 0, cap_tab = 0, cap_lkp = 0, cap_sel = 0;
     OrbDev d{};
     LevelGeo* d_levels = nullptr; CellGeo* d_cells = nullptr; TileGeo* d_tiles = nullptr; int* d_itab = nullptr; short* d_stab = nullptr;
 
@@ -1157,7 +1190,7 @@ struct se2gpu_orb {
     int last_n = 0;
     se2gpu::Profiler prof;
     cudaStream_t side = nullptr;          // blur runs here, concurrently with FAST + selection
-    cudaEvent_t ev_pyr = nullptr, ev_blur = nullptr, ev_l1 = nullptr;
+    cudaEvent_t ev_pyr = nullptr, ev_blur = nullptr;
     // host-buffer path: two pipeline lanes (stream + side stream + events) so that the H2D of chunk c+1 and the D2H of
     // chunk c-1 overlap the kernels of chunk c
     cudaStream_t pipe[ORB_LANES] = {};   // host-path pipeline lanes (chunk k runs on lane k % lanes)
@@ -1178,7 +1211,7 @@ namespace {
 
 // level geometry exactly as ORBextractor::ComputePyramid / ComputeKeyPoints derive it (float32 arithmetic)
 int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes, size_t* cand_total, size_t* n_cells,
-                   size_t* n_tiles, size_t* tab_total, size_t* max_fast_smem, size_t* max_select_smem,
+                   size_t* n_tiles, size_t* tab_total, size_t* max_fast_smem,
                    std::vector<LevelGeo>* Lv, std::vector<CellGeo>* Cv, std::vector<TileGeo>* Tv, bool* fast_big_out = nullptr,
                    size_t* fast_tma_smem_out = nullptr) {
     (void)dry;
@@ -1186,10 +1219,10 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
     std::vector<LevelGeo> L(nl);
     std::vector<CellGeo> C;
     std::vector<TileGeo> T;
-    size_t poff = 0, coff = 0, toff = 0, fsm = 0, ssm = 0, fsm_big = 0, fsm_tma = 0;
+    size_t poff = 0, coff = 0, toff = 0, fsm = 0, fsm_big = 0, fsm_tma = 0;
     bool fast_big = false;   // some cell is too large for orb_fast_cells' shared-memory candidate list -> orb_fast_cells_big
     bool tma_ok = true;      // every level's cell patch fits a TMA box (<= 256 x 256) and 16-bit list offsets
-    int kp_off = 0;
+    int kp_off = 0, sel_off = 0;
     const float imageRatio = (float)w / (float)hgt;   // mvImagePyramid[0].cols/rows (:538)
     for (int l = 0; l < nl; ++l) {
         LevelGeo& g = L[l];
@@ -1262,8 +1295,9 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
                 fsm_tma = std::max(fsm_tma, (size_t)128 + ((pw * g.fbh + 15) & ~(size_t)15) + (((size_t)fastpx::nms_plane_bytes(g.fbw, chh) + 15) & ~(size_t)15) + bitmap + (size_t)cw * chh * 2 + 64);
             }
         }
-        if (h->harris) ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 8 + (size_t)g.nCells * 16 + (size_t)(SEL_STAGE / 2) * 8);
-        else ssm = std::max(ssm, (size_t)(2 * g.nDesired + 4 * g.nCells + 64) * 4 + (size_t)g.nCells * 16 + (size_t)SEL_STAGE * 4);
+        // level list: every cell's survivors, at most nToRetain each (the reference's cap on the concatenation)
+        g.sel_cap = 2 * g.nDesired + 4 * g.nCells + 64;
+        g.sel_off = sel_off; sel_off += g.sel_cap;
         // orb_blur: at least 2 strips of at most about BLUR_TH rows, of one height: with its 6 warm-up rows a strip is a whole number
         // of turns of the kernel's 7-row ring, and at most the ROI's height (h >= 39). A tile = 32 consecutive (strip, column group)
         // items. The tile count grows with w and h, so the table sized at create time holds every smaller frame's.
@@ -1278,7 +1312,7 @@ int build_geometry(se2gpu_orb* h, int w, int hgt, bool dry, size_t* plane_bytes,
     }
     *plane_bytes = poff; *cand_total = coff; *n_cells = C.size(); *n_tiles = T.size(); *tab_total = toff;
     if (fsm > 227 * 1024) fast_big = true;
-    *max_fast_smem = fast_big ? fsm_big : fsm; *max_select_smem = ssm;
+    *max_fast_smem = fast_big ? fsm_big : fsm;
     if (fast_big_out) *fast_big_out = fast_big;
     if (fast_tma_smem_out) *fast_tma_smem_out = (tma_ok && !fast_big && fsm_tma <= 227 * 1024) ? fsm_tma : 0;
     if (Lv) *Lv = L;
@@ -1307,10 +1341,15 @@ EncodeTiledFn tensor_map_encoder() {
 // a TMA kernel with 8-pixel items and per-warp candidate lists (whole step 0.72 ms against 0.74 / 0.76 ms); batched loads in
 // orb_orient_describe take it from 0.1045 to 0.097 ms against one dependent load pair per loop trip. The plain-load
 // instantiation stays for geometries whose cell patch exceeds a 256 x 256 TMA box and for drivers without the tensor-map encoder.
-// Blur group A = levels [0, BLUR_SPLIT) on the side stream once its last level exists, the rest behind FAST (run_device). Measured with
-// this orb_blur (same card, 64 frames of 640x480, range over 2 runs of 200 steps): 0.697-0.698 ms per step at 1, 0.709-0.711 at 2,
-// 0.709-0.710 at 3. The blur now costs less than the resize tail it would hide behind, and level 0 alone next to FAST finishes
-// before FAST does, so the levels left for the selection's idle SMs are the ones that shorten the step most.
+// Blur schedule (run_device): one event behind the last resize forks the blur onto the side stream as two back-to-back launches,
+// group A = levels [0, BLUR_SPLIT), then the rest; the main stream joins before the descriptors. Measured on an H100 SXM
+// (700 W), 64 frames of 640x480, ms per step with the two-launch selection (A fork / B fork; P = right behind level
+// BLUR_SPLIT-1, L = behind the last resize, F = behind the FAST launch):
+//   split 1: P/L 0.5633, P/F 0.5607-0.5646, L/F 0.5546-0.5583, L/L 0.5544-0.5584      split 2: P/L 0.5650, L/F 0.5545, L/L 0.5545
+//   split 3: P/L 0.5663                             one launch of every level behind the last resize: 0.5672
+// Blurring level 0 next to the resize chain lengthens the pyramid (0.132 -> 0.158 ms span) by more than it hides, and a
+// fork behind FAST leaves the blur later than the selection, now that the selection is short. The event between the last
+// resize and FAST does not keep FAST from starting before the resize ends (tools/orb_pyramid_trace.py: -3.7 us).
 constexpr int BLUR_SPLIT = 1;
 // host-buffer pipeline shape (orb_enqueue): se2gpu_orb_extract splits a batch into PIPE_CHUNKS chunks round-robin over all
 // pipeline lanes, the first PIPE_FIRST_PCT percent of an even share so that less of the initial H2D copy is exposed;
@@ -1338,9 +1377,9 @@ bool encode_fast_maps(se2gpu_orb* h, size_t frame_plane_bytes) {
 
 int set_geometry(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
     if (w == h->cur_w && hgt == h->cur_h) return SE2GPU_OK;
-    size_t pb, ct, nc, nt, tt, fsm, ssm, fsm_tma = 0;
+    size_t pb, ct, nc, nt, tt, fsm, fsm_tma = 0;
     bool big = false;
-    int rc = build_geometry(h, w, hgt, false, &pb, &ct, &nc, &nt, &tt, &fsm, &ssm, &h->levels, &h->cells, &h->tiles, &big, &fsm_tma);
+    int rc = build_geometry(h, w, hgt, false, &pb, &ct, &nc, &nt, &tt, &fsm, &h->levels, &h->cells, &h->tiles, &big, &fsm_tma);
     if (rc != SE2GPU_OK) return rc;
     if (pb > h->cap_plane || ct > h->cap_cand || nc > h->cap_cells || nt > h->cap_tiles || tt > h->cap_tab)
         return fail(SE2GPU_ERR_CAPACITY, "frame %dx%d exceeds the capacity this extractor was created with (%dx%d)", w, hgt, h->max_w, h->max_h);
@@ -1379,7 +1418,7 @@ int set_geometry(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
     SE2_CUDA(cudaMemcpyAsync(h->d_itab, itab.data(), sizeof(int) * itab.size(), cudaMemcpyHostToDevice, s));
     SE2_CUDA(cudaMemcpyAsync(h->d_stab, stab.data(), sizeof(short) * stab.size(), cudaMemcpyHostToDevice, s));
     SE2_CUDA(cudaStreamSynchronize(s));
-    h->fast_smem = fsm; h->select_smem = ssm; h->fast_big = big;
+    h->fast_smem = fsm; h->fast_big = big;
     {   // consecutive pyramid levels differ by mvScaleFactor[1] up to rounding of the level sizes
         double ratio = 1.0;
         for (size_t l = 1; l < h->levels.size(); ++l)
@@ -1406,10 +1445,25 @@ int set_geometry(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
     h->fast_tma = fsm_tma > 0 && encode_fast_maps(h, pb);
     h->fast_tma_smem = fsm_tma;
     if (h->fast_tma) SE2_CUDA(cudaFuncSetAttribute(orb_fast_cells<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(fsm_tma, 1024)));
-    if (h->harris && ssm > 227 * 1024) return fail(SE2GPU_ERR_CAPACITY, "the Harris-score selection of a %dx%d frame needs %zu B of shared memory", w, hgt, ssm);
-    if (h->harris) SE2_CUDA(cudaFuncSetAttribute(orb_select<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(ssm, 1024)));
-    else SE2_CUDA(cudaFuncSetAttribute(orb_select<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(ssm, 1024)));
+    int max_cells = 0, sel_total = 0, max_sel_cap = 0, max_cand = 0;
+    for (const LevelGeo& g : h->levels) { max_cells = std::max(max_cells, g.nCells); max_sel_cap = std::max(max_sel_cap, g.sel_cap); sel_total += g.sel_cap; }
+    for (const CellGeo& c : h->cells) max_cand = std::max(max_cand, c.skipped ? 0 : c.cand_cap);
+    const int rec = h->harris ? 8 : 4;
+    const int stage_n = std::min((max_cand + 31) & ~31, SEL_STAGE_BYTES / rec);
+    const size_t ssm = (size_t)SEL_WARPS * ((size_t)stage_n * rec + 2 * 4 * (size_t)max_cells);
+    if ((size_t)sel_total > h->cap_sel) return fail(SE2GPU_ERR_CAPACITY, "frame %dx%d exceeds the selection capacity this extractor was created with", w, hgt);
+    const size_t lsm = (size_t)max_sel_cap * (h->harris ? 8 : 4);
+    if (ssm > 227 * 1024 || lsm > 227 * 1024) return fail(SE2GPU_ERR_CAPACITY, "the selection of a %dx%d frame needs %zu / %zu B of shared memory", w, hgt, ssm, lsm);
+    if (h->harris) {
+        SE2_CUDA(cudaFuncSetAttribute(orb_select_cells<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
+        SE2_CUDA(cudaFuncSetAttribute(orb_select_levels<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
+    } else {
+        SE2_CUDA(cudaFuncSetAttribute(orb_select_cells<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
+        SE2_CUDA(cudaFuncSetAttribute(orb_select_levels<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
+    }
+    h->select_smem = ssm; h->select_levels_smem = lsm; h->sel_max_cells = max_cells; h->sel_stage_n = stage_n;
     OrbDev& d = h->d;
+    d.sel_total = sel_total;
     d.n_cells = (int)h->cells.size(); d.n_tiles = (int)h->tiles.size();
     d.frame_plane_bytes = pb; d.cand_total = ct;
     int lk = 0; for (auto& g : h->levels) lk += g.kp_cap;
@@ -1492,6 +1546,20 @@ int ensure_undistort_map(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
     return SE2GPU_OK;
 }
 
+// a launch that may begin while its predecessor in the stream drains (programmatic dependent launch): the kernel reads what
+// its predecessor wrote only behind griddepcontrol.wait, which returns once that grid has completed and its writes are visible
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    ::se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed);
+    return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
 int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int stride, size_t frame_stride,
                se2gpu_keypoint* d_kps, uint8_t* d_desc, int* d_counts, cudaStream_t s, int frame0 = 0, int lane = -1) {
     int rc = set_geometry(h, w, hgt, s);
@@ -1518,10 +1586,7 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
             SE2_LAUNCH(orb_pyr0, grid, dim3(64, 4), 0, s, d, g, d_imgs, stride, frame_stride, nvec);
         }
     }
-    // blur schedule on the side stream: group A = levels [0, splitA) starts as soon as level splitA-1 exists; group B = the rest starts
-    // when FAST has been launched, i.e. it runs next to the selection kernel, whose level-0 CTAs leave most SMs idle, instead of
-    // competing with the issue-bound FAST kernel
-    const int splitA = std::min(BLUR_SPLIT, h->nlevels);
+    const bool overlap = !pr.on && side != nullptr;
     for (int l = 1; l < h->nlevels; ++l) {
         const LevelGeo& g = h->levels[l];
         cudaLaunchConfig_t cfg = {};
@@ -1539,41 +1604,41 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
         if (tall) SE2_CUDA(cudaLaunchKernelEx(&cfg, orb_resize_w<RESIZE_TR_TALL>, d, g, h->levels[l - 1], h->resize_tall_rows, h->resize_raw_pitch));
         else SE2_CUDA(cudaLaunchKernelEx(&cfg, orb_resize_w<RESIZE_TR>, d, g, h->levels[l - 1], h->resize_rows, h->resize_raw_pitch));
         ::se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed);
-        if (l == splitA - 1 && side && !pr.on) SE2_CUDA(cudaEventRecord(h->ev_l1, s));
     }
-    if (splitA - 1 <= 0 && side && !pr.on) SE2_CUDA(cudaEventRecord(h->ev_l1, s));   // level 0 alone is group A (or there is only one level)
+    // the blur is forked here, behind the whole pyramid (see BLUR_SPLIT); with the profiler on everything stays on one stream
+    // so that the per-kernel event times are not polluted by the overlap
+    if (overlap) SE2_CUDA(cudaEventRecord(ev_pyr, s));
     pr.end(s);
     nvtxRangePop();
-    // The blur of a level only needs that level's plane: on the side stream the blur of group A (no shared memory, so it co-resides
-    // with the resize and FAST CTAs) starts once its last level exists - with BLUR_SPLIT = 1 that is level 0 alone (about a third of
-    // the pixels), behind the whole pyramid, next to FAST; the remaining levels are blurred behind the FAST launch,
-    // next to the selection. The main stream joins before the descriptors are sampled. With the
-    // profiler on everything stays on one stream so that the per-kernel event times are not polluted by the overlap.
-    const bool overlap = !pr.on && side != nullptr;
     auto launch_blur = [&](cudaStream_t st, int t0, int t1) {
         if (t1 > t0) SE2_LAUNCH(orb_blur, dim3((t1 - t0 + BLUR_WARPS - 1) / BLUR_WARPS, n), BLUR_WARPS * 32, 0, st, d, t0, t1);
     };
-    const int tilesA = splitA < h->nlevels ? h->levels[splitA].tile_base : d.n_tiles;
+    const int split = std::min(BLUR_SPLIT, h->nlevels);
+    const int tilesA = split < h->nlevels ? h->levels[split].tile_base : d.n_tiles;
     if (overlap) {
-        SE2_CUDA(cudaStreamWaitEvent(side, h->ev_l1, 0));
-        launch_blur(side, 0, tilesA);
-    }
-    SE2_NVTX("se2gpu.orb.fast_select_blur_describe");
-    pr.begin(1, s);
-    if (h->fast_big) SE2_LAUNCH(orb_fast_cells_big, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d);
-    else if (h->fast_tma) SE2_LAUNCH(orb_fast_cells<true>, dim3(d.n_cells, n), FAST_THREADS, h->fast_tma_smem, s, d, h->fast_maps);
-    else SE2_LAUNCH(orb_fast_cells<false>, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d, h->fast_maps);
-    if (h->harris) SE2_LAUNCH(orb_harris, dim3(d.n_cells, n), HARRIS_THREADS, 0, s, d, h->hb.cand64);   // timed with FAST (group 1)
-    pr.end(s);
-    if (overlap) {      // group B behind FAST in stream order, concurrent with the selection
-        SE2_CUDA(cudaEventRecord(ev_pyr, s));
         SE2_CUDA(cudaStreamWaitEvent(side, ev_pyr, 0));
+        launch_blur(side, 0, tilesA);
         launch_blur(side, tilesA, d.n_tiles);
         SE2_CUDA(cudaEventRecord(ev_blur, side));
     }
+    SE2_NVTX("se2gpu.orb.fast_select_blur_describe");
+    pr.begin(1, s);
+    // FAST is a programmatic dependent of the last resize; orb_fast_cells_big, for cells too large for it, keeps a plain launch
+    if (h->fast_big) SE2_LAUNCH(orb_fast_cells_big, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d);
+    else if (h->fast_tma) SE2_CUDA(launch_pdl(orb_fast_cells<true>, dim3(d.n_cells, n), FAST_THREADS, h->fast_tma_smem, s, d, h->fast_maps));
+    else SE2_CUDA(launch_pdl(orb_fast_cells<false>, dim3(d.n_cells, n), FAST_THREADS, h->fast_smem, s, d, h->fast_maps));
+    if (h->harris) SE2_LAUNCH(orb_harris, dim3(d.n_cells, n), HARRIS_THREADS, 0, s, d, h->hb.cand64);   // timed with FAST (group 1)
+    pr.end(s);
     pr.begin(2, s);
-    if (h->harris) SE2_LAUNCH(orb_select<true>, dim3(h->nlevels, n), SEL_THREADS, h->select_smem, s, d, h->hb);
-    else SE2_LAUNCH(orb_select<false>, dim3(h->nlevels, n), SEL_THREADS, h->select_smem, s, d, h->hb);
+    // frames vary fastest in the CTA order: the CTAs of every frame's first cells (level 0) are dispatched together, first
+    const dim3 sel_grid(n, (d.n_cells + SEL_WARPS - 1) / SEL_WARPS);
+    if (h->harris) {
+        SE2_CUDA(launch_pdl(orb_select_cells<true>, sel_grid, SEL_WARPS * 32, h->select_smem, s, d, h->hb, h->sel_max_cells, h->sel_stage_n));
+        SE2_CUDA(launch_pdl(orb_select_levels<true>, dim3(h->nlevels, n), 32, h->select_levels_smem, s, d, h->hb));
+    } else {
+        SE2_CUDA(launch_pdl(orb_select_cells<false>, sel_grid, SEL_WARPS * 32, h->select_smem, s, d, h->hb, h->sel_max_cells, h->sel_stage_n));
+        SE2_CUDA(launch_pdl(orb_select_levels<false>, dim3(h->nlevels, n), 32, h->select_levels_smem, s, d, h->hb));
+    }
     pr.end(s);
     if (overlap) {
         SE2_CUDA(cudaStreamWaitEvent(s, ev_blur, 0));
@@ -1583,9 +1648,10 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
         pr.end(s);
     }
     const int warps = 8;
+    const dim3 desc_grid((h->nfeatures + warps - 1) / warps, n);
     pr.begin(4, s);
-    if (h->harris) SE2_LAUNCH(orb_orient_describe<true>, dim3((h->nfeatures + warps - 1) / warps, n), warps * 32, 0, s, d, d_kps, d_desc, d_counts, h->hb.lresp);
-    else SE2_LAUNCH(orb_orient_describe<false>, dim3((h->nfeatures + warps - 1) / warps, n), warps * 32, 0, s, d, d_kps, d_desc, d_counts, h->hb.lresp);
+    if (h->harris) SE2_CUDA(launch_pdl(orb_orient_describe<true>, desc_grid, warps * 32, 0, s, d, d_kps, d_desc, d_counts, (const float*)h->hb.lresp));
+    else SE2_CUDA(launch_pdl(orb_orient_describe<false>, desc_grid, warps * 32, 0, s, d, d_kps, d_desc, d_counts, (const float*)h->hb.lresp));
     pr.end(s);
     h->last_n = std::max(h->last_n * (frame0 > 0), frame0 + n);
     return SE2GPU_OK;
@@ -1631,25 +1697,26 @@ se2gpu_orb* se2gpu_orb_create_scored(int nfeatures, float scale_factor, int nlev
     }
     float gk[7];
     { double g[7], s = 0; for (int i = 0; i < 7; ++i) { double x = i - 3; g[i] = std::exp(-0.5 * x * x / 4.0); s += g[i]; } for (int i = 0; i < 7; ++i) gk[i] = (float)(g[i] * (1. / s)); }
-    size_t pb, ct, nc, nt, tt, fsm, ssm;
-    int rc = build_geometry(h, max_w, max_h, true, &pb, &ct, &nc, &nt, &tt, &fsm, &ssm, nullptr, nullptr, nullptr);
+    size_t pb, ct, nc, nt, tt, fsm;
+    int rc = build_geometry(h, max_w, max_h, true, &pb, &ct, &nc, &nt, &tt, &fsm, nullptr, nullptr, nullptr);
     if (rc != SE2GPU_OK) { delete h; return nullptr; }
     // head-room so that smaller frames (different cell rounding) always fit
     h->cap_plane = pb + 4096; h->cap_cand = ct + ct / 8 + 4096; h->cap_cells = nc + 64; h->cap_tiles = nt + 64; h->cap_tab = tt + 64;
     h->cap_lkp = nfeatures + 64;
+    h->cap_sel = 2 * (size_t)nfeatures + 4 * h->cap_cells + 64 * (size_t)nlevels;   // the level lists' sel_cap summed over levels
     const size_t B = max_batch;
     bool ok = true;
     auto A = [&](auto** p, size_t c) { ok = ok && h->bufs.alloc(p, c) == cudaSuccess; };
     OrbDev& d = h->d;
     A(&h->d_levels, (size_t)nlevels); A(&h->d_cells, h->cap_cells); A(&h->d_tiles, h->cap_tiles); A(&h->d_itab, h->cap_tab); A(&h->d_stab, 2 * h->cap_tab);
     A(&d.plain, B * h->cap_plane); A(&d.blurred, B * h->cap_plane);
-    A(&d.cand, B * h->cap_cand); A(&d.hdr, B * h->cap_cells); A(&d.lkp, B * h->cap_lkp); A(&d.lcount, B * nlevels); A(&d.err, 1);
+    A(&d.cand, B * h->cap_cand); A(&d.hdr, B * h->cap_cells); A(&d.lkp, B * h->cap_lkp); A(&d.lcount, B * nlevels); A(&d.sel, B * h->cap_sel); A(&d.err, 1);
     A(&h->d_in, B * (size_t)max_w * max_h); A(&h->d_kps, B * nfeatures); A(&h->d_desc, B * nfeatures * 32); A(&h->d_counts, B);
     if (h->harris) { A(&h->hb.cand64, B * h->cap_cand); A(&h->hb.lresp, B * h->cap_lkp); }
     if (!ok) { fail(SE2GPU_ERR_CUDA, "device allocation failed (%s)", cudaGetErrorString(cudaGetLastError())); se2gpu_orb_destroy(h); return nullptr; }
     cudaMemset(d.err, 0, sizeof(int));
     if (cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_pyr, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->ev_blur, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_l1, cudaEventDisableTiming) != cudaSuccess) { h->side = nullptr; cudaGetLastError(); }
+        cudaEventCreateWithFlags(&h->ev_blur, cudaEventDisableTiming) != cudaSuccess) { h->side = nullptr; cudaGetLastError(); }
     for (int l = 0; l < ORB_LANES && h->side; ++l)
         if (cudaStreamCreateWithFlags(&h->pipe[l], cudaStreamNonBlocking) != cudaSuccess) { h->pipe[l] = nullptr; cudaGetLastError(); break; }
     cudaMemcpyToSymbol(c_umax, umax, sizeof umax);
@@ -1679,7 +1746,6 @@ void se2gpu_orb_destroy(se2gpu_orb* h) {
     if (h->d_und_m1) cudaFree(h->d_und_m1);
     if (h->d_und_m2) cudaFree(h->d_und_m2);
     if (h->ev_blur) cudaEventDestroy(h->ev_blur);
-    if (h->ev_l1) cudaEventDestroy(h->ev_l1);
     if (h->pin_counts) cudaFreeHost(h->pin_counts);
     if (h->pin_kps) cudaFreeHost(h->pin_kps);
     if (h->pin_desc) cudaFreeHost(h->pin_desc);

@@ -6,7 +6,9 @@ usage: orb_pyramid_trace.py OUT_DIR [--steps K] [--warmup W]
 
 Writes OUT_DIR/orb_trace.json (every kernel launch of the traced steps: name, start relative to the step's first kernel,
 duration, in launch order) and OUT_DIR/orb_trace.txt (per kernel name: launches per step, mean duration, and the wall time from
-the step's first pyramid kernel to the end of its last one), and prints the text table."""
+the step's first pyramid kernel to the end of its last one; then the whole step: each launch's mean start and end, the gaps
+across the chain's edges - last resize to FAST, FAST to the selection, selection to the descriptors; a negative gap is a
+launch that began before its predecessor ended - and where the blur launches sit), and prints the text table."""
 from __future__ import annotations
 
 import argparse
@@ -25,6 +27,42 @@ PYRAMID_KERNELS = ("orb_pyr0", "orb_resize")
 def short_name(name: str) -> str:
     name = name.replace("(anonymous namespace)::", "").split("(")[0].replace("void ", "").strip()
     return name.split("::")[-1].split("<")[0]
+
+
+def step_timeline(steps) -> list:
+    """Per launch of a step (in launch order, repeated names numbered): mean start / end in us from the step's first kernel;
+    then the mean gaps across the chain's edges and the step's span."""
+    import numpy as np
+    table, gaps = OrderedDict(), OrderedDict()
+    for s in steps:
+        t0 = s[0].time_range.start
+        seen = {}
+        for e in s:
+            n = short_name(e.name)
+            seen[n] = seen.get(n, 0) + 1
+            key = f"{n} #{seen[n]}" if n.startswith(("orb_resize", "orb_blur")) else n
+            table.setdefault(key, []).append((e.time_range.start - t0, e.time_range.end - t0))
+
+        def first(prefix, last=False):
+            m = [e for e in s if short_name(e.name).startswith(prefix)]
+            return (m[-1] if last else m[0]) if m else None
+        rz, fast, sel0, sel1, desc = (first("orb_resize", True), first("orb_fast_cells"), first("orb_select"),
+                                      first("orb_select", True), first("orb_orient_describe"))
+        for name, a, b in (("last resize end -> FAST start", rz, fast), ("FAST end -> selection start", fast, sel0),
+                           ("selection end -> descriptors start", sel1, desc)):
+            if a is not None and b is not None:
+                gaps.setdefault(name, []).append(b.time_range.start - a.time_range.end)
+        if sel0 is not None and sel1 is not sel0:
+            gaps.setdefault("selection launch 1 end -> launch 2 start", []).append(sel1.time_range.start - sel0.time_range.end)
+        gaps.setdefault("step span (first start..last end)", []).append(max(e.time_range.end for e in s) - t0)
+    out = ["", "whole step, per launch (us from the step's first kernel start)", f"{'launch':32s} {'start':>9s} {'end':>9s}"]
+    for k, v in table.items():
+        a = np.array(v)
+        out.append(f"{k:32s} {a[:, 0].mean():9.1f} {a[:, 1].mean():9.1f}")
+    out += ["", f"{'edge':44s} {'mean us':>9s} {'min us':>9s} {'max us':>9s}"]
+    for k, v in gaps.items():
+        out.append(f"{k:44s} {np.mean(v):9.1f} {np.min(v):9.1f} {np.max(v):9.1f}")
+    return out
 
 
 def main() -> None:
@@ -97,6 +135,7 @@ def main() -> None:
         lines.append(f"{n:32s} {len(v) / max(len(steps), 1):13.1f} {np.mean(v):9.1f} {np.min(v):9.1f} {np.max(v):9.1f}")
     if pyr_span:
         lines.append(f"{'pyramid span (first start..last end)':40s} mean {np.mean(pyr_span):7.1f} us, min {np.min(pyr_span):7.1f}, max {np.max(pyr_span):7.1f}")
+    lines += step_timeline(steps)
     text = "\n".join(lines)
     with open(os.path.join(args.out_dir, "orb_trace.txt"), "w") as f:
         f.write(text + "\n")
