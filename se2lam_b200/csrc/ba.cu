@@ -37,69 +37,16 @@
 #include <vector>
 #include <algorithm>
 
-#include "common.h"
-#include "ba_band.h"
+#include "ba_context.h"
 #include "sym3.h"
+
+using namespace se2ba;
 
 namespace {
 
 using se2gpu::fail;
 
-constexpr int EB = 12;             // doubles per edge record (9 used + padding to 96 B = 3 L2 sectors)
-constexpr int LM_THREADS = 128;   // threads per block in per-landmark kernels
 constexpr int CHOL_THREADS = 512;
-constexpr int SMEM_CHOL_MAX_N = 156;  // ldlt_smem_bytes(n) <= 227 KB, n a multiple of 3
-
-struct Cam {
-    double fx, cx, cy, Rcb[9], tcb[3], delta;
-};
-
-struct LMState {  // device-resident scalars of the LM loop (host mirrors it once per trial)
-    double lambda, ni, chi_cur, chi_before, chi_trial, scale, rho, max_diag;
-    int cur, solve_ok, accepted, trials, terminate, retry, iter, stop_all;   // stop_all: abort flag, OR-ed over the ranks of a sharded run
-    long long epoch;   // sharded persistent kernel: last exchange epoch used (continues across optimize() calls)
-    int error, pad;    // 1: a peer did not show up within the exchange timeout
-};
-
-struct Dev {  // all device pointers of one context (passed by value to kernels)
-    int P, L, E, O, nf, n, nblk;
-    int rank, world;
-    int sbw;   // 0: S dense [n*n]; > 0: S in band storage, row r holds columns r-sbw..r (large windows, ba_band.cu)
-    // two-sided ("twisted") reduced solve of the persistent kernel: pose blocks [0, tw_m0) are eliminated top-down by CTA 0,
-    // blocks [tw_m0 + tw_w, nf) bottom-up by CTA 1, the tw_w separator blocks in between last (tw_m0 == 0: off)
-    int tw_m0, tw_w;
-    const int* tw_cmax1;   // [3 (nf - tw_m0)] envelope of the mirrored bottom part
-    double* tw_buf;        // CTA 1 -> CTA 0: separator Schur complement | rhs | ok; CTA 0 -> CTA 1 at TW_XM: separator solution, mirrored
-    unsigned* tw_flag;     // [0] bottom part ready (sequence number), [1] published separator entries (count), [2] (sequence << 1) | ok
-    // state
-    double* xp[2];
-    double* xl[2];
-    LMState* st;
-    // edges, landmark-sorted
-    const int *e_pose, *e_hidx, *lm_ptr;
-    const double *e_u, *e_v, *e_w00, *e_w01, *e_w11;
-    const int* hidx;
-    // odometry edges
-    const int *o_i, *o_j;
-    const double *o_m, *o_w;  // [3][O], [6][O]
-    // per-edge / per-landmark outputs (SoA, component-major)
-    // per-edge records, array-of-structures with a 96 B stride so that one record is exactly 3 L2 sectors:
-    //   Hpl[e] = 3x3 pose-landmark block; PH[e] = pose-side Hessian (6 unique) + gradient (3); Y[e] = Hpl Hll^-1 (9) + g (3)
-    double *Hpl, *PH, *Y;
-    double *Hll, *bl, *HllInv;            // [6][L] [3][L] [6][L]
-    double *oAii, *oAij, *oAjj, *obi, *obj;  // [6][O] [9][O] [6][O] [3][O] [3][O]
-    // pose-side gathers
-    const int *pose_ptr, *pose_edges, *pose_odo_ptr, *pose_odo;
-    double *Hpp, *bp;                     // [6][nf], [n]
-    // reduced system
-    const int *blk_a, *blk_b, *blk_pair_ptr, *pair_e1, *pair_e2, *blk_odo_ptr, *blk_odo;
-    const int* colmax;                    // [n] envelope of the reduced system (last structurally non-zero row per column)
-    const int* blk_order;                 // [nord] serving order of the persistent kernel: position p belongs to worker p % W; -1 = hole
-    int nord;
-    double *S, *bs, *scal, *dxp, *dxl;    // S [n*n] | bs [n] | scal [8] contiguous (all-reduce buffer)
-    double *part_chi, *part_scale;
-    int nb_lm, nb_odo;
-};
 
 // A per-edge record is 96 bytes (three 32-byte sectors), 32-byte aligned: gathers read it with 16-byte loads - the record gathers of the
 // Schur phase are bound by L1 wavefronts (every lane hits a different record), so halving the load instructions per record halves them.
@@ -694,7 +641,7 @@ struct GmemIO {   // same interface on byte offsets from a global base (reduced 
     static __device__ __forceinline__ void sti2(unsigned long long a, int x, int y) { sti(a, x); sti(a + 4, y); }
 };
 
-// Block LDL^T of the reduced system (see the comment above ldlt_smem_bytes for the algorithm).
+// Block LDL^T of the reduced system (see "Reduced solve, one CTA" above for the algorithm).
 //   ADDR = unsigned (shared window) or unsigned long long (global); aA, aY, aW, aC, aT are the byte addresses of
 //   A [n*n], y [n] (= row n of A when the two are adjacent), W records [8 per pose, 16-byte aligned inside a 9-per-pose area],
 //   cmax (int) [n], scratch {3 unused, ok (int), 2 x 3 back-substitution exchange slots}.
@@ -710,7 +657,6 @@ struct LdltOpt {
     double* pub = nullptr; unsigned* pub_cnt = nullptr; int pub_kb = 0;
     unsigned* okword = nullptr; unsigned okval = 0;     // thread 0 writes okval | ok right after the factorisation
 };
-constexpr int TW_MAX_W = 16;                            // separator blocks
 constexpr int TW_XM = 3 * TW_MAX_W * (3 * TW_MAX_W + 1) + 16;
 constexpr int TW_BUF_DOUBLES = TW_XM + 3 * TW_MAX_W + 16;
 
@@ -916,9 +862,6 @@ __device__ void ldlt_block_solve(double* G, double* ywork, int n, const int* col
         ldlt_block_solve_impl<GmemIO, unsigned long long>(gA, gY, gW, (unsigned long long)colmax_g, gT, n, bs, dxp, st);
     }
 }
-
-// bytes of dynamic shared memory the SMEM variant needs for n unknowns
-__host__ __device__ inline size_t ldlt_smem_bytes(int n) { return ((size_t)n * n + n + 3 * (size_t)n + 2) * 8 + (size_t)n * 4 + 16 + 128; }
 
 // S (n*n doubles, rounded up to 16 B: the tail lands in y, which is initialised afterwards) and the envelope -> shared
 // memory. One elected thread issues a single bulk copy; everybody waits on the mbarrier phase `parity`.
@@ -1139,7 +1082,6 @@ __global__ void __launch_bounds__(256) ba_decide(Dev d, int nb_scale, int phase,
 // CTA from the same fixed-order partial sums, so no host round trip happens inside an optimize() call.
 // Per-landmark work is spread over LPL lanes (edges strided over the lanes, xor-tree over the lane group).
 namespace cg = cooperative_groups;
-constexpr int PK_THREADS = 512;
 constexpr int FALLBACK_CLOCK_KHZ = 1980000;   // H100 SXM maximum SM clock: cycle <-> time conversion if the device does not report one
 
 struct PKArgs {
@@ -1158,7 +1100,6 @@ struct PKArgs {
     double* part_max;         // [gridDim.x]
     long long* phase_cycles;  // [8] SM cycles CTA 0 spent per phase incl. the barrier that ends it (profiling aid)
     int dyn_smem_bytes;       // dynamic shared memory of the launch (arena size of the non-zero CTAs)
-    int dbg_sysfence;         // diagnostic: CTA 0 issues a system-scope fence after every chi2 phase (single-GPU runs)
     long long* cta_work;      // [gridDim.x][8] per-CTA busy cycles per phase (debug aid, null = off)
 };
 
@@ -1288,11 +1229,7 @@ __device__ void pk_phase_linearize(const Dev& d, const Cam& cam, int xi, double*
 // Static work lists of a persistent CTA, cached once per optimize() in its (otherwise unused) dynamic shared memory:
 // the (edge, edge) pair lists of the blocks of S it owns and, for diagonal blocks, the pose's edge list. This removes
 // the dependent L2 round trips for index data from every Schur / pose-gather phase (only the payload is gathered).
-constexpr int PK_MAXOWN = 16;
 struct PKOwn { int blk, a, b, p0, np, e0, ne; };
-constexpr int PK_RED_SCRATCH_BYTES = (PK_THREADS / 32) * 21 * 33 * 8;   // per-warp reduction scratch at the top of a worker's arena
-// dynamic shared memory of the persistent launch: CTA 0's reduced solve, and on worker CTAs pair lists + reduction scratch
-inline size_t pk_dyn_smem_bytes(int n) { return std::max(ldlt_smem_bytes(n), (size_t)160 * 1024); }
 
 // block (a >= b) of the reduced system; pairs interleaved (e1,e2) in `pairs` (shared) or null -> global lists at gp0.
 // Its gather loops are written out rather than calling schur_pairs / schur_odo / schur_pose_sweep: with the shared loops here
@@ -1779,7 +1716,6 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
                 if (threadIdx.x == 0) pa.part_chi[nparts + blockIdx.x] = totc;
             }
             if (blockIdx.x == 0 && threadIdx.x == 0) pa.abort_dev[1] = *pa.abort_host;
-            if (pa.dbg_sysfence && blockIdx.x == 0 && threadIdx.x == 0) __threadfence_system();
             PK_WORK(5);
             grid.sync();
             PK_TICK(5);
@@ -1841,93 +1777,17 @@ __global__ void __launch_bounds__(256) ba_writeback_f32(const double* __restrict
 }  // namespace
 
 // =================================================================================================
-using se2gpu::PinnedArena;
-
-struct se2gpu_ba {
-    PinnedArena* arena = nullptr;   // page-locked staging of set_problem's uploads
-    PinnedArena* arena2 = nullptr;  // page-locked arrays that set_problem builds in place (per-edge and per-pair lists)
-    int device = 0;
-    int maxP = 0, maxL = 0, maxE = 0, maxO = 0, maxN = 0;
-    size_t cap_pairs = 0, cap_blk = 0;
-    cudaStream_t stream = nullptr;
-    int rank = 0, world = 1;
-    se2gpu_allreduce_fn allreduce = nullptr;
-    // sharded persistent kernel: exchange through peer memory (se2gpu_ba_peer_export / _import / _peer_attach_local)
-    double* xch = nullptr;                      // this rank's exchange block: flags + 2 scalar slots (own cudaMalloc: exported by IPC handle)
-    int xslot = 0;                              // doubles per scalar slot
-    double* ssum = nullptr;                     // rank-summed [S | bs]
-    long long* go = nullptr;                    // [2] local hand-off words of pk_wait_peers
-    int* env_idx = nullptr; int nenv = 0; size_t env_cap = 0;   // envelope entries of [S | bs] (what the exchange sums)
-    void* peer_opened[16] = {};                 // mappings opened with cudaIpcOpenMemHandle (closed on destroy)
-    const double* peer_red[8] = {};
-    const double* peer_xch[8] = {};
-    bool peer_on = false;
-    long long peer_epoch = 0;
-    double peer_timeout_s = 10.0;
-    void* ar_user = nullptr;
-    Dev d{};
-    Cam cam{};
-    se2gpu::DeviceBuffers bufs;   // owned device buffers
-    int *e_pose = nullptr, *e_hidx = nullptr, *lm_ptr = nullptr, *hidx = nullptr, *o_i = nullptr, *o_j = nullptr;
-    double *e_u = nullptr, *e_v = nullptr, *e_w00 = nullptr, *e_w01 = nullptr, *e_w11 = nullptr, *o_m = nullptr, *o_w = nullptr;
-    int *pose_ptr = nullptr, *pose_edges = nullptr, *pose_odo_ptr = nullptr, *pose_odo = nullptr;
-    int *blk_a = nullptr, *blk_b = nullptr, *blk_pair_ptr = nullptr, *pair_e1 = nullptr, *pair_e2 = nullptr, *blk_odo_ptr = nullptr, *blk_odo = nullptr;
-    double* red = nullptr;     // all-reduce buffer [maxN*maxN + maxN + 8]
-    double* ywork = nullptr;
-    int* colmax = nullptr;
-    int* tw_cmax1 = nullptr; double* tw_buf = nullptr; unsigned* tw_flag = nullptr;   // twisted reduced solve (persistent kernel)
-    int* blk_order = nullptr;
-    se2gpu_ba_iter_stats* stats_dev = nullptr;
-    int max_stats = 64;
-    LMState* st_host = nullptr;  // pinned
-    std::vector<int> perm;       // sorted edge position -> original edge index
-    int P = 0, L = 0, E = 0, O = 0;
-    int nb_scale = 0;
-    bool loaded = false;
-    double *xp0 = nullptr, *xl0 = nullptr;   // estimates as loaded (se2gpu_ba_reset)
-    se2gpu::Profiler prof;
-    // persistent cooperative path
-    int mode = 0;              // 0 auto, 1 multi-launch, 2 persistent
-    int pk_grid = 0;           // co-resident CTAs (0 = unavailable)
-    double *pk_part_chi = nullptr, *pk_part_scale = nullptr, *pk_part_max = nullptr;
-    int* abort_host = nullptr; int* abort_host_dev = nullptr; int* abort_dev = nullptr;
-    double *trace_p = nullptr, *trace_l = nullptr; size_t trace_cap_p = 0, trace_cap_l = 0;
-    long long* phase_cycles = nullptr;   // device [8]
-    long long* cta_work = nullptr;       // device [1024][8]
-    int pk_launches = 0, clock_khz = 0;
-    // topology of the loaded window (host copies): a set_problem with the same graph structure only refreshes the values
-    std::vector<int> t_edge_pose, t_edge_point, t_odo_i, t_odo_j; std::vector<uint8_t> t_fixed; int t_rank = -1, t_world = -1;
-    se2band::Plan band;        // partitioned band solver for reduced systems beyond one CTA's shared memory
-    int smem_optin = 0;
-    int plan[SE2GPU_BA_PLAN_FIELDS] = {};   // host-side decisions of the last full set_problem (se2gpu_ba_debug_plan)
-};
-
 namespace {
 
-template <class T>
-int upload(T* dst, const std::vector<T>& src, cudaStream_t s) {
-    if (src.empty()) return SE2GPU_OK;
-    SE2_CUDA(cudaMemcpyAsync(dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, s));
-    return SE2GPU_OK;
-}
-
-
-int ensure_cap(se2gpu_ba* h, size_t npairs, size_t nblk, size_t nblk_odo) {
-    if (npairs > h->cap_pairs) {
-        size_t cap = npairs + npairs / 4 + 1024;
-        int *a, *b;
-        if (h->bufs.alloc(&a, cap) != cudaSuccess || h->bufs.alloc(&b, cap) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "pair list alloc failed");
-        h->pair_e1 = a; h->pair_e2 = b; h->cap_pairs = cap;
-    }
-    if (nblk + 1 > h->cap_blk) {
-        size_t cap = nblk + nblk / 4 + 1024;
-        int* p[6];
-        for (int i = 0; i < 6; ++i) if (h->bufs.alloc(&p[i], cap + 1) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "block list alloc failed");
-        h->blk_a = p[0]; h->blk_b = p[1]; h->blk_pair_ptr = p[2]; h->blk_odo_ptr = p[3]; h->blk_odo = p[4]; h->blk_order = p[5];
-        h->cap_blk = cap;
-    }
-    (void)nblk_odo;
-    return SE2GPU_OK;
+// the only place the BA reads the environment
+Switches read_switches() {
+    Switches sw;
+    if (const char* g = getenv("SE2GPU_BA_PK_GRID")) sw.pk_grid_limit = atoi(g);
+    if (const char* t = getenv("SE2GPU_BA_PEER_TIMEOUT_S")) { if (atof(t) > 0) sw.peer_timeout_s = atof(t); }
+    sw.debug = getenv("SE2GPU_BA_DEBUG") != nullptr;
+    sw.no_band = getenv("SE2GPU_BA_NO_BAND") != nullptr;
+    sw.no_twist = getenv("SE2GPU_BA_NO_TWIST") != nullptr;
+    return sw;
 }
 
 }  // namespace
@@ -1940,6 +1800,7 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
     const size_t maxN = 3 * (size_t)max_poses;
     if (maxN * maxN * 8 > (size_t)8 << 30) { fail(SE2GPU_ERR_CAPACITY, "dense reduced system for %d poses exceeds this build's limit", max_poses); return nullptr; }
     se2gpu_ba* h = new se2gpu_ba;
+    h->sw = read_switches();
     h->device = device; h->maxP = max_poses; h->maxL = max_points; h->maxE = max_edges; h->maxO = max_odo; h->maxN = (int)maxN;
     const size_t P = max_poses, L = max_points, E = max_edges, O = max_odo ? max_odo : 1;
     int rc = SE2GPU_OK;
@@ -1948,15 +1809,15 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
         if (rc == SE2GPU_OK && h->bufs.alloc(p, c) != cudaSuccess) rc = fail(SE2GPU_ERR_CUDA, "cudaMalloc of %zu bytes failed", c * sizeof **p);
     };
     A(&d.xp[0], 3 * P); A(&d.xp[1], 3 * P); A(&d.xl[0], 3 * L); A(&d.xl[1], 3 * L); A(&d.st, 1);
-    A(&h->e_pose, E); A(&h->e_hidx, E); A(&h->lm_ptr, L + 1); A(&h->hidx, P);
-    A(&h->e_u, E); A(&h->e_v, E); A(&h->e_w00, E); A(&h->e_w01, E); A(&h->e_w11, E);
-    A(&h->o_i, O); A(&h->o_j, O); A(&h->o_m, 3 * O); A(&h->o_w, 6 * O);
+    A(&d.e_pose, E); A(&d.e_hidx, E); A(&d.lm_ptr, L + 1); A(&d.hidx, P);
+    A(&d.e_u, E); A(&d.e_v, E); A(&d.e_w00, E); A(&d.e_w01, E); A(&d.e_w11, E);
+    A(&d.o_i, O); A(&d.o_j, O); A(&d.o_m, 3 * O); A(&d.o_w, 6 * O);
     A(&d.Hpl, EB * E); A(&d.PH, EB * E); A(&d.Y, EB * E);
     A(&d.Hll, 6 * L); A(&d.bl, 3 * L); A(&d.HllInv, 6 * L);
     A(&d.oAii, 6 * O); A(&d.oAij, 9 * O); A(&d.oAjj, 6 * O); A(&d.obi, 3 * O); A(&d.obj, 3 * O);
-    A(&h->pose_ptr, P + 1); A(&h->pose_edges, E); A(&h->pose_odo_ptr, P + 1); A(&h->pose_odo, 2 * O);
+    A(&d.pose_ptr, P + 1); A(&d.pose_edges, E); A(&d.pose_odo_ptr, P + 1); A(&d.pose_odo, 2 * O);
     A(&d.Hpp, 6 * P); A(&d.bp, 3 * P);
-    A(&h->red, maxN * maxN + maxN + 8); A(&h->ywork, 4 * maxN + 32); A(&h->colmax, maxN); A(&h->tw_cmax1, maxN); A(&h->tw_buf, TW_BUF_DOUBLES); A(&h->tw_flag, 4); A(&d.dxp, maxN); A(&d.dxl, 3 * L);
+    A(&h->red, maxN * maxN + maxN + 8); A(&h->ywork, 4 * maxN + 32); A(&d.colmax, maxN); A(&d.tw_cmax1, maxN); A(&d.tw_buf, TW_BUF_DOUBLES); A(&d.tw_flag, 4); A(&d.dxp, maxN); A(&d.dxl, 3 * L);
     const size_t nb = (L + LM_THREADS - 1) / LM_THREADS + (O + LM_THREADS - 1) / LM_THREADS + (P + LM_THREADS - 1) / LM_THREADS + 4;
     A(&d.part_chi, nb); A(&d.part_scale, nb);
     A(&h->stats_dev, h->max_stats);
@@ -1978,7 +1839,7 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
         if (coop && cudaFuncSetAttribute(ba_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max) == cudaSuccess &&
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ba_persistent, PK_THREADS, smem_max) == cudaSuccess && occ >= 1)
             h->pk_grid = std::min(nsm, 1024);
-        if (const char* g = getenv("SE2GPU_BA_PK_GRID")) { const int lim = atoi(g); if (lim >= 2 && lim < h->pk_grid) h->pk_grid = lim; }   // test hook: several contexts on one GPU
+        if (h->sw.pk_grid_limit >= 2 && h->sw.pk_grid_limit < h->pk_grid) h->pk_grid = h->sw.pk_grid_limit;
         cudaGetLastError();
         if (cudaHostAlloc((void**)&h->abort_host, sizeof(int), cudaHostAllocMapped) != cudaSuccess ||
             cudaHostGetDevicePointer((void**)&h->abort_host_dev, h->abort_host, 0) != cudaSuccess) { h->pk_grid = 0; cudaGetLastError(); }
@@ -1991,18 +1852,14 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
 void se2gpu_ba_destroy(se2gpu_ba* h) {
     if (!h) return;
     cudaSetDevice(h->device);
-    if (h->trace_p) cudaFree(h->trace_p);
-    if (h->trace_l) cudaFree(h->trace_l);
     if (h->abort_host) cudaFreeHost(h->abort_host);
     se2band::release(h->band);
     for (void* m : h->peer_opened) if (m) cudaIpcCloseMemHandle(m);
+    // the peer exchange buffers are separate allocations (peer_alloc: a rank exports them by IPC handle); h->bufs frees the rest
     if (h->xch) cudaFree(h->xch);
     if (h->ssum) cudaFree(h->ssum);
     if (h->go) cudaFree(h->go);
-    if (h->env_idx) cudaFree(h->env_idx);
     if (h->st_host) cudaFreeHost(h->st_host);
-    delete h->arena;
-    delete h->arena2;
     delete h;
 }
 
@@ -2017,7 +1874,6 @@ static int peer_alloc(se2gpu_ba* h) {
     SE2_CUDA(cudaMemset(h->ssum, 0, sizeof(double) * ((size_t)SMEM_CHOL_MAX_N * SMEM_CHOL_MAX_N + SMEM_CHOL_MAX_N + 8)));
     SE2_CUDA(cudaMalloc((void**)&h->go, 2 * sizeof(long long)));
     SE2_CUDA(cudaMemset(h->go, 0, 2 * sizeof(long long)));
-    if (const char* t = getenv("SE2GPU_BA_PEER_TIMEOUT_S")) h->peer_timeout_s = atof(t) > 0 ? atof(t) : h->peer_timeout_s;
     return SE2GPU_OK;
 }
 
@@ -2093,383 +1949,6 @@ int se2gpu_ba_set_shard(se2gpu_ba* h, int rank, int world, se2gpu_allreduce_fn a
     return SE2GPU_OK;
 }
 
-int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, const uint8_t* fixed,
-                          const double* points, const int* edge_pose, const int* edge_point, const double* uv,
-                          const double* info, const int* odo_i, const int* odo_j, const double* odo_meas,
-                          const double* odo_info, double fx, double cx, double cy, const double* Tcb, double huber_delta) {
-    if (!h) return fail(SE2GPU_ERR_INVALID, "null handle");
-    if (P <= 0 || L < 0 || E < 0 || O < 0) return fail(SE2GPU_ERR_INVALID, "bad sizes");
-    SE2_NVTX("se2gpu.ba.set_problem");
-    if (P > h->maxP || L > h->maxL || E > h->maxE || O > h->maxO) return fail(SE2GPU_ERR_CAPACITY, "problem (%d,%d,%d,%d) exceeds capacity (%d,%d,%d,%d)", P, L, E, O, h->maxP, h->maxL, h->maxE, h->maxO);
-    SE2_CUDA(cudaSetDevice(h->device));
-    cudaStream_t s = h->stream;
-    static const bool dbg = getenv("SE2GPU_BA_DEBUG") != nullptr;
-    auto tnow = [] { return std::chrono::steady_clock::now(); };
-    auto t_begin = tnow();
-    for (int e = 0; e < E; ++e)
-        if (edge_pose[e] < 0 || edge_pose[e] >= P || edge_point[e] < 0 || edge_point[e] >= L) return fail(SE2GPU_ERR_INVALID, "edge %d references a missing vertex", e);
-    for (int o = 0; o < O; ++o)
-        if (odo_i[o] < 0 || odo_i[o] >= P || odo_j[o] < 0 || odo_j[o] >= P) return fail(SE2GPU_ERR_INVALID, "odometry edge %d references a missing vertex", o);
-
-    // --- same graph structure as the loaded window (same vertices, fixed flags, edge endpoints, shard): everything
-    // initializeOptimization / buildStructure derives is still valid on the device - only the values are refreshed
-    if (h->loaded && P == h->P && L == h->L && E == h->E && O == h->O && h->t_rank == h->rank && h->t_world == h->world &&
-        (int)h->t_edge_pose.size() == E && (int)h->t_odo_i.size() == O && (int)h->t_fixed.size() == P &&
-        memcmp(h->t_fixed.data(), fixed, P) == 0 && (E == 0 || (memcmp(h->t_edge_pose.data(), edge_pose, sizeof(int) * E) == 0 && memcmp(h->t_edge_point.data(), edge_point, sizeof(int) * E) == 0)) &&
-        (O == 0 || (memcmp(h->t_odo_i.data(), odo_i, sizeof(int) * O) == 0 && memcmp(h->t_odo_j.data(), odo_j, sizeof(int) * O) == 0))) {
-        const int El = h->d.E, Ol = h->d.O;
-        if (!h->arena2) h->arena2 = new PinnedArena;
-        h->arena2->reserve((size_t)El * 40 + (size_t)Ol * 72 + 64 * 16);
-        if (!h->arena) h->arena = new PinnedArena;
-        h->arena->reserve(sizeof(double) * (3 * (size_t)P + 3 * (size_t)L) + (size_t)El * 40 + (size_t)Ol * 72 + 64 * 16);
-        PinnedArena& ar = *h->arena;
-        std::vector<double> fb[7];
-        auto dbls = [&](size_t cnt, std::vector<double>& f) { double* q = h->arena2->alloc<double>(cnt); if (!q) { f.resize(cnt); q = f.data(); } return q; };
-        double *e_u = dbls(El, fb[0]), *e_v = dbls(El, fb[1]), *w00 = dbls(El, fb[2]), *w01 = dbls(El, fb[3]), *w11 = dbls(El, fb[4]);
-        for (int k = 0; k < El; ++k) {
-            const int e = h->perm[k];
-            e_u[k] = uv[2 * e]; e_v[k] = uv[2 * e + 1];
-            w00[k] = info[3 * e]; w01[k] = info[3 * e + 1]; w11[k] = info[3 * e + 2];
-        }
-        double *om = dbls(3 * (size_t)Ol, fb[5]), *ow = dbls(6 * (size_t)Ol, fb[6]);
-        for (int o = 0; o < Ol; ++o) {
-            for (int q = 0; q < 3; ++q) om[q * (size_t)Ol + o] = odo_meas[3 * o + q];
-            for (int q = 0; q < 6; ++q) ow[q * (size_t)Ol + o] = odo_info[6 * o + q];
-        }
-#define UPV(dst, ptr, count) do { int _r = h->arena2->owns(ptr) ? (((size_t)(count)) ? (cudaMemcpyAsync(dst, ptr, sizeof(*(ptr)) * (size_t)(count), cudaMemcpyHostToDevice, s) == cudaSuccess ? SE2GPU_OK : fail(SE2GPU_ERR_CUDA, "upload failed")) : SE2GPU_OK) : ar.up(dst, ptr, (size_t)(count), s); if (_r != SE2GPU_OK) return _r; } while (0)
-        UPV(h->d.xp[0], poses, 3 * (size_t)P); UPV(h->d.xl[0], points, 3 * (size_t)L);
-        SE2_CUDA(cudaMemcpyAsync(h->d.xp[1], h->d.xp[0], sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice, s));
-        SE2_CUDA(cudaMemcpyAsync(h->d.xl[1], h->d.xl[0], sizeof(double) * 3 * L, cudaMemcpyDeviceToDevice, s));
-        SE2_CUDA(cudaMemcpyAsync(h->xp0, h->d.xp[0], sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice, s));
-        SE2_CUDA(cudaMemcpyAsync(h->xl0, h->d.xl[0], sizeof(double) * 3 * L, cudaMemcpyDeviceToDevice, s));
-        UPV(h->e_u, e_u, El); UPV(h->e_v, e_v, El); UPV(h->e_w00, w00, El); UPV(h->e_w01, w01, El); UPV(h->e_w11, w11, El);
-        UPV(h->o_m, om, 3 * (size_t)Ol); UPV(h->o_w, ow, 6 * (size_t)Ol);
-#undef UPV
-        LMState st0{};
-        st0.ni = 2;
-        *h->st_host = st0;
-        SE2_CUDA(cudaMemcpyAsync(h->d.st, h->st_host, sizeof(LMState), cudaMemcpyHostToDevice, s));
-        SE2_CUDA(cudaStreamSynchronize(s));
-        h->cam.fx = fx; h->cam.cx = cx; h->cam.cy = cy; h->cam.delta = huber_delta;
-        memcpy(h->cam.Rcb, Tcb, sizeof(double) * 9); memcpy(h->cam.tcb, Tcb + 9, sizeof(double) * 3);
-        if (dbg) fprintf(stderr, "[se2gpu_ba_set_problem] same topology: values refreshed in %.3f ms\n", std::chrono::duration<double, std::milli>(tnow() - t_begin).count());
-        return SE2GPU_OK;
-    }
-    h->loaded = false;
-
-    // --- index mapping (SparseOptimizer::buildIndexMapping): free poses in id order
-    std::vector<int> hidx(P, -1);
-    int nf = 0;
-    for (int i = 0; i < P; ++i) if (!fixed[i]) hidx[i] = nf++;
-    const int n = 3 * nf;
-    // --- shard: this rank keeps the edges of landmarks j % world == rank; odometry lives on rank 0
-    const int world = h->world, rank = h->rank;
-    std::vector<int> lm_ptr(L + 1, 0);
-    for (int e = 0; e < E; ++e) if (edge_point[e] % world == rank) lm_ptr[edge_point[e] + 1]++;
-    for (int j = 0; j < L; ++j) lm_ptr[j + 1] += lm_ptr[j];
-    const int El = lm_ptr[L];
-    std::vector<int> perm(El), cursor(lm_ptr.begin(), lm_ptr.end() - 1);
-    for (int e = 0; e < E; ++e) if (edge_point[e] % world == rank) perm[cursor[edge_point[e]]++] = e;
-    const int Ol = (rank == 0) ? O : 0;
-    // the per-edge and per-pair arrays are built directly in page-locked memory (no staging copy before the upload)
-    size_t pair_bound = 0;
-    for (int j = 0; j < L; ++j) { const size_t k = (size_t)(lm_ptr[j + 1] - lm_ptr[j]); pair_bound += k * (k + 1) / 2; }
-    if (!h->arena2) h->arena2 = new PinnedArena;
-    h->arena2->reserve((size_t)El * 48 + pair_bound * 8 + 64 * 16);
-    std::vector<int> fb_i[4];
-    std::vector<double> fb_d[5];
-    auto ints = [&](size_t cnt, std::vector<int>& fb) { int* q = h->arena2->alloc<int>(cnt); if (!q) { fb.resize(cnt); q = fb.data(); } return q; };
-    auto dbls = [&](size_t cnt, std::vector<double>& fb) { double* q = h->arena2->alloc<double>(cnt); if (!q) { fb.resize(cnt); q = fb.data(); } return q; };
-    int *e_pose = ints(El, fb_i[0]), *e_hidx = ints(El, fb_i[1]);
-    double *e_u = dbls(El, fb_d[0]), *e_v = dbls(El, fb_d[1]), *w00 = dbls(El, fb_d[2]), *w01 = dbls(El, fb_d[3]), *w11 = dbls(El, fb_d[4]);
-    for (int k = 0; k < El; ++k) {
-        const int e = perm[k];
-        e_pose[k] = edge_pose[e]; e_hidx[k] = hidx[edge_pose[e]];
-        e_u[k] = uv[2 * e]; e_v[k] = uv[2 * e + 1];
-        w00[k] = info[3 * e]; w01[k] = info[3 * e + 1]; w11[k] = info[3 * e + 2];
-    }
-    // --- pose CSR over sorted edges, and over odometry edges (code = 2*o + role)
-    std::vector<int> pose_ptr(nf + 1, 0), pose_edges;
-    for (int k = 0; k < El; ++k) if (e_hidx[k] >= 0) pose_ptr[e_hidx[k] + 1]++;
-    for (int a = 0; a < nf; ++a) pose_ptr[a + 1] += pose_ptr[a];
-    pose_edges.resize(pose_ptr[nf]);
-    { std::vector<int> cur(pose_ptr.begin(), pose_ptr.end() - 1); for (int k = 0; k < El; ++k) if (e_hidx[k] >= 0) pose_edges[cur[e_hidx[k]]++] = k; }
-    std::vector<int> pose_odo_ptr(nf + 1, 0), pose_odo;
-    for (int o = 0; o < Ol; ++o) { if (hidx[odo_i[o]] >= 0) pose_odo_ptr[hidx[odo_i[o]] + 1]++; if (hidx[odo_j[o]] >= 0) pose_odo_ptr[hidx[odo_j[o]] + 1]++; }
-    for (int a = 0; a < nf; ++a) pose_odo_ptr[a + 1] += pose_odo_ptr[a];
-    pose_odo.resize(pose_odo_ptr[nf]);
-    { std::vector<int> cur(pose_odo_ptr.begin(), pose_odo_ptr.end() - 1);
-      for (int o = 0; o < Ol; ++o) { int a = hidx[odo_i[o]], b = hidx[odo_j[o]]; if (a >= 0) pose_odo[cur[a]++] = 2 * o; if (b >= 0) pose_odo[cur[b]++] = 2 * o + 1; } }
-    // --- structure of the reduced system (BlockSolver::buildStructure): blocks (a>=b) touched by co-observation or odometry
-    // The (edge, edge) pair list of every block, blocks in key order (a*nf + b), pairs inside a block in landmark
-    // order: a stable counting sort over a dense nf x nf table when that is small, a comparison sort otherwise.
-    struct OdoB { long long key; int code; };
-    std::vector<OdoB> odob;
-    for (int o = 0; o < Ol; ++o) {
-        const int a = hidx[odo_i[o]], b = hidx[odo_j[o]];
-        if (a < 0 || b < 0 || a == b) continue;
-        // oAij has rows = vertex i, cols = vertex j; the stored block has rows = max index
-        if (a > b) odob.push_back({(long long)a * nf + b, 2 * o});
-        else odob.push_back({(long long)b * nf + a, 2 * o + 1});
-    }
-    std::stable_sort(odob.begin(), odob.end(), [](const OdoB& x, const OdoB& y) { return x.key < y.key; });
-    std::vector<long long> keys;
-    int *pe1 = nullptr, *pe2 = nullptr;
-    std::vector<int> blk_pair_ptr;
-    size_t npairs = 0;
-    if ((size_t)nf * nf <= ((size_t)1 << 22)) {
-        std::vector<int> cnt((size_t)nf * nf, 0);
-        std::vector<uint8_t> used((size_t)nf * nf, 0);
-        for (int j = 0; j < L; ++j)
-            for (int k1 = lm_ptr[j]; k1 < lm_ptr[j + 1]; ++k1) {
-                const int a = e_hidx[k1];
-                if (a < 0) continue;
-                for (int k2 = lm_ptr[j]; k2 < lm_ptr[j + 1]; ++k2) {
-                    const int b = e_hidx[k2];
-                    if (b >= 0 && b <= a) { cnt[(size_t)a * nf + b]++; ++npairs; }
-                }
-            }
-        for (int a = 0; a < nf; ++a) used[(size_t)a * nf + a] = 1;
-        for (auto& p : odob) used[(size_t)p.key] = 1;
-        size_t run = 0;
-        for (size_t k = 0; k < cnt.size(); ++k) {
-            const int c = cnt[k];
-            if (c || used[k]) { keys.push_back((long long)k); blk_pair_ptr.push_back((int)run); }
-            cnt[k] = (int)run;     // becomes the fill cursor of block k
-            run += c;
-        }
-        blk_pair_ptr.push_back((int)run);
-        pe1 = ints(npairs, fb_i[2]); pe2 = ints(npairs, fb_i[3]);
-        for (int j = 0; j < L; ++j)
-            for (int k1 = lm_ptr[j]; k1 < lm_ptr[j + 1]; ++k1) {
-                const int a = e_hidx[k1];
-                if (a < 0) continue;
-                for (int k2 = lm_ptr[j]; k2 < lm_ptr[j + 1]; ++k2) {
-                    const int b = e_hidx[k2];
-                    if (b >= 0 && b <= a) { const int at = cnt[(size_t)a * nf + b]++; pe1[at] = k1; pe2[at] = k2; }
-                }
-            }
-    } else {
-        struct Pair { long long key; int e1, e2; };
-        std::vector<Pair> pairs;
-        pairs.reserve((size_t)El * 4);
-        for (int j = 0; j < L; ++j)
-            for (int k1 = lm_ptr[j]; k1 < lm_ptr[j + 1]; ++k1) {
-                const int a = e_hidx[k1];
-                if (a < 0) continue;
-                for (int k2 = lm_ptr[j]; k2 < lm_ptr[j + 1]; ++k2) {
-                    const int b = e_hidx[k2];
-                    if (b < 0 || b > a) continue;
-                    pairs.push_back({(long long)a * nf + b, k1, k2});
-                }
-            }
-        std::stable_sort(pairs.begin(), pairs.end(), [](const Pair& x, const Pair& y) { return x.key < y.key; });
-        npairs = pairs.size();
-        for (int a = 0; a < nf; ++a) keys.push_back((long long)a * nf + a);
-        for (auto& p : pairs) keys.push_back(p.key);
-        for (auto& p : odob) keys.push_back(p.key);
-        std::sort(keys.begin(), keys.end());
-        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
-        pe1 = ints(npairs, fb_i[2]); pe2 = ints(npairs, fb_i[3]);
-        blk_pair_ptr.assign(keys.size() + 1, 0);
-        size_t ip = 0;
-        for (size_t b = 0; b < keys.size(); ++b) {
-            blk_pair_ptr[b] = (int)ip;
-            while (ip < npairs && pairs[ip].key == keys[b]) { pe1[ip] = pairs[ip].e1; pe2[ip] = pairs[ip].e2; ++ip; }
-        }
-        blk_pair_ptr[keys.size()] = (int)ip;
-    }
-    const int nblk = (int)keys.size();
-    std::vector<int> blk_a(nblk), blk_b(nblk), blk_odo_ptr(nblk + 1, 0), blk_odo(odob.size());
-    { size_t io = 0;
-      for (int b = 0; b < nblk; ++b) {
-          blk_a[b] = (int)(keys[b] / nf); blk_b[b] = (int)(keys[b] % nf);
-          blk_odo_ptr[b] = (int)io;
-          while (io < odob.size() && odob[io].key == keys[b]) { blk_odo[io] = odob[io].code; ++io; }
-      }
-      blk_odo_ptr[nblk] = (int)io; }
-    if (odob.size() + 1 > (size_t)2 * (h->maxO ? h->maxO : 1) + 1) return fail(SE2GPU_ERR_CAPACITY, "too many odometry blocks");
-    // envelope of the reduced system: last block row touching each block column, made monotone so that the
-    // fill-in of an LDL^T without pivoting stays inside it; in sharded mode every rank needs the envelope of the
-    // SUMMED system, i.e. of all landmarks, so it is rebuilt here from the unsharded edge list
-    std::vector<int> bmax(nf);
-    for (int a = 0; a < nf; ++a) bmax[a] = a;
-    {
-        std::vector<int> lo(L, nf), hi(L, -1);
-        for (int e = 0; e < E; ++e) { const int a = hidx[edge_pose[e]]; if (a < 0) continue; const int j = edge_point[e]; lo[j] = std::min(lo[j], a); hi[j] = std::max(hi[j], a); }
-        for (int j = 0; j < L; ++j) if (hi[j] >= 0) bmax[lo[j]] = std::max(bmax[lo[j]], hi[j]);
-        for (int o = 0; o < O; ++o) { const int a = hidx[odo_i[o]], b = hidx[odo_j[o]]; if (a < 0 || b < 0) continue; bmax[std::min(a, b)] = std::max(bmax[std::min(a, b)], std::max(a, b)); }
-        for (int a = 1; a < nf; ++a) bmax[a] = std::max(bmax[a], bmax[a - 1]);
-    }
-    std::vector<int> colmax(n);
-    for (int a = 0; a < nf; ++a) for (int r = 0; r < 3; ++r) colmax[3 * a + r] = 3 * bmax[a] + 2;
-    // sharded persistent kernel: the entries of [S | bs] the ranks exchange = lower triangle inside the envelope + right-hand side
-    std::vector<int> env_idx;
-    if (world > 1 && n <= SMEM_CHOL_MAX_N) {
-        for (int c = 0; c < n; ++c) for (int r = c; r <= colmax[c]; ++r) env_idx.push_back(r * n + c);
-        for (int r = 0; r < n; ++r) env_idx.push_back(n * n + r);
-        if (env_idx.size() > h->env_cap) {
-            if (h->env_idx) cudaFree(h->env_idx);
-            h->env_cap = env_idx.size() + env_idx.size() / 4 + 64;
-            if (cudaMalloc((void**)&h->env_idx, sizeof(int) * h->env_cap) != cudaSuccess) return fail(SE2GPU_ERR_CUDA, "envelope list alloc failed");
-        }
-        SE2_CUDA(cudaMemcpyAsync(h->env_idx, env_idx.data(), sizeof(int) * env_idx.size(), cudaMemcpyHostToDevice, s));
-        SE2_CUDA(cudaStreamSynchronize(s));
-    }
-    h->nenv = (int)env_idx.size();
-    if (h->ssum) SE2_CUDA(cudaMemsetAsync(h->ssum, 0, sizeof(double) * ((size_t)SMEM_CHOL_MAX_N * SMEM_CHOL_MAX_N + SMEM_CHOL_MAX_N + 8), s));   // zero outside the (new) envelope
-    // windows beyond one CTA's shared memory: partitioned band factorisation when the envelope is narrow (ba_band.cu),
-    // otherwise the single-CTA global-memory envelope factorisation
-    se2band::release(h->band);
-    if (n > SMEM_CHOL_MAX_N && !getenv("SE2GPU_BA_NO_BAND")) se2band::plan(h->band, nf, bmax, h->smem_optin);
-    const size_t S_elems = h->band.active ? h->band.band_elems : (size_t)n * n;
-    // serving order of the blocks for the persistent kernel: diagonal blocks (they also carry the pose-side gather) first,
-    // so that round-robin assignment gives every worker CTA at most one of them
-    // Longest-processing-time assignment: blocks by decreasing work (pairs + pose-side edges of a diagonal block) to the least
-    // loaded worker, at most 12 blocks per worker (the concurrent Schur phase gives every owned block its own warp group).
-    // Worker w serves positions w, w + W, w + 2W, ...; unused trailing positions are holes (-1).
-    // two-sided solve plan: split point m0 with separator w = bmax[m0-1] - m0 + 1 blocks (bmax is monotone), chain max(m0, m1) + w
-    int tw_m0 = 0, tw_w = 0;
-    std::vector<int> tw_cmax1;
-    if (n <= SMEM_CHOL_MAX_N && nf >= 16 && h->pk_grid >= 4 && !getenv("SE2GPU_BA_NO_TWIST")) {
-        int best = nf;
-        for (int m0 = 1; m0 < nf; ++m0) {
-            const int w = bmax[m0 - 1] - m0 + 1, m1 = nf - m0 - w;
-            if (w < 1 || w > TW_MAX_W || m1 < 1) continue;
-            const int chain = std::max(m0, m1 + 4) + w;            // + 4: the bottom part is staged element-wise, not by one bulk copy (~4 pivot steps)
-            if (chain < best) { best = chain; tw_m0 = m0; tw_w = w; }
-        }
-        if (best * 4 > nf * 3) tw_m0 = tw_w = 0;                  // not worth two hand-overs
-        if (tw_m0 > 0) {
-            // envelope of the index-reversed bottom part: block column b' <-> global block row R = nf-1-b', reaching up to the
-            // first block column whose envelope contains R
-            const int nb1 = nf - tw_m0;
-            std::vector<int> rminb(nf);
-            for (int R = 0, C = 0; R < nf; ++R) { while (bmax[C] < R) ++C; rminb[R] = C; }
-            tw_cmax1.resize(3 * (size_t)nb1);
-            for (int b = 0; b < nb1; ++b) {
-                int cb = std::min(nf - 1 - rminb[nf - 1 - b], nb1 - 1);
-                if (b >= nb1 - tw_w) cb = nb1 - 1;
-                for (int r = 0; r < 3; ++r) tw_cmax1[3 * b + r] = 3 * cb + 2;
-            }
-        }
-    }
-    std::vector<int> blk_order;
-    {
-        const int W = h->pk_grid > 1 ? h->pk_grid - (tw_m0 > 0 ? 2 : 1) : 1;
-        std::vector<std::pair<long long, int>> byw(nblk);
-        for (int b = 0; b < nblk; ++b) {
-            long long wt = blk_pair_ptr[b + 1] - blk_pair_ptr[b] + 8;
-            if (blk_a[b] == blk_b[b]) wt += pose_ptr[blk_a[b] + 1] - pose_ptr[blk_a[b]];
-            byw[b] = {-wt, b};
-        }
-        std::sort(byw.begin(), byw.end());
-        std::vector<std::vector<int>> lists(W);
-        std::vector<long long> load(W, 0);
-        const size_t cap = std::max<size_t>(12, (nblk + W - 1) / W);
-        for (auto& it : byw) {
-            int best = -1;
-            for (int w2 = 0; w2 < W; ++w2) if (lists[w2].size() < cap && (best < 0 || load[w2] < load[best])) best = w2;
-            lists[best].push_back(it.second); load[best] += -it.first;
-        }
-        size_t maxlen = 0;
-        for (auto& l : lists) maxlen = std::max(maxlen, l.size());
-        blk_order.assign((size_t)W * maxlen, -1);
-        for (int w2 = 0; w2 < W; ++w2) for (size_t i = 0; i < lists[w2].size(); ++i) blk_order[i * W + w2] = lists[w2][i];
-        // workers whose blocks do not all fit the shared-memory cache (the rule of ba_persistent's prologue): they run the
-        // sequential Schur sweep over pair lists in global memory
-        const int arena_ints = (int)(pk_dyn_smem_bytes(n) - PK_RED_SCRATCH_BYTES) / 4;
-        int uncached = 0;
-        for (auto& l : lists) {
-            int off = 0, no = 0;
-            for (int b : l) {
-                const int np = blk_pair_ptr[b + 1] - blk_pair_ptr[b], ne = blk_a[b] == blk_b[b] ? pose_ptr[blk_a[b] + 1] - pose_ptr[blk_a[b]] : 0;
-                if (no >= PK_MAXOWN || off + 2 * np + ne > arena_ints) break;
-                off += 2 * np + ne; ++no;
-            }
-            if (no < (int)l.size()) ++uncached;
-        }
-        int* pl = h->plan;
-        pl[0] = nf; pl[1] = n; pl[2] = (size_t)nf * nf <= ((size_t)1 << 22) ? 0 : 1;
-        pl[3] = 0; for (int a = 0; a < nf; ++a) pl[3] = std::max(pl[3], bmax[a] - a);
-        pl[4] = n <= SMEM_CHOL_MAX_N ? (tw_m0 > 0 ? 1 : 0) : (h->band.active ? 2 : 3);
-        pl[5] = tw_m0; pl[6] = tw_w; pl[7] = h->band.active ? h->band.w : 0; pl[8] = h->band.active ? h->band.p : 0;
-        pl[9] = h->pk_grid; pl[10] = W; pl[11] = nblk; pl[12] = (int)maxlen; pl[13] = uncached;
-    }
-    int rc = ensure_cap(h, npairs, std::max<size_t>(std::max<size_t>(nblk, blk_order.size()), odob.size()), odob.size());
-    if (rc != SE2GPU_OK) return rc;
-
-    // --- odometry SoA
-    std::vector<int> oi(Ol), oj(Ol);
-    std::vector<double> om(3 * (size_t)Ol), ow(6 * (size_t)Ol);
-    for (int o = 0; o < Ol; ++o) {
-        oi[o] = odo_i[o]; oj[o] = odo_j[o];
-        for (int q = 0; q < 3; ++q) om[q * (size_t)Ol + o] = odo_meas[3 * o + q];
-        for (int q = 0; q < 6; ++q) ow[q * (size_t)Ol + o] = odo_info[6 * o + q];
-    }
-    auto t_host = tnow();
-    // --- upload (staged through the page-locked arena, one synchronisation at the end)
-    if (!h->arena) h->arena = new PinnedArena;
-    {
-        size_t bytes = sizeof(double) * (3 * (size_t)P + 3 * (size_t)L) + 64 * 40;
-        bytes += sizeof(int) * (lm_ptr.size() + hidx.size() + oi.size() + oj.size() + pose_ptr.size() + pose_edges.size() +
-                                pose_odo_ptr.size() + pose_odo.size() + blk_a.size() + blk_b.size() + blk_pair_ptr.size() +
-                                blk_odo_ptr.size() + blk_odo.size() + colmax.size() + tw_cmax1.size() + blk_order.size());
-        bytes += sizeof(double) * (om.size() + ow.size());
-        if (!fb_i[0].empty()) bytes += (size_t)El * 48 + npairs * 8;   // arena2 unavailable: those arrays are staged too
-        h->arena->reserve(bytes);   // on failure the uploads fall back to pageable copies
-    }
-    PinnedArena& ar = *h->arena;
-    // arrays that already live in page-locked memory are uploaded in place, everything else is staged through `ar`
-#define UPP(dst, ptr, count) do { int _r = h->arena2->owns(ptr) ? (((size_t)(count)) ? (cudaMemcpyAsync(dst, ptr, sizeof(*(ptr)) * (size_t)(count), cudaMemcpyHostToDevice, s) == cudaSuccess ? SE2GPU_OK : fail(SE2GPU_ERR_CUDA, "upload failed")) : SE2GPU_OK) : ar.up(dst, ptr, (size_t)(count), s); if (_r != SE2GPU_OK) return _r; } while (0)
-#define UP(dst, src) UPP(dst, (src).data(), (src).size())
-    UPP(h->d.xp[0], poses, 3 * (size_t)P); UPP(h->d.xl[0], points, 3 * (size_t)L);
-    SE2_CUDA(cudaMemcpyAsync(h->d.xp[1], h->d.xp[0], sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice, s));
-    SE2_CUDA(cudaMemcpyAsync(h->d.xl[1], h->d.xl[0], sizeof(double) * 3 * L, cudaMemcpyDeviceToDevice, s));
-    SE2_CUDA(cudaMemcpyAsync(h->xp0, h->d.xp[0], sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice, s));
-    SE2_CUDA(cudaMemcpyAsync(h->xl0, h->d.xl[0], sizeof(double) * 3 * L, cudaMemcpyDeviceToDevice, s));
-    UPP(h->e_pose, e_pose, El); UPP(h->e_hidx, e_hidx, El); UP(h->lm_ptr, lm_ptr); UP(h->hidx, hidx);
-    UPP(h->e_u, e_u, El); UPP(h->e_v, e_v, El); UPP(h->e_w00, w00, El); UPP(h->e_w01, w01, El); UPP(h->e_w11, w11, El);
-    UP(h->o_i, oi); UP(h->o_j, oj); UP(h->o_m, om); UP(h->o_w, ow);
-    UP(h->pose_ptr, pose_ptr); UP(h->pose_edges, pose_edges); UP(h->pose_odo_ptr, pose_odo_ptr); UP(h->pose_odo, pose_odo);
-    UP(h->blk_a, blk_a); UP(h->blk_b, blk_b); UP(h->blk_pair_ptr, blk_pair_ptr); UPP(h->pair_e1, pe1, npairs); UPP(h->pair_e2, pe2, npairs);
-    UP(h->blk_odo_ptr, blk_odo_ptr); UP(h->blk_odo, blk_odo); UP(h->colmax, colmax); UP(h->tw_cmax1, tw_cmax1); UP(h->blk_order, blk_order);
-#undef UP
-#undef UPP
-    SE2_CUDA(cudaMemsetAsync(h->red, 0, sizeof(double) * (S_elems + n + 8), s));
-    LMState st0{};
-    st0.ni = 2;
-    *h->st_host = st0;
-    SE2_CUDA(cudaMemcpyAsync(h->d.st, h->st_host, sizeof(LMState), cudaMemcpyHostToDevice, s));
-    auto t_enq = tnow();
-    SE2_CUDA(cudaStreamSynchronize(s));
-    if (dbg) {
-        auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-        fprintf(stderr, "[se2gpu_ba_set_problem] host structure %.3f ms, stage+enqueue %.3f ms, drain %.3f ms (P %d L %d E %d blocks %d pairs %zu)\n",
-                ms(t_begin, t_host), ms(t_host, t_enq), ms(t_enq, tnow()), P, L, E, nblk, npairs);
-    }
-
-    Dev& d = h->d;
-    d.P = P; d.L = L; d.E = El; d.O = Ol; d.nf = nf; d.n = n; d.nblk = nblk; d.rank = rank; d.world = world;
-    d.e_pose = h->e_pose; d.e_hidx = h->e_hidx; d.lm_ptr = h->lm_ptr; d.hidx = h->hidx;
-    d.e_u = h->e_u; d.e_v = h->e_v; d.e_w00 = h->e_w00; d.e_w01 = h->e_w01; d.e_w11 = h->e_w11;
-    d.o_i = h->o_i; d.o_j = h->o_j; d.o_m = h->o_m; d.o_w = h->o_w;
-    d.pose_ptr = h->pose_ptr; d.pose_edges = h->pose_edges; d.pose_odo_ptr = h->pose_odo_ptr; d.pose_odo = h->pose_odo;
-    d.blk_a = h->blk_a; d.blk_b = h->blk_b; d.blk_pair_ptr = h->blk_pair_ptr; d.pair_e1 = h->pair_e1; d.pair_e2 = h->pair_e2;
-    d.blk_odo_ptr = h->blk_odo_ptr; d.blk_odo = h->blk_odo; d.colmax = h->colmax; d.blk_order = h->blk_order; d.nord = (int)blk_order.size();
-    d.tw_m0 = tw_m0; d.tw_w = tw_w; d.tw_cmax1 = h->tw_cmax1; d.tw_buf = h->tw_buf; d.tw_flag = h->tw_flag;
-    d.S = h->red; d.bs = h->red + S_elems; d.scal = d.bs + n; d.sbw = h->band.active ? h->band.bw : 0;
-    d.nb_lm = (L + LM_THREADS - 1) / LM_THREADS; d.nb_odo = (Ol + LM_THREADS - 1) / LM_THREADS;
-    h->nb_scale = (std::max(L, P) + LM_THREADS - 1) / LM_THREADS;
-    h->cam.fx = fx; h->cam.cx = cx; h->cam.cy = cy; h->cam.delta = huber_delta;
-    memcpy(h->cam.Rcb, Tcb, sizeof(double) * 9); memcpy(h->cam.tcb, Tcb + 9, sizeof(double) * 3);
-    h->perm = perm; h->P = P; h->L = L; h->E = E; h->O = O;
-    h->t_edge_pose.assign(edge_pose, edge_pose + E); h->t_edge_point.assign(edge_point, edge_point + E); h->t_odo_i.assign(odo_i, odo_i + O);
-    h->t_odo_j.assign(odo_j, odo_j + O); h->t_fixed.assign(fixed, fixed + P); h->t_rank = h->rank; h->t_world = h->world;
-    h->loaded = true;
-    return SE2GPU_OK;
-}
-
 }  // extern "C"
 
 namespace {
@@ -2494,27 +1973,43 @@ int launch_linearize(se2gpu_ba* h) {
     return SE2GPU_OK;
 }
 
-int launch_solve(se2gpu_ba* h) {
-    SE2_NVTX("se2gpu.ba.schur_solve");
+// elements of S as stored: dense for small windows, the band for large ones
+size_t stored_S_elems(const se2gpu_ba* h) { return h->band.active ? h->band.band_elems : (size_t)h->d.n * h->d.n; }
+
+// damping-dependent landmark terms at the current lambda, then this rank's reduced system [S | bs]
+int launch_schur(se2gpu_ba* h) {
     Dev& d = h->d;
     cudaStream_t s = h->stream;
     h->prof.begin(2, s);
     if (d.nb_lm > 0) SE2_LAUNCH(ba_lm_prep, d.nb_lm, LM_THREADS, 0, s, d);
     h->prof.end(s);
     // the global-memory Cholesky factorises S in place (fill-in outside the block list): re-zero it
-    const size_t S_elems = h->band.active ? h->band.band_elems : (size_t)d.n * d.n;
-    if (d.n > SMEM_CHOL_MAX_N) SE2_CUDA(cudaMemsetAsync(d.S, 0, sizeof(double) * S_elems, s));
+    if (d.n > SMEM_CHOL_MAX_N) SE2_CUDA(cudaMemsetAsync(d.S, 0, sizeof(double) * stored_S_elems(h), s));
     h->prof.begin(3, s);
     if (d.nblk > 0) SE2_LAUNCH(ba_schur, d.nblk, SCHUR_THREADS, 0, s, d);
     h->prof.end(s);
-    int rc = ar(h, d.S, S_elems + d.n, 0);     // the message is the stored pattern: dense for small windows, the band for large ones
-    if (rc != SE2GPU_OK) return rc;
+    return SE2GPU_OK;
+}
+
+// S dx_p = bs by the solver the window's size and envelope selected
+int launch_reduced_solve(se2gpu_ba* h) {
+    Dev& d = h->d;
+    cudaStream_t s = h->stream;
+    int rc = SE2GPU_OK;
     h->prof.begin(4, s);
     if (d.n <= SMEM_CHOL_MAX_N) SE2_LAUNCH(ba_chol_solve_smem, 1, CHOL_THREADS, ldlt_smem_bytes(d.n), s, d);   // n == 0: trivially ok
     else if (h->band.active) { if ((rc = se2band::solve(h->band, d.S, d.bs, d.dxp, &d.st->solve_ok, s)) != SE2GPU_OK) return rc; }
     else SE2_LAUNCH(ba_chol_solve_gmem, 1, CHOL_THREADS, 0, s, d, h->ywork);
     h->prof.end(s);
     return SE2GPU_OK;
+}
+
+int launch_solve(se2gpu_ba* h) {
+    SE2_NVTX("se2gpu.ba.schur_solve");
+    int rc = launch_schur(h);
+    if (rc != SE2GPU_OK) return rc;
+    if ((rc = ar(h, h->d.S, stored_S_elems(h) + h->d.n, 0)) != SE2GPU_OK) return rc;     // the message is the stored pattern
+    return launch_reduced_solve(h);
 }
 
 }  // namespace
@@ -2541,15 +2036,16 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
         if (max_iters == 0) return 0;
         if (h->world == 1 && stop_flag && *stop_flag) return 0;      // sharded: the kernel takes the decision collectively
         // the whole optimize() is ONE cooperative launch; the host only forwards the abort flag while it runs
+        // (a trace buffer that is replaced is idle: the launch that wrote it was waited for before optimize returned)
         if (trace_poses && h->trace_cap_p < (size_t)max_iters * 3 * h->P) {
-            if (h->trace_p) cudaFree(h->trace_p);
+            h->trace_cap_p = 0;
+            SE2_CUDA(h->bufs.regrow(&h->trace_p, (size_t)max_iters * 3 * h->P));
             h->trace_cap_p = (size_t)max_iters * 3 * h->P;
-            SE2_CUDA(cudaMalloc((void**)&h->trace_p, h->trace_cap_p * sizeof(double)));
         }
         if (trace_points && h->trace_cap_l < (size_t)max_iters * 3 * h->L) {
-            if (h->trace_l) cudaFree(h->trace_l);
+            h->trace_cap_l = 0;
+            SE2_CUDA(h->bufs.regrow(&h->trace_l, (size_t)max_iters * 3 * h->L));
             h->trace_cap_l = (size_t)max_iters * 3 * h->L;
-            SE2_CUDA(cudaMalloc((void**)&h->trace_l, h->trace_cap_l * sizeof(double)));
         }
         *h->abort_host = (stop_flag && *stop_flag) ? 1 : 0;
         PKShard shd{};
@@ -2558,11 +2054,11 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
             for (int r = 0; r < h->world; ++r) { shd.red[r] = h->peer_red[r]; shd.xch[r] = h->peer_xch[r]; }
             shd.my_xch = h->xch; shd.ssum = h->ssum; shd.go = h->go; shd.epoch0 = h->peer_epoch; shd.xslot = h->xslot;
             shd.env_idx = h->env_idx; shd.nenv = h->nenv;
-            shd.timeout_cycles = (long long)(h->peer_timeout_s * 1e3 * (double)(h->clock_khz > 0 ? h->clock_khz : FALLBACK_CLOCK_KHZ));
+            shd.timeout_cycles = (long long)(h->sw.peer_timeout_s * 1e3 * (double)(h->clock_khz > 0 ? h->clock_khz : FALLBACK_CLOCK_KHZ));
             SE2_CUDA(cudaMemsetAsync(h->go, 0, 2 * sizeof(long long), s));
         }
         PKArgs pa{max_iters, first_iteration, h->stats_dev, trace_poses ? h->trace_p : nullptr, trace_points ? h->trace_l : nullptr,
-                  h->abort_host_dev, h->abort_dev, h->pk_part_chi, h->pk_part_scale, h->pk_part_max, h->prof.on ? h->phase_cycles : nullptr, 0, getenv("SE2GPU_BA_DEBUG_SYSFENCE") ? 1 : 0, getenv("SE2GPU_BA_DEBUG") ? h->cta_work : nullptr};
+                  h->abort_host_dev, h->abort_dev, h->pk_part_chi, h->pk_part_scale, h->pk_part_max, h->prof.on ? h->phase_cycles : nullptr, 0, h->sw.debug ? h->cta_work : nullptr};
         if (h->prof.on) h->pk_launches++;
         const size_t smem = pk_dyn_smem_bytes(d.n);      // worker CTAs: pair lists + 87 KB of reduction scratch
         pa.dyn_smem_bytes = (int)smem;
@@ -2579,7 +2075,7 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
         const int done = h->st_host->iter;
         if (h->world > 1) {
             h->peer_epoch = h->st_host->epoch;
-            if (h->st_host->error) return fail(SE2GPU_ERR_CUDA, "sharded BA: a peer rank did not reach the exchange within %.1f s (rank %d of %d)", h->peer_timeout_s, h->rank, h->world);
+            if (h->st_host->error) return fail(SE2GPU_ERR_CUDA, "sharded BA: a peer rank did not reach the exchange within %.1f s (rank %d of %d)", h->sw.peer_timeout_s, h->rank, h->world);
         }
         if (pa.cta_work) {   // SE2GPU_BA_DEBUG=1: per-phase busy cycles of every CTA (max / mean / who) to stderr
             std::vector<long long> w((size_t)h->pk_grid * 10);
@@ -2675,10 +2171,7 @@ int se2gpu_ba_reset(se2gpu_ba* h) {
     if (!h || !h->loaded) return fail(SE2GPU_ERR_INVALID, "no problem loaded");
     SE2_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
-    LMState st0{};
-    st0.ni = 2;
-    *h->st_host = st0;
-    SE2_CUDA(cudaMemcpyAsync(h->d.st, h->st_host, sizeof(LMState), cudaMemcpyHostToDevice, s));
+    if (const int rc = reset_lm_state(h)) return rc;
     SE2_CUDA(cudaMemcpyAsync(h->d.xp[0], h->xp0, sizeof(double) * 3 * h->P, cudaMemcpyDeviceToDevice, s));
     SE2_CUDA(cudaMemcpyAsync(h->d.xl[0], h->xl0, sizeof(double) * 3 * h->L, cudaMemcpyDeviceToDevice, s));
     return SE2GPU_OK;
@@ -2764,10 +2257,9 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
     if (chi2) *chi2 = saved.chi_cur;
     h->st_host->lambda = lambda;
     SE2_CUDA(cudaMemcpyAsync(d.st, h->st_host, sizeof(LMState), cudaMemcpyHostToDevice, s));
-    if (d.nb_lm > 0) SE2_LAUNCH(ba_lm_prep, d.nb_lm, LM_THREADS, 0, s, d);
-    const size_t S_elems = h->band.active ? h->band.band_elems : (size_t)d.n * d.n;
-    if (d.n > SMEM_CHOL_MAX_N) SE2_CUDA(cudaMemsetAsync(d.S, 0, sizeof(double) * S_elems, s));
-    if (d.nblk > 0) SE2_LAUNCH(ba_schur, d.nblk, SCHUR_THREADS, 0, s, d);
+    if ((rc = launch_schur(h)) != SE2GPU_OK) return rc;
+    const size_t S_elems = stored_S_elems(h);
+    const int u6[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};   // (row, column) of the 6 stored entries of a symmetric 3x3 block
     std::vector<double> tmp;
     auto get = [&](const double* dev, size_t cnt) { tmp.resize(cnt); return cudaMemcpyAsync(tmp.data(), dev, cnt * 8, cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess; };
     if (S) {
@@ -2780,15 +2272,12 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
         }
     }
     if (bs) { if (!get(d.bs, n)) return fail(SE2GPU_ERR_CUDA, "copy bs"); memcpy(bs, tmp.data(), tmp.size() * 8); }
-    if (d.n <= SMEM_CHOL_MAX_N) SE2_LAUNCH(ba_chol_solve_smem, 1, CHOL_THREADS, ldlt_smem_bytes(d.n), s, d);
-    else if (h->band.active) { if ((rc = se2band::solve(h->band, d.S, d.bs, d.dxp, &d.st->solve_ok, s)) != SE2GPU_OK) return rc; }
-    else SE2_LAUNCH(ba_chol_solve_gmem, 1, CHOL_THREADS, 0, s, d, h->ywork);
+    if ((rc = launch_reduced_solve(h)) != SE2GPU_OK) return rc;
     SE2_LAUNCH(ba_backsub_update, h->nb_scale, LM_THREADS, 0, s, d);
     if (Hpp) {
         if (!get(d.Hpp, 6 * (size_t)nf)) return fail(SE2GPU_ERR_CUDA, "copy Hpp");
         // diagonal blocks only (off-diagonal odometry blocks are folded into S directly)
         memset(Hpp, 0, sizeof(double) * n * n);
-        const int u6[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
         for (int a = 0; a < nf; ++a)
             for (int q = 0; q < 6; ++q) {
                 Hpp[(size_t)(3 * a + u6[q][0]) * n + 3 * a + u6[q][1]] = tmp[q * (size_t)nf + a];
@@ -2798,7 +2287,6 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
     if (bp) { if (!get(d.bp, n)) return fail(SE2GPU_ERR_CUDA, "copy bp"); memcpy(bp, tmp.data(), tmp.size() * 8); }
     if (Hll) {
         if (!get(d.Hll, 6 * (size_t)L)) return fail(SE2GPU_ERR_CUDA, "copy Hll");
-        const int u6[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
         std::vector<int> lmp(L + 1);
         cudaMemcpy(lmp.data(), d.lm_ptr, sizeof(int) * (L + 1), cudaMemcpyDeviceToHost);
         for (int j = 0; j < L; ++j)

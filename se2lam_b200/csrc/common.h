@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdarg>
 #include <cstdint>
@@ -122,8 +123,16 @@ class DeviceBuffers {
     template <class T>
     cudaError_t alloc(T** p, size_t count) {
         const cudaError_t e = dev_alloc(p, count);
-        if (e == cudaSuccess) bufs_.push_back(*p);
+        if (e == cudaSuccess) bufs_.push_back((void*)*p);
         return e;
+    }
+    // a buffer that grows: *p, when this list owns it, is freed (its contents are not kept) and replaced by `count` elements
+    template <class T>
+    cudaError_t regrow(T** p, size_t count) {
+        const auto it = std::find(bufs_.begin(), bufs_.end(), (void*)*p);
+        if (*p && it != bufs_.end()) { cudaFree(*it); bufs_.erase(it); }
+        *p = nullptr;
+        return alloc(p, count);
     }
 
   private:
