@@ -380,7 +380,10 @@ void se2gpu_ba_destroy(se2gpu_ba* h);
  *   odo_i/odo_j [O] PreEdgeSE2 vertices (error = Ri^T(rj-ri)-m), odo_meas [O*3], odo_info [O*6] (00,01,02,11,12,22)
  *   fx,cx,cy       CamPara (single focal length), Tcb [12] = row-major Rcb then tcb (SE3 of setExtParameter, inverted)
  *   huber_delta    RobustKernelHuber delta of every EdgeSE2XYZ
- * All HOST pointers; copies and re-indexes synchronously. */
+ * All HOST pointers; copies and re-indexes synchronously. A context may be loaded again with any window within its
+ * capacities: a window with the loaded graph structure (vertices, fixed flags, edge endpoints, shard) only refreshes the
+ * values, any other is rebuilt. On any error the context holds NO window: optimize, get, get_f32, reset and the debug
+ * calls return SE2GPU_ERR_INVALID until a set_problem succeeds, and that one rebuilds. */
 int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, const uint8_t* fixed,
                           const double* points, const int* edge_pose, const int* edge_point, const double* uv,
                           const double* info, const int* odo_i, const int* odo_j, const double* odo_meas,

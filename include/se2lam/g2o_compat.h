@@ -164,6 +164,7 @@ public:
 
     // builds the SoA problem (poses in id order first, then points: g2o's index mapping) and uploads it
     bool initializeOptimization(int level = 0) {
+        ready_ = false;          // a rejected graph must not leave the previous window to optimize() (its vertices are gone)
         poses_.clear(); points_.clear();
         std::vector<double> xp, xl, uv, info, om, oinf;
         std::vector<uint8_t> fixed;
@@ -232,7 +233,7 @@ public:
         if (verbose_) for (int k = 0; k < n; ++k)
             std::fprintf(stderr, "iteration= %d\t chi2= %f\t lambda= %f\t levenbergIter= %d\n", k, stats_[k].chi2_after, stats_[k].lambda, stats_[k].trials);
         std::vector<double> xp(3 * poses_.size()), xl(3 * points_.size() + 3);
-        se2gpu_ba_get(ba_, xp.data(), xl.data());
+        if (se2gpu_ba_get(ba_, xp.data(), xl.data()) != SE2GPU_OK) { std::fprintf(stderr, "se2gpu: %s\n", se2gpu_last_error()); return 0; }
         for (size_t i = 0; i < poses_.size(); ++i) poses_[i]->est = SE2(xp[3 * i], xp[3 * i + 1], xp[3 * i + 2]);
         for (size_t j = 0; j < points_.size(); ++j) for (int k = 0; k < 3; ++k) points_[j]->est[k] = xl[3 * j + k];
         return n;

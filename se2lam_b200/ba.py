@@ -81,10 +81,11 @@ class LocalBA:
              c(prob.edge_point, np.int32), c(prob.uv, np.float64), c(prob.info, np.float64), c(prob.odo_i, np.int32),
              c(prob.odo_j, np.int32), c(prob.odo_meas, np.float64), c(prob.odo_info, np.float64)]
         tcb = c(prob.Tcb, np.float64)
-        self.P, self.L, self.E, self.O = prob.P, prob.L, prob.E, prob.O
+        self.P = self.L = self.E = self.O = 0          # a failed load leaves no window (se2gpu_ba_set_problem)
         check(lib().se2gpu_ba_set_problem(self.h, prob.P, prob.L, prob.E, prob.O, *[ptr(x) for x in a],
                                           float(prob.fx), float(prob.cx), float(prob.cy), ptr(tcb),
                                           float(prob.huber_delta)), "se2gpu_ba_set_problem")
+        self.P, self.L, self.E, self.O = prob.P, prob.L, prob.E, prob.O
 
     def optimize(self, iters, trace=False, stop_flag=None, first_iteration=0):
         """first_iteration > 0 continues the lambda / nu schedule of the previous call (g2o's solve(iteration) slices)."""

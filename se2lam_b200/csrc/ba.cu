@@ -1821,7 +1821,7 @@ se2gpu_ba* se2gpu_ba_create(int max_poses, int max_points, int max_edges, int ma
     const size_t nb = (L + LM_THREADS - 1) / LM_THREADS + (O + LM_THREADS - 1) / LM_THREADS + (P + LM_THREADS - 1) / LM_THREADS + 4;
     A(&d.part_chi, nb); A(&d.part_scale, nb);
     A(&h->stats_dev, h->max_stats);
-    A(&h->xp0, 3 * P); A(&h->xl0, 3 * L);
+    A(&h->xp0, 3 * P); A(&h->xl0, 3 * L); A(&h->wb32, 3 * P + 8 + 3 * L);
     A(&h->pk_part_chi, 2048); A(&h->pk_part_scale, 1024); A(&h->pk_part_max, 1024); A(&h->abort_dev, 2); A(&h->phase_cycles, 8); A(&h->cta_work, 1024 * 10);
     if (rc == SE2GPU_OK && cudaMallocHost((void**)&h->st_host, sizeof(LMState)) != cudaSuccess) rc = fail(SE2GPU_ERR_CUDA, "cudaMallocHost failed");
     if (rc == SE2GPU_OK) {
@@ -2229,10 +2229,9 @@ int se2gpu_ba_get_f32(se2gpu_ba* h, float* poses, float* points) {
     SE2_CUDA(cudaStreamSynchronize(s));
     const int cur = h->st_host->cur;
     const int n = std::max(h->P, h->L);
-    // narrow on the device into the (free) dxl / Y scratch, then one copy per array
-    float* fp = reinterpret_cast<float*>(h->d.Y);
+    // narrow on the device into the context's float write-back buffer, then one copy per array
+    float* fp = h->wb32;
     float* fl = fp + 3 * (size_t)h->P + 8;
-    if ((3 * (size_t)h->P + 8 + 3 * (size_t)h->L) * sizeof(float) > sizeof(double) * EB * (size_t)h->maxE) return fail(SE2GPU_ERR_CAPACITY, "scratch too small for the float write-back");
     SE2_LAUNCH(ba_writeback_f32, (n + 255) / 256, 256, 0, s, h->d.xp[cur], h->P, h->d.xl[cur], h->L, poses ? fp : nullptr, points ? fl : nullptr);
     if (poses) SE2_CUDA(cudaMemcpyAsync(poses, fp, sizeof(float) * 3 * h->P, cudaMemcpyDeviceToHost, s));
     if (points) SE2_CUDA(cudaMemcpyAsync(points, fl, sizeof(float) * 3 * h->L, cudaMemcpyDeviceToHost, s));

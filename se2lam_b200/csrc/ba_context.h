@@ -119,6 +119,7 @@ struct se2gpu_ba {
     int nb_scale = 0;
     bool loaded = false;
     double *xp0 = nullptr, *xl0 = nullptr;   // estimates as loaded (se2gpu_ba_reset)
+    float* wb32 = nullptr;                   // [3 maxP + 8 + 3 maxL] se2gpu_ba_get_f32's narrowed estimates
     se2gpu::Profiler prof;
     // persistent cooperative path
     int mode = 0;              // 0 auto, 1 multi-launch, 2 persistent

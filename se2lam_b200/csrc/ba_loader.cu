@@ -481,11 +481,21 @@ int se2gpu_ba_build_information(int P, int L, int E, const float* view_mp, const
     return st.finish();
 }
 
-int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, const uint8_t* fixed,
-                          const double* points, const int* edge_pose, const int* edge_point, const double* uv,
-                          const double* info, const int* odo_i, const int* odo_j, const double* odo_meas,
-                          const double* odo_info, double fx, double cx, double cy, const double* Tcb, double huber_delta) {
-    if (!h) return fail(SE2GPU_ERR_INVALID, "null handle");
+}  // extern "C"
+
+namespace {
+
+// no window loaded: optimize / get / reset / debug_* refuse to run, and the next set_problem rebuilds the structure
+void unload(se2gpu_ba* h) {
+    h->loaded = false;
+    h->t_edge_pose.clear(); h->t_edge_point.clear(); h->t_odo_i.clear(); h->t_odo_j.clear(); h->t_fixed.clear();
+    h->t_rank = h->t_world = -1;
+}
+
+int load_window(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, const uint8_t* fixed, const double* points,
+                const int* edge_pose, const int* edge_point, const double* uv, const double* info, const int* odo_i,
+                const int* odo_j, const double* odo_meas, const double* odo_info, double fx, double cx, double cy,
+                const double* Tcb, double huber_delta) {
     if (P <= 0 || L < 0 || E < 0 || O < 0) return fail(SE2GPU_ERR_INVALID, "bad sizes");
     SE2_NVTX("se2gpu.ba.set_problem");
     if (P > h->maxP || L > h->maxL || E > h->maxE || O > h->maxO) return fail(SE2GPU_ERR_CAPACITY, "problem (%d,%d,%d,%d) exceeds capacity (%d,%d,%d,%d)", P, L, E, O, h->maxP, h->maxL, h->maxE, h->maxO);
@@ -549,6 +559,21 @@ int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double
     h->t_odo_j.assign(odo_j, odo_j + O); h->t_fixed.assign(fixed, fixed + P); h->t_rank = h->rank; h->t_world = h->world;
     h->loaded = true;
     return SE2GPU_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int se2gpu_ba_set_problem(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, const uint8_t* fixed,
+                          const double* points, const int* edge_pose, const int* edge_point, const double* uv,
+                          const double* info, const int* odo_i, const int* odo_j, const double* odo_meas,
+                          const double* odo_info, double fx, double cx, double cy, const double* Tcb, double huber_delta) {
+    if (!h) return fail(SE2GPU_ERR_INVALID, "null handle");
+    const int rc = load_window(h, P, L, E, O, poses, fixed, points, edge_pose, edge_point, uv, info, odo_i, odo_j, odo_meas,
+                               odo_info, fx, cx, cy, Tcb, huber_delta);
+    if (rc != SE2GPU_OK) unload(h);   // a rejected window leaves none loaded, never the previous one
+    return rc;
 }
 
 }  // extern "C"

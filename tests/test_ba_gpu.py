@@ -107,7 +107,7 @@ def _assert_strict_trajectory(prob, iters, mode, need_reject=True):
         dp_o, dp_g = tp_o[k] - prev_p, tp_g[k] - prev_p
         dl_o, dl_g = tl_o[k] - prev_l, tl_g[k] - prev_l
         assert np.abs(dp_g - dp_o).max() <= REL * max(np.abs(dp_o).max(), 1e-12), f"pose step {k}"
-        assert np.abs(dl_g - dl_o).max() <= REL * max(np.abs(dl_o).max(), 1e-12), f"landmark step {k}"
+        assert np.abs(dl_g - dl_o).max(initial=0.0) <= REL * max(np.abs(dl_o).max(initial=0.0), 1e-12), f"landmark step {k}"
         prev_p, prev_l = tp_o[k], tl_o[k]
     return st_o
 
