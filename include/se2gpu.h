@@ -38,6 +38,9 @@
  *   se2gpu_pose_ba[_device]          Localizer::DoLocalBA (pose-only SE(3) BA, g2o LM)  src/Localizer.cpp:233-302,
  *                                    (addPlaneMotionSE3Expmap src/optimizer.cpp:236-314, EdgeSE3ExpmapPrior :159-189)
  *   se2gpu_localizer_ba_device       Localizer::MatchLocalMap's observations + DoLocalBA  src/Localizer.cpp:211-302
+ *   se2gpu_feat_edge[_device]        GlobalMapper::CreateFeatEdge (both overloads), OptKFPair, OptKFPairMatch
+ *                                    src/GlobalMapper.cpp:737-1032 (addVertexSE3PlaneMotion src/optimizer.cpp:337-468),
+ *                                    Sparsifier::DoMarginalizeSE3XYZ / InfoSE3  src/sparsifier.cpp:59-274
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -544,6 +547,65 @@ int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_
                                const float* d_inv_sigma2, int nlevels, float* d_Tcw, const se2gpu_pose_ba_params* params,
                                int min_edges, int* d_n_edges, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
                                double* d_pose, void* stream);
+
+/* ------------------------------------------------------------------------------------------ feature-graph constraints */
+/* GlobalMapper::CreateFeatEdge (src/GlobalMapper.cpp:737-843) for B keyframe pairs, one CTA each, everything on the device:
+ * the two-keyframe BA of OptKFPair / OptKFPairMatch (two VertexSE3 with the plane-motion EdgeSE3Prior of
+ * addVertexSE3PlaneMotion, one marginalised VertexPointXYZ per point with a Huber EdgeSE3PointXYZ to each keyframe, g2o's
+ * Levenberg-Marquardt with a Schur complement onto the poses), the chi2 outlier cut of OptKFPairMatch, and
+ * Sparsifier::DoMarginalizeSE3XYZ + InfoSE3 (src/sparsifier.cpp:59-274) with their forward-difference Jacobians, in double
+ * precision (DESIGN.md section 10).
+ * mode 0 is CreateFeatEdge(from, to, cnstr): keyframe 0 fixed, iterations[0] LM iterations, at least min_points[0] points.
+ * mode 1 is CreateFeatEdge(from, to, mapMatch, cnstr): both keyframes free, iterations[1] iterations, then every point with
+ * an edge of chi2 > chi2_cut is an outlier and leaves the marginalisation; at least min_points[1] matches (counted before
+ * the cut, as the reference does). A match belongs in the input only when both of its map points exist. */
+typedef struct se2gpu_feat_edge_params {
+    float Tbc[16];          /* Config::bTc, row-major 4x4 */
+    float xrot_info, yrot_info, z_info; /* Config::PLANEMOTION_XROT_INFO, _YROT_INFO, _Z_INFO */
+    float huber_delta;      /* RobustKernelHuber::setDelta(5.99) */
+    int iterations[2];      /* optimize(15) in OptKFPair, optimize(30) in OptKFPairMatch */
+    float chi2_cut;         /* dThreshChi2 = 5.0 */
+    int min_points[2];      /* numMinMPs = 10; mapMatch.size() < 3 */
+} se2gpu_feat_edge_params;
+/* the reference's values, with an identity Tbc to be replaced by Config::bTc */
+#define SE2GPU_FEAT_EDGE_PARAMS_INIT \
+    { {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}, 1e6f, 1e6f, 1.f, 5.99f, {15, 30}, 5.0f, {10, 3} }
+
+/* per-pair status */
+#define SE2GPU_FEAT_EDGE_OK 0
+#define SE2GPU_FEAT_EDGE_TOO_FEW 1  /* fewer points than min_points[mode]: the pair's outputs are left as they are */
+#define SE2GPU_FEAT_EDGE_NOT_PD 2   /* LM ended on an iteration whose 10 trials all failed the Cholesky; the constraint is
+                                       computed from the last accepted estimate */
+
+/* HOST buffers, synchronous. Pair b owns points point_ptr[b] .. point_ptr[b+1]-1 (point_ptr [B+1], point_ptr[0] = 0, P =
+ * point_ptr[B]). Tcw0 / Tcw1 [B*16] float row-major: KeyFrame::getPose() of the two keyframes. Per point: xyz [P*3] float,
+ * the start estimate (MapPoint::getPos; in mode 1 of the point seen in keyframe 0); z0 / z1 [P*3] float, mViewMPs[idx] in
+ * keyframe 0 / 1; info0 / info1 [P*9] double, mViewMPsInfo[idx], exactly as se2gpu_xyz_info writes them.
+ * Outputs: measure [B*16] float (toCvMat of KF0^-1 KF1) and info [B*36] float (toCvMat6f), the SE3Constraint; optional (may
+ * be NULL): status [B], iterations [B], stats [B*iterations[mode]] (rows past iterations[b] are zero), outlier [P] bytes
+ * (mode 1; zero in mode 0), poses [B*14] (vSe3KFs: qx, qy, qz, qw, tx, ty, tz per keyframe, camera-to-world), points [P*3]
+ * (every point's estimate, outliers included). Returns SE2GPU_ERR_INVALID before any launch on malformed input. */
+int se2gpu_feat_edge(int B, int mode, const float* Tcw0, const float* Tcw1, const int* point_ptr, const float* xyz,
+                     const float* z0, const float* z1, const double* info0, const double* info1,
+                     const se2gpu_feat_edge_params* params, float* measure, float* info, int* status, int* iterations,
+                     se2gpu_ba_iter_stats* stats, uint8_t* outlier, double* poses, double* points, int device);
+/* The same on DEVICE buffers, asynchronous on `stream` (params is a host pointer, read during the call). d_info0 / d_info1
+ * take se2gpu_xyz_info_device's outputs as they are. d_points [P*3] and d_work [P*3] doubles are required: the kernel keeps
+ * the point estimates and the trial step there. d_stats rows past an iteration count are not written. d_point_ptr is device
+ * memory and is trusted: it must start at 0 and ascend, and every array must hold d_point_ptr[B] points; the rejection of
+ * malformed input described above is the host entry's. */
+int se2gpu_feat_edge_device(int B, int mode, const float* d_Tcw0, const float* d_Tcw1, const int* d_point_ptr, const float* d_xyz,
+                            const float* d_z0, const float* d_z1, const double* d_info0, const double* d_info1,
+                            const se2gpu_feat_edge_params* params, float* d_measure, float* d_info, int* d_status,
+                            int* d_iterations, se2gpu_ba_iter_stats* d_stats, uint8_t* d_outlier, double* d_poses,
+                            double* d_points, double* d_work, void* stream);
+/* parity hook: se2gpu_feat_edge plus trace [B*iterations[mode]*24], both keyframes' estimates (rotation row-major, then
+ * translation) after every iteration (rows past the count zero) */
+int se2gpu_feat_edge_debug_trace(int B, int mode, const float* Tcw0, const float* Tcw1, const int* point_ptr, const float* xyz,
+                                 const float* z0, const float* z1, const double* info0, const double* info1,
+                                 const se2gpu_feat_edge_params* params, float* measure, float* info, int* status, int* iterations,
+                                 se2gpu_ba_iter_stats* stats, uint8_t* outlier, double* poses, double* points, double* trace,
+                                 int device);
 
 #ifdef __cplusplus
 }

@@ -34,6 +34,11 @@ class PoseBAParams(C.Structure):
                 ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float), ("iterations", C.c_int)]
 
 
+class FeatEdgeParams(C.Structure):
+    _fields_ = [("Tbc", C.c_float * 16), ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float),
+                ("huber_delta", C.c_float), ("iterations", C.c_int * 2), ("chi2_cut", C.c_float), ("min_points", C.c_int * 2)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -63,6 +68,7 @@ SYMBOLS = [
     "se2gpu_fundam_debug_niters",
     "se2gpu_pose_ba", "se2gpu_pose_ba_device", "se2gpu_pose_ba_debug_trace", "se2gpu_localizer_create", "se2gpu_localizer_destroy",
     "se2gpu_localizer_ba_device",
+    "se2gpu_feat_edge", "se2gpu_feat_edge_device", "se2gpu_feat_edge_debug_trace",
 ]
 
 
@@ -164,6 +170,9 @@ def lib():
     L.se2gpu_localizer_create.argtypes = [i, i]
     L.se2gpu_localizer_destroy.argtypes = [vp]
     L.se2gpu_localizer_ba_device.argtypes = [vp, vp, i, vp, vp, i, vp, vp, vp, i, vp, vp, i, vp, vp, vp, vp, vp, vp]
+    L.se2gpu_feat_edge.argtypes = [i, i] + [vp] * 17 + [i]
+    L.se2gpu_feat_edge_device.argtypes = [i, i] + [vp] * 19
+    L.se2gpu_feat_edge_debug_trace.argtypes = [i, i] + [vp] * 18 + [i]
     _lib = L
     return L
 
