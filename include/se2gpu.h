@@ -41,6 +41,9 @@
  *   se2gpu_feat_edge[_device]        GlobalMapper::CreateFeatEdge (both overloads), OptKFPair, OptKFPairMatch
  *                                    src/GlobalMapper.cpp:737-1032 (addVertexSE3PlaneMotion src/optimizer.cpp:337-468),
  *                                    Sparsifier::DoMarginalizeSE3XYZ / InfoSE3  src/sparsifier.cpp:59-274
+ *   se2gpu_global_ba[_device]        GlobalMapper::GlobalBA's pose graph and optimize(GLOBAL_ITER)  src/GlobalMapper.cpp:328-504
+ *                                    (addVertexSE3PlaneMotion src/optimizer.cpp:337-468, addEdgeSE3 :375-419)
+ *   se2gpu_global_ba_update_points[_device]  GlobalBA's map-point write-back  src/GlobalMapper.cpp:506-531
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -606,6 +609,65 @@ int se2gpu_feat_edge_debug_trace(int B, int mode, const float* Tcw0, const float
                                  const se2gpu_feat_edge_params* params, float* measure, float* info, int* status, int* iterations,
                                  se2gpu_ba_iter_stats* stats, uint8_t* outlier, double* poses, double* points, double* trace,
                                  int device);
+
+/* ------------------------------------------------------------------------------------------ global pose graph */
+/* GlobalMapper::GlobalBA (src/GlobalMapper.cpp:328-535): one VertexSE3 per keyframe (camera-to-world, start value
+ * toIsometry3D(cvu::inv(Tcw))) with the plane-motion EdgeSE3Prior of addVertexSE3PlaneMotion, one EdgeSE3 per odometry or
+ * feature constraint (e = toVectorMQT(Z^-1 Xfrom^-1 Xto), information in the same [trans, rot] order), optimised by
+ * Levenberg-Marquardt over the free vertices with a sparse direct solve, in double precision (DESIGN.md section 11). */
+typedef struct se2gpu_global_ba_params {
+    float Tbc[16];          /* Config::bTc, row-major 4x4 */
+    float xrot_info, yrot_info, z_info; /* Config::PLANEMOTION_XROT_INFO, _YROT_INFO, _Z_INFO */
+    int iterations;         /* Config::GLOBAL_ITER */
+} se2gpu_global_ba_params;
+/* the reference's values, with an identity Tbc to be replaced by Config::bTc */
+#define SE2GPU_GLOBAL_BA_PARAMS_INIT \
+    { {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}, 1e6f, 1e6f, 1.f, 15 }
+
+#define SE2GPU_GLOBAL_BA_OK 0
+#define SE2GPU_GLOBAL_BA_NOT_PD 2  /* LM ended on an iteration whose 10 trials all met a pivot block that is not positive
+                                      definite; the poses are the last accepted estimate */
+
+/* A context: grow-only device buffers for the plan and the solver, a page-locked staging arena and a stream, on device
+ * `device`. One context serves graphs of any size and topology; a call gives the same bytes as on a fresh context. Calls
+ * on one context may use different streams: each call's work waits for the previous call's kernel on the device. */
+typedef struct se2gpu_global_ba_ctx se2gpu_global_ba_ctx;
+se2gpu_global_ba_ctx* se2gpu_global_ba_create(int device);
+void se2gpu_global_ba_destroy(se2gpu_global_ba_ctx* h);
+
+/* HOST buffers, synchronous. N keyframes: Tcw [N*16] float row-major (KeyFrame::Tcw), fixed [N] (mIdKF == 0). E edges:
+ * edge_from / edge_to [E] vertex indices, measure [E*16] float (SE3Constraint::measure), info [E*36] float (its info).
+ * Outputs: Tcw_out [N*16] float (the pose setPose receives: cvu::inv(toCvMat(estimate))); optional (may be NULL): status,
+ * iterations, stats [params->iterations] (rows past the count are zero), poses [N*7] (the estimates as SE3Quat: qx, qy, qz,
+ * qw, tx, ty, tz, camera-to-world). With no free vertex no iteration runs, as in g2o. Returns SE2GPU_ERR_INVALID before any
+ * launch when N <= 0, an index is out of range, from == to, or a measurement or information is not finite or an
+ * information is not symmetric. */
+int se2gpu_global_ba(se2gpu_global_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, int E, const int* edge_from,
+                     const int* edge_to, const float* measure, const float* info, const se2gpu_global_ba_params* params,
+                     float* Tcw_out, int* status, int* iterations, se2gpu_ba_iter_stats* stats, double* poses);
+/* The same on DEVICE values, asynchronous on `stream`. The topology (fixed, edge_from, edge_to) is HOST memory: the
+ * ordering and the gather lists are planned on the host once per call. d_edge_status [E] (may be NULL) leaves out every
+ * edge whose entry is SE2GPU_FEAT_EDGE_TOO_FEW, so se2gpu_feat_edge_device can write the feature edges' d_measure / d_info /
+ * d_status straight into slices of these arrays; such an edge keeps its place in the plan and contributes nothing. The
+ * values are trusted: the finiteness and symmetry checks are the host entry's. */
+int se2gpu_global_ba_device(se2gpu_global_ba_ctx* h, int N, const float* d_Tcw, const uint8_t* fixed, int E, const int* edge_from,
+                            const int* edge_to, const float* d_measure, const float* d_info, const int* d_edge_status,
+                            const se2gpu_global_ba_params* params, float* d_Tcw_out, int* d_status, int* d_iterations,
+                            se2gpu_ba_iter_stats* d_stats, double* d_poses, void* stream);
+/* Phase timing of the kernel (a measurement aid; it adds a %globaltimer read per phase on one thread). on = 1 zeroes and
+ * starts it, on = 0 stops it. profile_read waits for the last call and returns ms [7], the time accumulated since
+ * profiling started in: setup (start values, priors, first chi2), linearisation, gather of H and b, copy and damping,
+ * factorisation, substitution, and trial (oplus, computeScale, chi2 at the trial state, the LM decision). */
+int se2gpu_global_ba_profile(se2gpu_global_ba_ctx* h, int on);
+int se2gpu_global_ba_profile_read(se2gpu_global_ba_ctx* h, double* ms);
+/* GlobalBA's map-point write-back: pos_out [M*3] = Rwc * view_mp + twc of keyframe kf_index[m], Twc the rigid inverse of
+ * Tcw [N*16] (normally se2gpu_global_ba's Tcw_out), in float. view_mp [M*3] is mViewMPs[idx] of the point's main keyframe.
+ * HOST buffers, synchronous; kf_index is checked against N. */
+int se2gpu_global_ba_update_points(int M, const int* kf_index, const float* view_mp, int N, const float* Tcw, float* pos_out,
+                                   int device);
+/* the same on DEVICE buffers, asynchronous on `stream`; d_kf_index is trusted */
+int se2gpu_global_ba_update_points_device(int M, const int* d_kf_index, const float* d_view_mp, const float* d_Tcw, float* d_pos_out,
+                                          void* stream);
 
 #ifdef __cplusplus
 }

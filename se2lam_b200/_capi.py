@@ -39,6 +39,11 @@ class FeatEdgeParams(C.Structure):
                 ("huber_delta", C.c_float), ("iterations", C.c_int * 2), ("chi2_cut", C.c_float), ("min_points", C.c_int * 2)]
 
 
+class GlobalBAParams(C.Structure):
+    _fields_ = [("Tbc", C.c_float * 16), ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float),
+                ("iterations", C.c_int)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -69,6 +74,9 @@ SYMBOLS = [
     "se2gpu_pose_ba", "se2gpu_pose_ba_device", "se2gpu_pose_ba_debug_trace", "se2gpu_localizer_create", "se2gpu_localizer_destroy",
     "se2gpu_localizer_ba_device",
     "se2gpu_feat_edge", "se2gpu_feat_edge_device", "se2gpu_feat_edge_debug_trace",
+    "se2gpu_global_ba_create", "se2gpu_global_ba_destroy", "se2gpu_global_ba", "se2gpu_global_ba_device",
+    "se2gpu_global_ba_update_points", "se2gpu_global_ba_update_points_device", "se2gpu_global_ba_profile",
+    "se2gpu_global_ba_profile_read",
 ]
 
 
@@ -173,6 +181,15 @@ def lib():
     L.se2gpu_feat_edge.argtypes = [i, i] + [vp] * 17 + [i]
     L.se2gpu_feat_edge_device.argtypes = [i, i] + [vp] * 19
     L.se2gpu_feat_edge_debug_trace.argtypes = [i, i] + [vp] * 18 + [i]
+    L.se2gpu_global_ba_create.restype = vp
+    L.se2gpu_global_ba_create.argtypes = [i]
+    L.se2gpu_global_ba_destroy.argtypes = [vp]
+    L.se2gpu_global_ba.argtypes = [vp, i, vp, vp, i] + [vp] * 10
+    L.se2gpu_global_ba_device.argtypes = [vp, i, vp, vp, i] + [vp] * 12
+    L.se2gpu_global_ba_update_points.argtypes = [i, vp, vp, i, vp, vp, i]
+    L.se2gpu_global_ba_update_points_device.argtypes = [i] + [vp] * 5
+    L.se2gpu_global_ba_profile.argtypes = [vp, i]
+    L.se2gpu_global_ba_profile_read.argtypes = [vp, vp]
     _lib = L
     return L
 

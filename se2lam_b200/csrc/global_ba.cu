@@ -1,0 +1,743 @@
+// Global pose graph: GlobalMapper::GlobalBA (reference src/GlobalMapper.cpp:328-535). One g2o VertexSE3 per keyframe with
+// the plane-motion EdgeSE3Prior of addVertexSE3PlaneMotion, one EdgeSE3 per odometry and per feature constraint, and
+// optimize(GLOBAL_ITER) under OptimizationAlgorithmLevenberg with a sparse direct solve over the free vertices
+// (DESIGN.md section 11).
+//
+// The symbolic phase (global_ba_plan.h) runs on the host once per call: reverse Cuthill-McKee order, 6 x 6 block envelope,
+// fixed-order gather lists. The numeric phase, the whole optimize(), is one persistent kernel on one CTA:
+//  * per iteration: every edge is linearised by one thread into its own blocks (H_ii, H_jj, H_ij, b_i, b_j), every free
+//    vertex's prior likewise; then H and b are gathered block entry by block entry, each entry one thread summing its
+//    contributions in ascending edge order (no atomics: the bytes do not depend on scheduling);
+//  * per trial: damping, a block-envelope Cholesky (LL^T, 6 x 6 pivots) in RCM order, forward and back substitution,
+//    oplus, chi2 at the trial state, accept or keep; phases are separated by __syncthreads.
+// All arithmetic is double precision; every reduction is a fixed tree over the CTA's threads.
+#include <cuda_runtime.h>
+
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+
+#include "common.h"
+#include "global_ba_plan.h"
+#include "se3iso.h"
+
+using namespace se2gpu;
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kLin = 120;  // per-edge linearisation: H_ii, H_jj, H_ij (36 each), b_i, b_j (6 each)
+
+struct KArgs {
+    int N, E, nf, S, iterations;
+    float Tbc[16];
+    float xrot, yrot, zinfo;
+    const float* Tcw;       // [N*16]
+    const float* measure;   // [E*16]
+    const float* info;      // [E*36]
+    const int* from;        // [E]
+    const int* to;          // [E]
+    const int* edge_status; // [E] or NULL: SE2GPU_FEAT_EDGE_TOO_FEW leaves the edge out
+    // plan
+    const int* pos; const int* vert; const int* first; const long long* rowoff;
+    const int* col_ptr; const int* col_rows; const int* diag_ptr; const int* diag_code;
+    const long long* off_blk; const int* off_ptr; const int* off_code;
+    // work
+    Iso* X[2];              // [N] current and trial estimates (which is which: s_cur)
+    Prior* prior;           // [N]
+    Iso* Zinv;              // [E]
+    double* Om;             // [E*36]
+    double* lin;            // [E*kLin]
+    double* pH;             // [nf*36] prior blocks, by position
+    double* pb;             // [nf*6]
+    double* Hs;             // [env*36] the gathered H (blocks outside the gather lists stay zero)
+    double* L;              // [env*36] damped H, factorised in place
+    double* b;              // [nf*6]
+    double* x;              // [nf*6]
+    // outputs
+    float* Tcw_out; int* status; int* iters; se2gpu_ba_iter_stats* stats; double* poses;
+    unsigned long long* prof;  // [kPhases] ns per phase, accumulated by thread 0 (NULL: not profiled)
+};
+
+// the phases se2gpu_global_ba_profile_read reports
+enum Phase { kSetup, kLinearise, kGather, kDamp, kFactor, kSubstitute, kTrial, kPhases };
+
+__device__ inline unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+__device__ inline bool edge_active(const KArgs& a, int e) {
+    return !a.edge_status || a.edge_status[e] != SE2GPU_FEAT_EDGE_TOO_FEW;
+}
+
+// cvu::inv of a float 4 x 4 rigid transform: R^T, and -R^T t accumulated in double (OpenCV's float gemm) and rounded once;
+// the products of two floats are exact in double, so the rounding does not depend on contraction
+__device__ inline void rigid_inv_f32(const float* T, float* out) {
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) out[i * 4 + j] = T[j * 4 + i];
+        const double s = ((double)T[i] * T[3] + (double)T[4 + i] * T[7]) + (double)T[8 + i] * T[11];
+        out[i * 4 + 3] = (float)(-s);
+    }
+    out[12] = 0.f; out[13] = 0.f; out[14] = 0.f; out[15] = 1.f;
+}
+
+// converter.cpp toIsometry3D(cv::Mat): the rotation through an un-normalised Quaterniond, the translation as it is
+__device__ inline Iso iso_from_f32(const float* T) {
+    Iso X;
+    const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+    quat_to_R(quat_from_R(R), X.R);
+    X.t[0] = T[3]; X.t[1] = T[7]; X.t[2] = T[11];
+    return X;
+}
+
+// EdgeSE3::computeError: e = toVectorMQT(Z^-1 Xi^-1 Xj); returns e^T Omega e. With J, the Jacobians through oplus on both
+// vertices, E = A D(di)^-1 B with A = Z^-1, B = Xi^-1 Xj and (v, w) the quaternion of E (w >= 0):
+//   Ji = [[-R_A, 2 R_A skew(t_B)], [0, -(w I - skew(v)) R_A]],  Jj = [[R_E, 0], [0, w I + skew(v)]]
+__device__ __noinline__ double edge_error(const Iso& Zinv, const double* Om, const Iso& Xi, const Iso& Xj, double* e, double* Ji,
+                                          double* Jj) {
+    const Iso B = iso_mul(iso_inv(Xi), Xj);
+    const Iso E = iso_mul(Zinv, B);
+    Quat q = quat_from_R(E.R);
+    normalize_rotation(q);
+    e[0] = E.t[0]; e[1] = E.t[1]; e[2] = E.t[2]; e[3] = q.x; e[4] = q.y; e[5] = q.z;
+    double chi = 0;
+    for (int r = 0; r < 6; ++r) {
+        double we = 0;
+        for (int c = 0; c < 6; ++c) we += Om[r * 6 + c] * e[c];
+        chi += e[r] * we;
+    }
+    if (!Ji) return chi;
+    for (int k = 0; k < 36; ++k) { Ji[k] = 0; Jj[k] = 0; }
+    const double* RA = Zinv.R;
+    double S[9], RS[9], W[9];
+    skew(B.t, S);
+    mul3(RA, S, RS);
+    // w I - skew(v)
+    W[0] = q.w;  W[1] = q.z;  W[2] = -q.y;
+    W[3] = -q.z; W[4] = q.w;  W[5] = q.x;
+    W[6] = q.y;  W[7] = -q.x; W[8] = q.w;
+    double WR[9];
+    mul3(W, RA, WR);
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) {
+            Ji[r * 6 + c] = -RA[r * 3 + c];
+            Ji[r * 6 + 3 + c] = 2 * RS[r * 3 + c];
+            Ji[(r + 3) * 6 + 3 + c] = -WR[r * 3 + c];
+            Jj[r * 6 + c] = E.R[r * 3 + c];
+        }
+    Jj[21] = q.w;  Jj[22] = -q.z; Jj[23] = q.y;
+    Jj[27] = q.z;  Jj[28] = q.w;  Jj[29] = -q.x;
+    Jj[33] = -q.y; Jj[34] = q.x;  Jj[35] = q.w;
+    return chi;
+}
+
+// one edge's blocks: H_ii, H_jj, H_ij = Ji^T Om Jj, b_i = -Ji^T Om e, b_j
+__device__ __noinline__ void edge_linearise(const Iso& Zinv, const double* Om, const Iso& Xi, const Iso& Xj, double* out) {
+    double e[6], J[2][36];
+    edge_error(Zinv, Om, Xi, Xj, e, J[0], J[1]);
+    double Oe[6];
+    for (int r = 0; r < 6; ++r) {
+        double acc = 0;
+        for (int c = 0; c < 6; ++c) acc += Om[r * 6 + c] * e[c];
+        Oe[r] = acc;
+    }
+    for (int s = 0; s < 2; ++s) {
+        double OJ[36];
+        for (int r = 0; r < 6; ++r)
+            for (int c = 0; c < 6; ++c) {
+                double acc = 0;
+                for (int m = 0; m < 6; ++m) acc += Om[r * 6 + m] * J[s][m * 6 + c];
+                OJ[r * 6 + c] = acc;
+            }
+        for (int r = 0; r < 6; ++r) {
+            for (int c = 0; c < 6; ++c) {
+                double acc = 0;
+                for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * OJ[m * 6 + c];
+                out[36 * s + r * 6 + c] = acc;  // s = 0: H_ii, s = 1: H_jj
+                if (s == 1) {
+                    double ij = 0;
+                    for (int m = 0; m < 6; ++m) ij += J[0][m * 6 + r] * OJ[m * 6 + c];
+                    out[72 + r * 6 + c] = ij;
+                }
+            }
+            double acc = 0;
+            for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * Oe[m];
+            out[108 + 6 * s + r] = -acc;
+        }
+    }
+}
+
+// sum of one value per thread, the same on every thread: xor-shuffle tree, then the warp sums in index order
+__device__ inline double block_sum(double v, double* s_red) {
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    __syncthreads();  // s_red may still be read from the previous sum
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = s_red[0];
+    for (int w = 1; w < kWarps; ++w) s += s_red[w];
+    return s;
+}
+
+__device__ inline double block_max(double v, double* s_red) {
+    for (int off = 16; off > 0; off >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, off));
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = s_red[0];
+    for (int w = 1; w < kWarps; ++w) s = fmax(s, s_red[w]);
+    return s;
+}
+
+// activeChi2 at the estimates X: every active edge and every vertex's prior (the fixed ones are constant, but g2o counts them)
+__device__ double total_chi2(const KArgs& a, const Iso* X, double* s_red) {
+    double acc = 0;
+    for (int e = threadIdx.x; e < a.E; e += kThreads) {
+        if (!edge_active(a, e)) continue;
+        double err[6];
+        acc += edge_error(a.Zinv[e], a.Om + 36 * (size_t)e, X[a.from[e]], X[a.to[e]], err, nullptr, nullptr);
+    }
+    for (int v = threadIdx.x; v < a.N; v += kThreads) acc += prior_terms(a.prior[v], X[v], nullptr, nullptr);
+    return block_sum(acc, s_red);
+}
+
+__device__ inline const double* blkp(const double* M, const KArgs& a, int p, int q) {
+    return M + 36 * (size_t)(a.rowoff[p] + (q - a.first[p]));
+}
+
+// block-envelope Cholesky of L in place (lower blocks, row-major 6 x 6); false when a pivot block is not positive definite
+__device__ bool factor(const KArgs& a, double* s_D, int* s_flag) {
+    double* L = a.L;
+    for (int k = 0; k < a.nf; ++k) {
+        const int fk = a.first[k];
+        if (threadIdx.x < 36) {  // the pivot block's Schur update
+            const int r = threadIdx.x / 6, c = threadIdx.x % 6;
+            double s = blkp(L, a, k, k)[r * 6 + c];
+            for (int j = fk; j < k; ++j) {
+                const double* Lkj = blkp(L, a, k, j);
+                for (int t = 0; t < 6; ++t) s -= Lkj[r * 6 + t] * Lkj[c * 6 + t];
+            }
+            s_D[r * 6 + c] = s;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {  // dense 6 x 6 LL^T of the pivot
+            int ok = 1;
+            for (int r = 0; r < 6 && ok; ++r)
+                for (int c = 0; c <= r; ++c) {
+                    double s = s_D[r * 6 + c];
+                    for (int t = 0; t < c; ++t) s -= s_D[r * 6 + t] * s_D[c * 6 + t];
+                    if (c == r) {
+                        if (!(s > 0.0) || !isfinite(s)) { ok = 0; break; }
+                        s_D[r * 6 + r] = sqrt(s);
+                    } else {
+                        s_D[r * 6 + c] = s / s_D[c * 6 + c];
+                    }
+                }
+            double* Lkk = L + 36 * (size_t)(a.rowoff[k] + (k - fk));
+            for (int r = 0; r < 6; ++r)
+                for (int c = 0; c < 6; ++c) Lkk[r * 6 + c] = c <= r ? s_D[r * 6 + c] : 0.0;
+            *s_flag = ok;
+        }
+        __syncthreads();
+        if (!*s_flag) return false;
+        const int r0 = a.col_ptr[k], nr = a.col_ptr[k + 1] - r0;
+        for (int idx = threadIdx.x; idx < nr * 36; idx += kThreads) {  // the rows below: A_ik - sum_j L_ij L_kj^T
+            const int i = a.col_rows[r0 + idx / 36], r = (idx % 36) / 6, c = idx % 6;
+            double* Lik = L + 36 * (size_t)(a.rowoff[i] + (k - a.first[i]));
+            double s = Lik[r * 6 + c];
+            for (int j = max(a.first[i], fk); j < k; ++j) {
+                const double* Lij = blkp(L, a, i, j);
+                const double* Lkj = blkp(L, a, k, j);
+                for (int t = 0; t < 6; ++t) s -= Lij[r * 6 + t] * Lkj[c * 6 + t];
+            }
+            Lik[r * 6 + c] = s;
+        }
+        __syncthreads();
+        for (int idx = threadIdx.x; idx < nr * 6; idx += kThreads) {  // ... times L_kk^-T
+            const int i = a.col_rows[r0 + idx / 6], r = idx % 6;
+            double* row = L + 36 * (size_t)(a.rowoff[i] + (k - a.first[i])) + r * 6;
+            for (int c = 0; c < 6; ++c) {
+                double s = row[c];
+                for (int t = 0; t < c; ++t) s -= row[t] * s_D[c * 6 + t];
+                row[c] = s / s_D[c * 6 + c];
+            }
+        }
+        __syncthreads();
+    }
+    return true;
+}
+
+// L L^T x = b by warp 0: forward over the rows of the envelope, back over its columns
+__device__ void substitute(const KArgs& a) {
+    if (threadIdx.x >= 32) return;
+    const int lane = threadIdx.x;
+    double* x = a.x;
+    for (int k = 0; k < a.nf; ++k) {
+        if (lane < 6) {
+            double s = a.b[6 * k + lane];
+            for (int j = a.first[k]; j < k; ++j) {
+                const double* Lkj = blkp(a.L, a, k, j);
+                for (int t = 0; t < 6; ++t) s -= Lkj[lane * 6 + t] * x[6 * j + t];
+            }
+            x[6 * k + lane] = s;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            const double* Lkk = blkp(a.L, a, k, k);
+            for (int r = 0; r < 6; ++r) {
+                double s = x[6 * k + r];
+                for (int t = 0; t < r; ++t) s -= Lkk[r * 6 + t] * x[6 * k + t];
+                x[6 * k + r] = s / Lkk[r * 6 + r];
+            }
+        }
+        __syncwarp();
+    }
+    for (int k = a.nf - 1; k >= 0; --k) {
+        if (lane < 6) {
+            double s = x[6 * k + lane];
+            for (int q = a.col_ptr[k]; q < a.col_ptr[k + 1]; ++q) {
+                const int i = a.col_rows[q];
+                const double* Lik = blkp(a.L, a, i, k);
+                for (int t = 0; t < 6; ++t) s -= Lik[t * 6 + lane] * x[6 * i + t];
+            }
+            x[6 * k + lane] = s;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            const double* Lkk = blkp(a.L, a, k, k);
+            for (int r = 5; r >= 0; --r) {
+                double s = x[6 * k + r];
+                for (int t = r + 1; t < 6; ++t) s -= Lkk[t * 6 + r] * x[6 * k + t];
+                x[6 * k + r] = s / Lkk[r * 6 + r];
+            }
+        }
+        __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
+    __shared__ double s_red[kWarps], s_D[36];
+    __shared__ double s_cur, s_lambda, s_ni;
+    __shared__ int s_flag, s_more, s_stop, s_buf;
+    const int tid = threadIdx.x;
+    const size_t env36 = 36 * (size_t)(a.nf ? a.rowoff[a.nf] : 0);
+    // phase timing: thread 0 stamps right after the barrier that ends a phase
+    unsigned long long t_last = (a.prof && tid == 0) ? global_ns() : 0;
+    auto stamp = [&](int phase) {
+        if (a.prof && tid == 0) {
+            const unsigned long long t = global_ns();
+            a.prof[phase] += t - t_last;
+            t_last = t;
+        }
+    };
+
+    for (int v = tid; v < a.N; v += kThreads) {  // vertices: toIsometry3D(cvu::inv(Tcw)) and their priors
+        float Twc[16];
+        rigid_inv_f32(a.Tcw + 16 * (size_t)v, Twc);
+        const Iso X = iso_from_f32(Twc);
+        a.X[0][v] = X;
+        a.X[1][v] = X;
+        plane_motion_prior(X, a.Tbc, a.xrot, a.yrot, a.zinfo, &a.prior[v]);
+    }
+    for (int e = tid; e < a.E; e += kThreads) {  // edges: toIsometry3D(measure).inverse(), toMatrix6d(info)
+        a.Zinv[e] = iso_inv(iso_from_f32(a.measure + 16 * (size_t)e));
+        for (int k = 0; k < 36; ++k) a.Om[36 * (size_t)e + k] = (double)a.info[36 * (size_t)e + k];
+    }
+    for (size_t i = tid; i < env36; i += kThreads) a.Hs[i] = 0;
+    if (tid == 0) { s_stop = 0; s_buf = 0; }
+    __syncthreads();
+    {
+        const double c = total_chi2(a, a.X[0], s_red);
+        if (tid == 0) s_cur = c;
+    }
+    stamp(kSetup);
+
+    // g2o's optimize() returns before its first iteration when no vertex is free
+    const int iterations = a.nf ? a.iterations : 0;
+    int it = 0, last_failed = 0;
+    for (; it < iterations; ++it) {
+        const Iso* X = a.X[s_buf];
+        Iso* Xt = a.X[s_buf ^ 1];
+        // linearise
+        for (int e = tid; e < a.E; e += kThreads)
+            if (edge_active(a, e)) edge_linearise(a.Zinv[e], a.Om + 36 * (size_t)e, X[a.from[e]], X[a.to[e]], a.lin + kLin * (size_t)e);
+        for (int p = tid; p < a.nf; p += kThreads) {
+            const int v = a.vert[p];
+            prior_terms(a.prior[v], X[v], a.pH + 36 * (size_t)p, a.pb + 6 * (size_t)p);
+        }
+        __syncthreads();
+        stamp(kLinearise);
+        // gather H and b in ascending edge order
+        for (int idx = tid; idx < a.nf * 42; idx += kThreads) {
+            const int p = idx / 42, rc = idx % 42;
+            const bool isb = rc >= 36;
+            double s = isb ? a.pb[6 * (size_t)p + rc - 36] : a.pH[36 * (size_t)p + rc];
+            for (int q = a.diag_ptr[p]; q < a.diag_ptr[p + 1]; ++q) {
+                const int code = a.diag_code[q], e = code >> 2, side = code & 3;
+                if (!edge_active(a, e)) continue;
+                s += isb ? a.lin[kLin * (size_t)e + 108 + 6 * side + rc - 36] : a.lin[kLin * (size_t)e + 36 * side + rc];
+            }
+            if (isb) a.b[6 * (size_t)p + rc - 36] = s;
+            else a.Hs[36 * (size_t)(a.rowoff[p] + (p - a.first[p])) + rc] = s;
+        }
+        for (int idx = tid; idx < a.S * 36; idx += kThreads) {
+            const int sl = idx / 36, rc = idx % 36, tr = (rc % 6) * 6 + rc / 6;
+            double s = 0;
+            for (int q = a.off_ptr[sl]; q < a.off_ptr[sl + 1]; ++q) {
+                const int code = a.off_code[q], e = code >> 2;
+                if (!edge_active(a, e)) continue;
+                s += a.lin[kLin * (size_t)e + 72 + ((code & 3) == gba::kOffDiag ? rc : tr)];
+            }
+            a.Hs[36 * (size_t)a.off_blk[sl] + rc] = s;
+        }
+        __syncthreads();
+        stamp(kGather);
+        if (it == 0) {  // computeLambdaInit: tau = 1e-5 times the largest diagonal entry of the free vertices
+            double m = 0;
+            for (int idx = tid; idx < a.nf * 6; idx += kThreads)
+                m = fmax(m, fabs(a.Hs[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7]));
+            m = block_max(m, s_red);
+            if (tid == 0) { s_lambda = 1e-5 * m; s_ni = 2; }
+        }
+        se2gpu_ba_iter_stats st{};
+        st.chi2_before = s_cur;
+        int qmax = 0, failed = 0;
+        double rho = 0;
+        for (;;) {
+            __syncthreads();
+            const double lambda = s_lambda;
+            for (size_t i = tid; i < env36; i += kThreads) a.L[i] = a.Hs[i];
+            __syncthreads();
+            for (int idx = tid; idx < a.nf * 6; idx += kThreads)
+                a.L[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7] += lambda;
+            __syncthreads();
+            stamp(kDamp);
+            const bool ok = factor(a, s_D, &s_flag);
+            stamp(kFactor);
+            double temp = DBL_MAX, scale = 0;
+            if (ok) {
+                substitute(a);
+                __syncthreads();
+                stamp(kSubstitute);
+                double sc = 0;
+                for (int p = tid; p < a.nf; p += kThreads) {
+                    const double* d = a.x + 6 * (size_t)p;
+                    const int v = a.vert[p];
+                    Xt[v] = oplus(X[v], d);
+                    for (int r = 0; r < 6; ++r) sc += d[r] * (lambda * d[r] + a.b[6 * (size_t)p + r]);
+                }
+                scale = block_sum(sc, s_red);
+                temp = total_chi2(a, Xt, s_red);
+            }
+            if (tid == 0) {
+                if (!ok) ++failed;
+                rho = (s_cur - temp) / (scale + 1e-3);
+                if (rho > 0 && isfinite(temp)) {
+                    double alpha = 1. - pow((2 * rho - 1), 3);
+                    alpha = fmin(alpha, 2. / 3.);
+                    s_lambda *= fmax(1. / 3., alpha);
+                    s_ni = 2;
+                    s_cur = temp;
+                    st.accepted = 1;
+                    s_buf ^= 1;
+                } else {
+                    s_lambda *= s_ni;
+                    s_ni *= 2;
+                }
+                ++qmax;
+                s_more = rho < 0 && qmax < 10;
+            }
+            __syncthreads();
+            stamp(kTrial);
+            if (!s_more) break;
+        }
+        if (tid == 0) {
+            st.chi2_after = s_cur; st.lambda = s_lambda; st.rho = rho; st.trials = qmax;
+            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
+            last_failed = st.terminate && failed == qmax;
+            if (a.stats) a.stats[it] = st;
+            s_stop = st.terminate;
+        }
+        __syncthreads();
+        // the fixed vertices are the same in both buffers; a free vertex's trial is rewritten before it is read
+        if (s_stop) { ++it; break; }
+    }
+
+    // write-back: cvu::inv(toCvMat(toSE3Quat(estimate)))
+    const Iso* X = a.X[s_buf];
+    for (int v = tid; v < a.N; v += kThreads) {
+        const SE3 T = se3_from_iso(X[v]);
+        double R[9];
+        quat_to_R(T.q, R);
+        float Twc[16];
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) Twc[r * 4 + c] = (float)R[r * 3 + c];
+            Twc[r * 4 + 3] = (float)T.t[r];
+        }
+        Twc[12] = 0.f; Twc[13] = 0.f; Twc[14] = 0.f; Twc[15] = 1.f;
+        rigid_inv_f32(Twc, a.Tcw_out + 16 * (size_t)v);
+        if (a.poses) {
+            double* p7 = a.poses + 7 * (size_t)v;
+            p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
+            p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
+        }
+    }
+    if (tid == 0) {
+        if (a.iters) *a.iters = it;
+        if (a.status) *a.status = last_failed ? SE2GPU_GLOBAL_BA_NOT_PD : SE2GPU_GLOBAL_BA_OK;
+    }
+}
+
+// GlobalBA's map-point write-back (:506-531): pos = Rwc * view + twc of the main keyframe, Twc its rigid inverse
+__global__ void k_update_points(int M, const int* __restrict__ kf, const float* __restrict__ view, const float* __restrict__ Tcw,
+                                float* __restrict__ pos) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= M) return;
+    float Twc[16];
+    rigid_inv_f32(Tcw + 16 * (size_t)kf[m], Twc);
+    const float* v = view + 3 * (size_t)m;
+    for (int r = 0; r < 3; ++r) {
+        const double s = ((double)Twc[r * 4] * v[0] + (double)Twc[r * 4 + 1] * v[1]) + (double)Twc[r * 4 + 2] * v[2];
+        pos[3 * (size_t)m + r] = (float)(s + (double)Twc[r * 4 + 3]);
+    }
+}
+
+int check_params(const se2gpu_global_ba_params* p) {
+    if (!p) return fail(SE2GPU_ERR_INVALID, "null parameters");
+    if (p->iterations < 0) return fail(SE2GPU_ERR_INVALID, "iterations = %d", p->iterations);
+    return SE2GPU_OK;
+}
+
+int check_topology(int N, const uint8_t* fixed, int E, const int* from, const int* to) {
+    if (N <= 0) return fail(SE2GPU_ERR_INVALID, "N = %d", N);
+    if (E < 0) return fail(SE2GPU_ERR_INVALID, "E = %d", E);
+    if (!fixed || (E && (!from || !to))) return fail(SE2GPU_ERR_INVALID, "null topology arrays");
+    for (int e = 0; e < E; ++e) {
+        if (from[e] < 0 || from[e] >= N || to[e] < 0 || to[e] >= N) return fail(SE2GPU_ERR_INVALID, "edge %d: vertex out of range", e);
+        if (from[e] == to[e]) return fail(SE2GPU_ERR_INVALID, "edge %d: from == to", e);
+    }
+    return SE2GPU_OK;
+}
+
+}  // namespace
+
+struct se2gpu_global_ba_ctx {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t uploaded = nullptr;  // the last plan upload out of the pinned arena has completed
+    cudaEvent_t done = nullptr;      // the last kernel, which reads the plan and work buffers, has completed
+    DeviceBuffers bufs;
+    int* d_int = nullptr; size_t cap_int = 0;
+    long long* d_ll = nullptr; size_t cap_ll = 0;
+    double* d_dbl = nullptr; size_t cap_dbl = 0;
+    unsigned long long* d_prof = nullptr;  // [kPhases] while profiling is on
+    unsigned long long* d_prof_buf = nullptr;
+    PinnedArena arena;
+};
+
+namespace {
+
+template <class T>
+int grow(se2gpu_global_ba_ctx* h, T** p, size_t* cap, size_t need) {
+    if (need <= *cap && *p) return SE2GPU_OK;
+    SE2_CUDA(cudaEventSynchronize(h->done));  // an earlier call, on any stream, may still read the buffer
+    SE2_CUDA(h->bufs.regrow(p, need));
+    *cap = need;
+    return SE2GPU_OK;
+}
+
+size_t al(size_t n) { return (n + 31) & ~(size_t)31; }
+
+// plans the call, uploads the plan on `stream` and launches the kernel there; every value array is device memory
+int run(se2gpu_global_ba_ctx* h, int N, const uint8_t* fixed, int E, const int* from, const int* to, const float* d_Tcw,
+        const float* d_measure, const float* d_info, const int* d_from, const int* d_to, const int* d_edge_status,
+        const se2gpu_global_ba_params* prm, float* d_Tcw_out, int* d_status, int* d_iters, se2gpu_ba_iter_stats* d_stats,
+        double* d_poses, cudaStream_t stream) {
+    const gba::Plan P = gba::make_plan(N, fixed, E, from, to);
+    const int nf = P.n_free, S = (int)P.off_blk.size();
+    const size_t env = (size_t)P.env_blocks();
+    // int arrays: from, to (when not given on the device), pos, vert, first, col_ptr, col_rows, diag_ptr, diag_code, off_ptr, off_code
+    const size_t n_int[11] = {d_from ? 0 : (size_t)E, d_to ? 0 : (size_t)E, (size_t)N, (size_t)nf, (size_t)nf, (size_t)nf + 1,
+                              P.col_rows.size(), (size_t)nf + 1, P.diag_code.size(), (size_t)S + 1, P.off_code.size()};
+    const int* src_int[11] = {from, to, P.pos.data(), P.vert.data(), P.first.data(), P.col_ptr.data(), P.col_rows.data(),
+                              P.diag_ptr.data(), P.diag_code.data(), P.off_ptr.data(), P.off_code.data()};
+    size_t o_int[12] = {0};
+    for (int i = 0; i < 11; ++i) o_int[i + 1] = o_int[i] + al(n_int[i]);
+    const size_t o_ll[3] = {0, al((size_t)nf + 1), al((size_t)nf + 1) + al((size_t)S)};
+    // doubles: X[2] (12 N each), prior (48 N), Zinv (12 E), Om (36 E), lin (120 E), pH (36 nf), pb, b, x (6 nf each), Hs, L (36 env)
+    const size_t n_dbl[11] = {12 * (size_t)N, 12 * (size_t)N, sizeof(Prior) / 8 * (size_t)N, 12 * (size_t)E, 36 * (size_t)E,
+                              kLin * (size_t)E, 36 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 36 * env};
+    size_t o_dbl[13] = {0};
+    for (int i = 0; i < 11; ++i) o_dbl[i + 1] = o_dbl[i] + al(n_dbl[i]);
+    o_dbl[12] = o_dbl[11] + al(36 * env);
+    { const int rc = grow(h, &h->d_int, &h->cap_int, o_int[11]); if (rc) return rc; }
+    { const int rc = grow(h, &h->d_ll, &h->cap_ll, o_ll[2]); if (rc) return rc; }
+    { const int rc = grow(h, &h->d_dbl, &h->cap_dbl, o_dbl[12]); if (rc) return rc; }
+    // the plan goes up through the page-locked arena; the previous call's copies out of it must have completed
+    SE2_CUDA(cudaEventSynchronize(h->uploaded));
+    // the previous call's kernel may run on another stream: this call's plan copies and kernel overwrite what it reads
+    SE2_CUDA(cudaStreamWaitEvent(stream, h->done, 0));
+    size_t bytes = 0;
+    for (int i = 0; i < 11; ++i) bytes += 4 * al(n_int[i]) + 64;
+    bytes += 8 * o_ll[2] + 128;
+    h->arena.reserve(bytes);
+    for (int i = 0; i < 11; ++i) {
+        const int rc = h->arena.up(h->d_int + o_int[i], src_int[i], n_int[i], stream);
+        if (rc) return rc;
+    }
+    { const int rc = h->arena.up((long long*)h->d_ll, (const long long*)P.rowoff.data(), (size_t)nf + 1, stream); if (rc) return rc; }
+    { const int rc = h->arena.up(h->d_ll + o_ll[1], (const long long*)P.off_blk.data(), (size_t)S, stream); if (rc) return rc; }
+    SE2_CUDA(cudaEventRecord(h->uploaded, stream));
+
+    KArgs a{};
+    a.N = N; a.E = E; a.nf = nf; a.S = S; a.iterations = prm->iterations;
+    std::memcpy(a.Tbc, prm->Tbc, sizeof a.Tbc);
+    a.xrot = prm->xrot_info; a.yrot = prm->yrot_info; a.zinfo = prm->z_info;
+    a.Tcw = d_Tcw; a.measure = d_measure; a.info = d_info;
+    a.from = d_from ? d_from : h->d_int + o_int[0];
+    a.to = d_to ? d_to : h->d_int + o_int[1];
+    a.edge_status = d_edge_status;
+    int* I = h->d_int;
+    a.pos = I + o_int[2]; a.vert = I + o_int[3]; a.first = I + o_int[4]; a.col_ptr = I + o_int[5]; a.col_rows = I + o_int[6];
+    a.diag_ptr = I + o_int[7]; a.diag_code = I + o_int[8]; a.off_ptr = I + o_int[9]; a.off_code = I + o_int[10];
+    a.rowoff = h->d_ll; a.off_blk = h->d_ll + o_ll[1];
+    double* D = h->d_dbl;
+    a.X[0] = (Iso*)(D + o_dbl[0]); a.X[1] = (Iso*)(D + o_dbl[1]); a.prior = (Prior*)(D + o_dbl[2]); a.Zinv = (Iso*)(D + o_dbl[3]);
+    a.Om = D + o_dbl[4]; a.lin = D + o_dbl[5]; a.pH = D + o_dbl[6]; a.pb = D + o_dbl[7]; a.b = D + o_dbl[8]; a.x = D + o_dbl[9];
+    a.Hs = D + o_dbl[10]; a.L = D + o_dbl[11];
+    a.Tcw_out = d_Tcw_out; a.status = d_status; a.iters = d_iters; a.stats = d_stats; a.poses = d_poses;
+    a.prof = h->d_prof;
+    if (d_stats && prm->iterations)
+        SE2_CUDA(cudaMemsetAsync(d_stats, 0, sizeof(se2gpu_ba_iter_stats) * (size_t)prm->iterations, stream));
+    SE2_NVTX("se2gpu_global_ba");
+    SE2_LAUNCH(k_global_ba, 1, kThreads, 0, stream, a);
+    SE2_CUDA(cudaGetLastError());
+    SE2_CUDA(cudaEventRecord(h->done, stream));
+    return SE2GPU_OK;
+}
+
+}  // namespace
+
+se2gpu_global_ba_ctx* se2gpu_global_ba_create(int device) {
+    if (select_device(device)) return nullptr;
+    se2gpu_global_ba_ctx* h = new se2gpu_global_ba_ctx;
+    h->device = device;
+    if (cudaStreamCreate(&h->stream) != cudaSuccess || cudaEventCreateWithFlags(&h->uploaded, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
+        fail(SE2GPU_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
+        se2gpu_global_ba_destroy(h);
+        return nullptr;
+    }
+    return h;
+}
+
+void se2gpu_global_ba_destroy(se2gpu_global_ba_ctx* h) {
+    if (!h) return;
+    cudaSetDevice(h->device);
+    if (h->done) cudaEventSynchronize(h->done);
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    if (h->uploaded) cudaEventDestroy(h->uploaded);
+    if (h->done) cudaEventDestroy(h->done);
+    if (h->stream) cudaStreamDestroy(h->stream);
+    delete h;
+}
+
+int se2gpu_global_ba(se2gpu_global_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, int E, const int* edge_from,
+                     const int* edge_to, const float* measure, const float* info, const se2gpu_global_ba_params* params,
+                     float* Tcw_out, int* status, int* iterations, se2gpu_ba_iter_stats* stats, double* poses) {
+    if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
+    { const int rc = check_params(params); if (rc) return rc; }
+    { const int rc = check_topology(N, fixed, E, edge_from, edge_to); if (rc) return rc; }
+    if (!Tcw || !Tcw_out || (E && (!measure || !info))) return fail(SE2GPU_ERR_INVALID, "null arrays");
+    for (int e = 0; e < E; ++e) {
+        const float* I = info + 36 * (size_t)e;
+        for (int r = 0; r < 6; ++r)
+            for (int c = 0; c < 6; ++c) {
+                if (!std::isfinite(I[r * 6 + c])) return fail(SE2GPU_ERR_INVALID, "edge %d: information not finite", e);
+                if (I[r * 6 + c] != I[c * 6 + r]) return fail(SE2GPU_ERR_INVALID, "edge %d: information not symmetric", e);
+            }
+        for (int k = 0; k < 16; ++k)
+            if (!std::isfinite(measure[16 * (size_t)e + k])) return fail(SE2GPU_ERR_INVALID, "edge %d: measurement not finite", e);
+    }
+    HostStage st(h->device);
+    if (const int rc = st.status()) return rc;
+    const float* dT = st.upload(Tcw, 16 * (size_t)N);
+    const float* dm = st.upload(measure, 16 * (size_t)E);
+    const float* di = st.upload(info, 36 * (size_t)E);
+    const int* df = st.upload(edge_from, (size_t)E);
+    const int* dt = st.upload(edge_to, (size_t)E);
+    float* dout = st.output(Tcw_out, 16 * (size_t)N);
+    int* dst = status ? st.output(status, 1) : nullptr;
+    int* dit = iterations ? st.output(iterations, 1) : nullptr;
+    se2gpu_ba_iter_stats* dstats = stats && params->iterations ? st.output(stats, (size_t)params->iterations) : nullptr;
+    double* dposes = poses ? st.output(poses, 7 * (size_t)N) : nullptr;
+    if (const int rc = st.status()) return rc;
+    // h->stream is a blocking stream: the staged copies on the legacy stream order themselves around the kernel
+    { const int rc = run(h, N, fixed, E, edge_from, edge_to, dT, dm, di, df, dt, nullptr, params, dout, dst, dit, dstats, dposes, h->stream); if (rc) return rc; }
+    return st.finish();
+}
+
+int se2gpu_global_ba_device(se2gpu_global_ba_ctx* h, int N, const float* d_Tcw, const uint8_t* fixed, int E, const int* edge_from,
+                            const int* edge_to, const float* d_measure, const float* d_info, const int* d_edge_status,
+                            const se2gpu_global_ba_params* params, float* d_Tcw_out, int* d_status, int* d_iterations,
+                            se2gpu_ba_iter_stats* d_stats, double* d_poses, void* stream) {
+    if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
+    { const int rc = check_params(params); if (rc) return rc; }
+    { const int rc = check_topology(N, fixed, E, edge_from, edge_to); if (rc) return rc; }
+    if (!d_Tcw || !d_Tcw_out || (E && (!d_measure || !d_info))) return fail(SE2GPU_ERR_INVALID, "null arrays");
+    { const int rc = select_device(h->device); if (rc) return rc; }
+    return run(h, N, fixed, E, edge_from, edge_to, d_Tcw, d_measure, d_info, nullptr, nullptr, d_edge_status, params, d_Tcw_out,
+               d_status, d_iterations, d_stats, d_poses, (cudaStream_t)stream);
+}
+
+int se2gpu_global_ba_update_points(int M, const int* kf_index, const float* view_mp, int N, const float* Tcw, float* pos_out,
+                                   int device) {
+    if (M < 0 || N <= 0 || !Tcw || (M && (!kf_index || !view_mp || !pos_out))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    for (int m = 0; m < M; ++m)
+        if (kf_index[m] < 0 || kf_index[m] >= N) return fail(SE2GPU_ERR_INVALID, "kf_index[%d] = %d out of range", m, kf_index[m]);
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
+    if (M == 0) return SE2GPU_OK;
+    const int* dk = st.upload(kf_index, (size_t)M);
+    const float* dv = st.upload(view_mp, 3 * (size_t)M);
+    const float* dT = st.upload(Tcw, 16 * (size_t)N);
+    float* dp = st.output(pos_out, 3 * (size_t)M);
+    if (const int rc = st.status()) return rc;
+    { const int rc = se2gpu_global_ba_update_points_device(M, dk, dv, dT, dp, nullptr); if (rc) return rc; }
+    return st.finish();
+}
+
+int se2gpu_global_ba_update_points_device(int M, const int* d_kf_index, const float* d_view_mp, const float* d_Tcw, float* d_pos_out,
+                                          void* stream) {
+    if (M < 0 || (M && (!d_kf_index || !d_view_mp || !d_Tcw || !d_pos_out))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = require_device(); if (rc) return rc; }
+    if (M == 0) return SE2GPU_OK;
+    SE2_NVTX("se2gpu_global_ba_update_points");
+    SE2_LAUNCH(k_update_points, (M + 255) / 256, 256, 0, (cudaStream_t)stream, M, d_kf_index, d_view_mp, d_Tcw, d_pos_out);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+int se2gpu_global_ba_profile(se2gpu_global_ba_ctx* h, int on) {
+    if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
+    { const int rc = select_device(h->device); if (rc) return rc; }
+    SE2_CUDA(cudaEventSynchronize(h->done));
+    if (!on) { h->d_prof = nullptr; return SE2GPU_OK; }
+    if (!h->d_prof_buf) SE2_CUDA(h->bufs.alloc(&h->d_prof_buf, (size_t)kPhases));
+    SE2_CUDA(cudaMemset(h->d_prof_buf, 0, sizeof(unsigned long long) * kPhases));
+    h->d_prof = h->d_prof_buf;
+    return SE2GPU_OK;
+}
+
+int se2gpu_global_ba_profile_read(se2gpu_global_ba_ctx* h, double* ms) {
+    if (!h || !ms) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (!h->d_prof) return fail(SE2GPU_ERR_INVALID, "profiling is off");
+    { const int rc = select_device(h->device); if (rc) return rc; }
+    SE2_CUDA(cudaEventSynchronize(h->done));
+    unsigned long long ns[kPhases];
+    SE2_CUDA(cudaMemcpy(ns, h->d_prof, sizeof ns, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < kPhases; ++i) ms[i] = ns[i] * 1e-6;
+    return SE2GPU_OK;
+}
