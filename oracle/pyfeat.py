@@ -12,13 +12,13 @@ import subprocess
 
 import numpy as np
 
+from oracle.pyoracle import BA_STATS_DTYPE
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "feat_edge_oracle.cpp")
 LIB_PATH = os.path.join(HERE, "libfeat_edge_oracle.so")
 CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=default", "-Wall",
             "-Wno-unused-function", "-Wno-maybe-uninitialized"]
-STATS_DTYPE = np.dtype([("chi2_before", "f8"), ("chi2_after", "f8"), ("lambda", "f8"), ("rho", "f8"),
-                        ("trials", "i4"), ("accepted", "i4"), ("terminate", "i4"), ("pad", "i4")])
 
 
 class Params(C.Structure):
@@ -85,7 +85,7 @@ def run(mode, Tcw0, Tcw1, xyz, z0, z1, info0, info1, prm=None, reverse=False, co
     nit = max(prm.iterations[mode], 1)
     measure = np.zeros(16, np.float32); info = np.zeros(36, np.float32)
     outlier = np.zeros(max(P, 1), np.uint8); poses = np.zeros(14); points = np.zeros(max(3 * P, 1))
-    stats = np.zeros(nit, STATS_DTYPE); trace = np.zeros(nit * 24); Hm = np.zeros(144)
+    stats = np.zeros(nit, BA_STATS_DTYPE); trace = np.zeros(nit * 24); Hm = np.zeros(144)
     status = C.c_int(0)
     pad = lambda a, w: a if P else np.zeros((1, w), a.dtype)
     n = lib().feat_edge_oracle_run(int(mode), _p(T0), _p(T1), P, _p(pad(xyz, 3)), _p(pad(z0, 3)), _p(pad(z1, 3)), _p(pad(o0, 9)),

@@ -12,7 +12,8 @@ import subprocess
 
 import numpy as np
 
-from oracle.pyfeat import CXXFLAGS, STATS_DTYPE
+from oracle.pyfeat import CXXFLAGS
+from oracle.pyoracle import BA_STATS_DTYPE
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "global_ba_oracle.cpp")
@@ -103,7 +104,7 @@ def run(g, prm, reverse=False, reverse_order=False):
     order_buf = order if len(order) else np.zeros(1, np.int32)
     out = np.zeros((N, 16), np.float32)
     poses = np.zeros((N, 7))
-    stats = np.zeros(max(prm.iterations, 1), STATS_DTYPE)
+    stats = np.zeros(max(prm.iterations, 1), BA_STATS_DTYPE)
     status = C.c_int(0)
     n = lib().global_ba_oracle_run(N, _p(T), _p(fixed), E, _p(fr), _p(to), _p(me), _p(inf), C.addressof(prm), _p(order_buf), _p(out), _p(poses),
                                    _p(stats), int(bool(reverse)), C.addressof(status))

@@ -11,13 +11,13 @@ import subprocess
 
 import numpy as np
 
+from oracle.pyoracle import BA_STATS_DTYPE
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "pose_ba_oracle.cpp")
 LIB_PATH = os.path.join(HERE, "libpose_ba_oracle.so")
 CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=default", "-Wall",
             "-Wno-unused-function", "-Wno-maybe-uninitialized"]
-STATS_DTYPE = np.dtype([("chi2_before", "f8"), ("chi2_after", "f8"), ("lambda", "f8"), ("rho", "f8"),
-                        ("trials", "i4"), ("accepted", "i4"), ("terminate", "i4"), ("pad", "i4")])
 
 
 def build(force: bool = False) -> str:
@@ -58,7 +58,7 @@ def _f(a, shape):
 
 def run(Tcw, xyz, uv, info, fx, cx, cy, Tbc, huber_delta, xrot=1e6, yrot=1e6, zinfo=1.0, iterations=30):
     """One DoLocalBA problem. Returns dict(Tcw [4,4] float32, pose [7] (qx,qy,qz,qw,tx,ty,tz), iterations, status,
-    stats [iterations done] STATS_DTYPE, trace [iterations done, 7])."""
+    stats [iterations done] BA_STATS_DTYPE, trace [iterations done, 7])."""
     T = _f(Tcw, 16).copy()
     xyz = _f(xyz, (-1, 3)); E = len(xyz)
     uv = _f(uv, (-1, 2)); w = _f(info, -1)
@@ -66,7 +66,7 @@ def run(Tcw, xyz, uv, info, fx, cx, cy, Tbc, huber_delta, xrot=1e6, yrot=1e6, zi
     xyz_ = xyz if E else np.zeros((1, 3), np.float32)
     uv_ = uv if E else np.zeros((1, 2), np.float32)
     w_ = w if E else np.zeros(1, np.float32)
-    stats = np.zeros(max(iterations, 1), STATS_DTYPE)
+    stats = np.zeros(max(iterations, 1), BA_STATS_DTYPE)
     trace = np.zeros((max(iterations, 1), 7))
     pose = np.zeros(7); status = C.c_int(0)
     n = lib().pose_ba_oracle_run(_p(T), E, _p(xyz_), _p(uv_), _p(w_), float(fx), float(cx), float(cy), _p(_f(Tbc, 16)),

@@ -15,8 +15,8 @@
 // Both modes call the same LM phase functions (section "LM phase functions" below): pk_landmark (EdgeSE2XYZ error, Huber
 // weighting, Hll/bl, Hpl/PH records), pk_odo (PreEdgeSE2), lm_damp (damping terms), pk_pose_item and pose_odo_gather
 // (pose-side gather), schur_pairs / schur_odo / schur_pose_sweep (Schur gathers of ba_schur and pk_phase_schur_par),
-// pose_oplus / pose_scale, lm_gain_step and lm_lambda_init (LM control), diag_absmax and cta_max (lambda_0); sym3_inverse
-// (sym3.h) is shared with the LDL^T solvers. pk_schur_item and the landmark back-substitution keep a copy per mode (see
+// pose_oplus / pose_scale, diag_absmax and cta_max (lambda_0); the LM control is lm.h's, and sym3_inverse (sym3.h) is
+// shared with the LDL^T solvers. pk_schur_item and the landmark back-substitution keep a copy per mode (see
 // there: register allocation of ba_persistent). The multi-launch kernels:
 //   ba_linearize<JAC>   per landmark (one thread, JAC) or robust chi2 only (!JAC, at x_trial); extra blocks do the
 //                       PreEdgeSE2 odometry edges
@@ -38,6 +38,7 @@
 #include <algorithm>
 
 #include "ba_context.h"
+#include "lm.h"
 #include "sym3.h"
 
 using namespace se2ba;
@@ -45,6 +46,10 @@ using namespace se2ba;
 namespace {
 
 using se2gpu::fail;
+using se2gpu::lm_gain_step;
+using se2gpu::lm_iter_stats;
+using se2gpu::lm_lambda_init;
+using se2gpu::lm_retry;
 
 constexpr int CHOL_THREADS = 512;
 
@@ -165,30 +170,6 @@ __device__ double cta_max(double v, double* sh) {
 // max |diagonal| of the symmetric 3x3 block j of a component-major array H [6][stride] (Hll or Hpp)
 __device__ __forceinline__ double diag_absmax(const double* H, size_t stride, int j) {
     return fmax(fabs(H[j]), fmax(fabs(H[3 * stride + j]), fabs(H[5 * stride + j])));
-}
-
-// OptimizationAlgorithmLevenberg::computeLambdaInit: lambda_0 = 1e-5 * max |diag H| over all free vertices
-__device__ __forceinline__ void lm_lambda_init(double max_diag, double& lambda, double& ni) {
-    lambda = 1e-5 * max_diag;
-    ni = 2.0;
-}
-
-// g2o's gain-ratio test and lambda schedule for one trial (OptimizationAlgorithmLevenberg::solve). tempChi: robust chi2 at
-// the trial point, scale: computeScale() partial sum; both are replaced by the values the test used (a failed solve rejects
-// the trial). Accepting a trial makes the trial buffers current (cur ^= 1). Returns rho.
-__device__ __forceinline__ double lm_gain_step(double& tempChi, double& scale, int solve_ok, double& chi_cur, double& lambda,
-                                               double& ni, int& cur, int& accepted) {
-    if (!solve_ok) { tempChi = DBL_MAX; scale = 0.0; }
-    scale += 1e-3;
-    const double rho = (chi_cur - tempChi) / scale;
-    if (rho > 0 && isfinite(tempChi)) {
-        double alpha = 1. - pow((2 * rho - 1), 3);
-        alpha = fmin(alpha, 2. / 3.);
-        lambda *= fmax(1. / 3., alpha); ni = 2; chi_cur = tempChi; cur ^= 1; accepted = 1;
-    } else {
-        lambda *= ni; ni *= 2;
-    }
-    return rho;
 }
 
 // Damping-dependent terms of landmark j from its sums Hll = {h00 .. h22} and bl = {b0, b1, b2}: (Hll + lambda I)^-1, stored
@@ -464,7 +445,7 @@ __global__ void __launch_bounds__(POSE_THREADS) ba_pose_reduce(Dev d) {
 }
 
 // start of an LM iteration: currentChi from the linearisation partials; lambda init at iteration 0
-// (OptimizationAlgorithmLevenberg::computeLambdaInit: 1e-5 * max |diag H| over all free vertices).
+// (lm_lambda_init over the max |diag H| of all free vertices).
 // In sharded mode the host has all-reduced scal[0] (chi) and scal[1] (max diag) before `finish` runs.
 __global__ void __launch_bounds__(256) ba_iter_begin(Dev d, int iter, int phase /*0: local partials -> scal, 1: consume scal*/, int itg /*g2o iteration number: lambda is initialised at 0 only*/) {
     __shared__ double sh[32];
@@ -1058,18 +1039,15 @@ __global__ void __launch_bounds__(256) ba_decide(Dev d, int nb_scale, int phase,
         if (threadIdx.x == 0) {
             LMState& s = *d.st;
             s.stop_all = d.scal[2] > 0.0 ? 1 : 0;
-            double tempChi = d.scal[0], scale = d.scal[1];
-            const double rho = lm_gain_step(tempChi, scale, s.solve_ok, s.chi_cur, s.lambda, s.ni, s.cur, s.accepted);
+            double tempChi = d.scal[0], scale = d.scal[1], rho;
+            if (lm_gain_step(tempChi, scale, s.solve_ok, s.chi_cur, s.lambda, s.ni, rho)) { s.cur ^= 1; s.accepted = 1; }
             s.chi_trial = tempChi; s.scale = scale; s.rho = rho;
             s.trials += 1;
-            s.retry = (rho < 0 && s.trials < 10 && !s.stop_all) ? 1 : 0;
+            s.retry = (lm_retry(rho, s.trials) && !s.stop_all) ? 1 : 0;
             if (!s.retry) {
-                s.terminate = (s.trials == 10 || rho == 0) ? 1 : 0;
-                if (stats_dev) {
-                    se2gpu_ba_iter_stats& o = stats_dev[s.iter];
-                    o.chi2_before = s.chi_before; o.chi2_after = s.chi_cur; o.lambda = s.lambda; o.rho = rho;
-                    o.trials = s.trials; o.accepted = s.accepted; o.terminate = s.terminate; o.pad = 0;
-                }
+                const se2gpu_ba_iter_stats o = lm_iter_stats(s.chi_before, s.chi_cur, s.lambda, rho, s.trials, s.accepted);
+                s.terminate = o.terminate;
+                if (stats_dev) stats_dev[s.iter] = o;
             }
         }
     }
@@ -1735,21 +1713,17 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
                 tempChi = 0; scale = 0; ab = 0;
                 for (int r = 0; r < shd.world; ++r) { const double* sl = xslot_of(r, epoch); tempChi += __ldcv(sl); scale += __ldcv(sl + 1); ab += __ldcv(sl + 2); }
             }
-            rho = lm_gain_step(tempChi, scale, solve_ok, chi_cur, lambda, ni, cur, accepted);
+            if (lm_gain_step(tempChi, scale, solve_ok, chi_cur, lambda, ni, rho)) { cur ^= 1; accepted = 1; }
             ++trials;
             stop = ab > 0.0;
-        } while (rho < 0 && trials < 10 && !stop);
+        } while (lm_retry(rho, trials) && !stop);
         if (peer_err) break;
-        const int terminate = (trials == 10 || rho == 0) ? 1 : 0;
-        if (blockIdx.x == 0 && threadIdx.x == 0 && pa.stats) {
-            se2gpu_ba_iter_stats& o = pa.stats[it];
-            o.chi2_before = chi_before; o.chi2_after = chi_cur; o.lambda = lambda; o.rho = rho;
-            o.trials = trials; o.accepted = accepted; o.terminate = terminate; o.pad = 0;
-        }
+        const se2gpu_ba_iter_stats o = lm_iter_stats(chi_before, chi_cur, lambda, rho, trials, accepted);
+        if (blockIdx.x == 0 && threadIdx.x == 0 && pa.stats) pa.stats[it] = o;
         if (pa.trace_p) for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * d.P; i += gridDim.x * blockDim.x) pa.trace_p[(size_t)it * 3 * d.P + i] = d.xp[cur][i];
         if (pa.trace_l) for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * d.L; i += gridDim.x * blockDim.x) pa.trace_l[(size_t)it * 3 * d.L + i] = d.xl[cur][i];
         ++done;
-        if (terminate) stop = true;
+        if (o.terminate) stop = true;
     }
     PK_TICK(6);
 #undef PK_TICK
@@ -2153,14 +2127,11 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
             stop_all = h->st_host->stop_all != 0;
         }
         const LMState& st = *h->st_host;
-        if (stats) {
-            se2gpu_ba_iter_stats o{st.chi_before, st.chi_cur, st.lambda, st.rho, st.trials, st.accepted,
-                                   (st.trials == 10 || st.rho == 0) ? 1 : 0, 0};
-            stats[it] = o;
-        }
+        const se2gpu_ba_iter_stats o = lm_iter_stats(st.chi_before, st.chi_cur, st.lambda, st.rho, st.trials, st.accepted);
+        if (stats) stats[it] = o;
         if (trace_poses) SE2_CUDA(cudaMemcpyAsync(trace_poses + (size_t)it * 3 * h->P, d.xp[st.cur], sizeof(double) * 3 * h->P, cudaMemcpyDeviceToHost, s));
         if (trace_points) SE2_CUDA(cudaMemcpyAsync(trace_points + (size_t)it * 3 * h->L, d.xl[st.cur], sizeof(double) * 3 * h->L, cudaMemcpyDeviceToHost, s));
-        ok = !(st.trials == 10 || st.rho == 0);
+        ok = !o.terminate;
         ++done;
     }
     SE2_CUDA(cudaStreamSynchronize(s));

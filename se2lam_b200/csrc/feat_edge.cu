@@ -22,6 +22,7 @@
 #include <cstring>
 
 #include "common.h"
+#include "lm.h"
 #include "se3iso.h"
 
 using namespace se2gpu;
@@ -304,53 +305,6 @@ __device__ __noinline__ void marg_pass(const SE3* KFi, const SE3 (*KFdi)[6], con
     }
 }
 
-// fixed-order block sum of N per-thread values: xor-shuffle tree, then the warps in index order by thread 0
-template <int N>
-__device__ inline void block_sum(double* a, double (*red)[kRed], double* out) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k)
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) a[k] += __shfl_xor_sync(0xffffffffu, a[k], off);
-    __syncthreads();  // red may still be read from the previous sum
-    if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < N; ++k) red[warp][k] = a[k];
-    __syncthreads();
-    if (threadIdx.x == 0)
-        for (int k = 0; k < N; ++k) {
-            double s = red[0][k];
-            for (int w = 1; w < kWarps; ++w) s += red[w][k];
-            out[k] = s;
-        }
-}
-
-// dense LL^T of the n x n system H (row stride 12) and x = H^-1 b; L is scratch; false when not positive definite
-__device__ bool chol_solve(int n, const double* H, const double* b, double* L, double* x) {
-    for (int r = 0; r < n; ++r)
-        for (int c = 0; c <= r; ++c) {
-            double s = H[r * 12 + c];
-            for (int k = 0; k < c; ++k) s -= L[r * 12 + k] * L[c * 12 + k];
-            if (c == r) {
-                if (!(s > 0.0) || !isfinite(s)) return false;
-                L[r * 12 + r] = sqrt(s);
-            } else {
-                L[r * 12 + c] = s / L[c * 12 + c];
-            }
-        }
-    for (int r = 0; r < n; ++r) {
-        double s = b[r];
-        for (int k = 0; k < r; ++k) s -= L[r * 12 + k] * x[k];
-        x[r] = s / L[r * 12 + r];
-    }
-    for (int r = n - 1; r >= 0; --r) {
-        double s = x[r];
-        for (int k = r + 1; k < n; ++k) s -= L[k * 12 + r] * x[k];
-        x[r] = s / L[r * 12 + r];
-    }
-    return true;
-}
-
 // inverse by LU with partial pivoting (what Eigen's inverse() does above 4 x 4); M is destroyed
 __device__ void lu_inverse(int n, double* M, double* inv) {
     for (int i = 0; i < n * n; ++i) inv[i] = 0;
@@ -462,11 +416,6 @@ __device__ __noinline__ void info_se3(const SE3& K1, const SE3& K2, double* Hm, 
         for (int c = 0; c < 6; ++c) I[r * 6 + c] = (S[r * 6 + c] + S[c * 6 + r]) / 2;
 }
 
-__device__ inline void store_pose(const SE3& T, double* p7) {
-    p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
-    p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
-}
-
 __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict__ Tcw0, const float* __restrict__ Tcw1,
                                                         const int* __restrict__ point_ptr, const float* __restrict__ xyz,
                                                         const float* __restrict__ z0, const float* __restrict__ z1,
@@ -479,7 +428,7 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
     extern __shared__ double s_stage[];  // [2][kStageMax*9] Omega, then [2][kStageMax*3] z as float
     __shared__ double s_red[kWarps][kRed];
     __shared__ double s_sum[3][kRed];    // the reduced blocks 00 (+ b0), 11 (+ b1 + chi2), 01
-    __shared__ double s_H[144], s_L[144], s_b[12], s_xp[12], s_w[432];
+    __shared__ double s_H[144], s_b[12], s_xp[12], s_w[432];
     __shared__ double s_Hprior[2][36], s_bprior[2][6];
     __shared__ Prior s_prior[2];
     __shared__ Iso s_X[2], s_trial[2];
@@ -527,30 +476,25 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
             for (int k = free0 ? 0 : 1; k < 2; ++k) s_pchi += prior_terms(s_prior[k], s_X[k], s_Hprior[k], s_bprior[k]);
             s_last_trial = 0;
         }
-        if (it == 0) {  // OptimizationAlgorithmLevenberg::computeLambdaInit over every free vertex, tau = 1e-5
+        if (it == 0) {  // computeLambdaInit over every free vertex
             double acc[13];
 #pragma unroll
             for (int k = 0; k < 13; ++k) acc[k] = 0;
             for (int j = tid; j < P; j += kThreads) point_pass<kDiag>(Xi, pts + 3 * j, m, j, p.delta, 0.0, free0, nullptr, acc, nullptr);
-            double hmax = acc[12];
-            for (int off = 16; off > 0; off >>= 1) hmax = fmax(hmax, __shfl_xor_sync(0xffffffffu, hmax, off));
-            acc[12] = 0;
-            block_sum<12>(acc, s_red, s_sum[0]);
-            __syncthreads();
-            if ((tid & 31) == 0) s_red[tid >> 5][0] = hmax;
-            __syncthreads();
+            const double hmax = acc[12];
+            cta_sum<12>(acc, s_red, s_sum[0]);
+            double mx = cta_max(hmax, s_red);
             if (tid == 0) {
-                double mx = 0;
-                for (int w = 0; w < kWarps; ++w) mx = fmax(mx, s_red[w][0]);
                 for (int k = free0 ? 0 : 1; k < 2; ++k)
                     for (int i = 0; i < 6; ++i) mx = fmax(mx, fabs(s_sum[0][6 * k + i] + s_Hprior[k][i * 7]));
-                s_lambda = 1e-5 * mx;
-                s_ni = 2;
+                lm_lambda_init(mx, s_lambda, s_ni);
             }
             __syncthreads();
         }
+        // the iteration's stats live in st from here on: with chi2_before in a scalar instead, nvcc 12.9 contracts the
+        // quat_to_R of iso_from_Tcw(Tcw0) above differently (another FMA), and the start rotation changes by an ulp
         se2gpu_ba_iter_stats st{};
-        int qmax = 0, failed = 0;
+        int qmax = 0, failed = 0, accepted = 0;
         double rho = 0;
         for (;;) {
             __syncthreads();
@@ -560,16 +504,16 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
 #pragma unroll
                 for (int k = 0; k < 34; ++k) acc[k] = 0;
                 for (int j = tid; j < P; j += kThreads) point_pass<kBlock11>(Xi, pts + 3 * j, m, j, p.delta, lambda, free0, nullptr, acc, nullptr);
-                block_sum<34>(acc, s_red, s_sum[1]);
+                cta_sum<34>(acc, s_red, s_sum[1]);
                 if (free0) {
 #pragma unroll
                     for (int k = 0; k < 34; ++k) acc[k] = 0;
                     for (int j = tid; j < P; j += kThreads) point_pass<kBlock00>(Xi, pts + 3 * j, m, j, p.delta, lambda, free0, nullptr, acc, nullptr);
-                    block_sum<34>(acc, s_red, s_sum[0]);
+                    cta_sum<34>(acc, s_red, s_sum[0]);
 #pragma unroll
                     for (int k = 0; k < 36; ++k) acc[k] = 0;
                     for (int j = tid; j < P; j += kThreads) point_pass<kBlock01>(Xi, pts + 3 * j, m, j, p.delta, lambda, free0, nullptr, acc, nullptr);
-                    block_sum<36>(acc, s_red, s_sum[2]);
+                    cta_sum<36>(acc, s_red, s_sum[2]);
                 }
             }
             double scale = 0;
@@ -593,7 +537,8 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
                     for (int r = 0; r < 6; ++r)
                         for (int c = 0; c < 6; ++c) { s_H[r * 12 + 6 + c] = s_sum[2][r * 6 + c]; s_H[(6 + c) * 12 + r] = s_sum[2][r * 6 + c]; }
                 double x[12];
-                const bool ok2 = chol_solve(n, s_H, s_b, s_L, x);
+                const bool ok2 = chol_factor(n, 12, s_H);
+                if (ok2) chol_solve(n, 12, s_H, s_b, x);
                 s_ok2 = ok2;
                 for (int i = 0; i < 12; ++i) s_xp[i] = 0;
                 double sp = 0;
@@ -626,7 +571,7 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
                     }
                 }
                 double tot[3];
-                block_sum<2>(a, s_red, tot);
+                cta_sum<2>(a, s_red, tot);
                 if (tid == 0) {
                     double pchi = 0;
                     for (int k = free0 ? 0 : 1; k < 2; ++k) pchi += prior_terms(s_prior[k], s_trial[k], nullptr, nullptr);
@@ -637,23 +582,10 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
             }
             if (tid == 0) {
                 if (!s_ok2) ++failed;
-                rho = (s_cur - temp) / (scale + 1e-3);
-                s_accept = 0;
-                if (rho > 0 && isfinite(temp)) {
-                    double alpha = 1. - pow((2 * rho - 1), 3);
-                    alpha = fmin(alpha, 2. / 3.);
-                    s_lambda *= fmax(1. / 3., alpha);
-                    s_ni = 2;
-                    s_cur = temp;
-                    s_X[0] = s_trial[0]; s_X[1] = s_trial[1];
-                    st.accepted = 1;
-                    s_accept = 1;
-                } else {
-                    s_lambda *= s_ni;
-                    s_ni *= 2;
-                }
+                s_accept = lm_gain_step(temp, scale, s_ok2, s_cur, s_lambda, s_ni, rho);
+                if (s_accept) { s_X[0] = s_trial[0]; s_X[1] = s_trial[1]; accepted = 1; }
                 ++qmax;
-                s_more = rho < 0 && qmax < 10;
+                s_more = lm_retry(rho, qmax);
             }
             __syncthreads();
             if (s_accept)
@@ -663,9 +595,8 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
             if (!s_more) break;
         }
         if (tid == 0) {
-            st.chi2_after = s_cur; st.lambda = s_lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            last_failed = st.terminate && failed == qmax;
+            st = lm_iter_stats(st.chi2_before, s_cur, s_lambda, rho, qmax, accepted);
+            last_failed = lm_not_pd(st, failed);
             if (stats) stats[(size_t)pb * p.iterations + it] = st;
             if (trace)
                 for (int k = 0; k < 2; ++k) {
@@ -713,8 +644,8 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
             else if (pass == 1) marg_pass<kBlock11>(s_KFi, s_KFdi, pts + 3 * j, m, j, acc);
             else marg_pass<kBlock01>(s_KFi, s_KFdi, pts + 3 * j, m, j, acc);
         }
-        if (pass < 2) block_sum<21>(acc, s_red, s_sum[pass]);
-        else block_sum<36>(acc, s_red, s_sum[2]);
+        if (pass < 2) cta_sum<21>(acc, s_red, s_sum[pass]);
+        else cta_sum<36>(acc, s_red, s_sum[2]);
     }
     __syncthreads();
     if (tid == 0) {
@@ -731,15 +662,7 @@ __global__ void __launch_bounds__(kThreads) k_feat_edge(const float* __restrict_
             for (int c = 0; c < 6; ++c) { s_H[r * 12 + 6 + c] = s_sum[2][r * 6 + c]; s_H[(6 + c) * 12 + r] = s_sum[2][r * 6 + c]; }
         double I[36];
         info_se3(s_KF[0], s_KF[1], s_H, s_w, I);
-        const SE3 zo = se3_mul(s_KFi[0], s_KF[1]);
-        double R[9];  // converter.cpp toCvMat(SE3Quat) / toCvMat6f
-        quat_to_R(zo.q, R);
-        float* M = measure + 16 * (size_t)pb;
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) M[r * 4 + c] = (float)R[r * 3 + c];
-            M[r * 4 + 3] = (float)zo.t[r];
-        }
-        M[12] = 0.f; M[13] = 0.f; M[14] = 0.f; M[15] = 1.f;
+        se3_to_f32(se3_mul(s_KFi[0], s_KF[1]), measure + 16 * (size_t)pb);
         for (int i = 0; i < 36; ++i) info[36 * (size_t)pb + i] = (float)I[i];
         if (iters) iters[pb] = it;
         if (status) status[pb] = last_failed ? SE2GPU_FEAT_EDGE_NOT_PD : SE2GPU_FEAT_EDGE_OK;

@@ -19,6 +19,7 @@
 
 #include "common.h"
 #include "global_ba_plan.h"
+#include "lm.h"
 #include "se3iso.h"
 
 using namespace se2gpu;
@@ -44,7 +45,7 @@ struct KArgs {
     const int* col_ptr; const int* col_rows; const int* diag_ptr; const int* diag_code;
     const long long* off_blk; const int* off_ptr; const int* off_code;
     // work
-    Iso* X[2];              // [N] current and trial estimates (which is which: s_cur)
+    Iso* X[2];              // [N] current and trial estimates (which is which: s_buf)
     Prior* prior;           // [N]
     Iso* Zinv;              // [E]
     double* Om;             // [E*36]
@@ -170,29 +171,9 @@ __device__ __noinline__ void edge_linearise(const Iso& Zinv, const double* Om, c
     }
 }
 
-// sum of one value per thread, the same on every thread: xor-shuffle tree, then the warp sums in index order
-__device__ inline double block_sum(double v, double* s_red) {
-    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    __syncthreads();  // s_red may still be read from the previous sum
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = s_red[0];
-    for (int w = 1; w < kWarps; ++w) s += s_red[w];
-    return s;
-}
-
-__device__ inline double block_max(double v, double* s_red) {
-    for (int off = 16; off > 0; off >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, off));
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = s_red[0];
-    for (int w = 1; w < kWarps; ++w) s = fmax(s, s_red[w]);
-    return s;
-}
-
-// activeChi2 at the estimates X: every active edge and every vertex's prior (the fixed ones are constant, but g2o counts them)
-__device__ double total_chi2(const KArgs& a, const Iso* X, double* s_red) {
+// activeChi2 at the estimates X: every active edge and every vertex's prior (the fixed ones are constant, but g2o counts them);
+// valid in thread 0
+__device__ double total_chi2(const KArgs& a, const Iso* X, double (&s_red)[kWarps][1]) {
     double acc = 0;
     for (int e = threadIdx.x; e < a.E; e += kThreads) {
         if (!edge_active(a, e)) continue;
@@ -200,7 +181,9 @@ __device__ double total_chi2(const KArgs& a, const Iso* X, double* s_red) {
         acc += edge_error(a.Zinv[e], a.Om + 36 * (size_t)e, X[a.from[e]], X[a.to[e]], err, nullptr, nullptr);
     }
     for (int v = threadIdx.x; v < a.N; v += kThreads) acc += prior_terms(a.prior[v], X[v], nullptr, nullptr);
-    return block_sum(acc, s_red);
+    double tot = 0;
+    cta_sum<1>(&acc, s_red, &tot);
+    return tot;
 }
 
 __device__ inline const double* blkp(const double* M, const KArgs& a, int p, int q) {
@@ -223,18 +206,7 @@ __device__ bool factor(const KArgs& a, double* s_D, int* s_flag) {
         }
         __syncthreads();
         if (threadIdx.x == 0) {  // dense 6 x 6 LL^T of the pivot
-            int ok = 1;
-            for (int r = 0; r < 6 && ok; ++r)
-                for (int c = 0; c <= r; ++c) {
-                    double s = s_D[r * 6 + c];
-                    for (int t = 0; t < c; ++t) s -= s_D[r * 6 + t] * s_D[c * 6 + t];
-                    if (c == r) {
-                        if (!(s > 0.0) || !isfinite(s)) { ok = 0; break; }
-                        s_D[r * 6 + r] = sqrt(s);
-                    } else {
-                        s_D[r * 6 + c] = s / s_D[c * 6 + c];
-                    }
-                }
+            const int ok = chol_factor(6, 6, s_D);
             double* Lkk = L + 36 * (size_t)(a.rowoff[k] + (k - fk));
             for (int r = 0; r < 6; ++r)
                 for (int c = 0; c < 6; ++c) Lkk[r * 6 + c] = c <= r ? s_D[r * 6 + c] : 0.0;
@@ -318,7 +290,7 @@ __device__ void substitute(const KArgs& a) {
 }
 
 __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
-    __shared__ double s_red[kWarps], s_D[36];
+    __shared__ double s_red[kWarps][1], s_D[36];
     __shared__ double s_cur, s_lambda, s_ni;
     __shared__ int s_flag, s_more, s_stop, s_buf;
     const int tid = threadIdx.x;
@@ -394,16 +366,15 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
         }
         __syncthreads();
         stamp(kGather);
-        if (it == 0) {  // computeLambdaInit: tau = 1e-5 times the largest diagonal entry of the free vertices
+        if (it == 0) {  // computeLambdaInit over the free vertices
             double m = 0;
             for (int idx = tid; idx < a.nf * 6; idx += kThreads)
                 m = fmax(m, fabs(a.Hs[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7]));
-            m = block_max(m, s_red);
-            if (tid == 0) { s_lambda = 1e-5 * m; s_ni = 2; }
+            m = cta_max(m, s_red);
+            if (tid == 0) lm_lambda_init(m, s_lambda, s_ni);
         }
-        se2gpu_ba_iter_stats st{};
-        st.chi2_before = s_cur;
-        int qmax = 0, failed = 0;
+        const double chi_before = s_cur;
+        int qmax = 0, failed = 0, accepted = 0;
         double rho = 0;
         for (;;) {
             __syncthreads();
@@ -428,35 +399,22 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
                     Xt[v] = oplus(X[v], d);
                     for (int r = 0; r < 6; ++r) sc += d[r] * (lambda * d[r] + a.b[6 * (size_t)p + r]);
                 }
-                scale = block_sum(sc, s_red);
+                cta_sum<1>(&sc, s_red, &scale);
                 temp = total_chi2(a, Xt, s_red);
             }
             if (tid == 0) {
                 if (!ok) ++failed;
-                rho = (s_cur - temp) / (scale + 1e-3);
-                if (rho > 0 && isfinite(temp)) {
-                    double alpha = 1. - pow((2 * rho - 1), 3);
-                    alpha = fmin(alpha, 2. / 3.);
-                    s_lambda *= fmax(1. / 3., alpha);
-                    s_ni = 2;
-                    s_cur = temp;
-                    st.accepted = 1;
-                    s_buf ^= 1;
-                } else {
-                    s_lambda *= s_ni;
-                    s_ni *= 2;
-                }
+                if (lm_gain_step(temp, scale, ok, s_cur, s_lambda, s_ni, rho)) { s_buf ^= 1; accepted = 1; }
                 ++qmax;
-                s_more = rho < 0 && qmax < 10;
+                s_more = lm_retry(rho, qmax);
             }
             __syncthreads();
             stamp(kTrial);
             if (!s_more) break;
         }
         if (tid == 0) {
-            st.chi2_after = s_cur; st.lambda = s_lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            last_failed = st.terminate && failed == qmax;
+            const se2gpu_ba_iter_stats st = lm_iter_stats(chi_before, s_cur, s_lambda, rho, qmax, accepted);
+            last_failed = lm_not_pd(st, failed);
             if (a.stats) a.stats[it] = st;
             s_stop = st.terminate;
         }
@@ -469,20 +427,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
     const Iso* X = a.X[s_buf];
     for (int v = tid; v < a.N; v += kThreads) {
         const SE3 T = se3_from_iso(X[v]);
-        double R[9];
-        quat_to_R(T.q, R);
         float Twc[16];
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) Twc[r * 4 + c] = (float)R[r * 3 + c];
-            Twc[r * 4 + 3] = (float)T.t[r];
-        }
-        Twc[12] = 0.f; Twc[13] = 0.f; Twc[14] = 0.f; Twc[15] = 1.f;
+        se3_to_f32(T, Twc);
         rigid_inv_f32(Twc, a.Tcw_out + 16 * (size_t)v);
-        if (a.poses) {
-            double* p7 = a.poses + 7 * (size_t)v;
-            p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
-            p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
-        }
+        if (a.poses) store_pose(T, a.poses + 7 * (size_t)v);
     }
     if (tid == 0) {
         if (a.iters) *a.iters = it;

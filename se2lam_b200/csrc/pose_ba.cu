@@ -18,6 +18,7 @@
 #include <cstring>
 
 #include "common.h"
+#include "lm.h"
 #include "se3quat.h"
 
 using namespace se2gpu;
@@ -166,58 +167,6 @@ __device__ inline void edge_terms(const SE3& T, const float* xyz, const float* u
     }
 }
 
-// fixed-order block sum of N per-thread values: xor-shuffle tree, then the warps in index order by thread 0
-template <int N>
-__device__ inline void block_sum(double* a, double (*red)[kAcc], double* out) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k)
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) a[k] += __shfl_xor_sync(0xffffffffu, a[k], off);
-    if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < N; ++k) red[warp][k] = a[k];
-    __syncthreads();
-    if (threadIdx.x == 0)
-        for (int k = 0; k < N; ++k) {
-            double s = red[0][k];
-            for (int w = 1; w < kWarps; ++w) s += red[w][k];
-            out[k] = s;
-        }
-}
-
-// dense LL^T of H + lam I (H full symmetric 6 x 6) and x = (H + lam I)^-1 b; false when not positive definite
-__device__ bool chol_solve6(const double* H, const double* b, double lam, double* x) {
-    double L[36];
-    for (int r = 0; r < 6; ++r)
-        for (int c = 0; c <= r; ++c) {
-            double s = H[r * 6 + c] + (r == c ? lam : 0.0);
-            for (int k = 0; k < c; ++k) s -= L[r * 6 + k] * L[c * 6 + k];
-            if (c == r) {
-                if (!(s > 0.0) || !isfinite(s)) return false;
-                L[r * 6 + r] = sqrt(s);
-            } else {
-                L[r * 6 + c] = s / L[c * 6 + c];
-            }
-        }
-    for (int r = 0; r < 6; ++r) {
-        double s = b[r];
-        for (int k = 0; k < r; ++k) s -= L[r * 6 + k] * x[k];
-        x[r] = s / L[r * 6 + r];
-    }
-    for (int r = 5; r >= 0; --r) {
-        double s = x[r];
-        for (int k = r + 1; k < 6; ++k) s -= L[k * 6 + r] * x[k];
-        x[r] = s / L[r * 6 + r];
-    }
-    return true;
-}
-
-__device__ inline void store_pose(const SE3& T, double* p7) {
-    p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
-    p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
-}
-
 __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, const int* __restrict__ edge_ptr,
                                                       const float* __restrict__ xyz, const float* __restrict__ uv,
                                                       const float* __restrict__ info, Params p, int min_edges,
@@ -271,9 +220,9 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
             for (int k = 0; k < kAcc; ++k) acc[k] = 0;
             const SE3 T = s_est;
             for (int e = tid; e < E; e += kThreads) edge_terms<true>(T, px + 3 * e, pu + 2 * e, pw[e], p, acc[27], acc);
-            block_sum<kAcc>(acc, s_red, s_sum);
+            cta_sum<kAcc>(acc, s_red, s_sum);
         }
-        se2gpu_ba_iter_stats st{};
+        double chi_before = 0;
         if (tid == 0) {
             double ep[6];
             const double pchi = prior_error(s_meas, s_info, s_est, ep);
@@ -286,22 +235,25 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
                 s_b[r] = s_sum[21 + r] + we;
             }
             s_cur = s_sum[27] + pchi;
-            if (it == 0) {  // OptimizationAlgorithmLevenberg::computeLambdaInit, tau = 1e-5
+            if (it == 0) {
                 double m = 0;
                 for (int r = 0; r < 6; ++r) m = fmax(m, fabs(s_H[r * 7]));
-                s_lambda = 1e-5 * m;
-                s_ni = 2;
+                lm_lambda_init(m, s_lambda, s_ni);
             }
-            st.chi2_before = s_cur;
+            chi_before = s_cur;
         }
-        int qmax = 0, failed = 0;
+        int qmax = 0, failed = 0, accepted = 0;
         double rho = 0;
         for (;;) {
             double x[6], scale = 0;
             if (tid == 0) {
-                const bool ok2 = chol_solve6(s_H, s_b, s_lambda, x);
+                double L[36];  // LL^T of H + lambda I
+                for (int r = 0; r < 6; ++r)
+                    for (int c = 0; c <= r; ++c) L[r * 6 + c] = s_H[r * 6 + c] + (r == c ? s_lambda : 0.0);
+                const bool ok2 = chol_factor(6, 6, L);
                 s_ok2 = ok2;
                 if (ok2) {
+                    chol_solve(6, 6, L, s_b, x);
                     s_trial = se3_mul(se3_exp(x), s_est);
                     for (int r = 0; r < 6; ++r) scale += x[r] * (s_lambda * x[r] + s_b[r]);
                 }
@@ -313,7 +265,7 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
                 const SE3 T = s_trial;
                 for (int e = tid; e < E; e += kThreads) edge_terms<false>(T, px + 3 * e, pu + 2 * e, pw[e], p, a[0], nullptr);
                 double tot[1];
-                block_sum<1>(a, s_red, tot);
+                cta_sum<1>(a, s_red, tot);
                 if (tid == 0) {
                     double ep[6];
                     temp = tot[0] + prior_error(s_meas, s_info, s_trial, ep);
@@ -321,29 +273,16 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
             }
             if (tid == 0) {
                 if (!s_ok2) ++failed;
-                rho = (s_cur - temp) / (scale + 1e-3);
-                if (rho > 0 && isfinite(temp)) {
-                    double alpha = 1. - pow((2 * rho - 1), 3);
-                    alpha = fmin(alpha, 2. / 3.);
-                    s_lambda *= fmax(1. / 3., alpha);
-                    s_ni = 2;
-                    s_cur = temp;
-                    s_est = s_trial;
-                    st.accepted = 1;
-                } else {
-                    s_lambda *= s_ni;
-                    s_ni *= 2;
-                }
+                if (lm_gain_step(temp, scale, s_ok2, s_cur, s_lambda, s_ni, rho)) { s_est = s_trial; accepted = 1; }
                 ++qmax;
-                s_more = rho < 0 && qmax < 10;
+                s_more = lm_retry(rho, qmax);
             }
             __syncthreads();
             if (!s_more) break;
         }
         if (tid == 0) {
-            st.chi2_after = s_cur; st.lambda = s_lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            last_failed = st.terminate && failed == qmax;
+            const se2gpu_ba_iter_stats st = lm_iter_stats(chi_before, s_cur, s_lambda, rho, qmax, accepted);
+            last_failed = lm_not_pd(st, failed);
             if (stats) stats[(size_t)pb * p.iterations + it] = st;
             if (trace) store_pose(s_est, trace + ((size_t)pb * p.iterations + it) * 7);
             s_stop = st.terminate;
@@ -355,13 +294,7 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
         if (iters) iters[pb] = it;
         if (status) status[pb] = last_failed ? SE2GPU_POSE_BA_NOT_PD : SE2GPU_POSE_BA_OK;
         if (pose_out) store_pose(s_est, pose_out + 7 * (size_t)pb);
-        double R[9];  // converter.cpp toCvMat(SE3Quat): to_homogeneous_matrix narrowed to float
-        quat_to_R(s_est.q, R);
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) T16[r * 4 + c] = (float)R[r * 3 + c];
-            T16[r * 4 + 3] = (float)s_est.t[r];
-        }
-        T16[12] = 0.f; T16[13] = 0.f; T16[14] = 0.f; T16[15] = 1.f;
+        se3_to_f32(s_est, T16);
     }
 }
 

@@ -1,7 +1,7 @@
 // g2o::VertexSE3 (an Eigen::Isometry3d estimate with oplus = X * fromVectorMQT) and the EdgeSE3Prior of
-// addVertexSE3PlaneMotion, restated for device code in double precision. Shared by the feature-graph constraint
-// (feat_edge.cu) and the global pose graph (global_ba.cu). The functions that are not inline keep internal linkage, as
-// they had inside feat_edge.cu, so each kernel file compiles them exactly as before.
+// addVertexSE3PlaneMotion, restated for device code in double precision, on top of se3quat.h. Used by the feature-graph
+// constraint (feat_edge.cu) and the global pose graph (global_ba.cu). The functions that are not inline keep internal
+// linkage, as they had inside feat_edge.cu, so each kernel file compiles them exactly as before.
 #pragma once
 #include "se3quat.h"
 

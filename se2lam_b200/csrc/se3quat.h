@@ -1,5 +1,6 @@
-// g2o::SE3Quat and the Eigen quaternion routines it rests on, restated for device code in double precision. Shared by the
-// pose-only BA (pose_ba.cu) and the feature-graph constraint (feat_edge.cu).
+// g2o::SE3Quat and the Eigen quaternion routines it rests on, restated for device code in double precision. Used by the
+// pose-only BA (pose_ba.cu), and through se3iso.h by the feature-graph constraint (feat_edge.cu) and the global pose graph
+// (global_ba.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -88,6 +89,23 @@ __device__ inline SE3 se3_from_f32(const float* T) {
     r.t[0] = T[3]; r.t[1] = T[7]; r.t[2] = T[11];
     normalize_rotation(r.q);
     return r;
+}
+
+// converter.cpp toCvMat(SE3Quat): to_homogeneous_matrix narrowed to a float 4x4 row-major
+__device__ inline void se3_to_f32(const SE3& T, float* M) {
+    double R[9];
+    quat_to_R(T.q, R);
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) M[r * 4 + c] = (float)R[r * 3 + c];
+        M[r * 4 + 3] = (float)T.t[r];
+    }
+    M[12] = 0.f; M[13] = 0.f; M[14] = 0.f; M[15] = 1.f;
+}
+
+// the pose as the library returns it: (qx, qy, qz, qw, tx, ty, tz)
+__device__ inline void store_pose(const SE3& T, double* p7) {
+    p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
+    p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
 }
 
 __device__ inline SE3 se3_mul(const SE3& a, const SE3& b) {

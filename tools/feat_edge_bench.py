@@ -2,7 +2,10 @@
 one call, 50 and 300 points per pair, both modes, through the host entry (copies included, host clock around a synchronous
 call) and the device entry (CUDA events around the launch on resident buffers), against the CPU oracle on one core.
 
-    python tools/feat_edge_bench.py [--reps 50] [--json out.json]
+    python tools/feat_edge_bench.py [--reps 50] [--json out.json] [--dump-outputs DIR]
+
+--dump-outputs writes, per mode and size, every output of the host entry (with the pose trace) and of the device entry, and
+the host entry's outputs for 256 pairs per mode whose start poses vary in yaw.
 """
 from __future__ import annotations
 
@@ -20,6 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import pyfeat  # noqa: E402
 from se2lam_b200 import _capi, featgraph  # noqa: E402
+from tools import dump  # noqa: E402
 from tools import featgraph_synth as S  # noqa: E402
 
 
@@ -36,6 +40,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last run of each size as DIR/<tag>_<name>.npy")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -79,6 +84,11 @@ def main():
                     ev[1].synchronize()
                     ms += ev[0].elapsed_time(ev[1])
                 dev_us = ms / a.reps * 1e3
+                if a.dump_outputs:
+                    tag = f"feat_m{mode}_P{P}_B{B}"
+                    dump.save(a.dump_outputs, tag, featgraph.UpdateFeatGraph(pairs, prm, mode=mode, trace=True))
+                    dump.save(a.dump_outputs, tag + "_device", dict(measure=meas.cpu().numpy(), info=info.cpu().numpy(),
+                                                                    status=st.cpu().numpy(), points=pts.cpu().numpy()))
                 assert meas.cpu().numpy().tobytes() == np.concatenate([r["measure"].ravel() for r in g]).tobytes()
                 oprm = pyfeat.params(Tbc=pairs[0]["Tbc"])
                 n_cpu = min(B, 8)
@@ -96,6 +106,15 @@ def main():
                                  device_us_per_pair=round(dev_us / B, 2), cpu_oracle_us=round(cpu_us, 1),
                                  cpu_oracle_us_per_pair=round(cpu_us / B, 1)))
                 print(json.dumps(rows[-1]), flush=True)
+    if a.dump_outputs:
+        # 256 pairs per mode with start poses at every yaw, so the dump covers general start rotations, not one
+        rng = np.random.default_rng(7)
+        for mode in (0, 1):
+            pairs = [S.scene(3000 + b, 60, start=(rng.uniform(-5, 5), rng.uniform(-5, 5), rng.uniform(-np.pi, np.pi)),
+                             motion=(rng.uniform(0.1, 0.6), rng.uniform(-0.1, 0.1), rng.uniform(-0.3, 0.3)),
+                             noise=0.3 if mode else 1.0, outlier_share=0.1 if mode else 0.0, outlier_size=(0.2, 0.4)) for b in range(256)]
+            dump.save(a.dump_outputs, f"feat_m{mode}_varied", featgraph.UpdateFeatGraph(pairs, featgraph.params(pairs[0]["Tbc"]), mode=mode,
+                                                                                          trace=True))
     res = dict(gpu=gpu_info(), cpu_oracle="one core, g++ -O2 -ffp-contract=off, ctypes call included", reps=a.reps, rows=rows)
     print(json.dumps(res))
     if a.json:

@@ -4,7 +4,8 @@ Graphs: circles driven several times (tools/posegraph_synth.py), odometry plus f
 keyframe) plus loop closures, 15 LM iterations. Per size: the host entry (uploads, plan, kernel, downloads), the device
 entry on device-resident values (plan upload and kernel), launches per call, the kernel's time per phase
 (se2gpu_global_ba_profile, in a separate run), and the CPU oracle. Prints one JSON line per
-size with the card's name and power limit."""
+size with the card's name and power limit. --dump-outputs DIR writes, per size, every output of the host entry and the
+device entry's poses."""
 from __future__ import annotations
 
 import argparse
@@ -21,6 +22,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import pyglobal  # noqa: E402
 from se2lam_b200 import _capi, globalba  # noqa: E402
+from tools import dump  # noqa: E402
 from tools import posegraph_synth as S  # noqa: E402
 
 
@@ -34,6 +36,7 @@ def main():
     ap.add_argument("--sizes", default="100,500,2000,5000")
     ap.add_argument("--runs", type=int, default=10)
     ap.add_argument("--oracle-runs", type=int, default=1)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last run of each size as DIR/<tag>_<name>.npy")
     a = ap.parse_args()
     import torch
     name = card()
@@ -64,6 +67,9 @@ def main():
         torch.cuda.synchronize()
         dev_ms = (time.perf_counter() - t) / a.runs * 1e3
         launches = (L.se2gpu_launch_count() - l0) / a.runs
+        if a.dump_outputs:
+            dump.save(a.dump_outputs, f"global_N{N}", r)
+            dump.save(a.dump_outputs, f"global_N{N}_device", dict(Tcw=out.cpu().numpy()))
         # the phase split, in a run of its own (the timer reads are not in the timed runs above)
         _capi.check(L.se2gpu_global_ba_profile(ctx.h, 1), "se2gpu_global_ba_profile")
         ctx.run(g["Tcw"], g["fixed"], g["edges"], prm)

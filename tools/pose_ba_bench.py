@@ -2,7 +2,9 @@
 30 LM iterations each, through the host entry (copies included, host clock around a synchronous call) and the device entry
 (CUDA events around the launch on resident buffers), against the CPU oracle on one core.
 
-    python tools/pose_ba_bench.py [--reps 50] [--json out.json]
+    python tools/pose_ba_bench.py [--reps 50] [--json out.json] [--dump-outputs DIR]
+
+--dump-outputs writes, per size, every output of the host entry (with the pose trace) and the device entry's poses.
 """
 from __future__ import annotations
 
@@ -20,6 +22,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import pypose  # noqa: E402
 from se2lam_b200 import pose as pba  # noqa: E402
+from tools import dump  # noqa: E402
 from tools import pose_synth as ps  # noqa: E402
 
 DELTA = math.sqrt(5.991)
@@ -38,6 +41,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last run of each size as DIR/<tag>_<name>.npy")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -68,6 +72,10 @@ def main():
                 ev[1].synchronize()
                 ms += ev[0].elapsed_time(ev[1])
             dev_us = ms / a.reps * 1e3
+            if a.dump_outputs:
+                tag = f"pose_E{E}_B{B}"
+                dump.save(a.dump_outputs, tag, pba.poseOnlyBA(T, ptr, x, u, w, prm, trace=True))
+                dump.save(a.dump_outputs, tag + "_device", dict(Tcw=dT.cpu().numpy()))
             n_cpu = max(1, min(B, 8))
             pypose.run(probs[0]["Tcw"], probs[0]["xyz"], probs[0]["uv"], probs[0]["info"], ps.FX, ps.CX, ps.CY, ps.Tbc_f32(), DELTA)
             cpu_reps = max(1, 16 // n_cpu)
