@@ -493,6 +493,42 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
 #define SE2GPU_BA_PLAN_FIELDS 14
 int se2gpu_ba_debug_plan(se2gpu_ba* h, int* out, int n_out);
 
+/* se2gpu_ba_set_problem with every array in DEVICE memory (same arguments, same layout; Tcb stays a host pointer): the
+ * graph structure (landmark sort, pose lists, block and pair lists of the reduced system, envelope) is built on the
+ * device, and only O(free poses + blocks) ints come back for the host's solver decisions. The inputs are read on the
+ * context's stream (se2gpu_ba_set_stream); the call returns once the window is loaded and the stream is synchronised, so
+ * the caller may then overwrite them. Same contract as se2gpu_ba_set_problem: same-structure windows refresh the values
+ * only, sharded contexts keep their landmarks, out-of-range endpoints return SE2GPU_ERR_INVALID (detected on the device),
+ * capacity errors SE2GPU_ERR_CAPACITY, and on any error the context holds no window. The context ends up holding the
+ * same device arrays, element for element, as after se2gpu_ba_set_problem of the same window. Loads by the other entry
+ * point always rebuild the structure. */
+int se2gpu_ba_set_problem_device(se2gpu_ba* h, int P, int L, int E, int O, const double* d_poses, const uint8_t* d_fixed,
+                                 const double* d_points, const int* d_edge_pose, const int* d_edge_point, const double* d_uv,
+                                 const double* d_info, const int* d_odo_i, const int* d_odo_j, const double* d_odo_meas,
+                                 const double* d_odo_info, double fx, double cx, double cy, const double* Tcb,
+                                 double huber_delta);
+
+/* se2gpu_ba_build_information on DEVICE buffers of the caller's current device, asynchronous on `stream`. An edge whose
+ * pose or landmark index is out of range gets NaN information (the host entry rejects the call instead). */
+int se2gpu_ba_build_information_device(int P, int L, int E, const float* d_view_mp, const int* d_edge_pose,
+                                       const int* d_edge_point, const int* d_octave, const float* d_kf_Rcw,
+                                       const float* d_kf_twb_xy, const float* d_mp_pos, const float* d_level_sigma2,
+                                       int nlevels, float fx, float xrot_info, float z_info, double* d_info, void* stream);
+
+/* test hook: copies min(n_out, length) elements of one structure array the context holds on the device to `out` and
+ * returns the array's length (for the double arrays: their raw 32-bit words, two per double), or SE2GPU_ERR_INVALID with
+ * no window loaded. Changes nothing; the same after either load path. */
+enum {
+    SE2GPU_BA_STRUCT_HIDX, SE2GPU_BA_STRUCT_LM_PTR, SE2GPU_BA_STRUCT_PERM, SE2GPU_BA_STRUCT_E_POSE, SE2GPU_BA_STRUCT_E_HIDX,
+    SE2GPU_BA_STRUCT_POSE_PTR, SE2GPU_BA_STRUCT_POSE_EDGES, SE2GPU_BA_STRUCT_POSE_ODO_PTR, SE2GPU_BA_STRUCT_POSE_ODO,
+    SE2GPU_BA_STRUCT_BLK_A, SE2GPU_BA_STRUCT_BLK_B, SE2GPU_BA_STRUCT_BLK_PAIR_PTR, SE2GPU_BA_STRUCT_PAIR_E1,
+    SE2GPU_BA_STRUCT_PAIR_E2, SE2GPU_BA_STRUCT_BLK_ODO_PTR, SE2GPU_BA_STRUCT_BLK_ODO, SE2GPU_BA_STRUCT_COLMAX,
+    SE2GPU_BA_STRUCT_TW_CMAX1, SE2GPU_BA_STRUCT_BLK_ORDER, SE2GPU_BA_STRUCT_ENV_IDX, SE2GPU_BA_STRUCT_ODO_I,
+    SE2GPU_BA_STRUCT_ODO_J, SE2GPU_BA_STRUCT_E_U, SE2GPU_BA_STRUCT_E_V, SE2GPU_BA_STRUCT_E_W00, SE2GPU_BA_STRUCT_E_W01,
+    SE2GPU_BA_STRUCT_E_W11, SE2GPU_BA_STRUCT_ODO_M, SE2GPU_BA_STRUCT_ODO_W, SE2GPU_BA_STRUCT_COUNT
+};
+int se2gpu_ba_debug_structure(se2gpu_ba* h, int which, int* out, int n_out);
+
 /* ------------------------------------------------------------------------------------------ pose-only BA */
 /* Localizer::DoLocalBA (src/Localizer.cpp:233-302) for B independent problems, one CTA each, every LM iteration on the
  * device: one VertexSE3Expmap (estimate toSE3Quat(Tcw)), the plane-motion EdgeSE3ExpmapPrior of addPlaneMotionSE3Expmap

@@ -87,6 +87,31 @@ class LocalBA:
                                           float(prob.huber_delta)), "se2gpu_ba_set_problem")
         self.P, self.L, self.E, self.O = prob.P, prob.L, prob.E, prob.O
 
+    def set_problem_device(self, P, L, E, O, poses, fixed, points, edge_pose, edge_point, uv, info, odo_i, odo_j, odo_meas,
+                           odo_info, fx, cx, cy, Tcb, huber_delta):
+        """set_problem from device memory (se2gpu_ba_set_problem_device): the same fields in the same order and layout, as
+        torch CUDA tensors or raw device pointers (float64 / uint8 / int32 as in set_problem); Tcb [12] stays on the host.
+        The structure is built on the device; the arrays are read on the context's stream (set_stream)."""
+        tcb = np.ascontiguousarray(Tcb, np.float64)
+        arrays = [poses, fixed, points, edge_pose, edge_point, uv, info, odo_i, odo_j, odo_meas, odo_info]
+        self.P = self.L = self.E = self.O = 0          # a failed load leaves no window
+        check(lib().se2gpu_ba_set_problem_device(self.h, int(P), int(L), int(E), int(O), *[ptr(x) for x in arrays], float(fx),
+                                                 float(cx), float(cy), ptr(tcb), float(huber_delta)), "se2gpu_ba_set_problem_device")
+        self.P, self.L, self.E, self.O = int(P), int(L), int(E), int(O)
+
+    STRUCTURE_ARRAYS = ("hidx", "lm_ptr", "perm", "e_pose", "e_hidx", "pose_ptr", "pose_edges", "pose_odo_ptr", "pose_odo", "blk_a",
+                        "blk_b", "blk_pair_ptr", "pair_e1", "pair_e2", "blk_odo_ptr", "blk_odo", "colmax", "tw_cmax1", "blk_order",
+                        "env_idx", "odo_i", "odo_j", "e_u", "e_v", "e_w00", "e_w01", "e_w11", "odo_m", "odo_w")
+    STRUCTURE_DOUBLES = ("e_u", "e_v", "e_w00", "e_w01", "e_w11", "odo_m", "odo_w")
+
+    def debug_structure(self, which):
+        """One device array of the loaded window (se2gpu_ba_debug_structure) by name; int32, or float64 for the values."""
+        k = self.STRUCTURE_ARRAYS.index(which)
+        n = check(lib().se2gpu_ba_debug_structure(self.h, k, None, 0), "se2gpu_ba_debug_structure")
+        out = np.zeros(n, np.int32)
+        check(lib().se2gpu_ba_debug_structure(self.h, k, ptr(out), n), "se2gpu_ba_debug_structure")
+        return out.view(np.float64) if which in self.STRUCTURE_DOUBLES else out
+
     def optimize(self, iters, trace=False, stop_flag=None, first_iteration=0):
         """first_iteration > 0 continues the lambda / nu schedule of the previous call (g2o's solve(iteration) slices)."""
         st = np.zeros(max(iters, 1), BA_STATS_DTYPE)
@@ -147,7 +172,7 @@ class LocalBA:
 
     PLAN_FIELDS = ("nf", "n", "structure", "env_w", "solver", "tw_m0", "tw_w", "band_w", "band_p", "pk_grid", "workers",
                    "nblk", "max_own", "uncached")
-    STRUCTURES = ("dense", "sorted")
+    STRUCTURES = ("dense", "sorted", "device")
     SOLVERS = ("smem", "twisted", "band", "envelope")
 
     def debug_plan(self):

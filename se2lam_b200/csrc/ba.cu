@@ -1834,6 +1834,7 @@ void se2gpu_ba_destroy(se2gpu_ba* h) {
     if (h->ssum) cudaFree(h->ssum);
     if (h->go) cudaFree(h->go);
     if (h->st_host) cudaFreeHost(h->st_host);
+    if (h->dl.sc_host) cudaFreeHost(h->dl.sc_host);
     delete h;
 }
 
@@ -2275,8 +2276,11 @@ int se2gpu_ba_debug_system(se2gpu_ba* h, double lambda, double* chi2, double* Hp
         if (!get(d.Hpl, EB * (size_t)E)) return fail(SE2GPU_ERR_CUDA, "copy Hpl");
         std::vector<int> eh(E);
         cudaMemcpy(eh.data(), d.e_hidx, sizeof(int) * E, cudaMemcpyDeviceToHost);
+        std::vector<int> dperm;   // a device load keeps the landmark sort on the device only
+        if (h->dl.valid) { dperm.resize(E); cudaMemcpy(dperm.data(), h->dl.perm, sizeof(int) * E, cudaMemcpyDeviceToHost); }
+        const int* perm = h->dl.valid ? dperm.data() : h->perm.data();
         memset(Hpl, 0, sizeof(double) * 9 * (size_t)h->E);
-        for (int k = 0; k < E; ++k) if (eh[k] >= 0) for (int q = 0; q < 9; ++q) Hpl[9 * (size_t)h->perm[k] + q] = tmp[(size_t)k * EB + q];
+        for (int k = 0; k < E; ++k) if (eh[k] >= 0) for (int q = 0; q < 9; ++q) Hpl[9 * (size_t)perm[k] + q] = tmp[(size_t)k * EB + q];
     }
     if (dx_p) { if (!get(d.dxp, n)) return fail(SE2GPU_ERR_CUDA, "copy dxp"); memcpy(dx_p, tmp.data(), tmp.size() * 8); }
     if (dx_l) { if (!get(d.dxl, 3 * (size_t)L)) return fail(SE2GPU_ERR_CUDA, "copy dxl"); memcpy(dx_l, tmp.data(), tmp.size() * 8); }

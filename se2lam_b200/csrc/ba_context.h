@@ -82,6 +82,26 @@ struct Switches {
     bool no_twist = false;          // SE2GPU_BA_NO_TWIST: the persistent kernel's reduced solve stays on one CTA
 };
 
+// What se2gpu_ba_set_problem_device keeps between calls (ba_loader.cu): the loaded topology as device copies, the
+// landmark sort as a device array, and the scratch of the structure build. Every buffer is allocated on first use and grown
+// on demand; the topology copies are valid only after a device load (a host load clears `valid`).
+struct DevLoad {
+    bool valid = false;
+    uint8_t* fixed = nullptr;                                          // [maxP]
+    int *edge_pose = nullptr, *edge_point = nullptr, *odo_i = nullptr, *odo_j = nullptr;   // [maxE], [maxE], [maxO], [maxO]
+    int* perm = nullptr;                                               // [maxE] sorted edge position -> original edge
+    int* sc = nullptr;                                                 // [16] device scalars of the build (DL_* in ba_loader.cu)
+    int* sc_host = nullptr;                                            // [16] page-locked mirror
+    int *k0 = nullptr, *v0 = nullptr, *k1 = nullptr, *v1 = nullptr;   // radix sort ping-pong keys / values
+    int *g1 = nullptr, *g2 = nullptr;                                  // pair (k1, k2) in generation order
+    int *hist = nullptr, *aux = nullptr;                               // radix digit counts, scan block totals
+    int *lo = nullptr, *hi = nullptr;                                  // [L] per-landmark first / last free pose
+    int *pair_off = nullptr;                                           // [El + 1] first pair of each sorted edge
+    unsigned* bits = nullptr; int* wprefix = nullptr;                  // nf x nf block bitmap, popcount prefix per word
+    int* planin = nullptr; std::vector<int> planin_host;               // bmax [nf] | pairs per block | pose edges per diagonal block
+    size_t cap_sort = 0, cap_pairs = 0, cap_hist = 0, cap_aux = 0, cap_lm = 0, cap_off = 0, cap_bits = 0, cap_wprefix = 0, cap_plan = 0;
+};
+
 }  // namespace se2ba
 
 struct se2gpu_ba {
@@ -135,6 +155,8 @@ struct se2gpu_ba {
     se2band::Plan band;        // partitioned band solver for reduced systems beyond one CTA's shared memory
     int smem_optin = 0;
     int plan[SE2GPU_BA_PLAN_FIELDS] = {};   // host-side decisions of the last full set_problem (se2gpu_ba_debug_plan)
+    se2ba::DevLoad dl;                      // se2gpu_ba_set_problem_device
+    long long struct_len[SE2GPU_BA_STRUCT_COUNT] = {};   // element count of each se2gpu_ba_debug_structure array
 };
 
 namespace se2ba {
