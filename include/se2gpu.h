@@ -705,6 +705,69 @@ int se2gpu_global_ba_update_points(int M, const int* kf_index, const float* view
 int se2gpu_global_ba_update_points_device(int M, const int* d_kf_index, const float* d_view_mp, const float* d_Tcw, float* d_pos_out,
                                           void* stream);
 
+/* ------------------------------------------------------------------------------------------ SE(3)-XYZ window BA */
+/* The window of Map::loadLocalGraph (src/Map.cpp:414-566) and Map::loadLocalGraphOnlyBa (:568-698) under g2o's
+ * Levenberg-Marquardt, as LocalMapper::removeOutlierChi2 (src/LocalMapper.cpp:172-230) and the TIME_TO_LOG_LOCAL_BA timing
+ * (:251-276) run it, in double precision (DESIGN.md section 12). One VertexSE3Expmap per keyframe (estimate toSE3Quat(Tcw)),
+ * with the plane-motion EdgeSE3ExpmapPrior of addPlaneMotionSE3Expmap where prior[k] is set; one EdgeSE3Expmap per odometry
+ * link (vertices[0] = from, vertices[1] = to, e = log(T_to^-1 Z T_from), information permuted from [trans rot] to
+ * [rot trans] as addEdgeSE3Expmap does); one marginalised VertexSBAPointXYZ per map point and one EdgeProjectXYZ2UV per
+ * observation (information inv_sigma2 * I, RobustKernelHuber(huber_delta)). loadLocalGraphOnlyBa is the same call with
+ * every prior[k] = 0 and no odometry. */
+typedef struct se2gpu_se3_ba_params {
+    float fx, cx, cy;       /* CamPara: Config::Kcam (0,0), (0,2), (1,2) */
+    float Tbc[16];          /* Config::bTc, row-major 4x4 */
+    float huber_delta;      /* Config::TH_HUBER */
+    float xrot_info, yrot_info, z_info; /* Config::PLANEMOTION_XROT_INFO, _YROT_INFO, _Z_INFO */
+    int iterations;         /* optimize(iterations): 10 in removeOutlierChi2, LOCAL_ITER in the timing path */
+    float chi2_cut;         /* an edge is an outlier when its raw chi2 e^T Omega e exceeds this: 25 in removeOutlierChi2 */
+} se2gpu_se3_ba_params;
+
+#define SE2GPU_SE3_BA_OK 0
+#define SE2GPU_SE3_BA_NOT_PD 2  /* LM ended on an iteration whose 10 trials all met a pivot block that is not positive
+                                   definite; the estimates are the last accepted ones */
+
+/* A context: grow-only device buffers for the plan and the solver, a page-locked staging arena and a stream, on device
+ * `device`. One context serves windows of any size and topology; a call gives the same bytes as on a fresh context. Calls
+ * on one context may use different streams: each call's work waits for the previous call's kernel on the device. */
+typedef struct se2gpu_se3_ba_ctx se2gpu_se3_ba_ctx;
+se2gpu_se3_ba_ctx* se2gpu_se3_ba_create(int device);
+void se2gpu_se3_ba_destroy(se2gpu_se3_ba_ctx* h);
+
+/* HOST buffers, synchronous. N keyframes: Tcw [N*16] float row-major, fixed [N] (nonzero: fixed vertex), prior [N] (nonzero:
+ * the keyframe has the plane-motion prior). O odometry links: odo_from / odo_to [O], odo_measure [O*16] float
+ * (mOdoMeasureFrom.second.measure), odo_info [O*36] float in KeyFrame's [trans rot] order. L points: xyz [L*3] float. E edges:
+ * edge_point / edge_kf [E], uv [E*2] float (keyPointsUn[idx].pt), inv_sigma2 [E] (mvInvLevelSigma2[octave]).
+ * Outputs: chi2 [E] the raw chi2 of every edge at the final estimate, outlier [E] (chi2 > params->chi2_cut). Optional (may
+ * be NULL): status, iterations, stats [params->iterations] (rows past the count are zero), poses [N*7] (qx, qy, qz, qw, tx,
+ * ty, tz), points [L*3] double, Tcw_out [N*16] float (toCvMat of the estimate), xyz_out [L*3] float. A fixed keyframe
+ * and a keyframe no edge touches come back in Tcw_out bit for bit as they went in; a point without edges is not in the
+ * optimised graph and comes back as it was. With no free vertex no iteration runs, as in g2o. Returns
+ * SE2GPU_ERR_INVALID before any launch when N <= 0, a count is negative, an index is out of range, an odometry link has
+ * from == to, a point has two edges to one keyframe, a value or parameter is not finite (chi2_cut may be infinite), an
+ * odometry information is not symmetric or an inv_sigma2 is not positive. */
+int se2gpu_se3_ba(se2gpu_se3_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, const uint8_t* prior, int O, const int* odo_from,
+                  const int* odo_to, const float* odo_measure, const float* odo_info, int L, const float* xyz, int E,
+                  const int* edge_point, const int* edge_kf, const float* uv, const float* inv_sigma2,
+                  const se2gpu_se3_ba_params* params, double* chi2, uint8_t* outlier, int* status, int* iterations,
+                  se2gpu_ba_iter_stats* stats, double* poses, double* points, float* Tcw_out, float* xyz_out);
+/* The same on DEVICE values and outputs, asynchronous on `stream` (every output may be NULL). The topology (fixed, prior,
+ * odo_from, odo_to, edge_point, edge_kf) is HOST memory and is checked; the values are trusted. */
+int se2gpu_se3_ba_device(se2gpu_se3_ba_ctx* h, int N, const float* d_Tcw, const uint8_t* fixed, const uint8_t* prior, int O,
+                         const int* odo_from, const int* odo_to, const float* d_odo_measure, const float* d_odo_info, int L,
+                         const float* d_xyz, int E, const int* edge_point, const int* edge_kf, const float* d_uv,
+                         const float* d_inv_sigma2, const se2gpu_se3_ba_params* params, double* d_chi2, uint8_t* d_outlier,
+                         int* d_status, int* d_iterations, se2gpu_ba_iter_stats* d_stats, double* d_poses, double* d_points,
+                         float* d_Tcw_out, float* d_xyz_out, void* stream);
+/* parity hook: se2gpu_se3_ba plus trace [iterations * (N*7 + L*3)], the estimate after every iteration (the N poses, then
+ * the L points; rows past the count zero) */
+int se2gpu_se3_ba_debug_trace(se2gpu_se3_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, const uint8_t* prior, int O,
+                              const int* odo_from, const int* odo_to, const float* odo_measure, const float* odo_info, int L,
+                              const float* xyz, int E, const int* edge_point, const int* edge_kf, const float* uv,
+                              const float* inv_sigma2, const se2gpu_se3_ba_params* params, double* chi2, uint8_t* outlier,
+                              int* status, int* iterations, se2gpu_ba_iter_stats* stats, double* poses, double* points,
+                              double* trace);
+
 #ifdef __cplusplus
 }
 #endif

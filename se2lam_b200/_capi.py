@@ -44,6 +44,12 @@ class GlobalBAParams(C.Structure):
                 ("iterations", C.c_int)]
 
 
+class SE3BAParams(C.Structure):
+    _fields_ = [("fx", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("Tbc", C.c_float * 16), ("huber_delta", C.c_float),
+                ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float), ("iterations", C.c_int),
+                ("chi2_cut", C.c_float)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -77,6 +83,7 @@ SYMBOLS = [
     "se2gpu_global_ba_create", "se2gpu_global_ba_destroy", "se2gpu_global_ba", "se2gpu_global_ba_device",
     "se2gpu_global_ba_update_points", "se2gpu_global_ba_update_points_device", "se2gpu_global_ba_profile",
     "se2gpu_global_ba_profile_read",
+    "se2gpu_se3_ba_create", "se2gpu_se3_ba_destroy", "se2gpu_se3_ba", "se2gpu_se3_ba_device", "se2gpu_se3_ba_debug_trace",
 ]
 
 
@@ -193,6 +200,12 @@ def lib():
     L.se2gpu_global_ba_update_points_device.argtypes = [i] + [vp] * 5
     L.se2gpu_global_ba_profile.argtypes = [vp, i]
     L.se2gpu_global_ba_profile_read.argtypes = [vp, vp]
+    L.se2gpu_se3_ba_create.restype = vp
+    L.se2gpu_se3_ba_create.argtypes = [i]
+    L.se2gpu_se3_ba_destroy.argtypes = [vp]
+    L.se2gpu_se3_ba.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 14
+    L.se2gpu_se3_ba_device.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 15
+    L.se2gpu_se3_ba_debug_trace.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 13
     _lib = L
     return L
 
