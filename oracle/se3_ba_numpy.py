@@ -41,8 +41,33 @@ class SE3:
 
     @staticmethod
     def from_f32(T):
+        """converter.cpp toSE3Quat: the float matrix widened, through Eigen's Quaterniond(Matrix3d), which projects a
+        matrix that float rounding left slightly off SO(3) differently from scipy's from_matrix"""
         T = np.asarray(T, np.float64).reshape(4, 4)
-        return SE3(T[:3, :3], T[:3, 3])
+        return SE3(Rotation.from_quat(eigen_quat(T[:3, :3])).as_matrix(), T[:3, 3])
+
+
+def eigen_quat(m):
+    """Eigen's Quaterniond(const Matrix3d&), (x, y, z, w) before normalisation: the w branch while the trace is positive,
+    else the branch of the largest diagonal entry"""
+    t = m[0, 0] + m[1, 1] + m[2, 2]
+    if t > 0:
+        t = np.sqrt(t + 1.0)
+        w, t = 0.5 * t, 0.5 / t
+        return np.array([(m[2, 1] - m[1, 2]) * t, (m[0, 2] - m[2, 0]) * t, (m[1, 0] - m[0, 1]) * t, w])
+    i = 0
+    if m[1, 1] > m[0, 0]:
+        i = 1
+    if m[2, 2] > m[i, i]:
+        i = 2
+    j, k = (i + 1) % 3, (i + 2) % 3
+    q = np.zeros(4)
+    t = np.sqrt(m[i, i] - m[j, j] - m[k, k] + 1.0)
+    q[i], t = 0.5 * t, 0.5 / t
+    q[3] = (m[k, j] - m[j, k]) * t
+    q[j] = (m[j, i] + m[i, j]) * t
+    q[k] = (m[k, i] + m[i, k]) * t
+    return q
 
 
 def se3_exp(u):

@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -624,6 +625,7 @@ struct se2gpu_se3_ba_ctx {
     cudaStream_t stream = nullptr;
     cudaEvent_t uploaded = nullptr;  // the last plan upload out of the pinned arena has completed
     cudaEvent_t done = nullptr;      // the last kernel, which reads the plan and work buffers, has completed
+    int grid_limit = 0;              // SE2GPU_SE3_BA_GRID: cap on the cooperative grid (several contexts on one GPU); 0 = none
     DeviceBuffers bufs;
     int* d_int = nullptr; size_t cap_int = 0;
     long long* d_ll = nullptr; size_t cap_ll = 0;
@@ -663,7 +665,8 @@ int run(se2gpu_se3_ba_ctx* h, int N, const uint8_t* fixed, const uint8_t* prior,
     SE2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_se3_ba, kThreads, 0));
     if (per_sm < 1) return fail(SE2GPU_ERR_CUDA, "k_se3_ba cannot be resident");
     const size_t work = std::max<size_t>({(size_t)E, (size_t)L * 3, env * 36, (size_t)N, (size_t)O});
-    const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)dev_sms * per_sm, (work + kThreads - 1) / kThreads));
+    int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)dev_sms * per_sm, (work + kThreads - 1) / kThreads));
+    if (h->grid_limit >= 1) grid = std::min(grid, h->grid_limit);
     // doubles: X[2] (7 N each), P[2] (3 L each), pmeas (7 N), pinfo (36 N), Z (7 O), Om (36 O), olin (120 O), lin (72 E), Y (18 E),
     // Hl (9 L), D (6 L), pH (36 nf), pb, bf, b, x (6 nf each), Hs, L (36 env), part (chunks), part_max (grid), ctl
     const size_t n_dbl[23] = {7 * (size_t)N, 7 * (size_t)N, 3 * (size_t)L, 3 * (size_t)L, 7 * (size_t)N, 36 * (size_t)N,
@@ -756,6 +759,7 @@ se2gpu_se3_ba_ctx* se2gpu_se3_ba_create(int device) {
     if (select_device(device)) return nullptr;
     se2gpu_se3_ba_ctx* h = new se2gpu_se3_ba_ctx;
     h->device = device;
+    if (const char* g = getenv("SE2GPU_SE3_BA_GRID")) h->grid_limit = atoi(g);  // the only place this BA reads the environment
     if (cudaStreamCreate(&h->stream) != cudaSuccess || cudaEventCreateWithFlags(&h->uploaded, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
         fail(SE2GPU_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");

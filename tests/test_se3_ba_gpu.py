@@ -32,7 +32,7 @@ def compare(g, o, rel=1e-9, est=1e-7):
         q = g["poses"].copy()
         qo = o["poses"]
         assert np.abs(q - qo).max() <= est * max(1.0, np.abs(qo).max())
-        assert np.abs(g["points"] - o["points"]).max() <= est * max(1.0, np.abs(o["points"]).max())
+        assert np.abs(g["points"] - o["points"]).max(initial=0.0) <= est * max(1.0, np.abs(o["points"]).max(initial=0.0))
         assert np.allclose(g["chi2"], o["chi2"], rtol=1e-6, atol=1e-6)  # e^T w e of estimates 1e-7 apart
         near = np.abs(o["chi2"] - 25.0) <= 1e-6 * 25.0
         assert np.array_equal(g["outlier"][~near], o["outlier"][~near])
