@@ -173,6 +173,10 @@ typedef struct se2gpu_grid_params {
  * thread (like the reference's stack-allocated ORBmatcher objects, the calls are not re-entrant on one context). */
 typedef struct se2gpu_matcher se2gpu_matcher;
 se2gpu_matcher* se2gpu_matcher_create(int max_queries, int max_db, int device);
+/* The same for the batched device entry points below, up to max_batch (<= 65535) frame pairs per call: the candidate table
+ * becomes max_batch x max_queries x max_db x 8 bytes (at most 4 GiB in all) and every pair gets its own scratch.
+ * se2gpu_matcher_create(q, d, dev) == se2gpu_matcher_create_batch(q, d, 1, dev). */
+se2gpu_matcher* se2gpu_matcher_create_batch(int max_queries, int max_db, int max_batch, int device);
 void se2gpu_matcher_destroy(se2gpu_matcher* m);
 
 /* MatchByWindow(frame1, frame2, vbPrevMatched, winSize, vnMatches12, levelOffset, minLevel, maxLevel) with nnratio =
@@ -194,6 +198,31 @@ int se2gpu_match_by_projection_device(se2gpu_matcher* m, const se2gpu_keypoint* 
                                       const float* d_mp_uv, int n_mp, const int* d_mp_octave, const uint8_t* d_mp_desc,
                                       se2gpu_grid_params grid, int win_size, int level_offset, float nnratio,
                                       int* d_matches_idx_mp, int* d_nmatches, void* stream);
+
+/* The two device entry points over a batch of B independent frame pairs in one call, with the extractor's layout (frame i
+ * at d_kps + i*nfeatures): pair b reads d_kp1 + b*cap1, d_desc1 + b*cap1*32, d_kp2 + b*cap2, d_desc2 + b*cap2*32 and
+ * the counts d_n1[b], d_n2[b] (either array may be NULL: every pair at its capacity), updates d_prev + b*cap1*2 and
+ * writes d_matches12 + b*cap1 and d_nmatches[b] (may be NULL) - so d_matches12 feeds se2gpu_remove_outliers_device as is.
+ * Pair b's outputs are the bytes the single-pair call makes for that pair alone with n1 = cap1, n2 = cap2 (matches,
+ * vbPrevMatched, match count, and the rounds / fallback flag of se2gpu_matcher_last_rounds_batch). All pairs share one
+ * grid: the reference's Frame grid bounds are static members, the same for every frame. The kernel launches are those of
+ * one single-pair call whatever B is. B > max_batch, cap1 > max_queries or cap2 > max_db: SE2GPU_ERR_CAPACITY; B < 0 or
+ * a NULL required pointer: SE2GPU_ERR_INVALID; B == 0 does nothing. */
+int se2gpu_match_by_window_batch_device(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kp1, const uint8_t* d_desc1, int cap1,
+                                        const int* d_n1, const se2gpu_keypoint* d_kp2, const uint8_t* d_desc2, int cap2,
+                                        const int* d_n2, float* d_prev, se2gpu_grid_params grid, int win_size, int level_offset,
+                                        int min_level, int max_level, float nnratio, int* d_matches12, int* d_nmatches,
+                                        void* stream);
+/* MatchByProjection for B (keyframe, map-point list) pairs: keyframe side as frame 2 above (d_kf_kp + b*cap_kf, d_kf_desc +
+ * b*cap_kf*32, d_n_kf[b], d_kf_observed + b*cap_kf, d_matches_idx_mp + b*cap_kf, d_nmatches[b]); map points in slots of
+ * cap_mp (d_mp_valid / d_mp_octave + b*cap_mp, d_mp_uv + b*cap_mp*2, d_mp_desc + b*cap_mp*32). A pair with fewer map
+ * points pads its slot with mp_valid = 0: the reference skips such a point (ORBmatcher.cpp:390-404) and the padding comes
+ * after every real one, so the result is that of the shorter list. */
+int se2gpu_match_by_projection_batch_device(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kf_kp, const uint8_t* d_kf_desc,
+                                            int cap_kf, const int* d_n_kf, const uint8_t* d_kf_observed,
+                                            const uint8_t* d_mp_valid, const float* d_mp_uv, int cap_mp, const int* d_mp_octave,
+                                            const uint8_t* d_mp_desc, se2gpu_grid_params grid, int win_size, int level_offset,
+                                            float nnratio, int* d_matches_idx_mp, int* d_nmatches, void* stream);
 
 /* HOST-buffer entry points on an explicit context (synchronous; one stream synchronisation per call).
  * MatchByWindow: prev [n1*2] is vbPrevMatched, updated in place. matches12 [n1]. Returns the number of matches (>=0)
@@ -243,6 +272,9 @@ int se2gpu_matcher_profile(se2gpu_matcher* m, int enable);
 int se2gpu_matcher_profile_read(se2gpu_matcher* m, double* ms, int* launches);
 /* diagnostics of the last resolve on this context: speculative rounds it took, and whether the sequential fallback ran */
 int se2gpu_matcher_last_rounds(se2gpu_matcher* m, int* rounds, int* used_fallback);
+/* the same for every pair of the last batched call: rounds [B], used_fallback [B] (either may be NULL); B larger than
+ * that call's batch is SE2GPU_ERR_INVALID */
+int se2gpu_matcher_last_rounds_batch(se2gpu_matcher* m, int B, int* rounds, int* used_fallback);
 
 /* ------------------------------------------------------------------------------------------ bag of words */
 /* DBoW2 vocabulary tree (TemplatedVocabulary<FORB::TDescriptor, FORB>, reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h)

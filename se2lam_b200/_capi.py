@@ -68,6 +68,8 @@ SYMBOLS = [
     "se2gpu_matcher_create", "se2gpu_matcher_destroy", "se2gpu_match_by_window_device", "se2gpu_keypoints_to_points_device",
     "se2gpu_match_by_projection_device", "se2gpu_matcher_match_by_window", "se2gpu_matcher_match_by_projection",
     "se2gpu_matcher_search_by_bow", "se2gpu_matcher_profile", "se2gpu_matcher_profile_read", "se2gpu_matcher_last_rounds",
+    "se2gpu_matcher_create_batch", "se2gpu_match_by_window_batch_device", "se2gpu_match_by_projection_batch_device",
+    "se2gpu_matcher_last_rounds_batch",
     "se2gpu_ba_create", "se2gpu_ba_destroy", "se2gpu_ba_set_problem", "se2gpu_ba_optimize", "se2gpu_ba_get",
     "se2gpu_ba_set_shard", "se2gpu_ba_peer_export", "se2gpu_ba_peer_import", "se2gpu_ba_set_stream", "se2gpu_ba_debug_system", "se2gpu_ba_reset", "se2gpu_ba_profile",
     "se2gpu_ba_profile_read", "se2gpu_ba_set_mode", "se2gpu_ba_get_f32", "se2gpu_ba_build_information", "se2gpu_ba_optimize_from", "se2gpu_ba_peer_attach_local",
@@ -134,16 +136,21 @@ def lib():
     L.se2gpu_search_by_bow.argtypes = [C.POINTER(BowKF), C.POINTER(BowKF), i, f, i, vp, i]
     L.se2gpu_matcher_create.restype = vp
     L.se2gpu_matcher_create.argtypes = [i, i, i]
+    L.se2gpu_matcher_create_batch.restype = vp
+    L.se2gpu_matcher_create_batch.argtypes = [i, i, i, i]
     L.se2gpu_matcher_destroy.argtypes = [vp]
     L.se2gpu_match_by_window_device.argtypes = [vp, vp, vp, i, vp, vp, vp, i, vp, vp, GridParams, i, i, i, i, f, vp, vp, vp]
     L.se2gpu_keypoints_to_points_device.argtypes = [vp, i, vp, vp, vp]
     L.se2gpu_match_by_projection_device.argtypes = [vp, vp, vp, i, vp, vp, vp, vp, i, vp, vp, GridParams, i, i, f, vp, vp, vp]
+    L.se2gpu_match_by_window_batch_device.argtypes = [vp, i, vp, vp, i, vp, vp, vp, i, vp, vp, GridParams, i, i, i, i, f, vp, vp, vp]
+    L.se2gpu_match_by_projection_batch_device.argtypes = [vp, i, vp, vp, i, vp, vp, vp, vp, i, vp, vp, GridParams, i, i, f, vp, vp, vp]
     L.se2gpu_matcher_match_by_window.argtypes = [vp, vp, vp, i, vp, vp, i, vp, GridParams, i, i, i, i, f, vp]
     L.se2gpu_matcher_match_by_projection.argtypes = [vp, vp, vp, i, vp, vp, vp, i, vp, vp, GridParams, i, i, f, vp]
     L.se2gpu_matcher_search_by_bow.argtypes = [vp, C.POINTER(BowKF), C.POINTER(BowKF), i, f, i, vp]
     L.se2gpu_matcher_profile.argtypes = [vp, i]
     L.se2gpu_matcher_profile_read.argtypes = [vp, vp, vp]
     L.se2gpu_matcher_last_rounds.argtypes = [vp, C.POINTER(i), C.POINTER(i)]
+    L.se2gpu_matcher_last_rounds_batch.argtypes = [vp, i, vp, vp]
     L.se2gpu_ba_create.restype = vp
     L.se2gpu_ba_create.argtypes = [i, i, i, i, i]
     L.se2gpu_ba_destroy.argtypes = [vp]

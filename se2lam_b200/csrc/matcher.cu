@@ -20,6 +20,9 @@
 //   k_fallback_*   the one-warp sequential loop, kept as the exact fallback when a database keypoint collects more
 //                  simultaneous claims than the shared-memory claim table holds (flag set by k_resolve; returns at once
 //                  otherwise).
+// The device entry points take a batch of B independent frame pairs (se2gpu_match_by_*_batch_device; the single-pair entry
+// points are B = 1): the grid and candidate kernels take the pair from blockIdx.y, k_resolve runs one CTA and k_fallback_*
+// one warp per pair, and every pair works in its own slice of the context's scratch. The launch count does not depend on B.
 #include <climits>
 #include <cstring>
 #include <mutex>
@@ -29,15 +32,17 @@
 
 struct se2gpu_matcher {
     int device = 0;
-    int max_q = 0, max_db = 0;
+    int max_q = 0, max_db = 0, max_batch = 1;
     cudaStream_t stream = nullptr;      // host entry points run here
-    // device scratch (sized at creation)
-    int *cell = nullptr, *order = nullptr, *nvalid = nullptr;
+    // device scratch (sized at creation), one slice per frame pair: pair b's slice starts at b * (the size given here)
+    int *cell = nullptr, *order = nullptr, *nvalid = nullptr;   // [max_db], [max_db], [1]
     int2* cand = nullptr;               // [max_q][max_db] (index, dist | octave << 16)
     int* ncand = nullptr;               // [max_q]
     int* work = nullptr;                // fallback: [2 * max_db + max_q]
     int* flags = nullptr;               // [0] fallback needed, [1] rounds of the last resolve
     int* nm = nullptr;                  // match count of the last call
+    std::vector<int> seq_flags;         // [max_batch][2] = {1, 0}: the flags of every pair when the sequential kernel runs alone
+    int last_batch = 0;                 // pairs of the last resolve
     // device + pinned staging of the host entry points
     se2gpu_keypoint *d_kp1 = nullptr, *d_kp2 = nullptr;
     uint8_t *d_desc1 = nullptr, *d_desc2 = nullptr, *d_u8a = nullptr, *d_u8b = nullptr;
@@ -68,6 +73,7 @@ __global__ void k_hamming_pairs(const uint32_t* a, const uint32_t* b, int n, int
 // insertion index) of the valid ones by rank counting. Every CTA computes ALL sort keys (cell << 13 | index, INT_MAX for
 // keypoints outside the grid) into its shared memory - redundant but cheaper than a grid-wide dependency - and ranks its
 // own 128 keypoints against them with broadcast shared-memory reads. CTA 0 also publishes the number of valid keypoints.
+// Pair blockIdx.y reads keypoints kp[b * n_cap ..] and count d_n[b], and writes cell / order [b * scr ..] and n_valid[b].
 constexpr int GRID_SMEM_KEYS = 8192;
 __device__ __forceinline__ int grid_cell_of(const se2gpu_keypoint& p, const se2gpu_grid_params& g) {
     const int px = (int)roundf(__fmul_rn(__fsub_rn(p.x, g.min_x), g.inv_w));
@@ -76,8 +82,11 @@ __device__ __forceinline__ int grid_cell_of(const se2gpu_keypoint& p, const se2g
 }
 __global__ void __launch_bounds__(128) k_grid_build(const se2gpu_keypoint* __restrict__ kp, int n_cap, const int* __restrict__ d_n,
                                                     se2gpu_grid_params g, int* __restrict__ cell, int* __restrict__ order,
-                                                    int* __restrict__ n_valid) {
+                                                    int* __restrict__ n_valid, int scr) {
     __shared__ int keys[GRID_SMEM_KEYS];
+    const int b = blockIdx.y;
+    kp += (size_t)b * n_cap; cell += (size_t)b * scr; order += (size_t)b * scr; n_valid += b;
+    if (d_n) d_n += b;
     const int n = count_of(d_n, n_cap);
     int nv = 0;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -107,12 +116,18 @@ __global__ void __launch_bounds__(128) k_grid_build(const se2gpu_keypoint* __res
 }
 // the same for more keypoints than the shared-memory key table holds: cells first, then ranks from global memory
 __global__ void k_grid_cell_big(const se2gpu_keypoint* __restrict__ kp, int n_cap, const int* __restrict__ d_n, se2gpu_grid_params g,
-                                int* __restrict__ cell) {
+                                int* __restrict__ cell, int scr) {
+    const int b = blockIdx.y;
+    kp += (size_t)b * n_cap; cell += (size_t)b * scr;
+    if (d_n) d_n += b;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count_of(d_n, n_cap)) cell[i] = grid_cell_of(kp[i], g);
 }
 __global__ void k_grid_order_big(const int* __restrict__ cell, int n_cap, const int* __restrict__ d_n, int* __restrict__ order,
-                                 int* __restrict__ n_valid) {
+                                 int* __restrict__ n_valid, int scr) {
+    const int b = blockIdx.y;
+    cell += (size_t)b * scr; order += (size_t)b * scr; n_valid += b;
+    if (d_n) d_n += b;
     const int n = count_of(d_n, n_cap);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -134,13 +149,29 @@ struct CandArgs {
     const uint32_t* qdesc;
     // database = keypoints of frame 2 / of the keyframe
     const se2gpu_keypoint* kp; const uint32_t* desc; const int* cell; const int* order; const int* n_valid; const uint8_t* db_skip;
+    int db_cap;                       // database items per pair (the pair stride of kp, desc, db_skip)
     se2gpu_grid_params g;
-    int cap; int2* cand; int* ncand;
+    int cap; int2* cand; int* ncand;  // cap = max_db: row stride of cand, pair stride of cell / order
+    int scr_q;                        // max_queries: rows of cand and entries of ncand per pair
 };
 
+// pair b's slice of every array (pair-strided inputs, context scratch)
+__device__ __forceinline__ void pair_slice(CandArgs& a, int b) {
+    const size_t q = (size_t)b * a.nq_cap, d = (size_t)b * a.db_cap;
+    if (a.d_nq) a.d_nq += b;
+    if (a.mode == MODE_WINDOW) { a.kp1 += q; a.prev += 2 * q; }
+    else { a.mp_valid += q; a.mp_uv += 2 * q; a.mp_octave += q; }
+    a.qdesc += 8 * q;
+    a.kp += d; a.desc += 8 * d;
+    if (a.db_skip) a.db_skip += d;
+    a.cell += (size_t)b * a.cap; a.order += (size_t)b * a.cap; a.n_valid += b;
+    a.cand += (size_t)b * a.scr_q * a.cap; a.ncand += (size_t)b * a.scr_q;
+}
+
 // Frame::GetFeaturesInArea (Frame.cpp:222-286) for one query per warp + DescriptorDistance of every hit.
-// cand[q*cap + k] = (i2, dist | octave << 16) in the reference's iteration order; ncand[q] = hits.
+// cand[q*cap + k] = (i2, dist | octave << 16) in the reference's iteration order; ncand[q] = hits. Pair = blockIdx.y.
 __global__ void __launch_bounds__(256) k_candidates(CandArgs a) {
+    pair_slice(a, blockIdx.y);
     const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     const int nq = count_of(a.d_nq, a.nq_cap);
     if (q >= a.nq_cap) return;
@@ -262,9 +293,24 @@ struct ResolveArgs {
     int* out; int n_out;              // WINDOW: matches12[n1]; PROJ: vMatchesIdxMP[n_kf]; BOW: matches12[n1]
     float* prev;                      // WINDOW: vbPrevMatched, updated in place
     int* nmatches; int* flags;
+    int scr_q;                        // max_queries: per-pair rows of cand (each `cap` wide) and entries of ncand
 };
 
-// Greedy resolution as speculative rounds, one CTA (see the file header). Per-query decision = (chosen database item or
+// pair b's slice (WINDOW / PROJ; SearchByBoW runs one pair): queries and database items are strided by nq_cap / n2_cap,
+// outputs by n_out, the context scratch by its capacities; work is the fallback's [2 * cap + scr_q] per pair
+__device__ __forceinline__ void pair_slice(ResolveArgs& a, int b) {
+    const size_t q = (size_t)b * a.nq_cap, d = (size_t)b * a.n2_cap;
+    if (a.d_nq) a.d_nq += b;
+    if (a.d_n2) a.d_n2 += b;
+    a.cand += (size_t)b * a.scr_q * a.cap; a.ncand += (size_t)b * a.scr_q;
+    if (a.ang1) { a.ang1 += q * a.stride1; a.ang2 += d * a.stride2; }
+    if (a.kp2) a.kp2 += d;
+    if (a.prev) a.prev += 2 * q;
+    a.out += (size_t)b * a.n_out; a.nmatches += b; a.flags += 2 * b;
+}
+__device__ __forceinline__ int* work_slice(const ResolveArgs& a, int* work, int b) { return work + (size_t)b * (2 * (size_t)a.cap + a.scr_q); }
+
+// Greedy resolution as speculative rounds, one CTA per pair (see the file header). Per-query decision = (chosen database item or
 // -1, its distance). Claim table: for every database item the (query, distance) pairs of the queries that currently
 // choose it; a query evaluates a candidate j against min{distance of claims by EARLIER queries} == vMatchesDistance[j]
 // at its turn of the sequential loop (the distance of successive claims on one item is strictly decreasing), in BOW
@@ -274,6 +320,9 @@ __global__ void __launch_bounds__(1024) k_resolve(ResolveArgs a) {
     extern __shared__ int smi[];
     __shared__ int hist[HISTO_LENGTH];
     __shared__ int s_over, s_nm, s_top[3];
+    // pair 0 needs no offsets; skipping them keeps a single pair's prologue as short as it was (one CTA on one SM runs the
+    // whole resolve, so every per-thread instruction before the rounds is on the critical path)
+    if (blockIdx.x != 0) pair_slice(a, blockIdx.x);
     const int tid = threadIdx.x, nt = blockDim.x;
     const int nq = count_of(a.d_nq, a.nq_cap), n2 = count_of(a.d_n2, a.n2_cap);
     const int K = a.K;
@@ -397,10 +446,13 @@ __device__ __forceinline__ Top2 top2_warp(Top2 t) {
     return t;
 }
 
-// Exact sequential fallbacks (one warp, queries in order); they return at once unless k_resolve raised flags[0].
+// Exact sequential fallbacks (one warp per pair, queries in order); a warp returns at once unless its pair's flags[0] is set.
 // work: [n2] vMatchesDistance, [n2] vnMatches21, [n1] bin_of
 __global__ void __launch_bounds__(32) k_fallback_window(ResolveArgs a, const se2gpu_keypoint* __restrict__ kp1, int* __restrict__ work) {
-    if (a.flags[0] == 0) return;
+    const int b = blockIdx.x;
+    if (a.flags[2 * b] == 0) return;
+    pair_slice(a, b);
+    kp1 += (size_t)b * a.nq_cap; work = work_slice(a, work, b);
     __shared__ int hist[HISTO_LENGTH];
     const int lane = threadIdx.x;
     const int n1 = count_of(a.d_nq, a.nq_cap), n2 = count_of(a.d_n2, a.n2_cap);
@@ -451,7 +503,10 @@ __global__ void __launch_bounds__(32) k_fallback_window(ResolveArgs a, const se2
 
 // MatchByProjection's sequential loop (:415-449). work: [n] vMatchesDistance
 __global__ void __launch_bounds__(32) k_fallback_projection(ResolveArgs a, int* __restrict__ work) {
-    if (a.flags[0] == 0) return;
+    const int b = blockIdx.x;
+    if (a.flags[2 * b] == 0) return;
+    pair_slice(a, b);
+    work = work_slice(a, work, b);
     const int lane = threadIdx.x;
     const int nmp = count_of(a.d_nq, a.nq_cap), n = count_of(a.d_n2, a.n2_cap);
     for (int i = lane; i < n; i += 32) work[i] = INT_MAX;
@@ -536,14 +591,16 @@ __global__ void k_kp_to_xy(const se2gpu_keypoint* __restrict__ kp, int n_cap, co
     if (i < count_of(d_n, n_cap)) { xy[2 * i] = kp[i].x; xy[2 * i + 1] = kp[i].y; }
 }
 
-int launch_grid(se2gpu_matcher* m, const se2gpu_keypoint* d_kp, int n, const int* d_n, se2gpu_grid_params grid, cudaStream_t s) {
+// the grids of B databases of n (capacity) keypoints each, pair b's at d_kp + b * n
+int launch_grid(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kp, int n, const int* d_n, se2gpu_grid_params grid, cudaStream_t s) {
+    const dim3 blocks((n + 127) / 128, B);
     m->prof.begin(0, s);
     if (n <= GRID_SMEM_KEYS) {
-        SE2_LAUNCH(k_grid_build, (n + 127) / 128, 128, 0, s, d_kp, n, d_n, grid, m->cell, m->order, m->nvalid);
+        SE2_LAUNCH(k_grid_build, blocks, 128, 0, s, d_kp, n, d_n, grid, m->cell, m->order, m->nvalid, m->max_db);
     } else {
-        SE2_CUDA(cudaMemsetAsync(m->nvalid, 0, sizeof(int), s));
-        SE2_LAUNCH(k_grid_cell_big, (n + 127) / 128, 128, 0, s, d_kp, n, d_n, grid, m->cell);
-        SE2_LAUNCH(k_grid_order_big, (n + 127) / 128, 128, 0, s, m->cell, n, d_n, m->order, m->nvalid);
+        SE2_CUDA(cudaMemsetAsync(m->nvalid, 0, sizeof(int) * B, s));
+        SE2_LAUNCH(k_grid_cell_big, blocks, 128, 0, s, d_kp, n, d_n, grid, m->cell, m->max_db);
+        SE2_LAUNCH(k_grid_order_big, blocks, 128, 0, s, m->cell, n, d_n, m->order, m->nvalid, m->max_db);
     }
     m->prof.end(s);
     return SE2GPU_OK;
@@ -557,23 +614,25 @@ int pick_K(const se2gpu_matcher* m, int nq, int n2) {
     return 0;
 }
 
-// common tail of the three device paths: resolve + guarded fallback
+// common tail of the three device paths for B pairs (SearchByBoW: 1): resolve + guarded fallback. K depends on the caps only,
+// so it is the same for every pair.
 template <int MODE>
-int launch_resolve(se2gpu_matcher* m, ResolveArgs ra, const se2gpu_keypoint* kp1, cudaStream_t s) {
+int launch_resolve(se2gpu_matcher* m, int B, ResolveArgs ra, const se2gpu_keypoint* kp1, cudaStream_t s) {
     const int K = (ra.nq_cap < 65536) ? pick_K(m, ra.nq_cap, ra.n2_cap) : 0;
-    SE2_CUDA(cudaMemsetAsync(m->flags, 0, 2 * sizeof(int), s));
+    ra.scr_q = m->max_q;
+    m->last_batch = B;
+    SE2_CUDA(cudaMemsetAsync(m->flags, 0, 2 * sizeof(int) * B, s));
     m->prof.begin(2, s);
     if (K >= 2) {
         ra.K = K;
-        SE2_LAUNCH(k_resolve<MODE>, 1, 1024, resolve_smem(ra.nq_cap, ra.n2_cap, K), s, ra);
-    } else {
-        const int one = 1;       // inputs too large for the shared-memory claim table: sequential kernel directly
-        SE2_CUDA(cudaMemcpyAsync(m->flags, &one, sizeof(int), cudaMemcpyHostToDevice, s));
+        SE2_LAUNCH(k_resolve<MODE>, B, 1024, resolve_smem(ra.nq_cap, ra.n2_cap, K), s, ra);
+    } else {                     // inputs too large for the shared-memory claim table: sequential kernel directly
+        SE2_CUDA(cudaMemcpyAsync(m->flags, m->seq_flags.data(), 2 * sizeof(int) * B, cudaMemcpyHostToDevice, s));
     }
     m->prof.end(s);
     m->prof.begin(3, s);
-    if (MODE == MODE_WINDOW) SE2_LAUNCH(k_fallback_window, 1, 32, 0, s, ra, kp1, m->work);
-    else if (MODE == MODE_PROJ) SE2_LAUNCH(k_fallback_projection, 1, 32, 0, s, ra, m->work);
+    if (MODE == MODE_WINDOW) SE2_LAUNCH(k_fallback_window, B, 32, 0, s, ra, kp1, m->work);
+    else if (MODE == MODE_PROJ) SE2_LAUNCH(k_fallback_projection, B, 32, 0, s, ra, m->work);
     else SE2_LAUNCH(k_fallback_bow, 1, 32, 0, s, ra, m->work);
     m->prof.end(s);
     return SE2GPU_OK;
@@ -587,16 +646,26 @@ se2gpu_matcher* g_default[se2gpu::kMaxDevices] = {};
 extern "C" {
 
 se2gpu_matcher* se2gpu_matcher_create(int max_queries, int max_db, int device) {
-    if (max_queries <= 0 || max_db <= 0) { fail(SE2GPU_ERR_INVALID, "bad capacities"); return nullptr; }
-    if ((size_t)max_queries * max_db * sizeof(int2) > ((size_t)4 << 30)) { fail(SE2GPU_ERR_CAPACITY, "candidate table %d x %d too large", max_queries, max_db); return nullptr; }
+    return se2gpu_matcher_create_batch(max_queries, max_db, 1, device);
+}
+
+se2gpu_matcher* se2gpu_matcher_create_batch(int max_queries, int max_db, int max_batch, int device) {
+    if (max_queries <= 0 || max_db <= 0 || max_batch <= 0) { fail(SE2GPU_ERR_INVALID, "bad capacities"); return nullptr; }
+    if (max_batch > 65535) { fail(SE2GPU_ERR_CAPACITY, "%d pairs per call: at most 65535 (the grid's y dimension)", max_batch); return nullptr; }
+    if ((size_t)max_queries * max_db * sizeof(int2) > (((size_t)4 << 30) / max_batch)) {
+        fail(SE2GPU_ERR_CAPACITY, "candidate table %d x %d x %d too large", max_batch, max_queries, max_db);
+        return nullptr;
+    }
     if (se2gpu::select_device(device) != SE2GPU_OK) return nullptr;
     se2gpu_matcher* m = new se2gpu_matcher;
-    m->device = device; m->max_q = max_queries; m->max_db = max_db;
-    const size_t Q = max_queries, D = max_db, N = std::max(Q, D);
+    m->device = device; m->max_q = max_queries; m->max_db = max_db; m->max_batch = max_batch;
+    m->seq_flags.assign(2 * (size_t)max_batch, 0);
+    for (int b = 0; b < max_batch; ++b) m->seq_flags[2 * b] = 1;
+    const size_t Q = max_queries, D = max_db, N = std::max(Q, D), P = max_batch;
     bool ok = true;
     auto A = [&](auto** p, size_t count) { ok = ok && m->bufs.alloc(p, count) == cudaSuccess; };
-    A(&m->cell, D); A(&m->order, D); A(&m->nvalid, 1);
-    A(&m->cand, Q * D); A(&m->ncand, Q); A(&m->work, 2 * D + Q); A(&m->flags, 2); A(&m->nm, 1);
+    A(&m->cell, P * D); A(&m->order, P * D); A(&m->nvalid, P);
+    A(&m->cand, P * Q * D); A(&m->ncand, P * Q); A(&m->work, P * (2 * D + Q)); A(&m->flags, 2 * P); A(&m->nm, P);
     A(&m->d_kp1, N); A(&m->d_kp2, N); A(&m->d_desc1, N * 32); A(&m->d_desc2, N * 32);
     A(&m->d_u8a, N); A(&m->d_u8b, N); A(&m->d_f1, 2 * N); A(&m->d_f2, 2 * N);
     A(&m->d_i1, N + 1); A(&m->d_i2, N + 1); A(&m->d_i3, N + 1); A(&m->d_i4, N + 1); A(&m->d_out, N);
@@ -648,6 +717,20 @@ int se2gpu_matcher_last_rounds(se2gpu_matcher* m, int* rounds, int* used_fallbac
     return SE2GPU_OK;
 }
 
+int se2gpu_matcher_last_rounds_batch(se2gpu_matcher* m, int B, int* rounds, int* used_fallback) {
+    if (!m) return fail(SE2GPU_ERR_INVALID, "null handle");
+    if (B < 0 || B > m->last_batch) return fail(SE2GPU_ERR_INVALID, "%d pairs asked for, the last resolve had %d", B, m->last_batch);
+    if (B == 0) return SE2GPU_OK;
+    SE2_CUDA(cudaSetDevice(m->device));
+    std::vector<int> f(2 * (size_t)B);
+    SE2_CUDA(cudaMemcpy(f.data(), m->flags, sizeof(int) * f.size(), cudaMemcpyDeviceToHost));
+    for (int b = 0; b < B; ++b) {
+        if (used_fallback) used_fallback[b] = f[2 * b];
+        if (rounds) rounds[b] = f[2 * b + 1];
+    }
+    return SE2GPU_OK;
+}
+
 int se2gpu_keypoints_to_points_device(const se2gpu_keypoint* d_kp, int n, const int* d_n, float* d_xy, void* stream) {
     if (n < 0 || (n && (!d_kp || !d_xy))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     { const int rc = se2gpu::require_device(); if (rc) return rc; }
@@ -661,67 +744,88 @@ int se2gpu_match_by_window_device(se2gpu_matcher* m, const se2gpu_keypoint* d_kp
                                   const se2gpu_keypoint* d_kp2, const uint8_t* d_desc2, int n2, const int* d_n2, float* d_prev,
                                   se2gpu_grid_params grid, int win_size, int level_offset, int min_level, int max_level, float nnratio,
                                   int* d_matches12, int* d_nmatches, void* stream) {
+    return se2gpu_match_by_window_batch_device(m, 1, d_kp1, d_desc1, n1, d_n1, d_kp2, d_desc2, n2, d_n2, d_prev, grid, win_size, level_offset,
+                                               min_level, max_level, nnratio, d_matches12, d_nmatches, stream);
+}
+
+int se2gpu_match_by_window_batch_device(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kp1, const uint8_t* d_desc1, int cap1,
+                                        const int* d_n1, const se2gpu_keypoint* d_kp2, const uint8_t* d_desc2, int cap2, const int* d_n2,
+                                        float* d_prev, se2gpu_grid_params grid, int win_size, int level_offset, int min_level,
+                                        int max_level, float nnratio, int* d_matches12, int* d_nmatches, void* stream) {
     if (!m) return fail(SE2GPU_ERR_INVALID, "null handle");
-    if (n1 < 0 || n2 < 0) return fail(SE2GPU_ERR_INVALID, "negative sizes");
-    if (n1 > m->max_q || n2 > m->max_db) return fail(SE2GPU_ERR_CAPACITY, "%d x %d exceeds the matcher's capacity %d x %d", n1, n2, m->max_q, m->max_db);
+    if (B < 0 || cap1 < 0 || cap2 < 0) return fail(SE2GPU_ERR_INVALID, "negative sizes");
+    if (B > m->max_batch || cap1 > m->max_q || cap2 > m->max_db)
+        return fail(SE2GPU_ERR_CAPACITY, "%d pairs of %d x %d exceed the matcher's capacity %d pairs of %d x %d", B, cap1, cap2, m->max_batch, m->max_q, m->max_db);
     SE2_NVTX("se2gpu.match_by_window");
-    if (n1 && (!d_kp1 || !d_desc1 || !d_prev || !d_matches12)) return fail(SE2GPU_ERR_INVALID, "null argument");
-    if (n2 && (!d_kp2 || !d_desc2)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (B == 0) return SE2GPU_OK;
+    if (cap1 && (!d_kp1 || !d_desc1 || !d_prev || !d_matches12)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (cap2 && (!d_kp2 || !d_desc2)) return fail(SE2GPU_ERR_INVALID, "null argument");
     SE2_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = (cudaStream_t)stream;
     int* nm = d_nmatches ? d_nmatches : m->nm;
-    if (n1 == 0 || n2 == 0) {
-        if (n1) SE2_CUDA(cudaMemsetAsync(d_matches12, 0xff, sizeof(int) * n1, s));
-        SE2_CUDA(cudaMemsetAsync(nm, 0, sizeof(int), s));
+    if (cap1 == 0 || cap2 == 0) {
+        if (cap1) SE2_CUDA(cudaMemsetAsync(d_matches12, 0xff, sizeof(int) * cap1 * B, s));
+        SE2_CUDA(cudaMemsetAsync(nm, 0, sizeof(int) * B, s));
         return SE2GPU_OK;
     }
-    { const int rc = launch_grid(m, d_kp2, n2, d_n2, grid, s); if (rc != SE2GPU_OK) return rc; }
+    { const int rc = launch_grid(m, B, d_kp2, cap2, d_n2, grid, s); if (rc != SE2GPU_OK) return rc; }
     CandArgs ca{};
-    ca.mode = MODE_WINDOW; ca.nq_cap = n1; ca.d_nq = d_n1; ca.kp1 = d_kp1; ca.prev = d_prev; ca.min_level = min_level; ca.max_level = max_level;
+    ca.mode = MODE_WINDOW; ca.nq_cap = cap1; ca.d_nq = d_n1; ca.kp1 = d_kp1; ca.prev = d_prev; ca.min_level = min_level; ca.max_level = max_level;
     ca.level_offset = level_offset; ca.win_size = win_size; ca.qdesc = reinterpret_cast<const uint32_t*>(d_desc1);
     ca.kp = d_kp2; ca.desc = reinterpret_cast<const uint32_t*>(d_desc2); ca.cell = m->cell; ca.order = m->order; ca.n_valid = m->nvalid; ca.db_skip = nullptr;
-    ca.g = grid; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand;
+    ca.db_cap = cap2; ca.g = grid; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand; ca.scr_q = m->max_q;
     m->prof.begin(1, s);
-    SE2_LAUNCH(k_candidates, (n1 * 32 + 255) / 256, 256, 0, s, ca);
+    SE2_LAUNCH(k_candidates, dim3((cap1 * 32 + 255) / 256, B), 256, 0, s, ca);
     m->prof.end(s);
     ResolveArgs ra{};
-    ra.nq_cap = n1; ra.d_nq = d_n1; ra.n2_cap = n2; ra.d_n2 = d_n2; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;
+    ra.nq_cap = cap1; ra.d_nq = d_n1; ra.n2_cap = cap2; ra.d_n2 = d_n2; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;
     ra.ang1 = &d_kp1->angle; ra.stride1 = sizeof(se2gpu_keypoint) / 4; ra.ang2 = &d_kp2->angle; ra.stride2 = sizeof(se2gpu_keypoint) / 4; ra.check_ori = 1;
-    ra.qid = nullptr; ra.kp2 = d_kp2; ra.out = d_matches12; ra.n_out = n1; ra.prev = d_prev; ra.nmatches = nm; ra.flags = m->flags;
-    return launch_resolve<MODE_WINDOW>(m, ra, d_kp1, s);
+    ra.qid = nullptr; ra.kp2 = d_kp2; ra.out = d_matches12; ra.n_out = cap1; ra.prev = d_prev; ra.nmatches = nm; ra.flags = m->flags;
+    return launch_resolve<MODE_WINDOW>(m, B, ra, d_kp1, s);
 }
 
 int se2gpu_match_by_projection_device(se2gpu_matcher* m, const se2gpu_keypoint* d_kf_kp, const uint8_t* d_kf_desc, int n_kf, const int* d_n_kf,
                                       const uint8_t* d_kf_observed, const uint8_t* d_mp_valid, const float* d_mp_uv, int n_mp,
                                       const int* d_mp_octave, const uint8_t* d_mp_desc, se2gpu_grid_params grid, int win_size,
                                       int level_offset, float nnratio, int* d_matches_idx_mp, int* d_nmatches, void* stream) {
+    return se2gpu_match_by_projection_batch_device(m, 1, d_kf_kp, d_kf_desc, n_kf, d_n_kf, d_kf_observed, d_mp_valid, d_mp_uv, n_mp, d_mp_octave,
+                                                   d_mp_desc, grid, win_size, level_offset, nnratio, d_matches_idx_mp, d_nmatches, stream);
+}
+
+int se2gpu_match_by_projection_batch_device(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kf_kp, const uint8_t* d_kf_desc, int cap_kf,
+                                            const int* d_n_kf, const uint8_t* d_kf_observed, const uint8_t* d_mp_valid, const float* d_mp_uv,
+                                            int cap_mp, const int* d_mp_octave, const uint8_t* d_mp_desc, se2gpu_grid_params grid,
+                                            int win_size, int level_offset, float nnratio, int* d_matches_idx_mp, int* d_nmatches,
+                                            void* stream) {
     if (!m) return fail(SE2GPU_ERR_INVALID, "null handle");
-    if (n_kf < 0 || n_mp < 0) return fail(SE2GPU_ERR_INVALID, "negative sizes");
-    if (n_mp > m->max_q || n_kf > m->max_db) return fail(SE2GPU_ERR_CAPACITY, "%d x %d exceeds the matcher's capacity %d x %d", n_mp, n_kf, m->max_q, m->max_db);
+    if (B < 0 || cap_kf < 0 || cap_mp < 0) return fail(SE2GPU_ERR_INVALID, "negative sizes");
+    if (B > m->max_batch || cap_mp > m->max_q || cap_kf > m->max_db)
+        return fail(SE2GPU_ERR_CAPACITY, "%d pairs of %d x %d exceed the matcher's capacity %d pairs of %d x %d", B, cap_mp, cap_kf, m->max_batch, m->max_q, m->max_db);
     SE2_NVTX("se2gpu.match_by_projection");
-    if (n_kf && (!d_kf_kp || !d_kf_desc || !d_kf_observed || !d_matches_idx_mp)) return fail(SE2GPU_ERR_INVALID, "null argument");
-    if (n_mp && (!d_mp_valid || !d_mp_uv || !d_mp_octave || !d_mp_desc)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (B == 0) return SE2GPU_OK;
+    if (cap_kf && (!d_kf_kp || !d_kf_desc || !d_kf_observed || !d_matches_idx_mp)) return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (cap_mp && (!d_mp_valid || !d_mp_uv || !d_mp_octave || !d_mp_desc)) return fail(SE2GPU_ERR_INVALID, "null argument");
     SE2_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = (cudaStream_t)stream;
     int* nm = d_nmatches ? d_nmatches : m->nm;
-    if (n_kf == 0 || n_mp == 0) {
-        if (n_kf) SE2_CUDA(cudaMemsetAsync(d_matches_idx_mp, 0xff, sizeof(int) * n_kf, s));
-        SE2_CUDA(cudaMemsetAsync(nm, 0, sizeof(int), s));
+    if (cap_kf == 0 || cap_mp == 0) {
+        if (cap_kf) SE2_CUDA(cudaMemsetAsync(d_matches_idx_mp, 0xff, sizeof(int) * cap_kf * B, s));
+        SE2_CUDA(cudaMemsetAsync(nm, 0, sizeof(int) * B, s));
         return SE2GPU_OK;
     }
-    { const int rc = launch_grid(m, d_kf_kp, n_kf, d_n_kf, grid, s); if (rc != SE2GPU_OK) return rc; }
+    { const int rc = launch_grid(m, B, d_kf_kp, cap_kf, d_n_kf, grid, s); if (rc != SE2GPU_OK) return rc; }
     CandArgs ca{};
-    ca.mode = MODE_PROJ; ca.nq_cap = n_mp; ca.d_nq = nullptr; ca.mp_valid = d_mp_valid; ca.mp_uv = d_mp_uv; ca.mp_octave = d_mp_octave;
+    ca.mode = MODE_PROJ; ca.nq_cap = cap_mp; ca.d_nq = nullptr; ca.mp_valid = d_mp_valid; ca.mp_uv = d_mp_uv; ca.mp_octave = d_mp_octave;
     ca.level_offset = level_offset; ca.win_size = win_size; ca.qdesc = reinterpret_cast<const uint32_t*>(d_mp_desc);
     ca.kp = d_kf_kp; ca.desc = reinterpret_cast<const uint32_t*>(d_kf_desc); ca.cell = m->cell; ca.order = m->order; ca.n_valid = m->nvalid; ca.db_skip = d_kf_observed;
-    ca.g = grid; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand;
+    ca.db_cap = cap_kf; ca.g = grid; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand; ca.scr_q = m->max_q;
     m->prof.begin(1, s);
-    SE2_LAUNCH(k_candidates, (n_mp * 32 + 255) / 256, 256, 0, s, ca);
+    SE2_LAUNCH(k_candidates, dim3((cap_mp * 32 + 255) / 256, B), 256, 0, s, ca);
     m->prof.end(s);
     ResolveArgs ra{};
-    ra.nq_cap = n_mp; ra.d_nq = nullptr; ra.n2_cap = n_kf; ra.d_n2 = d_n_kf; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;
-    ra.check_ori = 0; ra.out = d_matches_idx_mp; ra.n_out = n_kf; ra.nmatches = nm; ra.flags = m->flags;
-    return launch_resolve<MODE_PROJ>(m, ra, nullptr, s);
+    ra.nq_cap = cap_mp; ra.d_nq = nullptr; ra.n2_cap = cap_kf; ra.d_n2 = d_n_kf; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;
+    ra.check_ori = 0; ra.out = d_matches_idx_mp; ra.n_out = cap_kf; ra.nmatches = nm; ra.flags = m->flags;
+    return launch_resolve<MODE_PROJ>(m, B, ra, nullptr, s);
 }
 
 }  // extern "C"
@@ -857,7 +961,7 @@ int se2gpu_matcher_search_by_bow(se2gpu_matcher* m, const se2gpu_bow_kf* k1, con
     ra.nq_cap = nq; ra.d_nq = nullptr; ra.n2_cap = k2->n; ra.d_n2 = nullptr; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;
     ra.ang1 = m->d_f1; ra.stride1 = 1; ra.ang2 = m->d_f2; ra.stride2 = 1; ra.check_ori = check_orientation;
     ra.qid = m->d_i1; ra.out = m->d_out; ra.n_out = k1->n; ra.nmatches = m->nm; ra.flags = m->flags;
-    int rc = launch_resolve<MODE_BOW>(m, ra, nullptr, s);
+    int rc = launch_resolve<MODE_BOW>(m, 1, ra, nullptr, s);
     if (rc != SE2GPU_OK) return rc;
     int* h_m = st.alloc<int>(k1->n); int* h_nm = st.alloc<int>(1);
     if (!h_m || !h_nm) return fail(SE2GPU_ERR_CAPACITY, "staging exhausted");

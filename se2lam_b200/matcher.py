@@ -36,19 +36,19 @@ class FrameView:
 
 
 class ORBmatcher:
-    """ORBmatcher(nnratio, checkOri). With `max_queries` / `max_db` it owns a matcher context (se2gpu_matcher_create: all
-    device buffers allocated once) and offers the device-resident entry points; without, the per-device default context
-    of the library is used."""
+    """ORBmatcher(nnratio, checkOri). With `max_queries` / `max_db` it owns a matcher context (se2gpu_matcher_create_batch:
+    all device buffers allocated once, for up to `max_batch` frame pairs per batched call) and offers the device-resident
+    entry points; without, the per-device default context of the library is used."""
     TH_HIGH, TH_LOW, HISTO_LENGTH = 100, 75, 30   # ORBmatcher.cpp:45-47
     PROFILE_GROUPS = ("k_grid_build", "k_candidates", "k_resolve", "k_fallback")
 
-    def __init__(self, nnratio=0.6, checkOri=True, device=0, max_queries=None, max_db=None):
+    def __init__(self, nnratio=0.6, checkOri=True, device=0, max_queries=None, max_db=None, max_batch=1):
         self.mfNNratio, self.mbCheckOrientation, self.device = float(nnratio), bool(checkOri), device
         self.h = None
         if max_queries is not None or max_db is not None:
-            self.h = lib().se2gpu_matcher_create(int(max_queries or max_db), int(max_db or max_queries), device)
+            self.h = lib().se2gpu_matcher_create_batch(int(max_queries or max_db), int(max_db or max_queries), int(max_batch), device)
             if not self.h:
-                raise _capi.Se2GpuError("se2gpu_matcher_create failed: " + _capi.last_error())
+                raise _capi.Se2GpuError("se2gpu_matcher_create_batch failed: " + _capi.last_error())
 
     def close(self):
         if getattr(self, "h", None):
@@ -84,6 +84,26 @@ class ORBmatcher:
                                                       ptr(d_nmatches), C.c_void_p(int(stream) if stream else 0)),
               "se2gpu_match_by_projection_device")
 
+    # ---- batched device entry points: B frame pairs, pair b at slot b of every array (see include/se2gpu.h)
+    def MatchByWindowBatchDevice(self, B, d_kp1, d_desc1, cap1, d_kp2, d_desc2, cap2, d_prev, grid: GridParams, winSize, d_matches12,
+                                 d_nmatches=None, d_n1=None, d_n2=None, levelOffset=1, minLevel=0, maxLevel=8, stream=0):
+        assert self.h, "device entry points need an owned context (pass max_queries / max_db)"
+        check(lib().se2gpu_match_by_window_batch_device(self.h, int(B), ptr(d_kp1), ptr(d_desc1), int(cap1), ptr(d_n1), ptr(d_kp2),
+                                                        ptr(d_desc2), int(cap2), ptr(d_n2), ptr(d_prev), grid, int(winSize), levelOffset,
+                                                        minLevel, maxLevel, self.mfNNratio, ptr(d_matches12), ptr(d_nmatches),
+                                                        C.c_void_p(int(stream) if stream else 0)), "se2gpu_match_by_window_batch_device")
+
+    def MatchByProjectionBatchDevice(self, B, d_kf_kp, d_kf_desc, cap_kf, d_kf_observed, d_mp_valid, d_mp_uv, cap_mp, d_mp_octave,
+                                     d_mp_desc, grid: GridParams, winSize, levelOffset, d_matches_idx_mp, d_nmatches=None, d_n_kf=None,
+                                     stream=0):
+        assert self.h, "device entry points need an owned context (pass max_queries / max_db)"
+        check(lib().se2gpu_match_by_projection_batch_device(self.h, int(B), ptr(d_kf_kp), ptr(d_kf_desc), int(cap_kf), ptr(d_n_kf),
+                                                            ptr(d_kf_observed), ptr(d_mp_valid), ptr(d_mp_uv), int(cap_mp),
+                                                            ptr(d_mp_octave), ptr(d_mp_desc), grid, int(winSize), int(levelOffset),
+                                                            self.mfNNratio, ptr(d_matches_idx_mp), ptr(d_nmatches),
+                                                            C.c_void_p(int(stream) if stream else 0)),
+              "se2gpu_match_by_projection_batch_device")
+
     def profile(self, enable=True):
         check(lib().se2gpu_matcher_profile(self.h, int(enable)), "se2gpu_matcher_profile")
 
@@ -96,6 +116,12 @@ class ORBmatcher:
         r, f = C.c_int(), C.c_int()
         check(lib().se2gpu_matcher_last_rounds(self.h, C.byref(r), C.byref(f)), "se2gpu_matcher_last_rounds")
         return r.value, bool(f.value)
+
+    def last_rounds_batch(self, B):
+        """(rounds [B] int32, used_fallback [B] bool) of every pair of the last batched call."""
+        r, f = np.zeros(B, np.int32), np.zeros(B, np.int32)
+        check(lib().se2gpu_matcher_last_rounds_batch(self.h, int(B), ptr(r), ptr(f)), "se2gpu_matcher_last_rounds_batch")
+        return r, f.astype(bool)
 
     @staticmethod
     def DescriptorDistance(a, b, device=0):
