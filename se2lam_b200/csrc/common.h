@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -223,6 +224,117 @@ struct PinnedArena {
         return SE2GPU_OK;
     }
 };
+
+// Element offsets of the arrays that share one device buffer, each starting on a 32-element boundary: `o.x = L.take(n)`
+// names the next n elements x, and L.size is the buffer's length.
+struct Layout {
+    size_t size = 0;
+    size_t take(size_t n) {
+        const size_t o = size;
+        size += (n + 31) & ~(size_t)31;
+        return o;
+    }
+};
+
+// A Layout whose arrays are host data, packed (zero-padded) into one vector for one upload.
+template <class T>
+struct Packed : Layout {
+    std::vector<T> data;
+    template <class U>
+    size_t put(const U* p, size_t n) {
+        const size_t o = take(n);
+        data.resize(size);
+        std::copy(p, p + n, data.begin() + o);
+        return o;
+    }
+    template <class V>
+    size_t put(const V& v) { return put(v.data(), v.size()); }
+};
+
+// The context of a solver that plans each call on the host (global_ba.cu, se3_ba.cu): its device, a blocking stream for
+// the host entries, grow-only device buffers for the plan (ints, long longs) and the work (doubles), and the pinned arena
+// the plan goes up through. create_plan_context makes one; delete destroys it once its last call has completed.
+struct PlanContext {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t uploaded = nullptr;  // the last plan upload out of the pinned arena has completed
+    cudaEvent_t done = nullptr;      // the last kernel, which reads the plan and work buffers, has completed
+    DeviceBuffers bufs;
+    int* d_int = nullptr; size_t cap_int = 0;
+    long long* d_ll = nullptr; size_t cap_ll = 0;
+    double* d_dbl = nullptr; size_t cap_dbl = 0;
+    PinnedArena arena;
+
+    ~PlanContext() {
+        cudaSetDevice(device);
+        if (done) cudaEventSynchronize(done);
+        if (stream) cudaStreamSynchronize(stream);
+        if (uploaded) cudaEventDestroy(uploaded);
+        if (done) cudaEventDestroy(done);
+        if (stream) cudaStreamDestroy(stream);
+    }
+
+    template <class T>
+    int grow(T** p, size_t* cap, size_t need) {
+        if (need <= *cap && *p) return SE2GPU_OK;
+        SE2_CUDA(cudaEventSynchronize(done));  // an earlier call, on any stream, may still read the buffer
+        SE2_CUDA(bufs.regrow(p, need));
+        *cap = need;
+        return SE2GPU_OK;
+    }
+
+    // Grows d_int / d_ll to the plan and copies it there on stream s, ordered against the calls before on any stream:
+    //  * the plan goes up through the pinned arena, so the previous call's copies out of it must have completed;
+    //  * the previous call's kernel may run on another stream, and this call's copies and kernel overwrite what it reads,
+    //    so s waits for it.
+    // The caller launches its kernel on s and then records `done` there.
+    int upload_plan(const std::vector<int>& ints, const std::vector<long long>& lls, cudaStream_t s) {
+        { const int rc = grow(&d_int, &cap_int, ints.size()); if (rc) return rc; }
+        { const int rc = grow(&d_ll, &cap_ll, lls.size()); if (rc) return rc; }
+        SE2_CUDA(cudaEventSynchronize(uploaded));
+        SE2_CUDA(cudaStreamWaitEvent(s, done, 0));
+        arena.reserve(4 * ints.size() + 8 * lls.size() + 128);
+        { const int rc = arena.up(d_int, ints.data(), ints.size(), s); if (rc) return rc; }
+        { const int rc = arena.up(d_ll, lls.data(), lls.size(), s); if (rc) return rc; }
+        SE2_CUDA(cudaEventRecord(uploaded, s));
+        return SE2GPU_OK;
+    }
+};
+
+template <class Ctx>
+Ctx* create_plan_context(int device) {
+    if (select_device(device)) return nullptr;
+    Ctx* h = new Ctx;
+    h->device = device;
+    if (cudaStreamCreate(&h->stream) != cudaSuccess || cudaEventCreateWithFlags(&h->uploaded, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
+        fail(SE2GPU_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
+        delete h;
+        return nullptr;
+    }
+    return h;
+}
+
+// n SE(3) links between N nodes (the global graph's edges, the window's odometry): from / to in range and distinct; with
+// measure [16 n] and info [36 n] (host entries) also every measurement finite and every information finite and symmetric.
+// `link` and `node` name them in the message.
+inline int check_se3_links(int N, int n, const int* from, const int* to, const float* measure, const float* info, const char* link,
+                           const char* node) {
+    for (int e = 0; e < n; ++e) {
+        if (from[e] < 0 || from[e] >= N || to[e] < 0 || to[e] >= N) return fail(SE2GPU_ERR_INVALID, "%s %d: %s out of range", link, e, node);
+        if (from[e] == to[e]) return fail(SE2GPU_ERR_INVALID, "%s %d: from == to", link, e);
+        if (!measure) continue;
+        for (int k = 0; k < 16; ++k)
+            if (!std::isfinite(measure[16 * (size_t)e + k])) return fail(SE2GPU_ERR_INVALID, "%s %d: measurement not finite", link, e);
+        const float* I = info + 36 * (size_t)e;
+        for (int r = 0; r < 6; ++r)
+            for (int c = 0; c < 6; ++c) {
+                if (!std::isfinite(I[r * 6 + c])) return fail(SE2GPU_ERR_INVALID, "%s %d: information not finite", link, e);
+                if (I[r * 6 + c] != I[c * 6 + r]) return fail(SE2GPU_ERR_INVALID, "%s %d: information not symmetric", link, e);
+            }
+    }
+    return SE2GPU_OK;
+}
 
 // ---------------------------------------------------------------------------------------------- shared device helpers
 // number of valid entries: *d_n clamped to [0, cap], or cap when there is no device-side count

@@ -29,7 +29,6 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kLin = 120;  // per-edge linearisation: H_ii, H_jj, H_ij (36 each), b_i, b_j (6 each)
 
 struct KArgs {
     int N, E, nf, S, iterations;
@@ -50,7 +49,7 @@ struct KArgs {
     Prior* prior;           // [N]
     Iso* Zinv;              // [E]
     double* Om;             // [E*36]
-    double* lin;            // [E*kLin]
+    double* lin;            // [E*kEdgeRec]
     double* pH;             // [nf*36] prior blocks, by position
     double* pb;             // [nf*6]
     double* Hs;             // [env*36] the gathered H (blocks outside the gather lists stay zero)
@@ -136,40 +135,11 @@ __device__ __noinline__ double edge_error(const Iso& Zinv, const double* Om, con
     return chi;
 }
 
-// one edge's blocks: H_ii, H_jj, H_ij = Ji^T Om Jj, b_i = -Ji^T Om e, b_j
+// one edge's record (envelope.h): H_ii, H_jj, H_ij = Ji^T Om Jj, b_i = -Ji^T Om e, b_j
 __device__ __noinline__ void edge_linearise(const Iso& Zinv, const double* Om, const Iso& Xi, const Iso& Xj, double* out) {
     double e[6], J[2][36];
     edge_error(Zinv, Om, Xi, Xj, e, J[0], J[1]);
-    double Oe[6];
-    for (int r = 0; r < 6; ++r) {
-        double acc = 0;
-        for (int c = 0; c < 6; ++c) acc += Om[r * 6 + c] * e[c];
-        Oe[r] = acc;
-    }
-    for (int s = 0; s < 2; ++s) {
-        double OJ[36];
-        for (int r = 0; r < 6; ++r)
-            for (int c = 0; c < 6; ++c) {
-                double acc = 0;
-                for (int m = 0; m < 6; ++m) acc += Om[r * 6 + m] * J[s][m * 6 + c];
-                OJ[r * 6 + c] = acc;
-            }
-        for (int r = 0; r < 6; ++r) {
-            for (int c = 0; c < 6; ++c) {
-                double acc = 0;
-                for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * OJ[m * 6 + c];
-                out[36 * s + r * 6 + c] = acc;  // s = 0: H_ii, s = 1: H_jj
-                if (s == 1) {
-                    double ij = 0;
-                    for (int m = 0; m < 6; ++m) ij += J[0][m * 6 + r] * OJ[m * 6 + c];
-                    out[72 + r * 6 + c] = ij;
-                }
-            }
-            double acc = 0;
-            for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * Oe[m];
-            out[108 + 6 * s + r] = -acc;
-        }
-    }
+    edge_record(Om, e, J, out);
 }
 
 // activeChi2 at the estimates X: every active edge and every vertex's prior (the fixed ones are constant, but g2o counts them);
@@ -232,7 +202,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
         Iso* Xt = a.X[s_buf ^ 1];
         // linearise
         for (int e = tid; e < a.E; e += kThreads)
-            if (edge_active(a, e)) edge_linearise(a.Zinv[e], a.Om + 36 * (size_t)e, X[a.from[e]], X[a.to[e]], a.lin + kLin * (size_t)e);
+            if (edge_active(a, e)) edge_linearise(a.Zinv[e], a.Om + 36 * (size_t)e, X[a.from[e]], X[a.to[e]], a.lin + kEdgeRec * (size_t)e);
         for (int p = tid; p < a.nf; p += kThreads) {
             const int v = a.vert[p];
             prior_terms(a.prior[v], X[v], a.pH + 36 * (size_t)p, a.pb + 6 * (size_t)p);
@@ -240,34 +210,15 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
         __syncthreads();
         stamp(kLinearise);
         // gather H and b in ascending edge order
-        for (int idx = tid; idx < a.nf * 42; idx += kThreads) {
-            const int p = idx / 42, rc = idx % 42;
-            const bool isb = rc >= 36;
-            double s = isb ? a.pb[6 * (size_t)p + rc - 36] : a.pH[36 * (size_t)p + rc];
-            for (int q = a.diag_ptr[p]; q < a.diag_ptr[p + 1]; ++q) {
-                const int code = a.diag_code[q], e = code >> 2, side = code & 3;
-                if (!edge_active(a, e)) continue;
-                s += isb ? a.lin[kLin * (size_t)e + 108 + 6 * side + rc - 36] : a.lin[kLin * (size_t)e + 36 * side + rc];
-            }
-            if (isb) a.b[6 * (size_t)p + rc - 36] = s;
-            else a.Hs[36 * (size_t)(a.rowoff[p] + (p - a.first[p])) + rc] = s;
-        }
-        for (int idx = tid; idx < a.S * 36; idx += kThreads) {
-            const int sl = idx / 36, rc = idx % 36, tr = (rc % 6) * 6 + rc / 6;
-            double s = 0;
-            for (int q = a.off_ptr[sl]; q < a.off_ptr[sl + 1]; ++q) {
-                const int code = a.off_code[q], e = code >> 2;
-                if (!edge_active(a, e)) continue;
-                s += a.lin[kLin * (size_t)e + 72 + ((code & 3) == gba::kOffDiag ? rc : tr)];
-            }
-            a.Hs[36 * (size_t)a.off_blk[sl] + rc] = s;
-        }
+        const auto active = [&](int e) { return edge_active(a, e); };
+        gather_diag(a, a.lin, a.b, tid, kThreads, active, [](int, int, double s) { return s; });
+        gather_off(a, a.lin, tid, kThreads, active);
         __syncthreads();
         stamp(kGather);
         if (it == 0) {  // computeLambdaInit over the free vertices
             double m = 0;
             for (int idx = tid; idx < a.nf * 6; idx += kThreads)
-                m = fmax(m, fabs(a.Hs[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7]));
+                m = fmax(m, fabs(blkp(a.Hs, a, idx / 6, idx / 6)[(idx % 6) * 7]));
             m = cta_max(m, s_red);
             if (tid == 0) lm_lambda_init(m, s_lambda, s_ni);
         }
@@ -279,8 +230,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_global_ba(KArgs a) {
             const double lambda = s_lambda;
             for (size_t i = tid; i < env36; i += kThreads) a.L[i] = a.Hs[i];
             __syncthreads();
-            for (int idx = tid; idx < a.nf * 6; idx += kThreads)
-                a.L[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7] += lambda;
+            damp(a, a.L, lambda, tid, kThreads);
             __syncthreads();
             stamp(kDamp);
             const bool ok = env_factor<kThreads>(a, s_D, &s_flag);
@@ -356,45 +306,22 @@ int check_params(const se2gpu_global_ba_params* p) {
     return SE2GPU_OK;
 }
 
-int check_topology(int N, const uint8_t* fixed, int E, const int* from, const int* to) {
+// the graph; with measure / info (host entries) also the edges' values
+int check_graph(int N, const uint8_t* fixed, int E, const int* from, const int* to, const float* measure, const float* info) {
     if (N <= 0) return fail(SE2GPU_ERR_INVALID, "N = %d", N);
     if (E < 0) return fail(SE2GPU_ERR_INVALID, "E = %d", E);
     if (!fixed || (E && (!from || !to))) return fail(SE2GPU_ERR_INVALID, "null topology arrays");
-    for (int e = 0; e < E; ++e) {
-        if (from[e] < 0 || from[e] >= N || to[e] < 0 || to[e] >= N) return fail(SE2GPU_ERR_INVALID, "edge %d: vertex out of range", e);
-        if (from[e] == to[e]) return fail(SE2GPU_ERR_INVALID, "edge %d: from == to", e);
-    }
-    return SE2GPU_OK;
+    return check_se3_links(N, E, from, to, measure, info, "edge", "vertex");
 }
 
 }  // namespace
 
-struct se2gpu_global_ba_ctx {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t uploaded = nullptr;  // the last plan upload out of the pinned arena has completed
-    cudaEvent_t done = nullptr;      // the last kernel, which reads the plan and work buffers, has completed
-    DeviceBuffers bufs;
-    int* d_int = nullptr; size_t cap_int = 0;
-    long long* d_ll = nullptr; size_t cap_ll = 0;
-    double* d_dbl = nullptr; size_t cap_dbl = 0;
+struct se2gpu_global_ba_ctx : se2gpu::PlanContext {
     unsigned long long* d_prof = nullptr;  // [kPhases] while profiling is on
     unsigned long long* d_prof_buf = nullptr;
-    PinnedArena arena;
 };
 
 namespace {
-
-template <class T>
-int grow(se2gpu_global_ba_ctx* h, T** p, size_t* cap, size_t need) {
-    if (need <= *cap && *p) return SE2GPU_OK;
-    SE2_CUDA(cudaEventSynchronize(h->done));  // an earlier call, on any stream, may still read the buffer
-    SE2_CUDA(h->bufs.regrow(p, need));
-    *cap = need;
-    return SE2GPU_OK;
-}
-
-size_t al(size_t n) { return (n + 31) & ~(size_t)31; }
 
 // plans the call, uploads the plan on `stream` and launches the kernel there; every value array is device memory
 int run(se2gpu_global_ba_ctx* h, int N, const uint8_t* fixed, int E, const int* from, const int* to, const float* d_Tcw,
@@ -404,55 +331,42 @@ int run(se2gpu_global_ba_ctx* h, int N, const uint8_t* fixed, int E, const int* 
     const gba::Plan P = gba::make_plan(N, fixed, E, from, to);
     const int nf = P.n_free, S = (int)P.off_blk.size();
     const size_t env = (size_t)P.env_blocks();
-    // int arrays: from, to (when not given on the device), pos, vert, first, col_ptr, col_rows, diag_ptr, diag_code, off_ptr, off_code
-    const size_t n_int[11] = {d_from ? 0 : (size_t)E, d_to ? 0 : (size_t)E, (size_t)N, (size_t)nf, (size_t)nf, (size_t)nf + 1,
-                              P.col_rows.size(), (size_t)nf + 1, P.diag_code.size(), (size_t)S + 1, P.off_code.size()};
-    const int* src_int[11] = {from, to, P.pos.data(), P.vert.data(), P.first.data(), P.col_ptr.data(), P.col_rows.data(),
-                              P.diag_ptr.data(), P.diag_code.data(), P.off_ptr.data(), P.off_code.data()};
-    size_t o_int[12] = {0};
-    for (int i = 0; i < 11; ++i) o_int[i + 1] = o_int[i] + al(n_int[i]);
-    const size_t o_ll[3] = {0, al((size_t)nf + 1), al((size_t)nf + 1) + al((size_t)S)};
-    // doubles: X[2] (12 N each), prior (48 N), Zinv (12 E), Om (36 E), lin (120 E), pH (36 nf), pb, b, x (6 nf each), Hs, L (36 env)
-    const size_t n_dbl[11] = {12 * (size_t)N, 12 * (size_t)N, sizeof(Prior) / 8 * (size_t)N, 12 * (size_t)E, 36 * (size_t)E,
-                              kLin * (size_t)E, 36 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 36 * env};
-    size_t o_dbl[13] = {0};
-    for (int i = 0; i < 11; ++i) o_dbl[i + 1] = o_dbl[i] + al(n_dbl[i]);
-    o_dbl[12] = o_dbl[11] + al(36 * env);
-    { const int rc = grow(h, &h->d_int, &h->cap_int, o_int[11]); if (rc) return rc; }
-    { const int rc = grow(h, &h->d_ll, &h->cap_ll, o_ll[2]); if (rc) return rc; }
-    { const int rc = grow(h, &h->d_dbl, &h->cap_dbl, o_dbl[12]); if (rc) return rc; }
-    // the plan goes up through the page-locked arena; the previous call's copies out of it must have completed
-    SE2_CUDA(cudaEventSynchronize(h->uploaded));
-    // the previous call's kernel may run on another stream: this call's plan copies and kernel overwrite what it reads
-    SE2_CUDA(cudaStreamWaitEvent(stream, h->done, 0));
-    size_t bytes = 0;
-    for (int i = 0; i < 11; ++i) bytes += 4 * al(n_int[i]) + 64;
-    bytes += 8 * o_ll[2] + 128;
-    h->arena.reserve(bytes);
-    for (int i = 0; i < 11; ++i) {
-        const int rc = h->arena.up(h->d_int + o_int[i], src_int[i], n_int[i], stream);
-        if (rc) return rc;
-    }
-    { const int rc = h->arena.up((long long*)h->d_ll, (const long long*)P.rowoff.data(), (size_t)nf + 1, stream); if (rc) return rc; }
-    { const int rc = h->arena.up(h->d_ll + o_ll[1], (const long long*)P.off_blk.data(), (size_t)S, stream); if (rc) return rc; }
-    SE2_CUDA(cudaEventRecord(h->uploaded, stream));
+    // the plan (from / to only when they are not given on the device), then the work
+    Packed<int> ints;
+    Packed<long long> lls;
+    Layout dbl;
+    struct {
+        size_t from, to, pos, vert, first, col_ptr, col_rows, diag_ptr, diag_code, off_ptr, off_code;  // ints
+        size_t rowoff, off_blk;                                                                      // long longs
+        size_t X[2], prior, Zinv, Om, lin, pH, pb, b, x, Hs, L;                                      // doubles
+    } o;
+    o.from = ints.put(from, d_from ? 0 : (size_t)E); o.to = ints.put(to, d_to ? 0 : (size_t)E);
+    o.pos = ints.put(P.pos); o.vert = ints.put(P.vert); o.first = ints.put(P.first); o.col_ptr = ints.put(P.col_ptr);
+    o.col_rows = ints.put(P.col_rows); o.diag_ptr = ints.put(P.diag_ptr); o.diag_code = ints.put(P.diag_code);
+    o.off_ptr = ints.put(P.off_ptr); o.off_code = ints.put(P.off_code);
+    o.rowoff = lls.put(P.rowoff); o.off_blk = lls.put(P.off_blk);
+    o.X[0] = dbl.take(12 * (size_t)N); o.X[1] = dbl.take(12 * (size_t)N); o.prior = dbl.take(sizeof(Prior) / 8 * (size_t)N);
+    o.Zinv = dbl.take(12 * (size_t)E); o.Om = dbl.take(36 * (size_t)E); o.lin = dbl.take(kEdgeRec * (size_t)E);
+    o.pH = dbl.take(36 * (size_t)nf); o.pb = dbl.take(6 * (size_t)nf); o.b = dbl.take(6 * (size_t)nf); o.x = dbl.take(6 * (size_t)nf);
+    o.Hs = dbl.take(36 * env); o.L = dbl.take(36 * env);
+    { const int rc = h->grow(&h->d_dbl, &h->cap_dbl, dbl.size); if (rc) return rc; }
+    { const int rc = h->upload_plan(ints.data, lls.data, stream); if (rc) return rc; }
 
     KArgs a{};
     a.N = N; a.E = E; a.nf = nf; a.S = S; a.iterations = prm->iterations;
     std::memcpy(a.Tbc, prm->Tbc, sizeof a.Tbc);
     a.xrot = prm->xrot_info; a.yrot = prm->yrot_info; a.zinfo = prm->z_info;
     a.Tcw = d_Tcw; a.measure = d_measure; a.info = d_info;
-    a.from = d_from ? d_from : h->d_int + o_int[0];
-    a.to = d_to ? d_to : h->d_int + o_int[1];
+    const int* I = h->d_int;
+    a.from = d_from ? d_from : I + o.from;
+    a.to = d_to ? d_to : I + o.to;
     a.edge_status = d_edge_status;
-    int* I = h->d_int;
-    a.pos = I + o_int[2]; a.vert = I + o_int[3]; a.first = I + o_int[4]; a.col_ptr = I + o_int[5]; a.col_rows = I + o_int[6];
-    a.diag_ptr = I + o_int[7]; a.diag_code = I + o_int[8]; a.off_ptr = I + o_int[9]; a.off_code = I + o_int[10];
-    a.rowoff = h->d_ll; a.off_blk = h->d_ll + o_ll[1];
+    a.pos = I + o.pos; a.vert = I + o.vert; a.first = I + o.first; a.col_ptr = I + o.col_ptr; a.col_rows = I + o.col_rows;
+    a.diag_ptr = I + o.diag_ptr; a.diag_code = I + o.diag_code; a.off_ptr = I + o.off_ptr; a.off_code = I + o.off_code;
+    a.rowoff = h->d_ll + o.rowoff; a.off_blk = h->d_ll + o.off_blk;
     double* D = h->d_dbl;
-    a.X[0] = (Iso*)(D + o_dbl[0]); a.X[1] = (Iso*)(D + o_dbl[1]); a.prior = (Prior*)(D + o_dbl[2]); a.Zinv = (Iso*)(D + o_dbl[3]);
-    a.Om = D + o_dbl[4]; a.lin = D + o_dbl[5]; a.pH = D + o_dbl[6]; a.pb = D + o_dbl[7]; a.b = D + o_dbl[8]; a.x = D + o_dbl[9];
-    a.Hs = D + o_dbl[10]; a.L = D + o_dbl[11];
+    a.X[0] = (Iso*)(D + o.X[0]); a.X[1] = (Iso*)(D + o.X[1]); a.prior = (Prior*)(D + o.prior); a.Zinv = (Iso*)(D + o.Zinv);
+    a.Om = D + o.Om; a.lin = D + o.lin; a.pH = D + o.pH; a.pb = D + o.pb; a.b = D + o.b; a.x = D + o.x; a.Hs = D + o.Hs; a.L = D + o.L;
     a.Tcw_out = d_Tcw_out; a.status = d_status; a.iters = d_iters; a.stats = d_stats; a.poses = d_poses;
     a.prof = h->d_prof;
     if (d_stats && prm->iterations)
@@ -466,47 +380,17 @@ int run(se2gpu_global_ba_ctx* h, int N, const uint8_t* fixed, int E, const int* 
 
 }  // namespace
 
-se2gpu_global_ba_ctx* se2gpu_global_ba_create(int device) {
-    if (select_device(device)) return nullptr;
-    se2gpu_global_ba_ctx* h = new se2gpu_global_ba_ctx;
-    h->device = device;
-    if (cudaStreamCreate(&h->stream) != cudaSuccess || cudaEventCreateWithFlags(&h->uploaded, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
-        fail(SE2GPU_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
-        se2gpu_global_ba_destroy(h);
-        return nullptr;
-    }
-    return h;
-}
+se2gpu_global_ba_ctx* se2gpu_global_ba_create(int device) { return create_plan_context<se2gpu_global_ba_ctx>(device); }
 
-void se2gpu_global_ba_destroy(se2gpu_global_ba_ctx* h) {
-    if (!h) return;
-    cudaSetDevice(h->device);
-    if (h->done) cudaEventSynchronize(h->done);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    if (h->uploaded) cudaEventDestroy(h->uploaded);
-    if (h->done) cudaEventDestroy(h->done);
-    if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-}
+void se2gpu_global_ba_destroy(se2gpu_global_ba_ctx* h) { delete h; }
 
 int se2gpu_global_ba(se2gpu_global_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, int E, const int* edge_from,
                      const int* edge_to, const float* measure, const float* info, const se2gpu_global_ba_params* params,
                      float* Tcw_out, int* status, int* iterations, se2gpu_ba_iter_stats* stats, double* poses) {
     if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
     { const int rc = check_params(params); if (rc) return rc; }
-    { const int rc = check_topology(N, fixed, E, edge_from, edge_to); if (rc) return rc; }
     if (!Tcw || !Tcw_out || (E && (!measure || !info))) return fail(SE2GPU_ERR_INVALID, "null arrays");
-    for (int e = 0; e < E; ++e) {
-        const float* I = info + 36 * (size_t)e;
-        for (int r = 0; r < 6; ++r)
-            for (int c = 0; c < 6; ++c) {
-                if (!std::isfinite(I[r * 6 + c])) return fail(SE2GPU_ERR_INVALID, "edge %d: information not finite", e);
-                if (I[r * 6 + c] != I[c * 6 + r]) return fail(SE2GPU_ERR_INVALID, "edge %d: information not symmetric", e);
-            }
-        for (int k = 0; k < 16; ++k)
-            if (!std::isfinite(measure[16 * (size_t)e + k])) return fail(SE2GPU_ERR_INVALID, "edge %d: measurement not finite", e);
-    }
+    { const int rc = check_graph(N, fixed, E, edge_from, edge_to, measure, info); if (rc) return rc; }
     HostStage st(h->device);
     if (const int rc = st.status()) return rc;
     const float* dT = st.upload(Tcw, 16 * (size_t)N);
@@ -531,8 +415,8 @@ int se2gpu_global_ba_device(se2gpu_global_ba_ctx* h, int N, const float* d_Tcw, 
                             se2gpu_ba_iter_stats* d_stats, double* d_poses, void* stream) {
     if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
     { const int rc = check_params(params); if (rc) return rc; }
-    { const int rc = check_topology(N, fixed, E, edge_from, edge_to); if (rc) return rc; }
     if (!d_Tcw || !d_Tcw_out || (E && (!d_measure || !d_info))) return fail(SE2GPU_ERR_INVALID, "null arrays");
+    { const int rc = check_graph(N, fixed, E, edge_from, edge_to, nullptr, nullptr); if (rc) return rc; }
     { const int rc = select_device(h->device); if (rc) return rc; }
     return run(h, N, fixed, E, edge_from, edge_to, d_Tcw, d_measure, d_info, nullptr, nullptr, d_edge_status, params, d_Tcw_out,
                d_status, d_iterations, d_stats, d_poses, (cudaStream_t)stream);

@@ -4,8 +4,8 @@
 // EdgeSE3Expmap per odometry link, one marginalised VertexSBAPointXYZ per map point and one Huber EdgeProjectXYZ2UV per
 // observation.
 //
-// The host plans the call (the reduced system's RCM order and 6 x 6 block envelope from global_ba_plan.h, and fixed-order
-// gather lists); the whole optimize() is then ONE cooperative kernel over as many CTAs as are co-resident, its phases
+// The host plans the call (se3_ba_plan.h: the reduced system's RCM order and 6 x 6 block envelope, and fixed-order gather
+// lists); the whole optimize() is then ONE cooperative kernel over as many CTAs as are co-resident, its phases
 // separated by grid-wide barriers. Landmark work (linearisation, Hll, (Hll + lambda I)^-1, the Schur complement, the back
 // substitution, the trial chi2) is spread over every CTA; the reduced system is factorised and solved by CTA 0 with
 // envelope.h. Every sum is a gather in a fixed order, and every reduction over items runs over fixed chunks of 256 items
@@ -23,8 +23,8 @@
 
 #include "common.h"
 #include "envelope.h"
-#include "global_ba_plan.h"
 #include "lm.h"
+#include "se3_ba_plan.h"
 #include "se3expmap.h"
 #include "sym3.h"
 
@@ -37,7 +37,6 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kChunk = kThreads;  // items per partial sum
 constexpr int kLin = 72;          // per projection edge: Hpp (36), bp (6), Hpl (18, pose-major), Hll (6 upper), bl (3), pad
-constexpr int kOdoLin = 120;      // per odometry edge: H_ii, H_jj, H_ij (36 each), b_i, b_j (6 each)
 
 struct Ctl {  // the LM state, written by CTA 0's thread 0 between barriers
     double cur, lambda, ni, rho, chi_before;
@@ -65,7 +64,7 @@ struct KArgs {
     SE3* X[2];        // [N] poses, current / trial
     double* P[2];     // [3 L] points
     SE3* pmeas; double* pinfo;   // [N], [36 N] priors
-    SE3* Z; double* Om; double* olin;  // odometry
+    SE3* Z; double* Om; double* olin;  // odometry: measurements, informations, records [O * kEdgeRec]
     double* lin;      // [E * kLin]
     double* Y;        // [E * 18] Hpl_e (Hll + lambda I)^-1, pose-major
     double* Hl;       // [L * 9] Hll upper, bl
@@ -90,10 +89,6 @@ struct Env {
     const int* first; const long long* rowoff; const int* col_ptr; const int* col_rows;
     double* L; double* b; double* x;
 };
-
-__device__ inline double* blk(double* M, const KArgs& a, int p, int q) {
-    return M + 36 * (size_t)(a.rowoff[p] + (q - a.first[p]));
-}
 
 // one EdgeProjectXYZ2UV at the poses X and points P: robust chi2 (raw into *raw when given)
 __device__ inline double proj_chi2(const KArgs& a, const SE3* X, const double* P, int e, double* raw) {
@@ -202,39 +197,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_se3_ba(KArgs a) {
             }
         }
         for (int o = gt; o < a.O; o += gs) {
-            double e[6], J[2][36], Oe[6];
+            double e[6], J[2][36];
             const double* Om = a.Om + 36 * (size_t)o;
             expmap_edge(a.Z[o], Om, X[a.odo_from[o]], X[a.odo_to[o]], e, J[0], J[1]);
-            double* out = a.olin + kOdoLin * (size_t)o;
-            for (int r = 0; r < 6; ++r) {
-                double acc = 0;
-                for (int c = 0; c < 6; ++c) acc += Om[r * 6 + c] * e[c];
-                Oe[r] = acc;
-            }
-            for (int s = 0; s < 2; ++s) {
-                double OJ[36];
-                for (int r = 0; r < 6; ++r)
-                    for (int c = 0; c < 6; ++c) {
-                        double acc = 0;
-                        for (int m = 0; m < 6; ++m) acc += Om[r * 6 + m] * J[s][m * 6 + c];
-                        OJ[r * 6 + c] = acc;
-                    }
-                for (int r = 0; r < 6; ++r) {
-                    for (int c = 0; c < 6; ++c) {
-                        double acc = 0;
-                        for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * OJ[m * 6 + c];
-                        out[36 * s + r * 6 + c] = acc;
-                        if (s == 1) {
-                            double ij = 0;
-                            for (int m = 0; m < 6; ++m) ij += J[0][m * 6 + r] * OJ[m * 6 + c];
-                            out[72 + r * 6 + c] = ij;
-                        }
-                    }
-                    double acc = 0;
-                    for (int m = 0; m < 6; ++m) acc += J[s][m * 6 + r] * Oe[m];
-                    out[108 + 6 * s + r] = -acc;
-                }
-            }
+            edge_record(Om, e, J, a.olin + kEdgeRec * (size_t)o);
         }
         for (int p = gt; p < a.nf; p += gs) {  // EdgeSE3ExpmapPrior, J = -I: H += Omega, b += Omega e
             const int v = a.vert[p];
@@ -266,30 +232,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_se3_ba(KArgs a) {
             for (int k = 0; k < 9; ++k) a.Hl[9 * (size_t)j + k] = h[k];
             m = fmax(m, fmax(fabs(h[0]), fmax(fabs(h[3]), fabs(h[5]))));
         }
-        for (int idx = gt; idx < a.nf * 42; idx += gs) {
-            const int p = idx / 42, rc = idx % 42;
-            const bool isb = rc >= 36;
-            double s = isb ? a.pb[6 * (size_t)p + rc - 36] : a.pH[36 * (size_t)p + rc];
-            for (int q = a.diag_ptr[p]; q < a.diag_ptr[p + 1]; ++q) {
-                const int code = a.diag_code[q], o = code >> 2, side = code & 3;
-                s += isb ? a.olin[kOdoLin * (size_t)o + 108 + 6 * side + rc - 36] : a.olin[kOdoLin * (size_t)o + 36 * side + rc];
-            }
+        const auto all = [](int) { return true; };
+        gather_diag(a, a.olin, a.bf, gt, gs, all, [&](int p, int rc, double s) {  // the projection edges after the odometry
             for (int q = a.kf_ptr[p]; q < a.kf_ptr[p + 1]; ++q) s += a.lin[kLin * (size_t)a.kf_edges[q] + rc];
-            if (isb) a.bf[6 * (size_t)p + rc - 36] = s;
-            else {
-                blk(a.Hs, a, p, p)[rc] = s;
-                if (rc % 7 == 0) m = fmax(m, fabs(s));
-            }
-        }
-        for (int idx = gt; idx < a.S * 36; idx += gs) {
-            const int sl = idx / 36, rc = idx % 36, tr = (rc % 6) * 6 + rc / 6;
-            double s = 0;
-            for (int q = a.off_ptr[sl]; q < a.off_ptr[sl + 1]; ++q) {
-                const int code = a.off_code[q], o = code >> 2;
-                s += a.olin[kOdoLin * (size_t)o + 72 + ((code & 3) == gba::kOffDiag ? rc : tr)];
-            }
-            a.Hs[36 * (size_t)a.off_blk[sl] + rc] = s;
-        }
+            if (rc < 36 && rc % 7 == 0) m = fmax(m, fabs(s));
+            return s;
+        });
+        gather_off(a, a.olin, gt, gs, all);
         if (it == 0) {
             m = cta_max(m, s_red);
             if (tid == 0) a.part_max[blockIdx.x] = m;
@@ -349,8 +298,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_se3_ba(KArgs a) {
                 a.b[idx] = s;
             }
             grid.sync();
-            for (int idx = gt; idx < a.nf * 6; idx += gs)  // damping of the pose blocks
-                a.L_[36 * (size_t)(a.rowoff[idx / 6] + (idx / 6 - a.first[idx / 6])) + (idx % 6) * 7] += lambda;
+            damp(a, a.L_, lambda, gt, gs);
             grid.sync();
             // the reduced solve on CTA 0
             if (blockIdx.x == 0) {
@@ -475,10 +423,7 @@ int check_topology(int N, const uint8_t* fixed, const uint8_t* prior, int O, con
                    const int* e_pt, const int* e_kf) {
     if (N <= 0 || O < 0 || L < 0 || E < 0) return fail(SE2GPU_ERR_INVALID, "N = %d, O = %d, L = %d, E = %d", N, O, L, E);
     if (!fixed || !prior || (O && (!from || !to)) || (E && (!e_pt || !e_kf))) return fail(SE2GPU_ERR_INVALID, "null topology arrays");
-    for (int o = 0; o < O; ++o) {
-        if (from[o] < 0 || from[o] >= N || to[o] < 0 || to[o] >= N) return fail(SE2GPU_ERR_INVALID, "odometry %d: keyframe out of range", o);
-        if (from[o] == to[o]) return fail(SE2GPU_ERR_INVALID, "odometry %d: from == to", o);
-    }
+    { const int rc = check_se3_links(N, O, from, to, nullptr, nullptr, "odometry", "keyframe"); if (rc) return rc; }
     std::vector<std::vector<int>> seen(L);
     for (int e = 0; e < E; ++e) {
         if (e_pt[e] < 0 || e_pt[e] >= L || e_kf[e] < 0 || e_kf[e] >= N) return fail(SE2GPU_ERR_INVALID, "edge %d: index out of range", e);
@@ -492,16 +437,11 @@ int check_topology(int N, const uint8_t* fixed, const uint8_t* prior, int O, con
     return SE2GPU_OK;
 }
 
-int check_values(int N, const float* Tcw, int O, const float* measure, const float* info, int L, const float* xyz, int E,
-                 const float* uv, const float* w) {
+int check_values(int N, const float* Tcw, int O, const int* from, const int* to, const float* measure, const float* info, int L,
+                 const float* xyz, int E, const float* uv, const float* w) {
     if (!Tcw || (O && (!measure || !info)) || (L && !xyz) || (E && (!uv || !w))) return fail(SE2GPU_ERR_INVALID, "null arrays");
     if (!finite_all(Tcw, 16 * (size_t)N)) return fail(SE2GPU_ERR_INVALID, "Tcw not finite");
-    if (!finite_all(measure, 16 * (size_t)O) || !finite_all(info, 36 * (size_t)O)) return fail(SE2GPU_ERR_INVALID, "odometry not finite");
-    for (int o = 0; o < O; ++o)
-        for (int r = 0; r < 6; ++r)
-            for (int c = 0; c < r; ++c)
-                if (info[36 * (size_t)o + r * 6 + c] != info[36 * (size_t)o + c * 6 + r])
-                    return fail(SE2GPU_ERR_INVALID, "odometry %d: information not symmetric", o);
+    { const int rc = check_se3_links(N, O, from, to, measure, info, "odometry", "keyframe"); if (rc) return rc; }
     if (!finite_all(xyz, 3 * (size_t)L) || !finite_all(uv, 2 * (size_t)E) || !finite_all(w, (size_t)E))
         return fail(SE2GPU_ERR_INVALID, "points or observations not finite");
     for (int e = 0; e < E; ++e)
@@ -509,142 +449,13 @@ int check_values(int N, const float* Tcw, int O, const float* measure, const flo
     return SE2GPU_OK;
 }
 
-// the host's half of initializeOptimization: which keyframes are free, the reduced system's order and envelope, and
-// every fixed-order gather list
-struct Plan {
-    std::vector<int> ints;
-    std::vector<long long> lls;
-    size_t o[22] = {0}, ol[4] = {0};
-    int nf = 0, S = 0;
-    long long env = 0;
-};
-
-Plan make_plan(int N, const uint8_t* fixed, const uint8_t* prior, int O, const int* from, const int* to, int L, int E,
-               const int* e_pt, const int* e_kf) {
-    // a keyframe no edge touches is not in the graph g2o optimises; a free one that is takes part in the reduced system
-    std::vector<uint8_t> active(N, 0), fx(N, 1);
-    for (int v = 0; v < N; ++v) active[v] = prior[v] ? 1 : 0;
-    for (int o = 0; o < O; ++o) active[from[o]] = active[to[o]] = 1;
-    for (int e = 0; e < E; ++e) active[e_kf[e]] = 1;
-    for (int v = 0; v < N; ++v) fx[v] = (fixed[v] || !active[v]) ? 1 : 0;
-    std::vector<int> pt_ptr(L + 1, 0), pt_edges(E);
-    for (int e = 0; e < E; ++e) ++pt_ptr[e_pt[e] + 1];
-    for (int j = 0; j < L; ++j) pt_ptr[j + 1] += pt_ptr[j];
-    {
-        std::vector<int> f(pt_ptr.begin(), pt_ptr.end() - 1);
-        for (int e = 0; e < E; ++e) pt_edges[f[e_pt[e]]++] = e;
-    }
-    // the block graph: odometry links, then every pair of free keyframes that observe a common point
-    std::vector<int> gf(from, from + O), gt(to, to + O);
-    {
-        std::vector<std::pair<int, int>> pr;
-        for (int j = 0; j < L; ++j)
-            for (int q = pt_ptr[j]; q < pt_ptr[j + 1]; ++q)
-                for (int r = q + 1; r < pt_ptr[j + 1]; ++r) {
-                    const int u = e_kf[pt_edges[q]], v = e_kf[pt_edges[r]];
-                    if (!fx[u] && !fx[v]) pr.push_back({std::min(u, v), std::max(u, v)});
-                }
-        std::sort(pr.begin(), pr.end());
-        pr.erase(std::unique(pr.begin(), pr.end()), pr.end());
-        for (const auto& x : pr) { gf.push_back(x.first); gt.push_back(x.second); }
-    }
-    const gba::Plan G = gba::make_plan(N, fx.data(), (int)gf.size(), gf.data(), gt.data());
-    const int nf = G.n_free;
-    // odometry contributions only (the co-observation links enter through the Schur complement)
-    std::vector<int> diag_ptr(nf + 1, 0), diag_code, off_ptr(1, 0), off_code;
-    std::vector<long long> off_blk;
-    for (int p = 0; p < nf; ++p) {
-        for (int q = G.diag_ptr[p]; q < G.diag_ptr[p + 1]; ++q)
-            if ((G.diag_code[q] >> 2) < O) diag_code.push_back(G.diag_code[q]);
-        diag_ptr[p + 1] = (int)diag_code.size();
-    }
-    for (size_t s = 0; s < G.off_blk.size(); ++s) {
-        const size_t before = off_code.size();
-        for (int q = G.off_ptr[s]; q < G.off_ptr[s + 1]; ++q)
-            if ((G.off_code[q] >> 2) < O) off_code.push_back(G.off_code[q]);
-        if (off_code.size() != before) { off_blk.push_back(G.off_blk[s]); off_ptr.push_back((int)off_code.size()); }
-    }
-    // projection edges per position, ascending
-    std::vector<int> kf_ptr(nf + 1, 0), kf_edges;
-    {
-        std::vector<std::vector<int>> by(nf);
-        for (int e = 0; e < E; ++e)
-            if (G.pos[e_kf[e]] >= 0) by[G.pos[e_kf[e]]].push_back(e);
-        for (int p = 0; p < nf; ++p) { kf_edges.insert(kf_edges.end(), by[p].begin(), by[p].end()); kf_ptr[p + 1] = (int)kf_edges.size(); }
-    }
-    // Schur pairs of every envelope block: the diagonal block of p lists (e, e) for p's edges in ascending edge order; block
-    // (p, q), p > q, lists (a, b) with a to p and b to q on one point, in ascending point order
-    const long long env = G.env_blocks();
-    std::vector<std::vector<std::pair<int, int>>> pb(env);
-    for (int p = 0; p < nf; ++p)
-        for (int q = kf_ptr[p]; q < kf_ptr[p + 1]; ++q) pb[G.blk(p, p)].push_back({kf_edges[q], kf_edges[q]});
-    for (int j = 0; j < L; ++j)
-        for (int q = pt_ptr[j]; q < pt_ptr[j + 1]; ++q)
-            for (int r = pt_ptr[j]; r < pt_ptr[j + 1]; ++r) {
-                const int ea = pt_edges[q], eb = pt_edges[r], pa = G.pos[e_kf[ea]], pq = G.pos[e_kf[eb]];
-                if (pa < 0 || pq < 0 || pa <= pq) continue;
-                pb[G.blk(pa, pq)].push_back({ea, eb});
-            }
-    std::vector<long long> pair_ptr(env + 1, 0);
-    std::vector<int> pair_a, pair_b;
-    for (long long k = 0; k < env; ++k) {
-        for (const auto& x : pb[k]) { pair_a.push_back(x.first); pair_b.push_back(x.second); }
-        pair_ptr[k + 1] = (long long)pair_a.size();
-    }
-    std::vector<int> flags(N), epos;
-    for (int v = 0; v < N; ++v) flags[v] = (fixed[v] ? 1 : 0) | (prior[v] ? 2 : 0);
-    Plan P;
-    P.nf = nf; P.S = (int)off_blk.size(); P.env = env;
-    const std::vector<int>* arrs[] = {&flags, &G.pos, &G.vert, &G.first, &G.col_ptr, &G.col_rows, &diag_ptr, &diag_code, &off_ptr,
-                                      &off_code, &kf_ptr, &kf_edges, &pt_ptr, &pt_edges, &pair_a, &pair_b};
-    const int n_arr = 16;
-    for (int i = 0; i < n_arr; ++i) {
-        P.o[i + 1] = P.o[i] + ((arrs[i]->size() + 31) & ~(size_t)31);
-    }
-    // e_pt, e_kf, odometry from / to follow
-    const size_t extra[4] = {(size_t)E, (size_t)E, (size_t)O, (size_t)O};
-    for (int i = 0; i < 4; ++i) P.o[n_arr + i + 1] = P.o[n_arr + i] + ((extra[i] + 31) & ~(size_t)31);
-    P.ints.assign(P.o[n_arr + 4], 0);
-    for (int i = 0; i < n_arr; ++i) std::copy(arrs[i]->begin(), arrs[i]->end(), P.ints.begin() + P.o[i]);
-    std::copy(e_pt, e_pt + E, P.ints.begin() + P.o[16]);
-    std::copy(e_kf, e_kf + E, P.ints.begin() + P.o[17]);
-    std::copy(from, from + O, P.ints.begin() + P.o[18]);
-    std::copy(to, to + O, P.ints.begin() + P.o[19]);
-    const std::vector<long long> rowoff(G.rowoff.begin(), G.rowoff.end());
-    const std::vector<long long>* larr[] = {&rowoff, &off_blk, &pair_ptr};
-    for (int i = 0; i < 3; ++i) P.ol[i + 1] = P.ol[i] + ((larr[i]->size() + 31) & ~(size_t)31);
-    P.lls.assign(P.ol[3], 0);
-    for (int i = 0; i < 3; ++i) std::copy(larr[i]->begin(), larr[i]->end(), P.lls.begin() + P.ol[i]);
-    return P;
-}
-
 }  // namespace
 
-struct se2gpu_se3_ba_ctx {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t uploaded = nullptr;  // the last plan upload out of the pinned arena has completed
-    cudaEvent_t done = nullptr;      // the last kernel, which reads the plan and work buffers, has completed
-    int grid_limit = 0;              // SE2GPU_SE3_BA_GRID: cap on the cooperative grid (several contexts on one GPU); 0 = none
-    DeviceBuffers bufs;
-    int* d_int = nullptr; size_t cap_int = 0;
-    long long* d_ll = nullptr; size_t cap_ll = 0;
-    double* d_dbl = nullptr; size_t cap_dbl = 0;
-    PinnedArena arena;
+struct se2gpu_se3_ba_ctx : se2gpu::PlanContext {
+    int grid_limit = 0;  // SE2GPU_SE3_BA_GRID: cap on the cooperative grid (several contexts on one GPU); 0 = none
 };
 
 namespace {
-
-template <class T>
-int grow(se2gpu_se3_ba_ctx* h, T** p, size_t* cap, size_t need) {
-    if (need <= *cap && *p) return SE2GPU_OK;
-    SE2_CUDA(cudaEventSynchronize(h->done));  // an earlier call, on any stream, may still read the buffer
-    SE2_CUDA(h->bufs.regrow(p, need ? need : 1));
-    *cap = need;
-    return SE2GPU_OK;
-}
-
-size_t al(size_t n) { return (n + 31) & ~(size_t)31; }
 
 struct Outs {
     float* Tcw; float* xyz; double* poses; double* points; double* chi2; uint8_t* outlier; int* status; int* iters;
@@ -655,9 +466,9 @@ int run(se2gpu_se3_ba_ctx* h, int N, const uint8_t* fixed, const uint8_t* prior,
         int E, const int* e_pt, const int* e_kf, const float* d_Tcw, const float* d_measure, const float* d_info,
         const float* d_xyz, const float* d_uv, const float* d_w, const se2gpu_se3_ba_params* prm, const Outs& out,
         cudaStream_t stream) {
-    const Plan P = make_plan(N, fixed, prior, O, from, to, L, E, e_pt, e_kf);
-    const int nf = P.nf;
-    const size_t env = (size_t)P.env;
+    const se3ba::Plan P = se3ba::make_plan(N, fixed, prior, O, from, to, L, E, e_pt, e_kf);
+    const int nf = P.G.n_free;
+    const size_t env = (size_t)P.G.env_blocks();
     const int n_items = std::max(E + N + O, nf + L);
     const int n_chunks = std::max(1, (n_items + kChunk - 1) / kChunk);
     int dev_sms = 0, per_sm = 0;
@@ -667,23 +478,31 @@ int run(se2gpu_se3_ba_ctx* h, int N, const uint8_t* fixed, const uint8_t* prior,
     const size_t work = std::max<size_t>({(size_t)E, (size_t)L * 3, env * 36, (size_t)N, (size_t)O});
     int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)dev_sms * per_sm, (work + kThreads - 1) / kThreads));
     if (h->grid_limit >= 1) grid = std::min(grid, h->grid_limit);
-    // doubles: X[2] (7 N each), P[2] (3 L each), pmeas (7 N), pinfo (36 N), Z (7 O), Om (36 O), olin (120 O), lin (72 E), Y (18 E),
-    // Hl (9 L), D (6 L), pH (36 nf), pb, bf, b, x (6 nf each), Hs, L (36 env), part (chunks), part_max (grid), ctl
-    const size_t n_dbl[23] = {7 * (size_t)N, 7 * (size_t)N, 3 * (size_t)L, 3 * (size_t)L, 7 * (size_t)N, 36 * (size_t)N,
-                              7 * (size_t)O, 36 * (size_t)O, kOdoLin * (size_t)O, kLin * (size_t)E, 18 * (size_t)E, 9 * (size_t)L,
-                              6 * (size_t)L, 36 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf, 6 * (size_t)nf,
-                              36 * env, 36 * env, (size_t)n_chunks, (size_t)grid, sizeof(Ctl) / 8 + 1};
-    size_t o_dbl[24] = {0};
-    for (int i = 0; i < 23; ++i) o_dbl[i + 1] = o_dbl[i] + al(n_dbl[i]);
-    { const int rc = grow(h, &h->d_int, &h->cap_int, P.ints.size()); if (rc) return rc; }
-    { const int rc = grow(h, &h->d_ll, &h->cap_ll, P.lls.size()); if (rc) return rc; }
-    { const int rc = grow(h, &h->d_dbl, &h->cap_dbl, o_dbl[23]); if (rc) return rc; }
-    SE2_CUDA(cudaEventSynchronize(h->uploaded));
-    SE2_CUDA(cudaStreamWaitEvent(stream, h->done, 0));
-    h->arena.reserve(4 * P.ints.size() + 8 * P.lls.size() + 256);
-    { const int rc = h->arena.up(h->d_int, P.ints.data(), P.ints.size(), stream); if (rc) return rc; }
-    { const int rc = h->arena.up(h->d_ll, P.lls.data(), P.lls.size(), stream); if (rc) return rc; }
-    SE2_CUDA(cudaEventRecord(h->uploaded, stream));
+    // the plan, the window's topology, then the work
+    Packed<int> ints;
+    Packed<long long> lls;
+    Layout dbl;
+    struct {
+        size_t flags, pos, vert, first, col_ptr, col_rows, diag_ptr, diag_code, off_ptr, off_code, kf_ptr, kf_edges, pt_ptr,
+            pt_edges, pair_a, pair_b, e_pt, e_kf, odo_from, odo_to;                                               // ints
+        size_t rowoff, off_blk, pair_ptr;                                                                       // long longs
+        size_t X[2], P[2], pmeas, pinfo, Z, Om, olin, lin, Y, Hl, D, pH, pb, bf, b, x, Hs, L, part, part_max, ctl;  // doubles
+    } o;
+    o.flags = ints.put(P.flags); o.pos = ints.put(P.G.pos); o.vert = ints.put(P.G.vert); o.first = ints.put(P.G.first);
+    o.col_ptr = ints.put(P.G.col_ptr); o.col_rows = ints.put(P.G.col_rows); o.diag_ptr = ints.put(P.diag_ptr);
+    o.diag_code = ints.put(P.diag_code); o.off_ptr = ints.put(P.off_ptr); o.off_code = ints.put(P.off_code);
+    o.kf_ptr = ints.put(P.kf_ptr); o.kf_edges = ints.put(P.kf_edges); o.pt_ptr = ints.put(P.pt_ptr); o.pt_edges = ints.put(P.pt_edges);
+    o.pair_a = ints.put(P.pair_a); o.pair_b = ints.put(P.pair_b); o.e_pt = ints.put(e_pt, (size_t)E); o.e_kf = ints.put(e_kf, (size_t)E);
+    o.odo_from = ints.put(from, (size_t)O); o.odo_to = ints.put(to, (size_t)O);
+    o.rowoff = lls.put(P.G.rowoff); o.off_blk = lls.put(P.off_blk); o.pair_ptr = lls.put(P.pair_ptr);
+    o.X[0] = dbl.take(7 * (size_t)N); o.X[1] = dbl.take(7 * (size_t)N); o.P[0] = dbl.take(3 * (size_t)L); o.P[1] = dbl.take(3 * (size_t)L);
+    o.pmeas = dbl.take(7 * (size_t)N); o.pinfo = dbl.take(36 * (size_t)N); o.Z = dbl.take(7 * (size_t)O); o.Om = dbl.take(36 * (size_t)O);
+    o.olin = dbl.take(kEdgeRec * (size_t)O); o.lin = dbl.take(kLin * (size_t)E); o.Y = dbl.take(18 * (size_t)E);
+    o.Hl = dbl.take(9 * (size_t)L); o.D = dbl.take(6 * (size_t)L); o.pH = dbl.take(36 * (size_t)nf); o.pb = dbl.take(6 * (size_t)nf);
+    o.bf = dbl.take(6 * (size_t)nf); o.b = dbl.take(6 * (size_t)nf); o.x = dbl.take(6 * (size_t)nf); o.Hs = dbl.take(36 * env);
+    o.L = dbl.take(36 * env); o.part = dbl.take((size_t)n_chunks); o.part_max = dbl.take((size_t)grid); o.ctl = dbl.take(sizeof(Ctl) / 8 + 1);
+    { const int rc = h->grow(&h->d_dbl, &h->cap_dbl, dbl.size); if (rc) return rc; }
+    { const int rc = h->upload_plan(ints.data, lls.data, stream); if (rc) return rc; }
 
     KArgs a{};
     a.N = N; a.O = O; a.L = L; a.E = E; a.nf = nf; a.iterations = prm->iterations; a.n_chunks = n_chunks;
@@ -692,17 +511,18 @@ int run(se2gpu_se3_ba_ctx* h, int N, const uint8_t* fixed, const uint8_t* prior,
     a.xrot = prm->xrot_info; a.yrot = prm->yrot_info; a.zinfo = prm->z_info;
     a.Tcw = d_Tcw; a.measure = d_measure; a.info = d_info; a.xyz = d_xyz; a.uv = d_uv; a.w = d_w;
     const int* I = h->d_int;
-    a.kf_flags = I + P.o[0]; a.pos = I + P.o[1]; a.vert = I + P.o[2]; a.first = I + P.o[3]; a.col_ptr = I + P.o[4];
-    a.col_rows = I + P.o[5]; a.diag_ptr = I + P.o[6]; a.diag_code = I + P.o[7]; a.off_ptr = I + P.o[8]; a.off_code = I + P.o[9];
-    a.kf_ptr = I + P.o[10]; a.kf_edges = I + P.o[11]; a.pt_ptr = I + P.o[12]; a.pt_edges = I + P.o[13]; a.pair_a = I + P.o[14];
-    a.pair_b = I + P.o[15]; a.e_pt = I + P.o[16]; a.e_kf = I + P.o[17]; a.odo_from = I + P.o[18]; a.odo_to = I + P.o[19];
-    a.rowoff = h->d_ll + P.ol[0]; a.off_blk = h->d_ll + P.ol[1]; a.pair_ptr = h->d_ll + P.ol[2]; a.S = P.S;
-    double* Dd = h->d_dbl;
-    a.X[0] = (SE3*)(Dd + o_dbl[0]); a.X[1] = (SE3*)(Dd + o_dbl[1]); a.P[0] = Dd + o_dbl[2]; a.P[1] = Dd + o_dbl[3];
-    a.pmeas = (SE3*)(Dd + o_dbl[4]); a.pinfo = Dd + o_dbl[5]; a.Z = (SE3*)(Dd + o_dbl[6]); a.Om = Dd + o_dbl[7];
-    a.olin = Dd + o_dbl[8]; a.lin = Dd + o_dbl[9]; a.Y = Dd + o_dbl[10]; a.Hl = Dd + o_dbl[11]; a.D = Dd + o_dbl[12];
-    a.pH = Dd + o_dbl[13]; a.pb = Dd + o_dbl[14]; a.bf = Dd + o_dbl[15]; a.b = Dd + o_dbl[16]; a.x = Dd + o_dbl[17];
-    a.Hs = Dd + o_dbl[18]; a.L_ = Dd + o_dbl[19]; a.part = Dd + o_dbl[20]; a.part_max = Dd + o_dbl[21]; a.ctl = (Ctl*)(Dd + o_dbl[22]);
+    a.kf_flags = I + o.flags; a.pos = I + o.pos; a.vert = I + o.vert; a.first = I + o.first; a.col_ptr = I + o.col_ptr;
+    a.col_rows = I + o.col_rows; a.diag_ptr = I + o.diag_ptr; a.diag_code = I + o.diag_code; a.off_ptr = I + o.off_ptr;
+    a.off_code = I + o.off_code; a.kf_ptr = I + o.kf_ptr; a.kf_edges = I + o.kf_edges; a.pt_ptr = I + o.pt_ptr;
+    a.pt_edges = I + o.pt_edges; a.pair_a = I + o.pair_a; a.pair_b = I + o.pair_b; a.e_pt = I + o.e_pt; a.e_kf = I + o.e_kf;
+    a.odo_from = I + o.odo_from; a.odo_to = I + o.odo_to;
+    a.rowoff = h->d_ll + o.rowoff; a.off_blk = h->d_ll + o.off_blk; a.pair_ptr = h->d_ll + o.pair_ptr; a.S = (int)P.off_blk.size();
+    double* D = h->d_dbl;
+    a.X[0] = (SE3*)(D + o.X[0]); a.X[1] = (SE3*)(D + o.X[1]); a.P[0] = D + o.P[0]; a.P[1] = D + o.P[1];
+    a.pmeas = (SE3*)(D + o.pmeas); a.pinfo = D + o.pinfo; a.Z = (SE3*)(D + o.Z); a.Om = D + o.Om; a.olin = D + o.olin;
+    a.lin = D + o.lin; a.Y = D + o.Y; a.Hl = D + o.Hl; a.D = D + o.D; a.pH = D + o.pH; a.pb = D + o.pb; a.bf = D + o.bf;
+    a.b = D + o.b; a.x = D + o.x; a.Hs = D + o.Hs; a.L_ = D + o.L; a.part = D + o.part; a.part_max = D + o.part_max;
+    a.ctl = (Ctl*)(D + o.ctl);
     a.Tcw_out = out.Tcw; a.xyz_out = out.xyz; a.poses = out.poses; a.points = out.points; a.chi2 = out.chi2; a.outlier = out.outlier;
     a.status = out.status; a.iters = out.iters; a.stats = out.stats; a.trace = out.trace;
     const size_t it = (size_t)prm->iterations;
@@ -725,7 +545,7 @@ int host_run(se2gpu_se3_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed
     if (!h) return fail(SE2GPU_ERR_INVALID, "null context");
     { const int rc = check_params(params); if (rc) return rc; }
     { const int rc = check_topology(N, fixed, prior, O, odo_from, odo_to, L, E, edge_point, edge_kf); if (rc) return rc; }
-    { const int rc = check_values(N, Tcw, O, odo_measure, odo_info, L, xyz, E, uv, inv_sigma2); if (rc) return rc; }
+    { const int rc = check_values(N, Tcw, O, odo_from, odo_to, odo_measure, odo_info, L, xyz, E, uv, inv_sigma2); if (rc) return rc; }
     if (E && (!chi2 || !outlier)) return fail(SE2GPU_ERR_INVALID, "null chi2 / outlier outputs");
     HostStage st(h->device);
     if (const int rc = st.status()) return rc;
@@ -756,29 +576,13 @@ int host_run(se2gpu_se3_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed
 }  // namespace
 
 se2gpu_se3_ba_ctx* se2gpu_se3_ba_create(int device) {
-    if (select_device(device)) return nullptr;
-    se2gpu_se3_ba_ctx* h = new se2gpu_se3_ba_ctx;
-    h->device = device;
-    if (const char* g = getenv("SE2GPU_SE3_BA_GRID")) h->grid_limit = atoi(g);  // the only place this BA reads the environment
-    if (cudaStreamCreate(&h->stream) != cudaSuccess || cudaEventCreateWithFlags(&h->uploaded, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
-        fail(SE2GPU_ERR_CUDA, "cudaStreamCreate / cudaEventCreate failed");
-        se2gpu_se3_ba_destroy(h);
-        return nullptr;
-    }
+    se2gpu_se3_ba_ctx* h = create_plan_context<se2gpu_se3_ba_ctx>(device);
+    if (h)
+        if (const char* g = getenv("SE2GPU_SE3_BA_GRID")) h->grid_limit = atoi(g);  // the only place this BA reads the environment
     return h;
 }
 
-void se2gpu_se3_ba_destroy(se2gpu_se3_ba_ctx* h) {
-    if (!h) return;
-    cudaSetDevice(h->device);
-    if (h->done) cudaEventSynchronize(h->done);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    if (h->uploaded) cudaEventDestroy(h->uploaded);
-    if (h->done) cudaEventDestroy(h->done);
-    if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-}
+void se2gpu_se3_ba_destroy(se2gpu_se3_ba_ctx* h) { delete h; }
 
 int se2gpu_se3_ba(se2gpu_se3_ba_ctx* h, int N, const float* Tcw, const uint8_t* fixed, const uint8_t* prior, int O, const int* odo_from,
                   const int* odo_to, const float* odo_measure, const float* odo_info, int L, const float* xyz, int E,

@@ -1,8 +1,8 @@
 """CPU checks of the directly built SE(3) windows (tools/se3_window_synth.DIRECT_SCENES): the C++ oracle agrees with the numpy
 restatement on a small version of each, the oracle's own spread on each is at least 10x below the GPU bounds, and the
 scenes keep the shapes they exist for — the reduced system's widest envelope column, both off-diagonal odometry codes,
-several RCM components (from global_ba_plan.h itself, tests/native/se3_plan_profile.cpp), every branch of Eigen's
-Quaterniond(Matrix3d) over the input rotations, the chunk boundaries and a window larger than the H100's 132 SMs x 256."""
+several RCM components (from the kernel's own plan, se3_ba_plan.h, through tests/native/se3_plan_profile.cpp), every
+branch of Eigen's Quaterniond(Matrix3d) over the input rotations, the chunk boundaries and a window larger than the H100's 132 SMs x 256."""
 from __future__ import annotations
 
 import os
@@ -58,25 +58,6 @@ def test_oracle_spread_is_far_below_the_gpu_bounds():
     assert worst[0] * 10 <= GPU_CHI2 and worst[1] * 10 <= GPU_EST and worst[2] * 10 <= GPU_EDGE, worst
 
 
-def block_graph(w):
-    """se3_ba.cu's make_plan: keyframes outside the graph count as fixed; the links are the odometry, then the sorted,
-    de-duplicated pairs of free keyframes that observe one point"""
-    N, O, L, E = w.sizes
-    active = w.prior.astype(bool).copy()
-    active[w.odo_from] = True; active[w.odo_to] = True; active[w.edge_kf] = True
-    fx = (w.fixed != 0) | ~active
-    pairs = set()
-    order = np.argsort(w.edge_point, kind="stable")
-    bounds = np.searchsorted(w.edge_point[order], np.arange(L + 1))
-    for j in range(L):
-        k = w.edge_kf[order[bounds[j]:bounds[j + 1]]]
-        k = k[~fx[k]]
-        a, b = np.triu_indices(len(k), 1)
-        pairs.update(zip(np.minimum(k[a], k[b]).tolist(), np.maximum(k[a], k[b]).tolist()))
-    links = list(zip(w.odo_from.tolist(), w.odo_to.tolist())) + sorted(pairs)
-    return fx, O, links
-
-
 @pytest.fixture(scope="module")
 def profile(tmp_path_factory):
     exe = str(tmp_path_factory.mktemp("native") / "se3_plan_profile")
@@ -85,8 +66,8 @@ def profile(tmp_path_factory):
     assert res.returncode == 0, res.stderr
 
     def run(w):
-        fx, O, links = block_graph(w)
-        text = f"{len(fx)} {O} {len(links)}\n" + " ".join(str(int(f)) for f in fx) + "\n" + "\n".join(f"{a} {b}" for a, b in links)
+        topo = [w.sizes, w.fixed, w.prior, np.stack([w.odo_from, w.odo_to], 1).ravel(), np.stack([w.edge_point, w.edge_kf], 1).ravel()]
+        text = "\n".join(" ".join(str(int(v)) for v in t) for t in topo) + "\n"
         res = subprocess.run([exe], input=text, capture_output=True, text=True)
         assert res.returncode == 0, res.stderr
         nf, rows, off, off_t, comps = (int(v) for v in res.stdout.split())
