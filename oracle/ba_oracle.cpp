@@ -9,7 +9,7 @@
 //
 // g2o (tag 20160424_git, README.MD:29) is an un-vendored dependency that is absent from
 // /root/reference and from this container: its published algorithm is restated here
-// (OptimizationAlgorithmLevenberg::solve, BlockSolver::buildSystem/solve with Schur complement,
+// (OptimizationAlgorithmLevenberg::solve in oracle/g2o_lm_oracle.h, BlockSolver::buildSystem/solve with Schur complement,
 // BaseBinaryEdge::constructQuadraticForm, RobustKernelHuber, VertexSE2/VertexSBAPointXYZ oplus).
 // PARITY UNPINNED against real g2o: no g2o build or golden vector exists (SURVEY.md section 8c).  The oracle
 // is instead pinned by self-consistency (tests/test_ba_oracle.py): analytic vs numeric Jacobians,
@@ -22,15 +22,11 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
-#include <limits>
 #include <vector>
 
-namespace {
+#include "g2o_lm_oracle.h"
 
-struct IterStats {  // must match se2gpu_ba_iter_stats (include/se2gpu.h)
-    double chi2_before, chi2_after, lambda, rho;
-    int trials, accepted, terminate, pad;
-};
+namespace {
 
 inline double normalize_theta(double theta) {  // g2o/stuff/misc.h
     if (theta >= -M_PI && theta < M_PI) return theta;
@@ -62,53 +58,6 @@ bool inv3(const double* A, double* R) {
     return true;
 }
 
-// Symmetric positive-definite matrix in lower skyline (profile) storage; Cholesky stays in profile.
-struct Skyline {
-    int n = 0;
-    std::vector<int> first;       // first stored column of row r
-    std::vector<size_t> off;      // offset of row r's first stored entry
-    std::vector<double> v;
-    void build(int n_, const std::vector<int>& first_) {
-        n = n_; first = first_; off.assign(n + 1, 0);
-        for (int r = 0; r < n; ++r) off[r + 1] = off[r] + (size_t)(r - first[r] + 1);
-        v.assign(off[n], 0.0);
-    }
-    inline double& at(int r, int c) { return v[off[r] + (c - first[r])]; }  // requires first[r] <= c <= r
-    inline double get(int r, int c) const { if (c > r) std::swap(r, c); return c < first[r] ? 0.0 : v[off[r] + (c - first[r])]; }
-    // in-place LL^T; false if not positive definite (CHOLMOD "minor != n")
-    bool cholesky() {
-        for (int r = 0; r < n; ++r) {
-            double* Lr = &v[off[r]];
-            for (int c = first[r]; c <= r; ++c) {
-                const double* Lc = &v[off[c]];
-                int k0 = std::max(first[r], first[c]);
-                double s = Lr[c - first[r]];
-                for (int k = k0; k < c; ++k) s -= Lr[k - first[r]] * Lc[k - first[c]];
-                if (c == r) {
-                    if (!(s > 0.0) || !std::isfinite(s)) return false;
-                    Lr[c - first[r]] = std::sqrt(s);
-                } else {
-                    Lr[c - first[r]] = s / Lc[c - first[c]];
-                }
-            }
-        }
-        return true;
-    }
-    void solve(double* x) const {  // x := (L L^T)^-1 x
-        for (int r = 0; r < n; ++r) {
-            const double* Lr = &v[off[r]];
-            double s = x[r];
-            for (int k = first[r]; k < r; ++k) s -= Lr[k - first[r]] * x[k];
-            x[r] = s / Lr[r - first[r]];
-        }
-        for (int r = n - 1; r >= 0; --r) {
-            const double* Lr = &v[off[r]];
-            x[r] /= Lr[r - first[r]];
-            for (int k = first[r]; k < r; ++k) x[k] -= Lr[k - first[r]] * x[r];
-        }
-    }
-};
-
 struct BA {
     int P, L, E, O;
     std::vector<double> pose, point, uv, info, odo_meas, odo_info;
@@ -126,7 +75,9 @@ struct BA {
     std::vector<int> first;
     std::vector<double> bp, Hll, bl, Hpl, bs, dx_p, dx_l, HllInv;
     std::vector<double> e_xyz, e_odo;
-    double lambda = 0, ni = 2;
+    std::vector<double> pose_bak, point_bak;
+    double* trace_poses = nullptr;
+    double* trace_points = nullptr;
 
     void indexing() {
         hidx.assign(P, -1); nf = 0;
@@ -208,7 +159,7 @@ struct BA {
     }
 
     // SparseOptimizer::computeActiveErrors + activeRobustChi2
-    double computeErrors() {
+    double chi2() {
         double chi = 0;
         for (int o = 0; o < O; ++o) {
             double* e = &e_odo[3 * o];
@@ -242,7 +193,7 @@ struct BA {
     }
 
     // BlockSolver::buildSystem: linearizeOplus + constructQuadraticForm over all active edges
-    void buildSystem() {
+    void build() {
         std::fill(Hpp.v.begin(), Hpp.v.end(), 0.0);
         std::fill(bp.begin(), bp.end(), 0.0);
         std::fill(Hll.begin(), Hll.end(), 0.0);
@@ -308,7 +259,7 @@ struct BA {
         }
     }
 
-    double maxDiag() const {  // OptimizationAlgorithmLevenberg::computeLambdaInit
+    double max_diag() const {  // OptimizationAlgorithmLevenberg::computeLambdaInit
         double m = 0;
         for (int r = 0; r < 3 * nf; ++r) m = std::max(m, std::fabs(Hpp.get(r, r)));
         for (int j = 0; j < L; ++j) if (lm_active[j]) for (int r = 0; r < 3; ++r) m = std::max(m, std::fabs(Hll[9 * (size_t)j + 4 * r]));
@@ -383,53 +334,21 @@ struct BA {
         return s;
     }
 
-    // SparseOptimizer::optimize(iterations) with OptimizationAlgorithmLevenberg::solve per iteration
-    int optimize(int iterations, IterStats* stats, double* trace_poses, double* trace_points, const volatile uint8_t* stop) {
-        int done = 0;
-        bool ok = true;
-        for (int it = 0; it < iterations && !(stop && *stop) && ok; ++it) {
-            IterStats st{};
-            double currentChi = computeErrors();
-            double tempChi = currentChi;
-            st.chi2_before = currentChi;
-            buildSystem();
-            if (it == 0) { lambda = 1e-5 * maxDiag(); ni = 2; }
-            double rho = 0;
-            int qmax = 0;
-            do {
-                std::vector<double> pose_bak = pose, point_bak = point;  // push()
-                bool ok2 = solve(lambda);
-                if (ok2) applyUpdate();
-                tempChi = computeErrors();
-                if (!ok2) tempChi = std::numeric_limits<double>::max();
-                rho = currentChi - tempChi;
-                double scale = ok2 ? computeScale(lambda) : 0.0;
-                scale += 1e-3;
-                rho /= scale;
-                if (rho > 0 && std::isfinite(tempChi)) {
-                    double alpha = 1. - std::pow((2 * rho - 1), 3);
-                    alpha = std::min(alpha, 2. / 3.);
-                    double scaleFactor = std::max(1. / 3., alpha);
-                    lambda *= scaleFactor;
-                    ni = 2;
-                    currentChi = tempChi;
-                    st.accepted = 1;
-                } else {
-                    lambda *= ni;
-                    ni *= 2;
-                    pose = pose_bak; point = point_bak;  // pop()
-                }
-                qmax++;
-            } while (rho < 0 && qmax < 10 && !(stop && *stop));
-            st.chi2_after = currentChi; st.lambda = lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            ok = !st.terminate;
-            if (stats) stats[it] = st;
-            if (trace_poses) memcpy(trace_poses + (size_t)it * 3 * P, pose.data(), sizeof(double) * 3 * P);
-            if (trace_points) memcpy(trace_points + (size_t)it * 3 * L, point.data(), sizeof(double) * 3 * L);
-            ++done;
-        }
-        return done;
+    // the other LM hooks of lm_optimize (build and max_diag are above); chi2 is evaluated at every iteration's start
+    double start_chi2(int, double) { return chi2(); }
+    bool trial(double lam, double* tempChi, double* scale) {
+        pose_bak = pose; point_bak = point;  // push()
+        const bool ok = solve(lam);
+        if (ok) applyUpdate();
+        *tempChi = chi2();
+        if (ok) *scale = computeScale(lam);
+        return ok;
+    }
+    void accept() {}
+    void reject() { pose = pose_bak; point = point_bak; }  // pop()
+    void record(int it) {
+        if (trace_poses) memcpy(trace_poses + (size_t)it * 3 * P, pose.data(), sizeof(double) * 3 * P);
+        if (trace_points) memcpy(trace_points + (size_t)it * 3 * L, point.data(), sizeof(double) * 3 * L);
     }
 };
 
@@ -456,8 +375,12 @@ void* ba_oracle_create(int P, int L, int E, int O, const double* poses, const ui
     return b;
 }
 void ba_oracle_destroy(void* h) { delete (BA*)h; }
+// SparseOptimizer::optimize(iters); stop (may be NULL) is polled like g2o's force-stop flag. The NOT_PD status is not reported.
 int ba_oracle_optimize(void* h, int iters, void* stats, double* trace_poses, double* trace_points, const volatile uint8_t* stop) {
-    return ((BA*)h)->optimize(iters, (IterStats*)stats, trace_poses, trace_points, stop);
+    BA* b = (BA*)h;
+    b->trace_poses = trace_poses; b->trace_points = trace_points;
+    bool not_pd = false;
+    return lm_optimize(*b, iters, (IterStats*)stats, &not_pd, stop);
 }
 void ba_oracle_get(void* h, double* poses, double* points) {
     BA* b = (BA*)h;
@@ -470,13 +393,13 @@ void ba_oracle_set(void* h, const double* poses, const double* points) {
     memcpy(b->point.data(), points, sizeof(double) * 3 * b->L);
 }
 int ba_oracle_num_free(void* h) { return ((BA*)h)->nf; }
-double ba_oracle_chi2(void* h) { return ((BA*)h)->computeErrors(); }
+double ba_oracle_chi2(void* h) { return ((BA*)h)->chi2(); }
 // introspection for kernel-level parity: errors + linear system at the current estimate.
 // Hpp_dense/S_dense are [3nf x 3nf] row-major full symmetric; Hll [L*9]; Hpl [E*9] (rows: pose, cols: point).
 double ba_oracle_linearize(void* h, double* Hpp_dense, double* bp, double* Hll, double* bl, double* Hpl) {
     BA* b = (BA*)h;
-    double chi = b->computeErrors();
-    b->buildSystem();
+    double chi = b->chi2();
+    b->build();
     int n = 3 * b->nf;
     if (Hpp_dense) for (int r = 0; r < n; ++r) for (int c = 0; c < n; ++c) Hpp_dense[(size_t)r * n + c] = b->Hpp.get(r, c);
     if (bp) memcpy(bp, b->bp.data(), sizeof(double) * n);

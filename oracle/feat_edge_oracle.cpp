@@ -6,11 +6,11 @@
 //   addEdgeSE3XYZ (:531-545), Sparsifier::JacobianSE3XYZ / HessianSE3XYZ / DoMarginalizeSE3XYZ / JacobianSE3 / InfoSE3
 //   (src/sparsifier.cpp:59-274).
 // g2o (tag 20160424) and Eigen are not vendored; their published definitions are restated: VertexSE3 (Isometry3D estimate,
-// oplus = estimate * fromVectorMQT), VertexPointXYZ, EdgeSE3PointXYZ and EdgeSE3Prior with an identity ParameterSE3Offset,
-// toVectorMQT / toCompactQuaternion, SE3Quat (operator*, inverse, map, toMinimalVector, fromMinimalVector),
+// oplus = estimate * fromVectorMQT) and EdgeSE3Prior with an identity ParameterSE3Offset (oracle/se3_oracle.h),
+// VertexPointXYZ, EdgeSE3PointXYZ, toVectorMQT / toCompactQuaternion, SE3Quat (map, toMinimalVector, fromMinimalVector),
 // RobustKernelHuber, BaseBinaryEdge / BaseUnaryEdge::constructQuadraticForm (rho' * Omega, no second-order term),
 // BlockSolver's Schur complement with lambda on the pose and the point diagonals, and
-// OptimizationAlgorithmLevenberg::solve as oracle/ba_oracle.cpp and oracle/pose_ba_oracle.cpp have it.
+// OptimizationAlgorithmLevenberg::solve (oracle/g2o_lm_oracle.h).
 //
 // What is decided here and not copied from anywhere:
 //  * The two edge Jacobians are the analytic first derivatives of the errors through the MQT oplus; they are unique, and
@@ -32,15 +32,12 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
-#include <limits>
 #include <vector>
 
-namespace {
+#include "g2o_lm_oracle.h"
+#include "se3_oracle.h"
 
-struct IterStats {  // must match se2gpu_ba_iter_stats (include/se2gpu.h)
-    double chi2_before, chi2_after, lambda, rho;
-    int trials, accepted, terminate, pad;
-};
+namespace {
 
 struct Params {  // must match se2gpu_feat_edge_params (include/se2gpu.h)
     float Tbc[16];
@@ -50,114 +47,6 @@ struct Params {  // must match se2gpu_feat_edge_params (include/se2gpu.h)
     float chi2_cut;
     int min_points[2];
 };
-
-struct Quat { double x, y, z, w; };
-struct SE3 { Quat q; double t[3]; };   // g2o::SE3Quat
-struct Iso { double R[9], t[3]; };     // Eigen::Isometry3d: rotation row-major, translation
-
-void cross(const double* a, const double* b, double* c) {
-    c[0] = a[1] * b[2] - a[2] * b[1];
-    c[1] = a[2] * b[0] - a[0] * b[2];
-    c[2] = a[0] * b[1] - a[1] * b[0];
-}
-
-// Eigen: Quaternion<double>(const Matrix3d&)
-Quat quat_from_R(const double* m) {
-    Quat q;
-    double t = m[0] + m[4] + m[8];
-    if (t > 0) {
-        t = std::sqrt(t + 1.0);
-        q.w = 0.5 * t;
-        t = 0.5 / t;
-        q.x = (m[7] - m[5]) * t;
-        q.y = (m[2] - m[6]) * t;
-        q.z = (m[3] - m[1]) * t;
-    } else {
-        int i = 0;
-        if (m[4] > m[0]) i = 1;
-        if (m[8] > m[i * 4]) i = 2;
-        int j = (i + 1) % 3, k = (j + 1) % 3;
-        double c[3];
-        t = std::sqrt(m[i * 4] - m[j * 4] - m[k * 4] + 1.0);
-        c[i] = 0.5 * t;
-        t = 0.5 / t;
-        q.w = (m[k * 3 + j] - m[j * 3 + k]) * t;
-        c[j] = (m[j * 3 + i] + m[i * 3 + j]) * t;
-        c[k] = (m[k * 3 + i] + m[i * 3 + k]) * t;
-        q.x = c[0]; q.y = c[1]; q.z = c[2];
-    }
-    return q;
-}
-
-// Eigen: QuaternionBase::toRotationMatrix
-void quat_to_R(const Quat& q, double* R) {
-    const double tx = 2 * q.x, ty = 2 * q.y, tz = 2 * q.z;
-    const double twx = tx * q.w, twy = ty * q.w, twz = tz * q.w;
-    const double txx = tx * q.x, txy = ty * q.x, txz = tz * q.x;
-    const double tyy = ty * q.y, tyz = tz * q.y, tzz = tz * q.z;
-    R[0] = 1 - (tyy + tzz); R[1] = txy - twz;       R[2] = txz + twy;
-    R[3] = txy + twz;       R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
-    R[6] = txz - twy;       R[7] = tyz + twx;       R[8] = 1 - (txx + tyy);
-}
-
-Quat qmul(const Quat& a, const Quat& b) {
-    return {a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-            a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z,
-            a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x,
-            a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z};
-}
-
-// Eigen: q * v
-void qrot(const Quat& q, const double* v, double* out) {
-    const double qv[3] = {q.x, q.y, q.z};
-    double uv[3], c[3];
-    cross(qv, v, uv);
-    uv[0] += uv[0]; uv[1] += uv[1]; uv[2] += uv[2];
-    cross(qv, uv, c);
-    for (int i = 0; i < 3; ++i) out[i] = v[i] + q.w * uv[i] + c[i];
-}
-
-// g2o SE3Quat::normalizeRotation
-void normalize_rotation(Quat& q) {
-    if (q.w < 0) { q.x = -q.x; q.y = -q.y; q.z = -q.z; q.w = -q.w; }
-    const double n2 = q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w;
-    if (n2 > 0) {
-        const double n = std::sqrt(n2);
-        q.x /= n; q.y /= n; q.z /= n; q.w /= n;
-    }
-}
-
-SE3 se3_from_Rt(const double* R, const double* t) {
-    SE3 T;
-    T.q = quat_from_R(R);
-    for (int i = 0; i < 3; ++i) T.t[i] = t[i];
-    normalize_rotation(T.q);
-    return T;
-}
-
-SE3 se3_from_f32(const float* T) {
-    const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
-    const double t[3] = {T[3], T[7], T[11]};
-    return se3_from_Rt(R, t);
-}
-
-SE3 se3_mul(const SE3& a, const SE3& b) {
-    SE3 r = a;
-    double rt[3];
-    qrot(a.q, b.t, rt);
-    for (int i = 0; i < 3; ++i) r.t[i] += rt[i];
-    r.q = qmul(a.q, b.q);
-    normalize_rotation(r.q);
-    return r;
-}
-
-SE3 se3_inv(const SE3& a) {
-    SE3 r;
-    r.q = {-a.q.x, -a.q.y, -a.q.z, a.q.w};
-    const double mt[3] = {a.t[0] * -1., a.t[1] * -1., a.t[2] * -1.};
-    qrot(r.q, mt, r.t);
-    return r;
-}
 
 // SE3Quat::map / operator*(Vector3D)
 void se3_map(const SE3& T, const double* p, double* out) {
@@ -181,73 +70,6 @@ SE3 se3_from_min(const double* v) {
     return T;
 }
 
-void mul3(const double* A, const double* B, double* C) {
-    for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) C[r * 3 + c] = A[r * 3] * B[c] + A[r * 3 + 1] * B[3 + c] + A[r * 3 + 2] * B[6 + c];
-}
-void mulv3(const double* A, const double* v, double* o) {
-    for (int r = 0; r < 3; ++r) o[r] = A[r * 3] * v[0] + A[r * 3 + 1] * v[1] + A[r * 3 + 2] * v[2];
-}
-
-Iso iso_mul(const Iso& a, const Iso& b) {
-    Iso r;
-    mul3(a.R, b.R, r.R);
-    mulv3(a.R, b.t, r.t);
-    for (int i = 0; i < 3; ++i) r.t[i] += a.t[i];
-    return r;
-}
-
-// Eigen Transform::inverse(Isometry): R^T, -R^T t
-Iso iso_inv(const Iso& a) {
-    Iso r;
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) r.R[i * 3 + j] = a.R[j * 3 + i];
-    double v[3];
-    mulv3(r.R, a.t, v);
-    for (int i = 0; i < 3; ++i) r.t[i] = -v[i];
-    return r;
-}
-
-// converter.cpp toIsometry3D(getPose().inv()): the rotation goes through an un-normalised Quaterniond
-Iso iso_from_Tcw(const float* T) {
-    Iso cw;
-    const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
-    std::memcpy(cw.R, R, sizeof R);
-    cw.t[0] = T[3]; cw.t[1] = T[7]; cw.t[2] = T[11];
-    Iso wc = iso_inv(cw);
-    quat_to_R(quat_from_R(wc.R), wc.R);
-    return wc;
-}
-
-// g2o::internal::toSE3Quat(Isometry3D)
-SE3 se3_from_iso(const Iso& X) { return se3_from_Rt(X.R, X.t); }
-Iso iso_from_se3(const SE3& T) {
-    Iso X;
-    quat_to_R(T.q, X.R);
-    std::memcpy(X.t, T.t, sizeof X.t);
-    return X;
-}
-
-// g2o::internal::fromVectorMQT: (t, qx, qy, qz), w = sqrt(1 - |q|^2); the normalised (0, q) when |q|^2 >= 1
-Iso iso_from_mqt(const double* d) {
-    const double n2 = d[3] * d[3] + d[4] * d[4] + d[5] * d[5];
-    const double w = 1. - n2;
-    Quat q;
-    if (w < 0) {
-        const double n = std::sqrt(n2);
-        q = {d[3] / n, d[4] / n, d[5] / n, 0};
-    } else {
-        q = {d[3], d[4], d[5], std::sqrt(w)};
-    }
-    Iso X;
-    quat_to_R(q, X.R);
-    X.t[0] = d[0]; X.t[1] = d[1]; X.t[2] = d[2];
-    return X;
-}
-
-// VertexSE3::oplusImpl
-Iso oplus(const Iso& X, const double* d) { return iso_mul(X, iso_from_mqt(d)); }
-
 // EdgeSE3PointXYZ::computeError with an identity offset: X^-1 p - z; pc = X^-1 p
 void xyz_error(const Iso& Xinv, const double* p, const double* z, double* e, double* pc) {
     mulv3(Xinv.R, p, pc);
@@ -263,78 +85,6 @@ void xyz_jacobians(const Iso& Xinv, const double* pc, double* Jp, double* Jl) {
     std::memcpy(Jl, Xinv.R, 9 * sizeof(double));
 }
 
-struct Prior {
-    Iso meas, meas_inv;
-    double info[36];
-};
-
-// addVertexSE3PlaneMotion (src/optimizer.cpp:429-455)
-Prior plane_motion_prior(const Iso& pose, const Params& p) {
-    const SE3 Tbc = se3_from_f32(p.Tbc);
-    SE3 Twb = se3_mul(se3_from_iso(pose), se3_inv(Tbc));
-    const Quat& q = Twb.q;  // Eigen 3.3 AngleAxisd(Quaterniond)
-    double n = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z), angle = 0, axis_z = 0;
-    if (n != 0) {
-        angle = 2 * std::atan2(n, std::fabs(q.w));
-        if (q.w < 0) n = -n;
-        axis_z = q.z / n;
-    }
-    const double ha = 0.5 * (angle * axis_z), s = std::sin(ha);
-    Twb.q = {s * 0.0, s * 0.0, s * 1.0, std::cos(ha)};  // setRotation does not normalise
-    Twb.t[2] = 0;
-    Prior pr;
-    pr.meas = iso_from_se3(se3_mul(Twb, Tbc));
-    pr.meas_inv = iso_inv(pr.meas);
-    // AdjTR (src/optimizer.cpp:93-102): [[R, skew(t) R], [0, R]]
-    double R[9], SR[9], A[36];
-    quat_to_R(Tbc.q, R);
-    const double* t = Tbc.t;
-    const double S[9] = {0, -t[2], t[1], t[2], 0, -t[0], -t[1], t[0], 0};
-    mul3(S, R, SR);
-    for (int k = 0; k < 36; ++k) A[k] = 0;
-    for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) {
-            A[r * 6 + c] = R[r * 3 + c];
-            A[(r + 3) * 6 + c + 3] = R[r * 3 + c];
-            A[r * 6 + c + 3] = SR[r * 3 + c];
-        }
-    const double d[6] = {1e-4, 1e-4, (double)p.zinfo, (double)p.xrot, (double)p.yrot, 1e-4};
-    for (int r = 0; r < 6; ++r)
-        for (int c = 0; c < 6; ++c) {
-            double acc = 0;
-            for (int k = 0; k < 6; ++k) acc += (A[k * 6 + r] * d[k]) * A[k * 6 + c];
-            pr.info[r * 6 + c] = acc;
-        }
-    return pr;
-}
-
-// EdgeSE3Prior::computeError: toVectorMQT(Z^-1 X); J [36] (may be NULL) its derivative through oplus
-void prior_error(const Prior& pr, const Iso& X, double* e, double* J) {
-    const Iso E = iso_mul(pr.meas_inv, X);
-    Quat q = quat_from_R(E.R);
-    normalize_rotation(q);
-    e[0] = E.t[0]; e[1] = E.t[1]; e[2] = E.t[2];
-    e[3] = q.x; e[4] = q.y; e[5] = q.z;
-    if (!J) return;
-    for (int k = 0; k < 36; ++k) J[k] = 0;
-    for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) J[r * 6 + c] = E.R[r * 3 + c];
-    // vec(q (x) (w_d, d)) = w d + w_d v + v x d: derivative w I + skew(v) at d = 0
-    J[21] = q.w;  J[22] = -q.z; J[23] = q.y;
-    J[27] = q.z;  J[28] = q.w;  J[29] = -q.x;
-    J[33] = -q.y; J[34] = q.x;  J[35] = q.w;
-}
-
-double quad(const double* M, const double* e, int n) {
-    double chi = 0;
-    for (int r = 0; r < n; ++r) {
-        double we = 0;
-        for (int c = 0; c < n; ++c) we += M[r * n + c] * e[c];
-        chi += e[r] * we;
-    }
-    return chi;
-}
-
 // Eigen fixed-size 3 x 3 inverse: cofactors over the determinant
 void inv3(const double* m, double* o) {
     const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
@@ -342,33 +92,6 @@ void inv3(const double* m, double* o) {
     o[0] = c00 * id; o[1] = (m[2] * m[7] - m[1] * m[8]) * id; o[2] = (m[1] * m[5] - m[2] * m[4]) * id;
     o[3] = c01 * id; o[4] = (m[0] * m[8] - m[2] * m[6]) * id; o[5] = (m[2] * m[3] - m[0] * m[5]) * id;
     o[6] = c02 * id; o[7] = (m[1] * m[6] - m[0] * m[7]) * id; o[8] = (m[0] * m[4] - m[1] * m[3]) * id;
-}
-
-// dense LL^T solve of the n x n system; false when not positive definite
-bool chol_solve(int n, const double* H, const double* b, double* x) {
-    std::vector<double> L((size_t)n * n);
-    for (int r = 0; r < n; ++r)
-        for (int c = 0; c <= r; ++c) {
-            double s = H[r * n + c];
-            for (int k = 0; k < c; ++k) s -= L[r * n + k] * L[c * n + k];
-            if (c == r) {
-                if (!(s > 0.0) || !std::isfinite(s)) return false;
-                L[r * n + r] = std::sqrt(s);
-            } else {
-                L[r * n + c] = s / L[c * n + c];
-            }
-        }
-    for (int r = 0; r < n; ++r) {
-        double s = b[r];
-        for (int k = 0; k < r; ++k) s -= L[r * n + k] * x[k];
-        x[r] = s / L[r * n + r];
-    }
-    for (int r = n - 1; r >= 0; --r) {
-        double s = x[r];
-        for (int k = r + 1; k < n; ++k) s -= L[k * n + r] * x[k];
-        x[r] = s / L[r * n + r];
-    }
-    return true;
 }
 
 // inverse by LU with partial pivoting (Eigen's inverse() above 4 x 4)
@@ -582,9 +305,10 @@ struct PairBA {
     Params prm;
     int mode = 0, P = 0, nfree = 0, fk[2] = {0, 0};
     bool reverse = false;
-    Iso X[2], lastX[2];
+    Iso X[2], lastX[2], bak[2];
     Prior prior[2];
-    std::vector<double> pts, lastPts;
+    std::vector<double> pts, lastPts, bakp, xl;
+    double* trace = nullptr;
     const float *z[2] = {nullptr, nullptr};
     const double* om[2] = {nullptr, nullptr};
     // linearisation
@@ -603,7 +327,7 @@ struct PairBA {
         double chi = 0;
         for (int f = 0; f < nfree; ++f) {
             double e[6];
-            prior_error(prior[fk[f]], Xs[fk[f]], e, nullptr);
+            se3_prior_error(prior[fk[f]], Xs[fk[f]], e, nullptr);
             chi += quad(prior[fk[f]].info, e, 6);
         }
         const Iso Xi[2] = {iso_inv(Xs[0]), iso_inv(Xs[1])};
@@ -628,7 +352,7 @@ struct PairBA {
         for (int f = 0; f < nfree; ++f) {  // BaseUnaryEdge: H += J^T Omega J, b -= J^T Omega e
             const int k = fk[f];
             double e[6], J[36], OJ[36], Oe[6];
-            prior_error(prior[k], X[k], e, J);
+            se3_prior_error(prior[k], X[k], e, J);
             for (int r = 0; r < 6; ++r) {
                 Oe[r] = 0;
                 for (int c = 0; c < 6; ++c) {
@@ -683,7 +407,7 @@ struct PairBA {
             }
         }
     }
-    double maxDiag() const {  // computeLambdaInit over every free vertex
+    double max_diag() const {  // computeLambdaInit over every free vertex
         double m = 0;
         for (int f = 0; f < nfree; ++f)
             for (int i = 0; i < 6; ++i) m = std::max(m, std::fabs(Hpp[fk[f]][i * 7]));
@@ -725,7 +449,7 @@ struct PairBA {
                 }
             }
         }
-        if (!chol_solve(n, Hs.data(), bs.data(), xp)) return false;
+        if (!dense_llt_solve(n, Hs.data(), bs.data(), xp)) return false;
         double sc = 0;
         for (int f = 0; f < nfree; ++f)
             for (int r = 0; r < 6; ++r) sc += xp[f * 6 + r] * (lambda * xp[f * 6 + r] + bp[fk[f]][r]);
@@ -747,73 +471,32 @@ struct PairBA {
         return true;
     }
 
-    int optimize(int iterations, IterStats* stats, double* trace, int* not_pd) {
-        *not_pd = 0;
-        double lambda = 0, ni = 2;
-        int done = 0;
-        bool ok = true;
-        std::vector<double> xl((size_t)P * 3);
-        for (int it = 0; it < iterations && ok; ++it) {
-            IterStats st{};
-            double currentChi = chi2(X, pts);
-            lastX[0] = X[0]; lastX[1] = X[1]; lastPts = pts;
-            st.chi2_before = currentChi;
-            build();
-            if (it == 0) { lambda = 1e-5 * maxDiag(); ni = 2; }
-            double rho = 0;
-            int qmax = 0, failed = 0;
-            do {
-                const Iso bak[2] = {X[0], X[1]};
-                const std::vector<double> bakp = pts;
-                double xp[12], scale = 0;
-                const bool ok2 = solve(lambda, xp, xl, &scale);
-                double tempChi = std::numeric_limits<double>::max();
-                if (ok2) {
-                    for (int f = 0; f < nfree; ++f) X[fk[f]] = oplus(X[fk[f]], xp + 6 * f);
-                    for (size_t i = 0; i < pts.size(); ++i) pts[i] += xl[i];
-                    tempChi = chi2(X, pts);
-                    lastX[0] = X[0]; lastX[1] = X[1]; lastPts = pts;
-                } else {
-                    ++failed;
-                }
-                rho = (currentChi - tempChi) / (scale + 1e-3);
-                if (rho > 0 && std::isfinite(tempChi)) {
-                    double alpha = 1. - std::pow((2 * rho - 1), 3);
-                    alpha = std::min(alpha, 2. / 3.);
-                    lambda *= std::max(1. / 3., alpha);
-                    ni = 2;
-                    currentChi = tempChi;
-                    st.accepted = 1;
-                } else {
-                    lambda *= ni;
-                    ni *= 2;
-                    X[0] = bak[0]; X[1] = bak[1]; pts = bakp;
-                }
-                qmax++;
-            } while (rho < 0 && qmax < 10);
-            st.chi2_after = currentChi; st.lambda = lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            ok = !st.terminate;
-            if (st.terminate && failed == qmax) *not_pd = 1;
-            if (stats) stats[it] = st;
-            if (trace)
-                for (int k = 0; k < 2; ++k) {
-                    std::memcpy(trace + 24 * (size_t)it + 12 * k, X[k].R, 9 * sizeof(double));
-                    std::memcpy(trace + 24 * (size_t)it + 12 * k + 9, X[k].t, 3 * sizeof(double));
-                }
-            ++done;
-        }
-        return done;
+    // the LM hooks of lm_optimize. chi2 is evaluated at every iteration's start; that and a solved trial record the estimate
+    // whose errors OptKFPairMatch reads after optimize()
+    double start_chi2(int, double) {
+        lastX[0] = X[0]; lastX[1] = X[1]; lastPts = pts;
+        return chi2(X, pts);
+    }
+    bool trial(double lambda, double* tempChi, double* scale) {
+        bak[0] = X[0]; bak[1] = X[1]; bakp = pts;
+        double xp[12];
+        if (!solve(lambda, xp, xl, scale)) return false;
+        for (int f = 0; f < nfree; ++f) X[fk[f]] = oplus(X[fk[f]], xp + 6 * f);
+        for (size_t i = 0; i < pts.size(); ++i) pts[i] += xl[i];
+        *tempChi = chi2(X, pts);
+        lastX[0] = X[0]; lastX[1] = X[1]; lastPts = pts;
+        return true;
+    }
+    void accept() {}
+    void reject() { X[0] = bak[0]; X[1] = bak[1]; pts = bakp; }
+    void record(int it) {
+        if (trace)
+            for (int k = 0; k < 2; ++k) {
+                std::memcpy(trace + 24 * (size_t)it + 12 * k, X[k].R, 9 * sizeof(double));
+                std::memcpy(trace + 24 * (size_t)it + 12 * k + 9, X[k].t, 3 * sizeof(double));
+            }
     }
 };
-
-void pose_out(const SE3& T, double* p7) {
-    p7[0] = T.q.x; p7[1] = T.q.y; p7[2] = T.q.z; p7[3] = T.q.w;
-    p7[4] = T.t[0]; p7[5] = T.t[1]; p7[6] = T.t[2];
-}
-
-void iso_in(const double* v12, Iso* X) { std::memcpy(X->R, v12, 9 * sizeof(double)); std::memcpy(X->t, v12 + 9, 3 * sizeof(double)); }
-void iso_out(const Iso& X, double* v12) { std::memcpy(v12, X.R, 9 * sizeof(double)); std::memcpy(v12 + 9, X.t, 3 * sizeof(double)); }
 
 }  // namespace
 
@@ -839,13 +522,15 @@ int feat_edge_oracle_run(int mode, const float* Tcw0, const float* Tcw1, int P, 
     b.X[1] = iso_from_Tcw(Tcw1);
     if (mode == 0) { b.nfree = 1; b.fk[0] = 1; }
     else { b.nfree = 2; b.fk[0] = 0; b.fk[1] = 1; }
-    for (int f = 0; f < b.nfree; ++f) b.prior[b.fk[f]] = plane_motion_prior(b.X[b.fk[f]], b.prm);
+    for (int f = 0; f < b.nfree; ++f) b.prior[b.fk[f]] = plane_prior_se3(b.X[b.fk[f]], b.prm.Tbc, b.prm.xrot, b.prm.yrot, b.prm.zinfo);
     b.pts.resize((size_t)P * 3);
+    b.xl.resize((size_t)P * 3);
+    b.trace = trace;
     for (size_t i = 0; i < b.pts.size(); ++i) b.pts[i] = xyz[i];
     b.z[0] = z0; b.z[1] = z1; b.om[0] = info0; b.om[1] = info1;
     b.lastX[0] = b.X[0]; b.lastX[1] = b.X[1]; b.lastPts = b.pts;
-    int not_pd = 0;
-    const int done = b.optimize(b.prm.iterations[mode], (IterStats*)stats, trace, &not_pd);
+    bool not_pd = false;
+    const int done = lm_optimize(b, b.prm.iterations[mode], (IterStats*)stats, &not_pd);
     *status = not_pd ? 2 : 0;
     std::vector<int> keep;
     if (mode == 1) {  // EdgeSE3PointXYZ::chi2() on the errors of the last evaluated trial
@@ -866,13 +551,7 @@ int feat_edge_oracle_run(int mode, const float* Tcw0, const float* Tcw1, int P, 
     SE3 zo;
     double I[36];
     marginalize(KF, (int)keep.size(), keep.data(), b.pts.data(), z0, z1, info0, info1, b.reverse, (reverse & 2) != 0, &zo, I, Hm);
-    double R[9];  // converter.cpp toCvMat(SE3Quat) / toCvMat6f
-    quat_to_R(zo.q, R);
-    for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) measure[r * 4 + c] = (float)R[r * 3 + c];
-        measure[r * 4 + 3] = (float)zo.t[r];
-    }
-    measure[12] = 0; measure[13] = 0; measure[14] = 0; measure[15] = 1;
+    to_f32(zo, measure);  // converter.cpp toCvMat(SE3Quat) / toCvMat6f
     for (int i = 0; i < 36; ++i) info[i] = (float)I[i];
     if (poses) { pose_out(KF[0], poses); pose_out(KF[1], poses + 7); }
     if (points) std::memcpy(points, b.pts.data(), b.pts.size() * sizeof(double));
@@ -899,10 +578,10 @@ void feat_edge_oracle_prior(const double* X0_12, const void* params, const doubl
     Params p;
     std::memcpy(&p, params, sizeof p);
     Iso X0, X; iso_in(X0_12, &X0); iso_in(X12, &X);
-    const Prior pr = plane_motion_prior(X0, p);
+    const Prior pr = plane_prior_se3(X0, p.Tbc, p.xrot, p.yrot, p.zinfo);
     iso_out(pr.meas, meas12);
     std::memcpy(info36, pr.info, sizeof pr.info);
-    prior_error(pr, X, e, J);
+    se3_prior_error(pr, X, e, J);
 }
 // the singular-value clamp of InfoSE3 on a 6 x 6 matrix, in place
 void feat_edge_oracle_clamp(double* I36) { clamp_info(I36); }

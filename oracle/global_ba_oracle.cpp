@@ -6,8 +6,8 @@
 // optimize(GLOBAL_ITER) under OptimizationAlgorithmLevenberg with BlockSolverX and a sparse Cholesky.
 //
 // The SE(3) pieces — Isometry3d products and inverse, VertexSE3 oplus, toSE3Quat, the plane-motion prior with its analytic
-// Jacobian — are the feature-graph oracle's: feat_edge_oracle.cpp is compiled into this translation unit, so both oracles
-// run one definition of each.
+// Jacobian — are oracle/se3_oracle.h's, the Levenberg-Marquardt loop and the skyline Cholesky oracle/g2o_lm_oracle.h's: the
+// feature-graph oracle runs the same definitions.
 //
 // What is decided here and not copied from anywhere:
 //  * EdgeSE3's Jacobians are the analytic first derivatives of e = toVectorMQT(Z^-1 Xi^-1 Xj) through the MQT oplus of both
@@ -27,10 +27,14 @@
 //    The order changes only the rounding; the natural order of a graph with loop closures has an envelope too wide for the
 //    larger test scenes. A pivot <= 0 fails the trial, as CHOLMOD's minor != n does.
 // PARITY UNPINNED against real g2o (no g2o build exists here); pinned by self-consistency in tests/test_global_ba_oracle.py.
-// the feature-graph oracle's C entry points stay out of this library's exports
-#pragma GCC visibility push(hidden)
-#include "feat_edge_oracle.cpp"
-#pragma GCC visibility pop
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <cstring>
+#include <vector>
+
+#include "g2o_lm_oracle.h"
+#include "se3_oracle.h"
 
 namespace {
 
@@ -121,23 +125,21 @@ void atme(const double* A, const double* M, const double* e, double* out) {
 struct Graph {
     int N = 0, E = 0, n = 0;  // n = 6 * free vertices
     bool reverse = false;
-    std::vector<Iso> X, Zinv;
+    std::vector<Iso> X, Xt, Zinv;
     std::vector<Prior> prior;
     std::vector<double> Om;
     std::vector<int> from, to;
     std::vector<int> pos, vert;     // vertex -> elimination position (-1 fixed), position -> vertex
-    std::vector<int> fcol;          // [n] first scalar column of scalar row i
-    std::vector<int64_t> roff;      // [n + 1] skyline offsets
-    std::vector<double> H, b, L;
+    Skyline H, L;                   // one profile: a scalar row's first column is its block row's first block column
+    std::vector<double> b, x;
 
     int edge(int k) const { return reverse ? E - 1 - k : k; }
-    double& at(std::vector<double>& M, int i, int j) { return M[roff[i] + (j - fcol[i])]; }
 
     double chi2(const std::vector<Iso>& Xs) const {
         double chi = 0;
         for (int v = 0; v < N; ++v) {
             double e[6];
-            prior_error(prior[v], Xs[v], e, nullptr);
+            se3_prior_error(prior[v], Xs[v], e, nullptr);
             chi += quad(prior[v].info, e, 6);
         }
         for (int k = 0; k < E; ++k) {
@@ -152,17 +154,20 @@ struct Graph {
             for (int c = 0; c < 6; ++c) {
                 const int i = 6 * p + r, j = 6 * q + c;
                 if (j > i) continue;
-                at(H, i, j) += transpose ? M[c * 6 + r] : M[r * 6 + c];
+                H.at(i, j) += transpose ? M[c * 6 + r] : M[r * 6 + c];
             }
     }
+
+    // the LM hooks of lm_optimize
+    double start_chi2(int it, double carried) const { return it == 0 ? chi2(X) : carried; }  // carried after the first
     void build() {  // BlockSolver::buildSystem: priors first, then the edges in order
-        std::fill(H.begin(), H.end(), 0.0);
+        std::fill(H.v.begin(), H.v.end(), 0.0);
         std::fill(b.begin(), b.end(), 0.0);
         for (int v = 0; v < N; ++v) {
             const int p = pos[v];
             if (p < 0) continue;
             double e[6], J[36], Hb[36], bb[6];
-            prior_error(prior[v], X[v], e, J);
+            se3_prior_error(prior[v], X[v], e, J);
             atmb(J, prior[v].info, J, Hb);
             atme(J, prior[v].info, e, bb);
             add_block(p, p, Hb, false);
@@ -190,86 +195,27 @@ struct Graph {
             }
         }
     }
+    double max_diag() {
+        double m = 0;
+        for (int i = 0; i < n; ++i) m = std::max(m, std::fabs(H.at(i, i)));
+        return m;
+    }
     // (H + lambda I) x = b by skyline Cholesky; false when a pivot is not positive
-    bool solve(double lambda, std::vector<double>& x) {
-        L = H;
-        for (int i = 0; i < n; ++i) at(L, i, i) += lambda;
-        for (int i = 0; i < n; ++i)
-            for (int j = fcol[i]; j <= i; ++j) {
-                double s = at(L, i, j);
-                for (int k = std::max(fcol[i], fcol[j]); k < j; ++k) s -= at(L, i, k) * at(L, j, k);
-                if (j < i) {
-                    at(L, i, j) = s / at(L, j, j);
-                } else {
-                    if (!(s > 0.0) || !std::isfinite(s)) return false;
-                    at(L, i, i) = std::sqrt(s);
-                }
-            }
+    bool trial(double lambda, double* tempChi, double* scale) {
+        L.v = H.v;
+        for (int i = 0; i < n; ++i) L.at(i, i) += lambda;
+        if (!L.cholesky()) return false;
         x = b;
-        for (int i = 0; i < n; ++i) {
-            double s = x[i];
-            for (int k = fcol[i]; k < i; ++k) s -= at(L, i, k) * x[k];
-            x[i] = s / at(L, i, i);
-        }
-        for (int i = n - 1; i >= 0; --i) {
-            x[i] /= at(L, i, i);
-            for (int k = fcol[i]; k < i; ++k) x[k] -= at(L, i, k) * x[i];
-        }
+        L.solve(x.data());
+        Xt = X;
+        for (int p = 0; p < (int)vert.size(); ++p) Xt[vert[p]] = oplus(X[vert[p]], &x[6 * (size_t)p]);
+        for (int i = 0; i < n; ++i) *scale += x[i] * (lambda * x[i] + b[i]);
+        *tempChi = chi2(Xt);
         return true;
     }
-
-    int optimize(int iterations, IterStats* stats, int* not_pd) {
-        *not_pd = 0;
-        if (n == 0) return 0;
-        double lambda = 0, ni = 2, currentChi = chi2(X);
-        std::vector<double> x(n);
-        int done = 0;
-        for (int it = 0; it < iterations; ++it) {
-            IterStats st{};
-            st.chi2_before = currentChi;
-            build();
-            if (it == 0) {
-                double m = 0;
-                for (int i = 0; i < n; ++i) m = std::max(m, std::fabs(at(H, i, i)));
-                lambda = 1e-5 * m; ni = 2;
-            }
-            double rho = 0;
-            int qmax = 0, failed = 0;
-            do {
-                const bool ok = solve(lambda, x);
-                double tempChi = std::numeric_limits<double>::max(), scale = 0;
-                std::vector<Iso> Xt = X;
-                if (ok) {
-                    for (int p = 0; p < (int)vert.size(); ++p) Xt[vert[p]] = oplus(X[vert[p]], &x[6 * (size_t)p]);
-                    for (int i = 0; i < n; ++i) scale += x[i] * (lambda * x[i] + b[i]);
-                    tempChi = chi2(Xt);
-                } else {
-                    ++failed;
-                }
-                rho = (currentChi - tempChi) / (scale + 1e-3);
-                if (rho > 0 && std::isfinite(tempChi)) {
-                    double alpha = 1. - std::pow((2 * rho - 1), 3);
-                    alpha = std::min(alpha, 2. / 3.);
-                    lambda *= std::max(1. / 3., alpha);
-                    ni = 2;
-                    currentChi = tempChi;
-                    X = Xt;
-                    st.accepted = 1;
-                } else {
-                    lambda *= ni;
-                    ni *= 2;
-                }
-                qmax++;
-            } while (rho < 0 && qmax < 10);
-            st.chi2_after = currentChi; st.lambda = lambda; st.rho = rho; st.trials = qmax;
-            st.terminate = (qmax == 10 || rho == 0) ? 1 : 0;
-            if (st.terminate && failed == qmax) *not_pd = 1;
-            if (stats) stats[it] = st;
-            ++done;
-            if (st.terminate) break;
-        }
-        return done;
-    }
+    void accept() { X = Xt; }
+    void reject() {}
+    void record(int) {}
 };
 
 }  // namespace
@@ -286,9 +232,6 @@ int global_ba_oracle_run(int N, const float* Tcw, const uint8_t* fixed, int E, c
                          int* status) {
     GParams gp;
     std::memcpy(&gp, params, sizeof gp);
-    Params fp{};
-    std::memcpy(fp.Tbc, gp.Tbc, sizeof fp.Tbc);
-    fp.xrot = gp.xrot; fp.yrot = gp.yrot; fp.zinfo = gp.zinfo;
     Graph g;
     g.N = N; g.E = E; g.reverse = reverse != 0;
     g.from.assign(from, from + E); g.to.assign(to, to + E);
@@ -297,7 +240,7 @@ int global_ba_oracle_run(int N, const float* Tcw, const uint8_t* fixed, int E, c
         float Twc[16];
         rigid_inv_f32(Tcw + 16 * (size_t)v, Twc);
         g.X[v] = iso_from_f32(Twc);
-        g.prior[v] = plane_motion_prior(g.X[v], fp);
+        g.prior[v] = plane_prior_se3(g.X[v], gp.Tbc, gp.xrot, gp.yrot, gp.zinfo);
     }
     g.Zinv.resize(E); g.Om.resize(36 * (size_t)E);
     for (int e = 0; e < E; ++e) {
@@ -316,25 +259,18 @@ int global_ba_oracle_run(int N, const float* Tcw, const uint8_t* fixed, int E, c
         if (a >= 0 && b >= 0) first[std::max(a, b)] = std::min(first[std::max(a, b)], std::min(a, b));
     }
     g.n = 6 * nf;
-    g.fcol.resize(g.n); g.roff.assign(g.n + 1, 0);
-    for (int i = 0; i < g.n; ++i) {
-        g.fcol[i] = 6 * first[i / 6];
-        g.roff[i + 1] = g.roff[i] + (i - g.fcol[i] + 1);
-    }
-    g.H.assign(g.roff[g.n], 0.0); g.b.assign(g.n, 0.0);
-    int not_pd = 0;
-    const int done = g.optimize(gp.iterations, (IterStats*)stats, &not_pd);
+    std::vector<int> fcol(g.n);
+    for (int i = 0; i < g.n; ++i) fcol[i] = 6 * first[i / 6];
+    g.H.build(g.n, fcol); g.L.build(g.n, fcol);
+    g.b.assign(g.n, 0.0);
+    bool not_pd = false;
+    // with no free vertex g2o's optimize() returns before any iteration
+    const int done = g.n > 0 ? lm_optimize(g, gp.iterations, (IterStats*)stats, &not_pd) : 0;
     *status = not_pd ? 2 : 0;
     for (int v = 0; v < N; ++v) {
         const SE3 T = se3_from_iso(g.X[v]);
-        double R[9];
-        quat_to_R(T.q, R);
         float Twc[16];
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) Twc[r * 4 + c] = (float)R[r * 3 + c];
-            Twc[r * 4 + 3] = (float)T.t[r];
-        }
-        Twc[12] = 0.f; Twc[13] = 0.f; Twc[14] = 0.f; Twc[15] = 1.f;
+        to_f32(T, Twc);
         rigid_inv_f32(Twc, Tcw_out + 16 * (size_t)v);
         if (poses) pose_out(T, poses + 7 * (size_t)v);
     }

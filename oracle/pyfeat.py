@@ -7,18 +7,10 @@ product package (se2lam_b200) never imports this module.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.pyoracle import BA_STATS_DTYPE
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "feat_edge_oracle.cpp")
-LIB_PATH = os.path.join(HERE, "libfeat_edge_oracle.so")
-CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=default", "-Wall",
-            "-Wno-unused-function", "-Wno-maybe-uninitialized"]
+from oracle.pyoracle import BA_STATS_DTYPE, make
 
 
 class Params(C.Structure):
@@ -37,22 +29,13 @@ def params(Tbc=None, xrot=1e6, yrot=1e6, zinfo=1.0, huber_delta=5.99, iterations
     return p
 
 
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or os.path.getmtime(SRC) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
-
-
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libfeat_edge_oracle.so"))
         vp, i = C.c_void_p, C.c_int
         L.feat_edge_oracle_run.argtypes = [i, vp, vp, i] + [vp] * 14 + [i, vp]
         L.feat_edge_oracle_from_Tcw.argtypes = [vp, vp]

@@ -7,24 +7,10 @@ The product package (se2lam_b200) never imports this module.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "fundam_oracle.cpp")
-LIB_PATH = os.path.join(HERE, "libfundam_oracle.so")
-CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=hidden", "-Wall",
-            "-Wno-unused-function"]
-
-
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or os.path.getmtime(SRC) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
+from oracle.pyoracle import make
 
 
 _lib = None
@@ -33,8 +19,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libfundam_oracle.so"))
         vp, i = C.c_void_p, C.c_int
         L.fundam_oracle_find.argtypes = [vp, vp, i, vp, vp, vp, vp]
         L.fundam_oracle_remove_outliers.argtypes = [vp, i, vp, i, vp, vp, vp]

@@ -6,23 +6,10 @@ The product package (se2lam_b200) never imports this module.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "geom_oracle.cpp")
-LIB_PATH = os.path.join(HERE, "libgeom_oracle.so")
-CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wno-unused-function"]
-
-
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or os.path.getmtime(SRC) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
+from oracle.pyoracle import make
 
 
 _lib = None
@@ -31,8 +18,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libgeom_oracle.so"))
         vp, i, f, d = C.c_void_p, C.c_int, C.c_float, C.c_double
         L.geom_oracle_svd4.argtypes = [vp, vp, vp]
         L.geom_oracle_svd4_libm_hypot.argtypes = [vp, vp, vp]

@@ -1,24 +1,16 @@
 """ctypes bindings of the global pose-graph oracle (oracle/libglobal_ba_oracle.so) — TEST INFRASTRUCTURE ONLY.
 
-A library of its own, built with the flags of the other oracles (no -march, -ffp-contract=off). It restates
-GlobalMapper::GlobalBA (oracle/global_ba_oracle.cpp), compiling the feature-graph oracle's SE(3) pieces into the same
-translation unit. The product package (se2lam_b200) never imports this module.
+A library of its own, built by oracle/Makefile with the flags of the other oracles (no -march, -ffp-contract=off). It
+restates GlobalMapper::GlobalBA (oracle/global_ba_oracle.cpp) on the SE(3) pieces the feature-graph oracle also runs
+(oracle/se3_oracle.h). The product package (se2lam_b200) never imports this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.pyfeat import CXXFLAGS
-from oracle.pyoracle import BA_STATS_DTYPE
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "global_ba_oracle.cpp")
-DEPS = [SRC, os.path.join(HERE, "feat_edge_oracle.cpp")]
-LIB_PATH = os.path.join(HERE, "libglobal_ba_oracle.so")
+from oracle.pyoracle import BA_STATS_DTYPE, make
 
 
 class Params(C.Structure):
@@ -35,22 +27,13 @@ def params(Tbc=None, xrot=1e6, yrot=1e6, zinfo=1.0, iterations=15):
     return p
 
 
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or max(os.path.getmtime(d) for d in DEPS) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
-
-
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libglobal_ba_oracle.so"))
         vp, i = C.c_void_p, C.c_int
         L.global_ba_oracle_run.argtypes = [i, vp, vp, i] + [vp] * 9 + [i, vp]
         L.global_ba_oracle_edge.argtypes = [vp] * 7

@@ -7,27 +7,10 @@ never imports this module.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from .pyoracle import KP_DTYPE
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "orb_harris_oracle.cpp")
-DEPS = [SRC, os.path.join(HERE, "orb_oracle.cpp"), os.path.join(HERE, "..", "se2lam_b200", "csrc", "orb_pattern_31.inc")]
-LIB_PATH = os.path.join(HERE, "liborb_harris_oracle.so")
-CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=hidden", "-Wall",
-            "-Wno-unused-function"]
-
-
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or any(os.path.getmtime(d) > os.path.getmtime(LIB_PATH) for d in DEPS):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
+from .pyoracle import KP_DTYPE, make
 
 
 _lib = None
@@ -36,8 +19,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("liborb_harris_oracle.so"))
         vp, i, f = C.c_void_p, C.c_int, C.c_float
         L.orb_harris_oracle_create.restype = vp
         L.orb_harris_oracle_create.argtypes = [i, f, i, i]

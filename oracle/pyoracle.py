@@ -12,7 +12,6 @@ import subprocess
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "liboracle.so")
 
 KP_DTYPE = np.dtype([("x", "f4"), ("y", "f4"), ("size", "f4"), ("angle", "f4"), ("response", "f4"),
                      ("octave", "i4"), ("class_id", "i4")])
@@ -20,15 +19,12 @@ BA_STATS_DTYPE = np.dtype([("chi2_before", "f8"), ("chi2_after", "f8"), ("lambda
                            ("trials", "i4"), ("accepted", "i4"), ("terminate", "i4"), ("pad", "i4")])
 
 
-def build(force: bool = False) -> str:
-    srcs = [os.path.join(HERE, f) for f in ("orb_oracle.cpp", "ba_oracle.cpp", "matcher_oracle.cpp", "undistort_oracle.cpp", "bow_oracle.cpp")]
-    stale = force or not os.path.exists(LIB_PATH) or any(
-        os.path.exists(s) and os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
-    if stale:
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        subprocess.run(["make", "-C", HERE, "-s", "CXX=g++"], check=True, env=env)
-    return LIB_PATH
+def make(lib: str = "") -> str:
+    """Bring oracle/<lib> (every oracle library when lib is empty) up to date with oracle/Makefile, which decides what is
+    stale, and return its path. g++ with the Makefile's flags, whatever CXX / CXXFLAGS the environment holds."""
+    env = {k: v for k, v in os.environ.items() if k not in ("CXX", "CXXFLAGS")}
+    subprocess.run(["make", "-C", HERE, "-s", "CXX=g++"] + ([lib] if lib else []), check=True, env=env)
+    return os.path.join(HERE, lib)
 
 
 _lib = None
@@ -37,8 +33,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("liboracle.so"))
         vp, i, f, d = C.c_void_p, C.c_int, C.c_float, C.c_double
         L.orb_oracle_create.restype = vp
         L.orb_oracle_create.argtypes = [i, f, i, i]

@@ -6,26 +6,10 @@ Localizer::DoLocalBA's g2o graph (oracle/pose_ba_oracle.cpp). The product packag
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.pyoracle import BA_STATS_DTYPE
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "pose_ba_oracle.cpp")
-LIB_PATH = os.path.join(HERE, "libpose_ba_oracle.so")
-CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fvisibility=default", "-Wall",
-            "-Wno-unused-function", "-Wno-maybe-uninitialized"]
-
-
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or os.path.getmtime(SRC) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
+from oracle.pyoracle import BA_STATS_DTYPE, make
 
 
 _lib = None
@@ -34,8 +18,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libpose_ba_oracle.so"))
         vp, i, f, d = C.c_void_p, C.c_int, C.c_float, C.c_double
         L.pose_ba_oracle_run.argtypes = [vp, i, vp, vp, vp, f, f, f, vp, f, f, f, f, i, vp, vp, vp, vp]
         L.pose_ba_oracle_from_f32.argtypes = [vp, vp]

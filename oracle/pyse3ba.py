@@ -1,32 +1,17 @@
 """ctypes binding of the SE(3)-XYZ window BA oracle (oracle/libse3_ba_oracle.so) — TEST INFRASTRUCTURE ONLY.
 
-A library of its own, built with the flags of the other oracles (no -march, -ffp-contract=off). It restates the window of
-Map::loadLocalGraph / loadLocalGraphOnlyBa and removeOutlierChi2's cut (oracle/se3_ba_oracle.cpp), compiling the pose-only
-BA oracle's SE3Quat pieces into the same translation unit. The product package (se2lam_b200) never imports this module.
+A library of its own, built by oracle/Makefile with the flags of the other oracles (no -march, -ffp-contract=off). It
+restates the window of Map::loadLocalGraph / loadLocalGraphOnlyBa and removeOutlierChi2's cut (oracle/se3_ba_oracle.cpp) on
+the SE3Quat pieces the pose-only BA oracle also runs (oracle/se3_oracle.h). The product package (se2lam_b200) never imports
+this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.pyfeat import CXXFLAGS
-from oracle.pyoracle import BA_STATS_DTYPE
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, "se3_ba_oracle.cpp")
-DEPS = [SRC, os.path.join(HERE, "pose_ba_oracle.cpp")]
-LIB_PATH = os.path.join(HERE, "libse3_ba_oracle.so")
-
-
-def build(force: bool = False) -> str:
-    if force or not os.path.exists(LIB_PATH) or max(os.path.getmtime(d) for d in DEPS) > os.path.getmtime(LIB_PATH):
-        tmp = LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.run(["g++", *CXXFLAGS, "-shared", "-o", tmp, SRC], check=True)
-        os.replace(tmp, LIB_PATH)
-    return LIB_PATH
+from oracle.pyoracle import BA_STATS_DTYPE, make
 
 
 _lib = None
@@ -35,8 +20,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(LIB_PATH)
+        L = C.CDLL(make("libse3_ba_oracle.so"))
         vp, i = C.c_void_p, C.c_int
         L.se3_ba_oracle_run.restype = i
         L.se3_ba_oracle_run.argtypes = [i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i, vp, vp, vp, vp, vp, i, i] + [vp] * 7

@@ -138,3 +138,21 @@ def test_oracle_spread_is_far_below_the_gpu_bounds():
             worst_est = max(worst_est, float(np.abs(base["poses"] - other["poses"]).max()))
     assert 10 * worst_chi2 <= G.CHI2_RTOL, worst_chi2
     assert 10 * worst_est <= G.EST_ATOL, worst_est
+
+
+def test_failed_factorisation_after_an_infinite_chi2_keeps_the_estimate():
+    """An infinite information entry on the first edge makes chi2 infinite and the system non-finite. The first trial fails
+    its factorisation yet passes the rho test (rho = +inf): it counts as accepted with chi2 DBL_MAX and leaves the estimate
+    as it was. The next iteration starts from that carried DBL_MAX, gets rho = 0 and terminates with NOT_PD."""
+    g = S.graph(seed=1, N=10)
+    i, j, m, info = g["edges"][0]
+    info = np.array(info, np.float32)
+    info[0, 0] = np.inf
+    g["edges"][0] = (i, j, m, info)
+    r = pyglobal.run(g, pyglobal.params(g["Tbc"]))
+    start = pyglobal.run(g, pyglobal.params(g["Tbc"], iterations=0))
+    big = np.finfo(np.float64).max
+    assert r["status"] == 2 and r["iterations"] == 2 and start["iterations"] == 0
+    assert [(int(s["trials"]), int(s["accepted"]), int(s["terminate"])) for s in r["stats"]] == [(1, 1, 0), (1, 0, 1)]
+    assert r["stats"]["chi2_before"].tolist() == [np.inf, big] and r["stats"]["chi2_after"].tolist() == [big, big]
+    assert np.array_equal(r["Tcw"], start["Tcw"]) and np.array_equal(r["poses"], start["poses"])

@@ -50,3 +50,20 @@ def test_oracle_spread_is_far_below_the_gpu_bounds():
             edge = (np.abs(a["chi2"] - b["chi2"]) / np.maximum(1.0, np.abs(b["chi2"]))).max()
             worst = np.maximum(worst, [chi, est, edge])
     assert worst[0] * 10 <= GPU_CHI2 and worst[1] * 10 <= GPU_EST and worst[2] * 10 <= GPU_EDGE, worst
+
+
+def test_failed_factorisation_after_an_infinite_chi2_keeps_the_estimate():
+    """A point on the free keyframe's camera plane makes chi2 infinite and the system non-finite. The first trial fails
+    its factorisation yet passes the rho test (rho = +inf): it counts as accepted with chi2 DBL_MAX and leaves the estimate
+    as it was. The next iteration starts from that carried DBL_MAX, gets rho = 0 and terminates with NOT_PD."""
+    prob, w = S.SCENES["one_free_kf"][0]()
+    k = int(np.flatnonzero(np.asarray(w.fixed) == 0)[0])
+    w.Tcw[k] = np.eye(4, dtype=np.float32).ravel()
+    w.xyz[w.edge_point[int(np.flatnonzero(np.asarray(w.edge_kf) == k)[0])]] = (1, 1, 0)
+    r = pyse3ba.run(w, S.window_params(prob), trace=True)
+    start = pyse3ba.run(w, S.window_params(prob, iterations=0))
+    big = np.finfo(np.float64).max
+    assert r["status"] == 2 and r["iterations"] == 2 and start["iterations"] == 0
+    assert decisions(r["stats"]) == [(1, 1, 0), (1, 0, 1)]
+    assert r["stats"]["chi2_before"].tolist() == [np.inf, big] and r["stats"]["chi2_after"].tolist() == [big, big]
+    assert np.array_equal(r["poses"], start["poses"]) and np.array_equal(r["points"], start["points"])
