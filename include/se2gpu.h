@@ -34,6 +34,9 @@
  *   se2gpu_track_triangulate[_device]  Track::doTriangulate                   src/Track.cpp:389-416
  *   se2gpu_xyz_info[_device]         Track::calcSE3toXYZInfo                  src/Track.cpp:259-306
  *   se2gpu_projection_observations[_device]  LocalMapper::findCorrespd, MatchByProjection branch  src/LocalMapper.cpp:119-141
+ *   se2gpu_mp_add_observations[_device]      MapPoint::addObservation   src/MapPoint.cpp:104-185, 228-292
+ *   se2gpu_mp_erase_observations[_device]    MapPoint::eraseObservation src/MapPoint.cpp:86-101
+ *   se2gpu_mp_update_measure[_device]        MapPoint::updateMeasureInKFs  src/MapPoint.cpp:294-305 (src/Map.cpp:779-780)
  *   se2gpu_remove_outliers[_device]  Track::removeOutliers (cv::findFundamentalMat)  src/Track.cpp:308-344
  *   se2gpu_pose_ba[_device]          Localizer::DoLocalBA (pose-only SE(3) BA, g2o LM)  src/Localizer.cpp:233-302,
  *                                    (addPlaneMotionSE3Expmap src/optimizer.cpp:236-314, EdgeSE3ExpmapPrior :159-189)
@@ -362,6 +365,87 @@ int se2gpu_projection_observations_device(const se2gpu_keypoint* d_kf_kp, int n_
                                           const float* d_mp_max_dist, const float* d_Tcw_table, const float* d_K, float lower_depth,
                                           float upper_depth, float fx, uint8_t* d_accept, float* d_pos_new_kf, double* d_info_new,
                                           void* stream);
+
+/* ------------------------------------------------------------------------------------------ map-point updates */
+/* MapPoint::addObservation (src/MapPoint.cpp:104-122, with updateMainKFandDescriptor :228-292 and updateParallax :124-185),
+ * MapPoint::eraseObservation (:86-101) and MapPoint::updateMeasureInKFs (:294-305) over many map points in one call,
+ * on the object graph flattened into the tables below (DESIGN.md section 13). Map points are independent: a point's
+ * updates touch its own table entries and the keyframe slots of its own observations only. The keyframe side
+ * (KeyFrame::addObservation / eraseObservation, and the erasure setNull makes there) is the caller's. */
+typedef struct se2gpu_mp_keyframes {
+    int n_kf;                    /* K */
+    const int* kf_id;            /* [K] mIdKF */
+    const uint8_t* kf_null;      /* [K] isNull() */
+    const float* Tcw;            /* [K*16] getPose(), row-major */
+    const int* kp_base;          /* [K] slot of each keyframe's keypoint 0 */
+    int n_slots;                 /* S */
+    const se2gpu_keypoint* kp;   /* [S] keyPointsUn[i].pt with keyPoints[i].octave */
+    const uint8_t* desc;         /* [S*32] descriptors */
+    float* view_mp;              /* [S*3] mViewMPs, in/out */
+    double* view_info;           /* [S*9] mViewMPsInfo, in/out */
+} se2gpu_mp_keyframes;
+
+/* The point table, in the layout se2gpu_match_by_projection_device (mp_desc, mp_octave) and
+ * se2gpu_projection_observations_device (mp_main_measure, mp_main_pose = main_kf, mp_main_octave, mp_normal, mp_min_dist,
+ * mp_max_dist) read. Point m observes obs_ptr[m] .. obs_ptr[m+1]-1 (obs_ptr[0] = 0): keyframe obs_kf[j], keypoint
+ * obs_idx[j] (slot kp_base[obs_kf[j]] + obs_idx[j]), in mObservations' own iteration order. */
+typedef struct se2gpu_mp_points {
+    int n_mp;                    /* M */
+    float* pos;                  /* [M*3] mPos */
+    uint8_t* good_prl;           /* [M] mbGoodParallax */
+    uint8_t* null;               /* [M] mbNull */
+    int* main_kf;                /* [M] keyframe index of mMainKF, -1 = NULL */
+    uint8_t* main_desc;          /* [M*32] mMainDescriptor */
+    int* main_octave;            /* [M] mMainOctave */
+    float* main_measure;         /* [M*2] getMainMeasure() */
+    float* level_scale;          /* [M] mLevelScaleFactor */
+    float* normal;               /* [M*3] mNormalVector */
+    float* min_dist;             /* [M] mMinDist */
+    float* max_dist;             /* [M] mMaxDist */
+    const int* obs_ptr;          /* [M+1] */
+    const int* obs_kf;           /* [obs_ptr[M]] */
+    const int* obs_idx;          /* [obs_ptr[M]] */
+} se2gpu_mp_points;
+
+#define SE2GPU_MP_MAX_LEVELS 32
+typedef struct se2gpu_mp_params {
+    float K[9];                  /* Config::Kcam, row-major */
+    float lower_depth, upper_depth; /* Config::LOWER_DEPTH / UPPER_DEPTH */
+    float fx;                    /* Config::fxCam */
+    int nlevels;                 /* mnScaleLevels, 1 .. SE2GPU_MP_MAX_LEVELS */
+    float scale_factors[SE2GPU_MP_MAX_LEVELS]; /* mvScaleFactors */
+} se2gpu_mp_params;
+
+/* addObservation for the updates of every point: point m inserts the entries at list positions upd_pos[upd_ptr[m]] ..
+ * upd_pos[upd_ptr[m+1]-1], in that order (upd_ptr [M+1], upd_ptr[0] = 0). A point's list is its list AFTER all of its
+ * insertions: while one update runs, the entries of its later updates are absent. Each update runs
+ * updateMainKFandDescriptor (null keyframes skipped; mMainOctave, mLevelScaleFactor and min/max distances kept when the main
+ * keyframe's mIdKF is unchanged), updateParallax (re-triangulation from the oldest observer within 6 keyframe ids, rewriting
+ * view_mp / view_info of every observer on success), the mNormalVector update and the final mbNull = false. abandoned [M]
+ * is set to 1 for a point updateParallax abandons (setNull) and to 0 otherwise; a later update of that point starts from
+ * an empty list. HOST buffers, synchronous; SE2GPU_ERR_INVALID, with nothing changed, for an index outside its table, an
+ * update position outside its point's list or repeated within it, or an octave outside nlevels. */
+int se2gpu_mp_add_observations(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* upd_ptr, const int* upd_pos,
+                               const se2gpu_mp_params* params, uint8_t* abandoned, int device);
+/* eraseObservation: the list given is the list BEFORE the call; the entry at upd_pos is absent once its update has run.
+ * A non-null point whose list becomes empty is setNull and reported in abandoned [M]; otherwise
+ * updateMainKFandDescriptor and the mNormalVector downdate run. Same rules as above. */
+int se2gpu_mp_erase_observations(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* upd_ptr, const int* upd_pos,
+                                 const se2gpu_mp_params* params, uint8_t* abandoned, int device);
+/* updateMeasureInKFs for the n points points[0 .. n-1] (after setPos: pos holds se2gpu_ba_get_f32's points):
+ * view_mp[slot] = se3map(Tcw, pos) for every observer that is not null. */
+int se2gpu_mp_update_measure(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, int n, const int* points, int device);
+/* The same on DEVICE buffers (the structs are host memory holding device pointers), asynchronous on `stream`. The
+ * input is checked on the device first: d_status [1] receives SE2GPU_OK, or SE2GPU_ERR_INVALID and then nothing else is
+ * written. */
+int se2gpu_mp_add_observations_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* d_upd_ptr,
+                                      const int* d_upd_pos, const se2gpu_mp_params* params, uint8_t* d_abandoned, int* d_status,
+                                      void* stream);
+int se2gpu_mp_erase_observations_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* d_upd_ptr,
+                                        const int* d_upd_pos, const se2gpu_mp_params* params, uint8_t* d_abandoned,
+                                        int* d_status, void* stream);
+int se2gpu_mp_update_measure_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, int n, const int* d_points,
+                                    int* d_status, void* stream);
 
 /* Test hook: the 4x4 Jacobi SVD behind cvu::triangulate (cv::SVD::compute, MODIFY_A|FULL_UV) on n row-major matrices
  * A [n*16]; w [n*4] singular values (descending), vt [n*16]. HOST buffers. */

@@ -50,6 +50,31 @@ class SE3BAParams(C.Structure):
                 ("chi2_cut", C.c_float)]
 
 
+vp_ = C.c_void_p
+
+
+class MpKeyframes(C.Structure):
+    """se2gpu_mp_keyframes"""
+    _fields_ = [("n_kf", C.c_int), ("kf_id", vp_), ("kf_null", vp_), ("Tcw", vp_), ("kp_base", vp_), ("n_slots", C.c_int),
+                ("kp", vp_), ("desc", vp_), ("view_mp", vp_), ("view_info", vp_)]
+
+
+class MpPoints(C.Structure):
+    """se2gpu_mp_points"""
+    _fields_ = [("n_mp", C.c_int), ("pos", vp_), ("good_prl", vp_), ("null", vp_), ("main_kf", vp_), ("main_desc", vp_),
+                ("main_octave", vp_), ("main_measure", vp_), ("level_scale", vp_), ("normal", vp_), ("min_dist", vp_),
+                ("max_dist", vp_), ("obs_ptr", vp_), ("obs_kf", vp_), ("obs_idx", vp_)]
+
+
+MP_MAX_LEVELS = 32   # SE2GPU_MP_MAX_LEVELS
+
+
+class MpParams(C.Structure):
+    """se2gpu_mp_params"""
+    _fields_ = [("K", C.c_float * 9), ("lower_depth", C.c_float), ("upper_depth", C.c_float), ("fx", C.c_float),
+                ("nlevels", C.c_int), ("scale_factors", C.c_float * MP_MAX_LEVELS)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -86,6 +111,8 @@ SYMBOLS = [
     "se2gpu_global_ba_update_points", "se2gpu_global_ba_update_points_device", "se2gpu_global_ba_profile",
     "se2gpu_global_ba_profile_read",
     "se2gpu_se3_ba_create", "se2gpu_se3_ba_destroy", "se2gpu_se3_ba", "se2gpu_se3_ba_device", "se2gpu_se3_ba_debug_trace",
+    "se2gpu_mp_add_observations", "se2gpu_mp_erase_observations", "se2gpu_mp_update_measure",
+    "se2gpu_mp_add_observations_device", "se2gpu_mp_erase_observations_device", "se2gpu_mp_update_measure_device",
 ]
 
 
@@ -213,6 +240,12 @@ def lib():
     L.se2gpu_se3_ba.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 14
     L.se2gpu_se3_ba_device.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 15
     L.se2gpu_se3_ba_debug_trace.argtypes = [vp, i, vp, vp, vp, i, vp, vp, vp, vp, i, vp, i] + [vp] * 13
+    L.se2gpu_mp_add_observations.argtypes = [vp] * 6 + [i]
+    L.se2gpu_mp_erase_observations.argtypes = [vp] * 6 + [i]
+    L.se2gpu_mp_update_measure.argtypes = [vp, vp, i, vp, i]
+    L.se2gpu_mp_add_observations_device.argtypes = [vp] * 8
+    L.se2gpu_mp_erase_observations_device.argtypes = [vp] * 8
+    L.se2gpu_mp_update_measure_device.argtypes = [vp, vp, i, vp, vp, vp]
     _lib = L
     return L
 

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "common.h"
+#include "median_desc.h"
 
 struct se2gpu_voc {
     int device = 0;
@@ -29,7 +30,6 @@ struct se2gpu_voc {
 namespace {
 
 using se2gpu::fail;
-using se2gpu::hamming256;
 
 // one warp per feature; root = node 0
 __global__ void __launch_bounds__(256) k_voc_transform(const uint32_t* __restrict__ feat, int n, const uint32_t* __restrict__ ndesc,
@@ -78,22 +78,12 @@ __global__ void __launch_bounds__(128) k_median_descriptor(const uint32_t* __res
     if (m >= M) return;
     const int p0 = ptr[m], N = ptr[m + 1] - p0;
     if (N <= 0) { if (threadIdx.x == 0) { best_idx[m] = -1; if (best_median) best_median[m] = INT_MAX; } return; }
-    for (int e = threadIdx.x; e < N * N; e += blockDim.x) {
-        const int i = e / N, j = e - i * N;
-        dist[e] = (unsigned short)(i == j ? 0 : hamming256(desc + 8 * (size_t)(p0 + i), desc + 8 * (size_t)(p0 + j)));
-    }
+    se2gpu::hamming_matrix(desc, [p0](int i) { return p0 + i; }, N, dist, threadIdx.x, blockDim.x);
     if (threadIdx.x == 0) s_best = INT_MAX;
     __syncthreads();
     const int kth = (int)(0.5 * (N - 1));          // vDists[0.5*(N-1)] after std::sort (MapPoint.cpp:263)
     for (int i = threadIdx.x; i < N; i += blockDim.x) {
-        const unsigned short* row = dist + (size_t)i * N;
-        int median = 0;
-        for (int j = 0; j < N; ++j) {
-            const int v = row[j];
-            int less = 0, leq = 0;
-            for (int t = 0; t < N; ++t) { less += row[t] < v; leq += row[t] <= v; }
-            if (less <= kth && kth < leq) { median = v; break; }
-        }
+        const int median = se2gpu::rank_select(dist + (size_t)i * N, N, kth);
         atomicMin(&s_best, (median << 16) | i);    // lexicographic (median, index): the first index of the least median (:264-267)
     }
     __syncthreads();

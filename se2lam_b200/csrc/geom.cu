@@ -1,14 +1,17 @@
 // Two-view geometry over matches: cvu::triangulate, Track::doTriangulate, Track::calcSE3toXYZInfo and the MatchByProjection
 // branch of LocalMapper::findCorrespd (DESIGN.md section 8). One thread per match; counts are reduced with warp ballots and
-// one atomic per warp.
+// one atomic per warp. Then the map-point updates MapPoint::addObservation / eraseObservation / updateMeasureInKFs
+// (DESIGN.md section 13): one warp per map point, no atomics.
 //
 // Every floating-point operation is written with an explicitly rounded intrinsic, in the order the reference and OpenCV
 // evaluate it on the host, so that the compiler cannot contract a multiply and an add the host keeps apart. The only fused
 // multiply-adds of the reference's arithmetic are the rows of A (cv::addWeighted's dispatched SIMD kernel on an AVX2 host).
 #include <cfloat>
 #include <cstdint>
+#include <type_traits>
 
 #include "common.h"
+#include "median_desc.h"
 
 using namespace se2gpu;
 
@@ -452,6 +455,423 @@ inline int blocks(int n) { return (n + kBlock - 1) / kBlock; }
 
 const float kMinCos[4] = {0.9998f, 0.9994f, 0.9986f, 0.9976f};   // cvu::checkParallax
 
+// ------------------------------------------------------------------------------------------ map-point updates (DESIGN.md section 13)
+// One warp per map point. A list of up to kMpCap entries keeps its descriptor distance matrix in the warp's shared memory;
+// a longer one recomputes distances row by row instead (the same median, found by bisection over the 257 distance values).
+constexpr int kMpWarps = 4;
+constexpr int kMpCap = 32;
+constexpr int kMpMaxList = (1 << 22) - 1;        // list positions share a 32-bit key with a median of at most 256
+constexpr unsigned kFull = 0xffffffffu;
+
+// Point m's list and updates are well-formed: every observation inside the keyframe and slot tables (with an octave below
+// nlevels when nlevels > 0), main_kf in [-1, K), and each update position inside the list and not repeated.
+__host__ __device__ inline bool mp_point_ok(const se2gpu_mp_keyframes& kf, const se2gpu_mp_points& mp, const int* upd_ptr,
+                                            const int* upd_pos, int nlevels, int m) {
+    const int p0 = mp.obs_ptr[m], p1 = mp.obs_ptr[m + 1];
+    if (p0 < 0 || p1 < p0 || p1 - p0 > kMpMaxList) return false;
+    for (int j = p0; j < p1; ++j) {
+        const int k = mp.obs_kf[j], idx = mp.obs_idx[j];
+        if (k < 0 || k >= kf.n_kf || idx < 0) return false;
+        const long long slot = (long long)kf.kp_base[k] + idx;
+        if (kf.kp_base[k] < 0 || slot >= kf.n_slots) return false;
+        if (nlevels > 0 && (kf.kp[slot].octave < 0 || kf.kp[slot].octave >= nlevels)) return false;
+    }
+    if (!upd_ptr) return true;
+    if (mp.main_kf[m] < -1 || mp.main_kf[m] >= kf.n_kf) return false;
+    const int u0 = upd_ptr[m], u1 = upd_ptr[m + 1];
+    if (u0 < 0 || u1 < u0) return false;
+    for (int u = u0; u < u1; ++u) {
+        if (upd_pos[u] < 0 || upd_pos[u] >= p1 - p0) return false;
+        for (int v = u0; v < u; ++v)
+            if (upd_pos[v] == upd_pos[u]) return false;
+    }
+    return true;
+}
+
+__global__ void __launch_bounds__(kBlock) k_mp_check(se2gpu_mp_keyframes kf, se2gpu_mp_points mp, const int* __restrict__ upd_ptr,
+                                                     const int* __restrict__ upd_pos, int nlevels, int n,
+                                                     const int* __restrict__ points, int* __restrict__ status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0 && (mp.obs_ptr[0] != 0 || (upd_ptr && upd_ptr[0] != 0))) *status = SE2GPU_ERR_INVALID;
+    if (i >= n) return;
+    const int m = points ? points[i] : i;
+    if (m < 0 || m >= mp.n_mp || !mp_point_ok(kf, mp, upd_ptr, upd_pos, nlevels, m)) *status = SE2GPU_ERR_INVALID;
+}
+
+// Which list positions of a point are present while its update u runs. add: the list given is the list after every
+// insertion, so the positions of later updates are absent, and after an abandonment (setNull at update `clear`) only the
+// insertions since then are present. erase: the list given is the list before the call, so every position erased so far
+// (this update's included) is absent.
+struct MpList {
+    const int* pos;
+    int u0, u1, u, clear;
+    bool add;
+    __device__ __forceinline__ bool has(int j) const {
+        if (!add) {
+            for (int v = u0; v <= u; ++v)
+                if (pos[v] == j) return false;
+            return true;
+        }
+        for (int v = u + 1; v < u1; ++v)
+            if (pos[v] == j) return false;
+        if (clear < 0) return true;
+        for (int v = clear + 1; v <= u; ++v)
+            if (pos[v] == j) return true;
+        return false;
+    }
+};
+
+__device__ __forceinline__ int mp_slot(const se2gpu_mp_keyframes& kf, const se2gpu_mp_points& mp, int j) {
+    return kf.kp_base[mp.obs_kf[j]] + mp.obs_idx[j];
+}
+
+// number of present entries of a list of L (warp-uniform)
+__device__ int mp_count(const MpList& ls, int L, int lane) {
+    int n = 0;
+    for (int j0 = 0; j0 < L; j0 += 32) n += __popc(__ballot_sync(kFull, j0 + lane < L && ls.has(j0 + lane)));
+    return n;
+}
+
+// p = o * (1.f / cv::norm(o)): the float / double quotient is a double, and Point3f * double rounds each product once
+__device__ __forceinline__ F3 mp_unit(F3 o) {
+    const double s = dd(1.0, norm3(o));
+    return {__double2float_rn(dm((double)o.x, s)), __double2float_rn(dm((double)o.y, s)), __double2float_rn(dm((double)o.z, s))};
+}
+
+// Rcw^T * M * Rcw as the float MatExpr evaluates it: cv::gemm(R, M, GEMM_1_T) (double sums), then (...) * R (small path).
+// T is the 4x4 pose, M a row-major 3x3.
+__device__ __forceinline__ void rt_m_r(const float* T, const float* M, float* out) {
+    float tmp[9];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            double s = 0;
+#pragma unroll
+            for (int q = 0; q < 3; q++) s = da(s, dm((double)T[q * 4 + i], (double)M[q * 3 + j]));
+            tmp[i * 3 + j] = __double2float_rn(dm(s, 1.0));
+        }
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) out[i * 3 + j] = gemm3_elem(tmp, 3, i, T, 4, j, 1.0);
+}
+
+// Rcw * M * Rcw^T: R * M (small path), then cv::gemm(..., R, GEMM_2_T) (double sums)
+__device__ __forceinline__ void r_m_rt(const float* T, const float* M, float* out) {
+    float tmp[9];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) tmp[i * 3 + j] = gemm3_elem(T, 4, i, M, 3, j, 1.0);
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            double s = 0;
+#pragma unroll
+            for (int q = 0; q < 3; q++) s = da(s, dm((double)tmp[i * 3 + q], (double)T[j * 4 + q]));
+            out[i * 3 + j] = __double2float_rn(dm(s, 1.0));
+        }
+}
+
+// Per-warp shared memory of the short-list median: the distance matrix and the compacted slots / list positions
+struct MpShared {
+    unsigned short dist[kMpCap * kMpCap];
+    int slot[kMpCap], pos[kMpCap];
+};
+
+// MapPoint::updateMainKFandDescriptor (MapPoint.cpp:228-292) over the present entries of point m's list
+__device__ void mp_update_main(const se2gpu_mp_keyframes& kf, const se2gpu_mp_points& mp, const se2gpu_mp_params& prm, int m,
+                               int p0, int L, const MpList& ls, MpShared& sh, int lane) {
+    if (mp.null[m]) return;
+    const uint32_t* desc = reinterpret_cast<const uint32_t*>(kf.desc);
+    auto valid = [&](int j) { return ls.has(j) && !kf.kf_null[mp.obs_kf[p0 + j]]; };
+    int key = INT_MAX;
+    if (L <= kMpCap) {
+        const bool v = lane < L && valid(lane);
+        const unsigned b = __ballot_sync(kFull, v);
+        const int N = __popc(b);
+        if (N == 0) return;
+        if (v) {
+            const int c = __popc(b & ((1u << lane) - 1));
+            sh.slot[c] = mp_slot(kf, mp, p0 + lane);
+            sh.pos[c] = lane;
+        }
+        __syncwarp();
+        hamming_matrix(desc, [&sh](int i) { return sh.slot[i]; }, N, sh.dist, lane, 32);
+        __syncwarp();
+        const int kth = (int)(0.5 * (N - 1));
+        if (lane < N) key = (rank_select(sh.dist + lane * N, N, kth) << 22) | sh.pos[lane];
+        __syncwarp();
+    } else {
+        int N = 0;
+        for (int j0 = 0; j0 < L; j0 += 32) N += __popc(__ballot_sync(kFull, j0 + lane < L && valid(j0 + lane)));
+        if (N == 0) return;
+        const int kth = (int)(0.5 * (N - 1));
+        for (int j = 0; j < L; ++j) {
+            if (!valid(j)) continue;
+            const uint32_t* dj = desc + 8 * (size_t)mp_slot(kf, mp, p0 + j);
+            int lo = 0, hi = 256;                  // the least v with more than kth distances <= v
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                int c = 0;
+                for (int t = lane; t < L; t += 32)
+                    if (valid(t)) c += (t == j ? 0 : hamming256(dj, desc + 8 * (size_t)mp_slot(kf, mp, p0 + t))) <= mid;
+                c = __reduce_add_sync(kFull, c);
+                if (c > kth) hi = mid; else lo = mid + 1;
+            }
+            key = min(key, (lo << 22) | j);
+        }
+    }
+    // lexicographic (median, position): the first entry of the least median (:264-267)
+    const int jb = __reduce_min_sync(kFull, key) & kMpMaxList;
+    const int k = mp.obs_kf[p0 + jb], slot = mp_slot(kf, mp, p0 + jb);
+    if (lane < 8) reinterpret_cast<uint32_t*>(mp.main_desc)[8 * (size_t)m + lane] = desc[8 * (size_t)slot + lane];
+    if (lane == 0) {
+        const se2gpu_keypoint p = kf.kp[slot];
+        mp.main_measure[2 * m] = p.x; mp.main_measure[2 * m + 1] = p.y;
+        const int cur = mp.main_kf[m];
+        if (!(cur >= 0 && kf.kf_id[cur] == kf.kf_id[k])) {
+            mp.main_kf[m] = k;
+            mp.main_octave[m] = p.octave;
+            const float scale = prm.scale_factors[p.octave];
+            mp.level_scale[m] = scale;
+            const float dist = __double2float_rn(norm3({kf.view_mp[3 * slot], kf.view_mp[3 * slot + 1], kf.view_mp[3 * slot + 2]}));
+            const float mx = fm(dist, scale);
+            mp.max_dist[m] = mx;
+            mp.min_dist[m] = fd(mx, prm.scale_factors[prm.nlevels - 1]);
+        }
+    }
+    __syncwarp();
+}
+
+// MapPoint::updateParallax(pKF) (MapPoint.cpp:124-185) for the entry at list position q; `size` is the present count.
+// Returns true when it abandons the point.
+__device__ bool mp_update_parallax(const se2gpu_mp_keyframes& kf, const se2gpu_mp_points& mp, const se2gpu_mp_params& prm, int m,
+                                   int p0, int L, const MpList& ls, int q, int size, int lane) {
+    if (mp.good_prl[m] || size <= 2) return false;
+    // pKF0: the least mIdKF among the observers at most 6 ids older than pKF (null keyframes included), first entry on ties
+    const int idn = kf.kf_id[mp.obs_kf[p0 + q]];
+    int best_id = INT_MAX, best_j = INT_MAX;
+    for (int j = lane; j < L; j += 32) {
+        const int id = kf.kf_id[mp.obs_kf[p0 + j]];
+        if (ls.has(j) && idn - id <= 6 && id < best_id) { best_id = id; best_j = j; }
+    }
+    const int id0 = __reduce_min_sync(kFull, best_id);
+    const int j0 = (int)__reduce_min_sync(kFull, (unsigned)(best_id == id0 ? best_j : INT_MAX));
+    const int k0 = mp.obs_kf[p0 + j0], k1 = mp.obs_kf[p0 + q];
+    const int s0 = mp_slot(kf, mp, p0 + j0), s1 = mp_slot(kf, mp, p0 + q);
+    bool ok = false;
+    F3 posW = {0.f, 0.f, 0.f};
+    float W[9];
+    if (lane == 0) {
+        float T0[16], T1[16], K[9], P0[12], P1[12];
+#pragma unroll
+        for (int i = 0; i < 16; i++) { T0[i] = kf.Tcw[16 * k0 + i]; T1[i] = kf.Tcw[16 * k1 + i]; }
+#pragma unroll
+        for (int i = 0; i < 9; i++) K[i] = prm.K[i];
+        projection(K, T0, P0);
+        projection(K, T1, P1);
+        const se2gpu_keypoint a = kf.kp[s0], b = kf.kp[s1];
+        posW = triangulate(a.x, a.y, b.x, b.y, P0, P1);
+        const F3 pos0 = se3map(T0, posW), pos1 = se3map(T1, posW);
+        if (pos0.z >= prm.lower_depth && pos0.z <= prm.upper_depth && pos1.z >= prm.lower_depth && pos1.z <= prm.upper_depth) {
+            float Ti0[16], Ti1[16];
+            inv4(T0, Ti0);
+            inv4(T1, Ti1);
+            const F3 v0 = sub3(posW, {Ti0[3], Ti0[7], Ti0[11]}), v1 = sub3(posW, {Ti1[3], Ti1[7], Ti1[11]});
+            const float cosp = __double2float_rn(dd(fabs((double)dot3(v0, v1)), dm(norm3(v0), norm3(v1))));
+            ok = cosp < 0.9994f;                 // checkParallax(..., 2)
+            if (ok) {
+                mp.pos[3 * m] = posW.x; mp.pos[3 * m + 1] = posW.y; mp.pos[3 * m + 2] = posW.z;
+                mp.good_prl[m] = 1;
+                double info0[9], info1[9];
+                xyz_info(pos0, T0, T1, prm.fx, info0, info1);
+                const F3 pv[2] = {pos0, pos1};
+                const double* iv[2] = {info0, info1};
+                const int sv[2] = {s0, s1};
+                for (int v = 0; v < 2; v++) {      // setViewMP of pKF0, then of pKF (the same slot when pKF0 == pKF)
+                    kf.view_mp[3 * sv[v]] = pv[v].x; kf.view_mp[3 * sv[v] + 1] = pv[v].y; kf.view_mp[3 * sv[v] + 2] = pv[v].z;
+#pragma unroll
+                    for (int e = 0; e < 9; e++) kf.view_info[9 * sv[v] + e] = iv[v][e];
+                }
+                float M0[9];
+#pragma unroll
+                for (int e = 0; e < 9; e++) M0[e] = (float)info0[e];    // toCvMat(Matrix3d): the float values, exactly
+                rt_m_r(T0, M0, W);
+            }
+        }
+    }
+    ok = __shfl_sync(kFull, ok, 0);
+    if (ok) {
+        posW = {__shfl_sync(kFull, posW.x, 0), __shfl_sync(kFull, posW.y, 0), __shfl_sync(kFull, posW.z, 0)};
+#pragma unroll
+        for (int e = 0; e < 9; e++) W[e] = __shfl_sync(kFull, W[e], 0);
+        const int id1 = kf.kf_id[k1];
+        for (int j = lane; j < L; j += 32) {       // the other observers
+            const int k = mp.obs_kf[p0 + j], id = kf.kf_id[k];
+            if (!ls.has(j) || id == id1 || id == id0) continue;
+            float Tk[16], Wk[9];
+#pragma unroll
+            for (int i = 0; i < 16; i++) Tk[i] = kf.Tcw[16 * k + i];
+            const F3 pk = se3map(Tk, posW);
+            r_m_rt(Tk, W, Wk);
+            const int s = mp_slot(kf, mp, p0 + j);
+            kf.view_mp[3 * s] = pk.x; kf.view_mp[3 * s + 1] = pk.y; kf.view_mp[3 * s + 2] = pk.z;
+#pragma unroll
+            for (int e = 0; e < 9; e++) kf.view_info[9 * s + e] = (double)Wk[e];
+        }
+    }
+    __syncwarp();
+    if (idn - id0 >= 6 && !ok) {                   // setNull (the point's own side)
+        if (lane == 0) { mp.null[m] = 1; mp.good_prl[m] = 0; }
+        __syncwarp();
+        return true;
+    }
+    return false;
+}
+
+__global__ void __launch_bounds__(kMpWarps * 32) k_mp_add(se2gpu_mp_keyframes kf, se2gpu_mp_points mp, const int* __restrict__ upd_ptr,
+                                                          const int* __restrict__ upd_pos, se2gpu_mp_params prm,
+                                                          uint8_t* __restrict__ abandoned, const int* __restrict__ status) {
+    __shared__ MpShared sh[kMpWarps];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, m = blockIdx.x * kMpWarps + w;
+    if (m >= mp.n_mp || *status) return;
+    const int p0 = mp.obs_ptr[m], L = mp.obs_ptr[m + 1] - p0;
+    MpList ls{upd_pos, upd_ptr[m], upd_ptr[m + 1], 0, -1, true};
+    bool gone = false;
+    for (int u = ls.u0; u < ls.u1; ++u) {
+        ls.u = u;
+        const int q = upd_pos[u];
+        const int size = mp_count(ls, L, lane);
+        mp_update_main(kf, mp, prm, m, p0, L, ls, sh[w], lane);
+        if (mp_update_parallax(kf, mp, prm, m, p0, L, ls, q, size, lane)) { gone = true; ls.clear = u; }
+        if (lane == 0) {                           // MapPoint.cpp:115-121, with the list size before the insert
+            const int s = mp_slot(kf, mp, p0 + q);
+            const F3 nn = mp_unit({kf.view_mp[3 * s], kf.view_mp[3 * s + 1], kf.view_mp[3 * s + 2]});
+            const float old = (float)(size - 1), f = fd(1.f, (float)size);
+            float* n = mp.normal + 3 * m;
+            n[0] = fm(fa(fm(n[0], old), nn.x), f);
+            n[1] = fm(fa(fm(n[1], old), nn.y), f);
+            n[2] = fm(fa(fm(n[2], old), nn.z), f);
+            mp.null[m] = 0;
+        }
+        __syncwarp();
+    }
+    if (lane == 0) abandoned[m] = gone;
+}
+
+__global__ void __launch_bounds__(kMpWarps * 32) k_mp_erase(se2gpu_mp_keyframes kf, se2gpu_mp_points mp, const int* __restrict__ upd_ptr,
+                                                            const int* __restrict__ upd_pos, se2gpu_mp_params prm,
+                                                            uint8_t* __restrict__ abandoned, const int* __restrict__ status) {
+    __shared__ MpShared sh[kMpWarps];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, m = blockIdx.x * kMpWarps + w;
+    if (m >= mp.n_mp || *status) return;
+    const int p0 = mp.obs_ptr[m], L = mp.obs_ptr[m + 1] - p0;
+    MpList ls{upd_pos, upd_ptr[m], upd_ptr[m + 1], 0, -1, false};
+    bool gone = false;
+    for (int u = ls.u0; u < ls.u1; ++u) {
+        ls.u = u;
+        const int s = mp_slot(kf, mp, p0 + upd_pos[u]);
+        const F3 np = mp_unit({kf.view_mp[3 * s], kf.view_mp[3 * s + 1], kf.view_mp[3 * s + 2]});   // before the erase
+        const int size = mp_count(ls, L, lane);
+        if (!mp.null[m] && size == 0) {            // setNull
+            if (lane == 0) { mp.null[m] = 1; mp.good_prl[m] = 0; }
+            gone = true;
+        } else {
+            mp_update_main(kf, mp, prm, m, p0, L, ls, sh[w], lane);
+            if (lane == 0) {
+                const float up = (float)(size + 1), f = fd(1.f, (float)size);
+                float* n = mp.normal + 3 * m;
+                n[0] = fm(fs(fm(n[0], up), np.x), f);
+                n[1] = fm(fs(fm(n[1], up), np.y), f);
+                n[2] = fm(fs(fm(n[2], up), np.z), f);
+            }
+        }
+        __syncwarp();
+    }
+    if (lane == 0) abandoned[m] = gone;
+}
+
+__global__ void __launch_bounds__(kMpWarps * 32) k_mp_update_measure(se2gpu_mp_keyframes kf, se2gpu_mp_points mp, int n,
+                                                                     const int* __restrict__ points, const int* __restrict__ status) {
+    const int i = blockIdx.x * kMpWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (i >= n || *status) return;
+    const int m = points[i];
+    const F3 pos = {mp.pos[3 * m], mp.pos[3 * m + 1], mp.pos[3 * m + 2]};
+    for (int j = mp.obs_ptr[m] + lane; j < mp.obs_ptr[m + 1]; j += 32) {
+        const int k = mp.obs_kf[j];
+        if (kf.kf_null[k]) continue;
+        float T[16];
+#pragma unroll
+        for (int e = 0; e < 16; e++) T[e] = kf.Tcw[16 * k + e];
+        const F3 p = se3map(T, pos);
+        const int s = mp_slot(kf, mp, j);
+        kf.view_mp[3 * s] = p.x; kf.view_mp[3 * s + 1] = p.y; kf.view_mp[3 * s + 2] = p.z;
+    }
+}
+
+bool mp_tables_set(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, bool updates) {
+    if (!kf || !mp || kf->n_kf < 0 || kf->n_slots < 0 || mp->n_mp < 0 || !mp->obs_ptr) return false;
+    if (kf->n_kf && (!kf->kf_id || !kf->kf_null || !kf->Tcw || !kf->kp_base)) return false;
+    if (kf->n_slots && (!kf->view_mp || (updates && (!kf->kp || !kf->desc || !kf->view_info)))) return false;
+    if (mp->n_mp && (!mp->pos || (updates && (!mp->good_prl || !mp->null || !mp->main_kf || !mp->main_desc || !mp->main_octave ||
+                                              !mp->main_measure || !mp->level_scale || !mp->normal || !mp->min_dist || !mp->max_dist))))
+        return false;
+    return true;
+}
+
+int mp_updates_device(bool add, const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* d_upd_ptr,
+                      const int* d_upd_pos, const se2gpu_mp_params* prm, uint8_t* d_abandoned, int* d_status, void* stream) {
+    if (!mp_tables_set(kf, mp, true) || !prm || !d_status || !d_upd_ptr || (mp->n_mp && (!d_upd_pos || !d_abandoned)))
+        return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (prm->nlevels < 1 || prm->nlevels > SE2GPU_MP_MAX_LEVELS) return fail(SE2GPU_ERR_INVALID, "nlevels out of range");
+    { const int rc = require_device(); if (rc) return rc; }
+    cudaStream_t s = (cudaStream_t)stream;
+    SE2_CUDA(cudaMemsetAsync(d_status, 0, sizeof(int), s));
+    SE2_LAUNCH(k_mp_check, blocks(std::max(mp->n_mp, 1)), kBlock, 0, s, *kf, *mp, d_upd_ptr, d_upd_pos, prm->nlevels, mp->n_mp,
+               nullptr, d_status);
+    if (mp->n_mp) {
+        const int grid = (mp->n_mp + kMpWarps - 1) / kMpWarps;
+        if (add) SE2_LAUNCH(k_mp_add, grid, kMpWarps * 32, 0, s, *kf, *mp, d_upd_ptr, d_upd_pos, *prm, d_abandoned, d_status);
+        else SE2_LAUNCH(k_mp_erase, grid, kMpWarps * 32, 0, s, *kf, *mp, d_upd_ptr, d_upd_pos, *prm, d_abandoned, d_status);
+    }
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+// Host form of both updates: the same checks on the host, then every table through the stage
+int mp_updates_host(bool add, const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* upd_ptr, const int* upd_pos,
+                    const se2gpu_mp_params* prm, uint8_t* abandoned, int device) {
+    if (!mp_tables_set(kf, mp, true) || !prm || !upd_ptr || (mp->n_mp && !abandoned)) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (prm->nlevels < 1 || prm->nlevels > SE2GPU_MP_MAX_LEVELS) return fail(SE2GPU_ERR_INVALID, "nlevels out of range");
+    const int M = mp->n_mp;
+    if (mp->obs_ptr[0] != 0 || upd_ptr[0] != 0) return fail(SE2GPU_ERR_INVALID, "obs_ptr[0] and upd_ptr[0] must be 0");
+    if (M && upd_ptr[M] > 0 && !upd_pos) return fail(SE2GPU_ERR_INVALID, "null upd_pos");
+    for (int m = 0; m < M; ++m)
+        if (!mp_point_ok(*kf, *mp, upd_ptr, upd_pos, prm->nlevels, m)) return fail(SE2GPU_ERR_INVALID, "map point %d: index out of range or repeated update", m);
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
+    if (M == 0) return SE2GPU_OK;
+    const size_t K = kf->n_kf, S = kf->n_slots, nobs = mp->obs_ptr[M], nupd = upd_ptr[M];
+    auto up = [&](auto* p, size_t n) { using T = std::remove_cv_t<std::remove_pointer_t<decltype(p)>>; return n ? st.upload(p, n) : st.scratch<T>(1); };
+    auto io = [&](auto* p, size_t n) { using T = std::remove_pointer_t<decltype(p)>; return n ? st.inout(p, n) : st.scratch<T>(1); };
+    se2gpu_mp_keyframes dk{kf->n_kf, up(kf->kf_id, K), up(kf->kf_null, K), up(kf->Tcw, 16 * K), up(kf->kp_base, K), kf->n_slots,
+                           up(kf->kp, S), up(kf->desc, 32 * S), io(kf->view_mp, 3 * S), io(kf->view_info, 9 * S)};
+    se2gpu_mp_points dm{M, io(mp->pos, 3 * (size_t)M), io(mp->good_prl, M), io(mp->null, M), io(mp->main_kf, M),
+                        io(mp->main_desc, 32 * (size_t)M), io(mp->main_octave, M), io(mp->main_measure, 2 * (size_t)M),
+                        io(mp->level_scale, M), io(mp->normal, 3 * (size_t)M), io(mp->min_dist, M), io(mp->max_dist, M),
+                        up(mp->obs_ptr, (size_t)M + 1), up(mp->obs_kf, nobs), up(mp->obs_idx, nobs)};
+    const int* d_ptr = up(upd_ptr, (size_t)M + 1);
+    const int* d_pos = up(upd_pos, nupd);
+    uint8_t* d_ab = st.output(abandoned, M);
+    int* d_status = st.scratch<int>(1);
+    if (const int rc = st.status()) return rc;
+    { const int rc = mp_updates_device(add, &dk, &dm, d_ptr, d_pos, prm, d_ab, d_status, nullptr); if (rc) return rc; }
+    return st.finish();
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------ device-buffer entries
@@ -634,5 +1054,67 @@ int se2gpu_debug_svd4(int n, const float* A, float* w, float* vt, int device) {
     if (const int rc = st.status()) return rc;
     SE2_LAUNCH(k_debug_svd4, blocks(n), kBlock, 0, (cudaStream_t)0, n, dA, dw, dv);
     st.check(cudaGetLastError(), "kernel launch");
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ map-point updates
+int se2gpu_mp_add_observations(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* upd_ptr, const int* upd_pos,
+                               const se2gpu_mp_params* params, uint8_t* abandoned, int device) {
+    return mp_updates_host(true, kf, mp, upd_ptr, upd_pos, params, abandoned, device);
+}
+
+int se2gpu_mp_erase_observations(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* upd_ptr, const int* upd_pos,
+                                 const se2gpu_mp_params* params, uint8_t* abandoned, int device) {
+    return mp_updates_host(false, kf, mp, upd_ptr, upd_pos, params, abandoned, device);
+}
+
+int se2gpu_mp_add_observations_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* d_upd_ptr,
+                                      const int* d_upd_pos, const se2gpu_mp_params* params, uint8_t* d_abandoned, int* d_status,
+                                      void* stream) {
+    return mp_updates_device(true, kf, mp, d_upd_ptr, d_upd_pos, params, d_abandoned, d_status, stream);
+}
+
+int se2gpu_mp_erase_observations_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, const int* d_upd_ptr,
+                                        const int* d_upd_pos, const se2gpu_mp_params* params, uint8_t* d_abandoned,
+                                        int* d_status, void* stream) {
+    return mp_updates_device(false, kf, mp, d_upd_ptr, d_upd_pos, params, d_abandoned, d_status, stream);
+}
+
+int se2gpu_mp_update_measure_device(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, int n, const int* d_points,
+                                    int* d_status, void* stream) {
+    if (!mp_tables_set(kf, mp, false) || n < 0 || !d_status || (n && !d_points)) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    { const int rc = require_device(); if (rc) return rc; }
+    cudaStream_t s = (cudaStream_t)stream;
+    SE2_CUDA(cudaMemsetAsync(d_status, 0, sizeof(int), s));
+    SE2_LAUNCH(k_mp_check, blocks(std::max(n, 1)), kBlock, 0, s, *kf, *mp, nullptr, nullptr, 0, n, d_points, d_status);
+    if (n) SE2_LAUNCH(k_mp_update_measure, (n + kMpWarps - 1) / kMpWarps, kMpWarps * 32, 0, s, *kf, *mp, n, d_points, d_status);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+
+int se2gpu_mp_update_measure(const se2gpu_mp_keyframes* kf, const se2gpu_mp_points* mp, int n, const int* points, int device) {
+    if (!mp_tables_set(kf, mp, false) || n < 0 || (n && !points)) return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    const int M = mp->n_mp;
+    if (mp->obs_ptr[0] != 0) return fail(SE2GPU_ERR_INVALID, "obs_ptr[0] must be 0");
+    for (int i = 0; i < n; ++i)
+        if (points[i] < 0 || points[i] >= M || !mp_point_ok(*kf, *mp, nullptr, nullptr, 0, points[i]))
+            return fail(SE2GPU_ERR_INVALID, "points[%d]: index out of range", i);
+    HostStage st(device);
+    if (const int rc = st.status()) return rc;
+    if (n == 0) return SE2GPU_OK;
+    const size_t K = kf->n_kf, S = kf->n_slots, nobs = mp->obs_ptr[M];
+    auto up = [&](auto* p, size_t c) { using T = std::remove_cv_t<std::remove_pointer_t<decltype(p)>>; return c ? st.upload(p, c) : st.scratch<T>(1); };
+    se2gpu_mp_keyframes dk{kf->n_kf, up(kf->kf_id, K), up(kf->kf_null, K), up(kf->Tcw, 16 * K), up(kf->kp_base, K), kf->n_slots,
+                           nullptr, nullptr, S ? st.inout(kf->view_mp, 3 * S) : st.scratch<float>(1), nullptr};
+    se2gpu_mp_points dm{};
+    dm.n_mp = M;
+    dm.pos = st.upload(mp->pos, 3 * (size_t)M);
+    dm.obs_ptr = up(mp->obs_ptr, (size_t)M + 1);
+    dm.obs_kf = up(mp->obs_kf, nobs);
+    dm.obs_idx = up(mp->obs_idx, nobs);
+    const int* d_points = up(points, n);
+    int* d_status = st.scratch<int>(1);
+    if (const int rc = st.status()) return rc;
+    { const int rc = se2gpu_mp_update_measure_device(&dk, &dm, n, d_points, d_status, nullptr); if (rc) return rc; }
     return st.finish();
 }

@@ -1,0 +1,51 @@
+"""Scenes for the map-point update tests (tests/test_mappoint_oracle.py, tests/test_mappoint_gpu.py): seeded scenes whose
+mix reaches every branch of addObservation / eraseObservation, and the single-point cases built for one branch each."""
+import numpy as np
+
+from tools import mappoint_scenes as ms
+
+# branch events of oracle/mappoint_numpy.py each scene family must reach
+ADD_EVENTS = {"short_list", "already_good", "pkf0_older", "pkf0_self", "observer_beyond_6", "depth_below", "depth_above",
+              "parallax_rejected", "triangulated", "abandoned", "null_reset", "main_unchanged", "main_changed",
+              "null_kf_skipped", "median_tie", "two_adds"}
+ERASE_EVENTS = {"erased_to_empty", "erase_main_changed", "main_unchanged", "null_kf_skipped"}
+
+
+def add_scenes():
+    """(name, scene) pairs of the add family: plain, no good parallax, many null keyframes and points, short lists"""
+    return [("mixed", ms.scene(300, seed=101)),
+            ("no_good_prl", ms.scene(300, seed=102, good_frac=0.0)),
+            ("null_heavy", ms.scene(200, seed=103, null_frac=0.3)),
+            ("short", ms.scene(200, seed=104, lengths=np.arange(200) % 3 + 1))]
+
+
+def erase_scenes():
+    return [("mixed", ms.scene(300, seed=201, mode="erase")),
+            ("short", ms.scene(200, seed=202, mode="erase", lengths=np.arange(200) % 3 + 1, n_upd=(0.2, 0.4, 0.4)))]
+
+
+def long_scene(mode="add"):
+    """every list at or past the 32-entry shared-memory list: 32, 33 and the long lengths"""
+    lengths = np.array([32, 33, 40, 47, 64, 97] * 6)
+    return ms.scene(len(lengths), seed=301 if mode == "add" else 302, lengths=lengths, mode=mode, good_frac=0.0)
+
+
+def split_updates(sc):
+    """the scene's two-update points as two calls: the first with the list before the second insertion and only the first
+    update, the second with the full list and only the second update. Returns (first, second) update sets and the lists
+    of the first call: (obs_ptr, obs_kf, obs_idx, upd_ptr, upd_pos) twice."""
+    mp, up, pos = sc["mp"], sc["upd_ptr"], sc["upd_pos"]
+    M = len(mp["obs_ptr"]) - 1
+    ptr1, kf1, idx1, u1p, u1 = [0], [], [], [0], []
+    u2p, u2 = [0], []
+    for m in range(M):
+        a, b = mp["obs_ptr"][m], mp["obs_ptr"][m + 1]
+        ups = list(pos[up[m]:up[m + 1]])
+        last = ups[-1] if len(ups) == 2 else None
+        keep = [j for j in range(b - a) if j != last]
+        kf1 += list(mp["obs_kf"][a:b][keep]); idx1 += list(mp["obs_idx"][a:b][keep]); ptr1.append(len(kf1))
+        first = [keep.index(q) for q in ups[:1 if last is not None else len(ups)]]
+        u1 += first; u1p.append(len(u1))
+        u2 += [last] if last is not None else []; u2p.append(len(u2))
+    i4 = lambda x: np.asarray(x, np.int32)
+    return (i4(ptr1), i4(kf1), i4(idx1), i4(u1p), i4(u1)), (i4(u2p), i4(u2))
