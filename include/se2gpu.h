@@ -339,6 +339,18 @@ int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, co
                                     const float* d_K, float lower_depth, float upper_depth, int min_parallax_deg,
                                     float* d_local_mps, uint8_t* d_good_prl, int* d_counts, void* stream);
 
+/* The same for B independent streams in one launch: stream b reads d_kp_kf + b*cap (d_n[b] keypoints, d_n may be NULL: cap),
+ * d_kp_frame + b*cap_frame, d_kf_observed + b*cap, d_kf_view_mp + 3*b*cap and d_Tcr + 16*b, and updates d_matches12 + b*cap,
+ * d_local_mps + 3*b*cap, d_good_prl + b*cap and d_counts[2b], d_counts[2b+1]. d_gate [B] (may be NULL: every stream runs) is
+ * the nMinFrames test: a stream with d_gate[b] == 0 returns at once and leaves its matches, local map points and flags as
+ * they were (its counts are 0). Stream b's outputs are the bytes se2gpu_track_triangulate_device makes for it alone;
+ * that call is this one with B = 1. B > 65535: SE2GPU_ERR_CAPACITY. */
+int se2gpu_track_triangulate_batch_device(int B, const se2gpu_keypoint* d_kp_kf, int cap, const int* d_n, const se2gpu_keypoint* d_kp_frame,
+                                          int cap_frame, int* d_matches12, const uint8_t* d_kf_observed, const float* d_kf_view_mp,
+                                          const float* d_Tcr, const int* d_gate, const float* d_K, float lower_depth,
+                                          float upper_depth, int min_parallax_deg, float* d_local_mps, uint8_t* d_good_prl,
+                                          int* d_counts, void* stream);
+
 /* Track::calcSE3toXYZInfo (src/Track.cpp:259-306) for n points: calcSE3toXYZInfo(xyz1[i], Tcw[pose1[i]], Tcw[pose2[i]]),
  * Tcw [n_pose*16], fx = Config::fxCam. info1/info2 [n*9] are the float matrices widened to double (toMatrix3d). */
 int se2gpu_xyz_info(int n, const float* xyz1, const int* pose1, const int* pose2, const float* Tcw, int n_pose, float fx,
@@ -474,6 +486,104 @@ int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const
  * and se2gpu_fundam_debug_niters evaluates the device lookup for ep = (n[i] - good[i]) / n[i] (HOST buffers). */
 void se2gpu_fundam_niters_table(double* thresholds);
 int se2gpu_fundam_debug_niters(int count, const int* n, const int* good, const int* max_iters, int* out, int device);
+
+/* ------------------------------------------------------------------------------------------ tracking */
+/* Track::mTrack (reference src/Track.cpp:124-160) for up to max_streams independent camera streams, with the tracking state
+ * (reference frame, mPrevMatched, mMatchIdx, mLocalMPs, mvbGoodPrl / mnGoodPrl, preSE2) kept on the device between calls
+ * (DESIGN.md section 14). One se2gpu_tracker_step takes one frame per stream and runs, per stream and in the reference's
+ * order, the extraction with the undistortion folded in, MatchByWindow(mRefFrame, mFrame, mPrevMatched, 20, mMatchIdx)
+ * with nnratio 0.9, removeOutliers, updateFramePose with the pre-integration, doTriangulate (gated by nMinFrames) and
+ * needNewKF. A stream without a reference frame runs mCreateFrame instead. updateFramePose, the pre-integration and
+ * needNewKF run on the host in float / double as the reference does (glibc cosf / sinf); the device work of a step is
+ * one CUDA graph, captured on the first step of each (B, w, h) and replayed after that. Keyframe creation, the local
+ * mapper and covisibility stay with the caller. One handle per calling thread; calls on one handle are not re-entrant. */
+typedef struct se2gpu_tracker se2gpu_tracker;
+
+typedef struct se2gpu_tracker_params {
+    int nfeatures;               /* Config::MaxFtrNumber: the extractor's nfeatures and needNewKF's c4 */
+    float scale_factor;          /* Config::ScaleFactor */
+    int nlevels;                 /* Config::MaxLevel */
+    int fast_th;                 /* the extractor's FAST threshold (the reference's default is 20) */
+    float K[9];                  /* Config::Kcam, row-major */
+    float dist[12];              /* Config::Dcam; frames are raw, the undistortion is folded into extraction */
+    int ndist;                   /* 0, 4, 5, 8 or 12 */
+    se2gpu_grid_params grid;     /* Frame's grid bounds (static members, the same for every frame) */
+    float lower_depth, upper_depth; /* Config::LOWER_DEPTH / UPPER_DEPTH */
+    float cTb[16], bTc[16];      /* Config::cTb / bTc, row-major */
+    float odo_noise[3];          /* Config::ODO_X_NOISE, ODO_Y_NOISE, ODO_T_NOISE */
+    int min_frames;              /* nMinFrames (the reference: 8) */
+    int max_frames;              /* nMaxFrames = Config::FPS */
+} se2gpu_tracker_params;
+
+/* the keyframe side of one stream for one step, from the caller's mpKF (read only for streams that track) */
+typedef struct se2gpu_track_kf {
+    const uint8_t* d_observed;   /* [nfeatures] mpKF->hasObservation(i), DEVICE (a slice of se2gpu_mp_keyframes fits) */
+    const float* d_view_mp;      /* [nfeatures*3] mpKF->mViewMPs, DEVICE */
+    int n_obs_mp;                /* mpKF->getSizeObsMP() */
+    int accept_new_kf;           /* mpLocalMapper->acceptNewKF() */
+    float odom[3];               /* mpKF->odom (x, y, theta) */
+} se2gpu_track_kf;
+
+/* what one step reports for one stream */
+typedef struct se2gpu_track_result {
+    int frame_id;                /* mFrame.id */
+    int first;                   /* 1: the frame went through mCreateFrame */
+    int n_keypoints;             /* mFrame.N */
+    int n_matched;               /* MatchByWindow's count */
+    int n_inlier;                /* removeOutliers' count, the nMatched needNewKF sees */
+    int n_tracked_old;           /* doTriangulate's return (0 when gated) */
+    int n_good_prl;              /* mnGoodPrl after the step (kept when gated) */
+    int triangulated;            /* 1: doTriangulate passed the nMinFrames test */
+    int new_kf;                  /* needNewKF() returned true, or a first frame has > 100 keypoints: the caller makes the
+                                    keyframe, then calls se2gpu_tracker_reset */
+    int abort_ba;                /* needNewKF called mpLocalMapper->setAbortBA() */
+} se2gpu_track_result;
+
+/* one stream's state: device arrays of nfeatures entries (the reference frame's and the current frame's keypoints and
+ * descriptors, their counts, mPrevMatched [2 per entry], mMatchIdx, mLocalMPs [3 per entry], mvbGoodPrl) and host copies of
+ * mFrame.Tcr, preSE2 (meas, cov column-major as Eigen stores it) and the ids */
+typedef struct se2gpu_track_state {
+    const se2gpu_keypoint* d_ref_kp; const uint8_t* d_ref_desc; const int* d_ref_n;
+    const se2gpu_keypoint* d_cur_kp; const uint8_t* d_cur_desc; const int* d_cur_n;
+    const float* d_prev; const int* d_matches; const float* d_local_mps; const uint8_t* d_good_prl;
+    float Tcr[16];
+    double pre_meas[3], pre_cov[9];
+    int frame_id, kf_id, has_ref, n_good_prl;
+} se2gpu_track_state;
+
+/* max_w x max_h frames, up to max_streams (<= 65535) per step, on `device`. NULL on failure (se2gpu_last_error). */
+se2gpu_tracker* se2gpu_tracker_create(int max_streams, int max_w, int max_h, const se2gpu_tracker_params* params, int device);
+void se2gpu_tracker_destroy(se2gpu_tracker* t);
+/* One step for streams 0 .. B-1 (the others are untouched): frames are 8-bit gray w x hgt, row stride `stride`, frame b at
+ * frames + b*frame_stride, in DEVICE memory when frames_on_device != 0 and HOST memory otherwise; odom [B*3] (x, y, theta);
+ * kf [B] the keyframe side (may be NULL when no stream 0 .. B-1 has a reference frame); out [B]. Synchronous: returns when
+ * out is filled. Invalid input (B outside 1 .. max_streams, frames larger than the capacity, NULL pointers, a tracking
+ * stream without its keyframe arrays) returns SE2GPU_ERR_INVALID / SE2GPU_ERR_CAPACITY and changes nothing. */
+int se2gpu_tracker_step(se2gpu_tracker* t, int B, const uint8_t* frames, int frames_on_device, int w, int hgt, int stride,
+                        size_t frame_stride, const float* odom, const se2gpu_track_kf* kf, se2gpu_track_result* out);
+/* The same after dropping the reference frame of streams 0 .. B-1 and restarting their frame ids (Frame::nextId = 0): every
+ * stream runs mCreateFrame. kf may be NULL. */
+int se2gpu_tracker_first(se2gpu_tracker* t, int B, const uint8_t* frames, int frames_on_device, int w, int hgt, int stride,
+                         size_t frame_stride, const float* odom, se2gpu_track_result* out);
+/* resetLocalTrack (src/Track.cpp:191-204) for the n streams streams[0 .. n-1] (distinct), after the caller made their
+ * current frame a keyframe: the reference frame becomes the current frame, mPrevMatched its keypoints, mLocalMPs
+ * d_view_mp[j] [nfeatures*3] (DEVICE) up to its keypoint count and (-1,-1,-1) past it, mMatchIdx -1, preSE2 and mnGoodPrl
+ * 0. A stream that has not extracted a frame since se2gpu_tracker_create, or a NULL pointer: SE2GPU_ERR_INVALID, nothing
+ * changed. Asynchronous on the tracker's stream; the next call sees its results. */
+int se2gpu_tracker_reset(se2gpu_tracker* t, int n, const int* streams, const float* const* d_view_mp);
+/* stream b's state (device pointers stay valid for the life of the handle; read them after the call that wrote them) */
+int se2gpu_tracker_state(se2gpu_tracker* t, int b, se2gpu_track_state* st);
+/* nodes of the step graph last captured: kernels [1] and all nodes [1] (either may be NULL); 0 before the first step */
+int se2gpu_tracker_graph_nodes(se2gpu_tracker* t, int* kernels, int* nodes);
+/* test hook: eager != 0 runs every later step by direct launches on the tracker's stream instead of the captured graph */
+int se2gpu_tracker_debug_eager(se2gpu_tracker* t, int eager);
+/* Test hooks of the host part (no device needed), exactly what a step runs. _pose: updateFramePose's Tcr [16] and the
+ * pre-integration of preSE2 (meas [3], cov [9] column-major, updated in place) for odometry odom / kf_odom / last_odom [3].
+ * _decide: needNewKF's (bNeedNewKF && acceptNewKF, setAbortBA) for frame_id - kf_id = dframes. */
+int se2gpu_track_host_pose(const se2gpu_tracker_params* p, const float* odom, const float* kf_odom, const float* last_odom,
+                           float* Tcr, double* meas, double* cov);
+int se2gpu_track_host_decide(const se2gpu_tracker_params* p, int dframes, int n_tracked_old, int n_obs_mp, int n_good_prl,
+                             int n_inlier, const float* odom, const float* kf_odom, int accept_new_kf, int* new_kf, int* abort_ba);
 
 /* ------------------------------------------------------------------------------------------ local BA */
 typedef struct se2gpu_ba se2gpu_ba;

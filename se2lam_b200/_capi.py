@@ -75,6 +75,37 @@ class MpParams(C.Structure):
                 ("nlevels", C.c_int), ("scale_factors", C.c_float * MP_MAX_LEVELS)]
 
 
+class TrackerParams(C.Structure):
+    """se2gpu_tracker_params"""
+    _fields_ = [("nfeatures", C.c_int), ("scale_factor", C.c_float), ("nlevels", C.c_int), ("fast_th", C.c_int),
+                ("K", C.c_float * 9), ("dist", C.c_float * 12), ("ndist", C.c_int), ("grid", GridParams),
+                ("lower_depth", C.c_float), ("upper_depth", C.c_float), ("cTb", C.c_float * 16), ("bTc", C.c_float * 16),
+                ("odo_noise", C.c_float * 3), ("min_frames", C.c_int), ("max_frames", C.c_int)]
+
+
+class TrackKF(C.Structure):
+    """se2gpu_track_kf"""
+    _fields_ = [("d_observed", vp_), ("d_view_mp", vp_), ("n_obs_mp", C.c_int), ("accept_new_kf", C.c_int),
+                ("odom", C.c_float * 3)]
+
+
+TRACK_RESULT_FIELDS = ["frame_id", "first", "n_keypoints", "n_matched", "n_inlier", "n_tracked_old", "n_good_prl",
+                       "triangulated", "new_kf", "abort_ba"]
+
+
+class TrackResult(C.Structure):
+    """se2gpu_track_result"""
+    _fields_ = [(n, C.c_int) for n in TRACK_RESULT_FIELDS]
+
+
+class TrackState(C.Structure):
+    """se2gpu_track_state"""
+    _fields_ = [("d_ref_kp", vp_), ("d_ref_desc", vp_), ("d_ref_n", vp_), ("d_cur_kp", vp_), ("d_cur_desc", vp_),
+                ("d_cur_n", vp_), ("d_prev", vp_), ("d_matches", vp_), ("d_local_mps", vp_), ("d_good_prl", vp_),
+                ("Tcr", C.c_float * 16), ("pre_meas", C.c_double * 3), ("pre_cov", C.c_double * 9), ("frame_id", C.c_int),
+                ("kf_id", C.c_int), ("has_ref", C.c_int), ("n_good_prl", C.c_int)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -113,6 +144,9 @@ SYMBOLS = [
     "se2gpu_se3_ba_create", "se2gpu_se3_ba_destroy", "se2gpu_se3_ba", "se2gpu_se3_ba_device", "se2gpu_se3_ba_debug_trace",
     "se2gpu_mp_add_observations", "se2gpu_mp_erase_observations", "se2gpu_mp_update_measure",
     "se2gpu_mp_add_observations_device", "se2gpu_mp_erase_observations_device", "se2gpu_mp_update_measure_device",
+    "se2gpu_track_triangulate_batch_device", "se2gpu_tracker_create", "se2gpu_tracker_destroy", "se2gpu_tracker_step",
+    "se2gpu_tracker_first", "se2gpu_tracker_reset", "se2gpu_tracker_state", "se2gpu_tracker_graph_nodes",
+    "se2gpu_tracker_debug_eager", "se2gpu_track_host_pose", "se2gpu_track_host_decide",
 ]
 
 
@@ -246,6 +280,18 @@ def lib():
     L.se2gpu_mp_add_observations_device.argtypes = [vp] * 8
     L.se2gpu_mp_erase_observations_device.argtypes = [vp] * 8
     L.se2gpu_mp_update_measure_device.argtypes = [vp, vp, i, vp, vp, vp]
+    L.se2gpu_track_triangulate_batch_device.argtypes = [i, vp, i, vp, vp, i, vp, vp, vp, vp, vp, vp, f, f, i, vp, vp, vp, vp]
+    L.se2gpu_tracker_create.restype = vp
+    L.se2gpu_tracker_create.argtypes = [i, i, i, vp, i]
+    L.se2gpu_tracker_destroy.argtypes = [vp]
+    L.se2gpu_tracker_step.argtypes = [vp, i, vp, i, i, i, i, sz, vp, vp, vp]
+    L.se2gpu_tracker_first.argtypes = [vp, i, vp, i, i, i, i, sz, vp, vp]
+    L.se2gpu_tracker_reset.argtypes = [vp, i, vp, vp]
+    L.se2gpu_tracker_state.argtypes = [vp, i, vp]
+    L.se2gpu_tracker_graph_nodes.argtypes = [vp, vp, vp]
+    L.se2gpu_tracker_debug_eager.argtypes = [vp, i]
+    L.se2gpu_track_host_pose.argtypes = [vp] * 7
+    L.se2gpu_track_host_decide.argtypes = [vp, i, i, i, i, i, vp, vp, i, vp, vp]
     _lib = L
     return L
 

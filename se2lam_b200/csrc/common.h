@@ -348,4 +348,26 @@ __device__ __forceinline__ int hamming256(const uint32_t* __restrict__ a, const 
            __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
 }
 
+// ---------------------------------------------------------------------------------------------- entries shared between units
+// Track::doTriangulate over B streams (geom.cu); see se2gpu_track_triangulate_batch_device. observed_tab / view_mp_tab, when
+// set, give each stream's keyframe arrays by pointer (device memory) instead of at b * cap in observed / view_mp.
+struct TrackTriArgs {
+    const se2gpu_keypoint* kp_kf; int cap; const int* d_n;
+    const se2gpu_keypoint* kp_fr; int cap_fr;
+    int* matches;
+    const uint8_t* observed; const float* view_mp;
+    const uint8_t* const* observed_tab; const float* const* view_mp_tab;
+    const float* Tcr; const int* gate; const float* K;
+    float lower, upper, min_cos;
+    float* local_mps; uint8_t* good_prl; int* counts;
+};
+int track_triangulate_launch(const TrackTriArgs& a, int B, cudaStream_t s);
+float track_min_cos(int min_parallax_deg);
+// The set-up a stream capture must not contain, done ahead of one: the extractor's geometry tables and undistortion map for
+// a w x hgt frame (orb.cu), the outlier kernel's table and shared-memory limit (fundam.cu); and whether MatchByWindow on
+// cap1 x cap2 keypoints takes the shared-memory resolve, whose launches hold no host-to-device copy (matcher.cu).
+int orb_prepare_shape(se2gpu_orb* h, int w, int hgt, cudaStream_t s);
+int fundam_prepare();
+bool matcher_window_capturable(const se2gpu_matcher* m, int cap1, int cap2);
+
 }  // namespace se2gpu

@@ -534,6 +534,8 @@ int prepare_device() {
 
 }  // namespace
 
+int se2gpu::fundam_prepare() { return prepare_device(); }
+
 int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const int* d_n1, int cap1, const se2gpu_keypoint* d_kp2,
                                   const int* d_n2, int cap2, int* d_matches12, int* d_ninliers, double* d_F, int* d_iters,
                                   void* stream) {

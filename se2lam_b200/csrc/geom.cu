@@ -325,20 +325,30 @@ __global__ void __launch_bounds__(kBlock) k_triangulate(int n, const float* __re
     xyz[3 * i] = r.x; xyz[3 * i + 1] = r.y; xyz[3 * i + 2] = r.z;
 }
 
-__global__ void __launch_bounds__(kBlock) k_track_triangulate(
-    const se2gpu_keypoint* __restrict__ kp_kf, int cap, const int* __restrict__ d_n, const se2gpu_keypoint* __restrict__ kp_fr,
-    int* __restrict__ matches, const uint8_t* __restrict__ observed, const float* __restrict__ view_mp,
-    const float* __restrict__ Tcr_g, const float* __restrict__ K_g, float lower, float upper, float min_cos,
-    float* __restrict__ local_mps, uint8_t* __restrict__ good_prl, int* __restrict__ counts) {
-    // P_KF = Config::PrjMtrxEye, P = Kcam * Tcr.rowRange(0,3) and Ocam = inv(Tcr).col(3) are the same for the whole launch:
+// Track::doTriangulate for B streams, stream b on blockIdx.y: its keyframe keypoints, matches, good-parallax flags and local
+// map points at b * cap, its frame keypoints at b * cap_fr, its Tcr at 16 b and its counts at 2 b. A stream whose gate is 0
+// (the nMinFrames early return) leaves every output untouched.
+__global__ void __launch_bounds__(kBlock) k_track_triangulate(se2gpu::TrackTriArgs a) {
+    const int b = blockIdx.y;
+    if (a.gate && !a.gate[b]) return;
+    const size_t base = (size_t)b * a.cap;
+    const se2gpu_keypoint* __restrict__ kp_kf = a.kp_kf + base;
+    const se2gpu_keypoint* __restrict__ kp_fr = a.kp_fr + (size_t)b * a.cap_fr;
+    int* __restrict__ matches = a.matches + base;
+    const uint8_t* __restrict__ observed = a.observed_tab ? a.observed_tab[b] : a.observed + base;
+    const float* __restrict__ view_mp = a.view_mp_tab ? a.view_mp_tab[b] : a.view_mp + 3 * base;
+    float* __restrict__ local_mps = a.local_mps + 3 * base;
+    uint8_t* __restrict__ good_prl = a.good_prl + base;
+    int* __restrict__ counts = a.counts + 2 * b;
+    // P_KF = Config::PrjMtrxEye, P = Kcam * Tcr.rowRange(0,3) and Ocam = inv(Tcr).col(3) are the same for the whole stream:
     // one thread per block builds them in shared memory
     __shared__ float sP[24], sO[3];
     if (threadIdx.x == 0) {
         float Tcr[16], K[9], Ti[16];
 #pragma unroll
-        for (int k = 0; k < 16; k++) Tcr[k] = Tcr_g[k];
+        for (int k = 0; k < 16; k++) Tcr[k] = a.Tcr[16 * b + k];
 #pragma unroll
-        for (int k = 0; k < 9; k++) K[k] = K_g[k];
+        for (int k = 0; k < 9; k++) K[k] = a.K[k];
         const float eye34[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
         projection(K, eye34, sP);
         projection(K, Tcr, sP + 12);
@@ -347,7 +357,7 @@ __global__ void __launch_bounds__(kBlock) k_track_triangulate(
     }
     __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n = count_of(d_n, cap);
+    const int n = count_of(a.d_n ? a.d_n + b : nullptr, a.cap);
     bool tracked = false, good = false;
     if (i < n) {
         good_prl[i] = 0;
@@ -360,14 +370,14 @@ __global__ void __launch_bounds__(kBlock) k_track_triangulate(
                 float P_KF[12], P[12];
 #pragma unroll
                 for (int k = 0; k < 12; k++) { P_KF[k] = sP[k]; P[k] = sP[12 + k]; }
-                const se2gpu_keypoint a = kp_kf[i], b = kp_fr[m];
-                const F3 pos = triangulate(a.x, a.y, b.x, b.y, P_KF, P);
-                if (pos.z >= lower && pos.z <= upper) {
+                const se2gpu_keypoint p = kp_kf[i], q = kp_fr[m];
+                const F3 pos = triangulate(p.x, p.y, q.x, q.y, P_KF, P);
+                if (pos.z >= a.lower && pos.z <= a.upper) {
                     local_mps[3 * i] = pos.x; local_mps[3 * i + 1] = pos.y; local_mps[3 * i + 2] = pos.z;
                     // cvu::checkParallax(0, Ocam, pos, deg)
                     const F3 p1 = sub3(pos, {0.f, 0.f, 0.f}), p2 = sub3(pos, {sO[0], sO[1], sO[2]});
                     const float cosp = __double2float_rn(dd(fabs((double)dot3(p1, p2)), dm(norm3(p1), norm3(p2))));
-                    if (cosp < min_cos) { good = true; good_prl[i] = 1; }
+                    if (cosp < a.min_cos) { good = true; good_prl[i] = 1; }
                 } else {
                     matches[i] = -1;
                 }
@@ -885,21 +895,44 @@ int se2gpu_triangulate_device(int n, const float* d_pt1, const float* d_pt2, con
     return SE2GPU_OK;
 }
 
+namespace se2gpu {
+int track_triangulate_launch(const TrackTriArgs& a, int B, cudaStream_t s) {
+    SE2_CUDA(cudaMemsetAsync(a.counts, 0, 2 * sizeof(int) * B, s));
+    if (B == 0 || a.cap == 0) return SE2GPU_OK;
+    SE2_LAUNCH(k_track_triangulate, dim3(blocks(a.cap), B), kBlock, 0, s, a);
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
+float track_min_cos(int min_parallax_deg) { return kMinCos[min_parallax_deg - 1]; }
+}  // namespace se2gpu
+
 int se2gpu_track_triangulate_device(const se2gpu_keypoint* d_kp_kf, int n_kf, const int* d_n_kf, const se2gpu_keypoint* d_kp_frame,
                                     int* d_matches12, const uint8_t* d_kf_observed, const float* d_kf_view_mp, const float* d_Tcr,
                                     const float* d_K, float lower_depth, float upper_depth, int min_parallax_deg,
                                     float* d_local_mps, uint8_t* d_good_prl, int* d_counts, void* stream) {
-    if (n_kf < 0 || !d_counts || min_parallax_deg < 1 || min_parallax_deg > 4 || !d_Tcr || !d_K) return fail(SE2GPU_ERR_INVALID, "bad arguments");
-    if (n_kf && (!d_kp_kf || !d_kp_frame || !d_matches12 || !d_kf_observed || !d_kf_view_mp || !d_local_mps || !d_good_prl))
+    return se2gpu_track_triangulate_batch_device(1, d_kp_kf, n_kf, d_n_kf, d_kp_frame, 0, d_matches12, d_kf_observed, d_kf_view_mp,
+                                                 d_Tcr, nullptr, d_K, lower_depth, upper_depth, min_parallax_deg, d_local_mps,
+                                                 d_good_prl, d_counts, stream);
+}
+
+int se2gpu_track_triangulate_batch_device(int B, const se2gpu_keypoint* d_kp_kf, int cap, const int* d_n, const se2gpu_keypoint* d_kp_frame,
+                                          int cap_frame, int* d_matches12, const uint8_t* d_kf_observed, const float* d_kf_view_mp,
+                                          const float* d_Tcr, const int* d_gate, const float* d_K, float lower_depth,
+                                          float upper_depth, int min_parallax_deg, float* d_local_mps, uint8_t* d_good_prl,
+                                          int* d_counts, void* stream) {
+    if (B < 0 || cap < 0 || cap_frame < 0 || !d_counts || min_parallax_deg < 1 || min_parallax_deg > 4 || !d_Tcr || !d_K)
+        return fail(SE2GPU_ERR_INVALID, "bad arguments");
+    if (B && cap && (!d_kp_kf || !d_kp_frame || !d_matches12 || !d_kf_observed || !d_kf_view_mp || !d_local_mps || !d_good_prl))
         return fail(SE2GPU_ERR_INVALID, "null argument");
+    if (B > 65535) return fail(SE2GPU_ERR_CAPACITY, "%d streams per call: at most 65535 (the grid's y dimension)", B);
     { const int rc = require_device(); if (rc) return rc; }
-    cudaStream_t s = (cudaStream_t)stream;
-    SE2_CUDA(cudaMemsetAsync(d_counts, 0, 2 * sizeof(int), s));
-    if (n_kf == 0) return SE2GPU_OK;
-    SE2_LAUNCH(k_track_triangulate, blocks(n_kf), kBlock, 0, s, d_kp_kf, n_kf, d_n_kf, d_kp_frame, d_matches12, d_kf_observed,
-               d_kf_view_mp, d_Tcr, d_K, lower_depth, upper_depth, kMinCos[min_parallax_deg - 1], d_local_mps, d_good_prl, d_counts);
-    SE2_CUDA(cudaGetLastError());
-    return SE2GPU_OK;
+    if (B == 0) return SE2GPU_OK;
+    TrackTriArgs a{};
+    a.kp_kf = d_kp_kf; a.cap = cap; a.d_n = d_n; a.kp_fr = d_kp_frame; a.cap_fr = cap_frame; a.matches = d_matches12;
+    a.observed = d_kf_observed; a.view_mp = d_kf_view_mp; a.Tcr = d_Tcr; a.gate = d_gate; a.K = d_K;
+    a.lower = lower_depth; a.upper = upper_depth; a.min_cos = kMinCos[min_parallax_deg - 1];
+    a.local_mps = d_local_mps; a.good_prl = d_good_prl; a.counts = d_counts;
+    return track_triangulate_launch(a, B, (cudaStream_t)stream);
 }
 
 int se2gpu_xyz_info_device(int n, const float* d_xyz1, const int* d_pose1, const int* d_pose2, const float* d_Tcw, float fx,

@@ -643,6 +643,10 @@ se2gpu_matcher* g_default[se2gpu::kMaxDevices] = {};
 
 }  // namespace
 
+bool se2gpu::matcher_window_capturable(const se2gpu_matcher* m, int cap1, int cap2) {
+    return cap1 < 65536 && pick_K(m, cap1, cap2) >= 2;
+}
+
 extern "C" {
 
 se2gpu_matcher* se2gpu_matcher_create(int max_queries, int max_db, int device) {

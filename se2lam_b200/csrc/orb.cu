@@ -1659,6 +1659,13 @@ int run_device(se2gpu_orb* h, const uint8_t* d_imgs, int n, int w, int hgt, int 
 
 }  // namespace
 
+int se2gpu::orb_prepare_shape(se2gpu_orb* h, int w, int hgt, cudaStream_t s) {
+    SE2_CUDA(cudaSetDevice(h->device));
+    int rc = set_geometry(h, w, hgt, s);
+    if (rc == SE2GPU_OK && h->und_on) rc = ensure_undistort_map(h, w, hgt, s);
+    return rc;
+}
+
 extern "C" {
 
 se2gpu_orb* se2gpu_orb_create_scored(int nfeatures, float scale_factor, int nlevels, int score_type, int fast_th, int max_w, int max_h,
