@@ -813,6 +813,107 @@ int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_
                                int min_edges, int* d_n_edges, se2gpu_ba_iter_stats* d_stats, int* d_iterations, int* d_status,
                                double* d_pose, void* stream);
 
+/* ------------------------------------------------------------------------------------------ localization */
+/* Localizer::run (reference src/Localizer.cpp:32-176) for up to max_streams camera streams against one static map kept on
+ * the device (DESIGN.md section 15). The map (keyframes, map points, observations, covisibility) goes up once at create;
+ * the Localizer never edits it. One se2gpu_loc_step takes one frame and one odometry reading per stream and runs, per
+ * stream: ReadFrameInfo (extraction, a new keyframe with no observations), UpdatePoseCurr on the host, and for a tracked
+ * stream MatchLocalMap, DoLocalBA (above 30 observations), UpdateCovisKFCurr, UpdateLocalMap(1) and DetectIfLost. The
+ * device work of a step is one CUDA graph per (B, w, h). Loop detection and verification stay with the caller, who runs
+ * se2gpu_loc_relocalize for the streams it verified. The local map is in ascending map-point index. One handle per
+ * calling thread; calls on one handle are not re-entrant.
+ *
+ * Not to be confused with se2gpu_localizer above, the pose-BA workspace. */
+typedef struct se2gpu_loc se2gpu_loc;
+
+/* the map, flattened (HOST arrays, copied once). K keyframes, M map points, keypoint slots in CSR. */
+typedef struct se2gpu_loc_map {
+    int n_kf, n_mp;
+    const float* kf_Tcw;         /* [K*16] row-major keyframe poses */
+    const int* kf_kp_ptr;        /* [K+1] keypoint slots of keyframe k: kf_kp_ptr[k] .. kf_kp_ptr[k+1]-1 */
+    const int* kf_obs_mp;        /* [kf_kp_ptr[K]] map point of mDualObservations[idx], -1 for none */
+    const int* kf_obs_ptr;       /* [K+1] CSR of mObservations: the map points keyframe k observes, strictly ascending */
+    const int* kf_obs;
+    const int* kf_cov_ptr;       /* [K+1] CSR of getAllCovisibleKFs() as keyframe indices, strictly ascending */
+    const int* kf_cov;
+    const float* mp_pos;         /* [M*3] getPos */
+    const uint8_t* mp_null;      /* [M] isNull */
+    const uint8_t* mp_good_prl;  /* [M] isGoodPrl */
+    const uint8_t* mp_desc;      /* [M*32] mMainDescriptor */
+    const int* mp_octave;        /* [M] mMainOctave, < nlevels */
+} se2gpu_loc_map;
+
+typedef struct se2gpu_loc_params {
+    int nfeatures;               /* Config::MaxFtrNumber */
+    float scale_factor;          /* Config::ScaleFactor */
+    int nlevels;                 /* Config::MaxLevel, at most 16 */
+    int fast_th;                 /* the extractor's FAST threshold */
+    float K[9];                  /* Config::Kcam, row-major */
+    float dist[12];              /* Config::Dcam; frames are raw, the undistortion is folded into extraction */
+    int ndist;                   /* 0, 4, 5, 8 or 12 */
+    se2gpu_grid_params grid;     /* Frame's grid origin and inverse cell sizes */
+    float min_x, max_x, min_y, max_y; /* Frame::minXUn, maxXUn, minYUn, maxYUn (inImgBound, inclusive) */
+    float cTb[16], bTc[16];      /* Config::cTb / bTc, row-major */
+    se2gpu_pose_ba_params ba;    /* DoLocalBA: fx, cx, cy, Tbc (= bTc), TH_HUBER, plane-motion information, 30 iterations */
+    float inv_level_sigma2[16];  /* mvInvLevelSigma2 [nlevels] */
+    int max_local_mps;           /* per-stream capacity of the local map-point list */
+} se2gpu_loc_params;
+
+/* what a step (or a relocalization) reports for one stream */
+typedef struct se2gpu_loc_result {
+    int tracked;                 /* mbIsTracked after the call */
+    int first;                   /* 1: the stream's first frame (mpKFRef == NULL): nothing but the extraction ran */
+    int n_keypoints;             /* mpKFCurr->N */
+    int n_matched;               /* MatchLocalMap's count (0 when it did not run) */
+    int n_obs_mp;                /* mpKFCurr->getSizeObsMP() */
+    int ba_status;               /* SE2GPU_POSE_BA_*: GATED at 30 observations or fewer, NO_EDGES when no BA ran */
+    int ba_iterations;
+    int n_local_kfs;             /* |mspKFLocal| */
+    int n_local_mps;             /* |mspMPLocal|, the full count even when it exceeds max_local_mps */
+    int overflow;                /* 1: n_local_mps > max_local_mps; every later call on this stream returns CAPACITY */
+    float Tcw[16];               /* mpKFCurr->Tcw after the call, row-major (WriteTrajFile's source) */
+} se2gpu_loc_result;
+
+/* one stream's state: device arrays (current keypoints / descriptors [nfeatures] and their count, obs_mp [nfeatures] the
+ * map point of each keypoint slot or -1, the local map-point list [max_local_mps] and its count, the local-keyframe
+ * bitmap [K] and the covisible-keyframe bitmap [K] of the current keyframe) and host copies of Tcw and the flags */
+typedef struct se2gpu_loc_stream_state {
+    const se2gpu_keypoint* d_kp; const uint8_t* d_desc; const int* d_n;
+    const int* d_obs_mp;
+    const int* d_local_mps; const int* d_n_local_mps;
+    const uint8_t* d_local_kfs; const uint8_t* d_covis_kfs;
+    float Tcw[16];
+    int has_frame, tracked, overflow;
+} se2gpu_loc_stream_state;
+
+/* Validates the map on the host before any allocation (indices in range, CSR monotone, octaves below nlevels): on any
+ * failure SE2GPU_ERR_INVALID and NULL. max_streams <= 65535. */
+se2gpu_loc* se2gpu_loc_create(int max_streams, int max_w, int max_h, const se2gpu_loc_params* params, const se2gpu_loc_map* map,
+                              int device);
+void se2gpu_loc_destroy(se2gpu_loc* h);
+/* One frame for streams 0 .. B-1: frames as se2gpu_tracker_step, odom [B*3] (x, y, theta), out [B]. Synchronous. Invalid
+ * input returns SE2GPU_ERR_INVALID / SE2GPU_ERR_CAPACITY and changes nothing; so does a step over a stream whose local
+ * map overflowed (SE2GPU_ERR_CAPACITY). */
+int se2gpu_loc_step(se2gpu_loc* h, int B, const uint8_t* frames, int frames_on_device, int w, int hgt, int stride,
+                    size_t frame_stride, const float* odom, se2gpu_loc_result* out);
+/* The verified branch of Localizer::run (Localizer.cpp:121-140) for the n distinct streams streams[j] whose last step
+ * began lost (ran the else branch, where DetectLoopClose runs; a stream that lost tracking during its last step waits a
+ * frame, as in the reference): setPose(kf_loop[j].Tcw), covisible = {kf_loop[j]}, UpdateLocalMap(3), MatchLoopClose over the pairs
+ * match_curr / match_loop [match_ptr[j] .. match_ptr[j+1]) (idxCurr strictly ascending), DoLocalBA, MatchLocalMap,
+ * DoLocalBA, DetectIfLost. out [n]; Tcw_first [n*16] (may be NULL) receives the pose after the first BA. Runs eagerly.
+ * Bad input: SE2GPU_ERR_INVALID, nothing changed. A local map past max_local_mps marks the stream (out[j].overflow) and
+ * returns SE2GPU_ERR_CAPACITY. */
+int se2gpu_loc_relocalize(se2gpu_loc* h, int n, const int* streams, const int* kf_loop, const int* match_ptr, const int* match_curr,
+                          const int* match_loop, se2gpu_loc_result* out, float* Tcw_first);
+int se2gpu_loc_state(se2gpu_loc* h, int b, se2gpu_loc_stream_state* st);
+/* nodes of the step graph last captured: kernels [1] and all nodes [1] (either may be NULL) */
+int se2gpu_loc_graph_nodes(se2gpu_loc* h, int* kernels, int* nodes);
+/* test hook: eager != 0 runs later steps by direct launches instead of the captured graph */
+int se2gpu_loc_debug_eager(se2gpu_loc* h, int eager);
+/* Test hook of the host part (no device needed): UpdatePoseCurr's Tcw [16] = cTb * Se2(ref_odom - odom).toCvSE3() * bTc *
+ * ref_Tcw, exactly what a step computes. */
+int se2gpu_loc_host_pose(const se2gpu_loc_params* p, const float* odom, const float* ref_odom, const float* ref_Tcw, float* Tcw);
+
 /* ------------------------------------------------------------------------------------------ feature-graph constraints */
 /* GlobalMapper::CreateFeatEdge (src/GlobalMapper.cpp:737-843) for B keyframe pairs, one CTA each, everything on the device:
  * the two-keyframe BA of OptKFPair / OptKFPairMatch (two VertexSE3 with the plane-motion EdgeSE3Prior of

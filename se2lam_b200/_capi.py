@@ -106,6 +106,38 @@ class TrackState(C.Structure):
                 ("kf_id", C.c_int), ("has_ref", C.c_int), ("n_good_prl", C.c_int)]
 
 
+class LocMap(C.Structure):
+    """se2gpu_loc_map"""
+    _fields_ = [("n_kf", C.c_int), ("n_mp", C.c_int), ("kf_Tcw", vp_), ("kf_kp_ptr", vp_), ("kf_obs_mp", vp_), ("kf_obs_ptr", vp_),
+                ("kf_obs", vp_), ("kf_cov_ptr", vp_), ("kf_cov", vp_), ("mp_pos", vp_), ("mp_null", vp_), ("mp_good_prl", vp_),
+                ("mp_desc", vp_), ("mp_octave", vp_)]
+
+
+class LocParams(C.Structure):
+    """se2gpu_loc_params"""
+    _fields_ = [("nfeatures", C.c_int), ("scale_factor", C.c_float), ("nlevels", C.c_int), ("fast_th", C.c_int),
+                ("K", C.c_float * 9), ("dist", C.c_float * 12), ("ndist", C.c_int), ("grid", GridParams),
+                ("min_x", C.c_float), ("max_x", C.c_float), ("min_y", C.c_float), ("max_y", C.c_float),
+                ("cTb", C.c_float * 16), ("bTc", C.c_float * 16), ("ba", PoseBAParams), ("inv_level_sigma2", C.c_float * 16),
+                ("max_local_mps", C.c_int)]
+
+
+LOC_RESULT_FIELDS = ["tracked", "first", "n_keypoints", "n_matched", "n_obs_mp", "ba_status", "ba_iterations", "n_local_kfs",
+                     "n_local_mps", "overflow"]
+
+
+class LocResult(C.Structure):
+    """se2gpu_loc_result"""
+    _fields_ = [(n, C.c_int) for n in LOC_RESULT_FIELDS] + [("Tcw", C.c_float * 16)]
+
+
+class LocStreamState(C.Structure):
+    """se2gpu_loc_stream_state"""
+    _fields_ = [("d_kp", vp_), ("d_desc", vp_), ("d_n", vp_), ("d_obs_mp", vp_), ("d_local_mps", vp_), ("d_n_local_mps", vp_),
+                ("d_local_kfs", vp_), ("d_covis_kfs", vp_), ("Tcw", C.c_float * 16), ("has_frame", C.c_int), ("tracked", C.c_int),
+                ("overflow", C.c_int)]
+
+
 class Se2GpuError(RuntimeError):
     pass
 
@@ -147,6 +179,8 @@ SYMBOLS = [
     "se2gpu_track_triangulate_batch_device", "se2gpu_tracker_create", "se2gpu_tracker_destroy", "se2gpu_tracker_step",
     "se2gpu_tracker_first", "se2gpu_tracker_reset", "se2gpu_tracker_state", "se2gpu_tracker_graph_nodes",
     "se2gpu_tracker_debug_eager", "se2gpu_track_host_pose", "se2gpu_track_host_decide",
+    "se2gpu_loc_create", "se2gpu_loc_destroy", "se2gpu_loc_step", "se2gpu_loc_relocalize", "se2gpu_loc_state",
+    "se2gpu_loc_graph_nodes", "se2gpu_loc_debug_eager", "se2gpu_loc_host_pose",
 ]
 
 
@@ -292,6 +326,15 @@ def lib():
     L.se2gpu_tracker_debug_eager.argtypes = [vp, i]
     L.se2gpu_track_host_pose.argtypes = [vp] * 7
     L.se2gpu_track_host_decide.argtypes = [vp, i, i, i, i, i, vp, vp, i, vp, vp]
+    L.se2gpu_loc_create.restype = vp
+    L.se2gpu_loc_create.argtypes = [i, i, i, vp, vp, i]
+    L.se2gpu_loc_destroy.argtypes = [vp]
+    L.se2gpu_loc_step.argtypes = [vp, i, vp, i, i, i, i, sz, vp, vp]
+    L.se2gpu_loc_relocalize.argtypes = [vp, i] + [vp] * 7
+    L.se2gpu_loc_state.argtypes = [vp, i, vp]
+    L.se2gpu_loc_graph_nodes.argtypes = [vp, vp, vp]
+    L.se2gpu_loc_debug_eager.argtypes = [vp, i]
+    L.se2gpu_loc_host_pose.argtypes = [vp] * 5
     _lib = L
     return L
 

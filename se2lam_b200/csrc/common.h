@@ -363,6 +363,13 @@ struct TrackTriArgs {
 };
 int track_triangulate_launch(const TrackTriArgs& a, int B, cudaStream_t s);
 float track_min_cos(int min_parallax_deg);
+// Localizer::DoLocalBA for B streams (pose_ba.cu): stream b's keypoints d_kp + b * cap_kf (d_n[b] of them) with their map
+// points d_obs_mp + b * cap_kf (-1: none); edges at b * cap_kf in d_xyz / d_uv / d_w, their count in d_edges[b];
+// d_best [B * n_mp]. d_run[b] == 0 leaves stream b as it is (NO_EDGES); min_obs >= 0 gates at that many observations.
+int loc_local_ba(int B, const se2gpu_keypoint* d_kp, int cap_kf, const int* d_n, const int* d_obs_mp, int n_mp, const float* d_mp_xyz,
+                 const uint8_t* d_mp_use, const float* d_inv_sigma2, int nlevels, const int* d_run, int min_obs, int* d_best,
+                 float* d_xyz, float* d_uv, float* d_w, int* d_edges, int* d_skip, int* d_n_obs, float* d_Tcw,
+                 const se2gpu_pose_ba_params* params, int* d_iterations, int* d_status, cudaStream_t s);
 // The set-up a stream capture must not contain, done ahead of one: the extractor's geometry tables and undistortion map for
 // a w x hgt frame (orb.cu), the outlier kernel's table and shared-memory limit (fundam.cu); and whether MatchByWindow on
 // cap1 x cap2 keypoints takes the shared-memory resolve, whose launches hold no host-to-device copy (matcher.cu).

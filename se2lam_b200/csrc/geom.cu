@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "common.h"
+#include "fround.h"
 #include "median_desc.h"
 
 using namespace se2gpu;
@@ -19,12 +20,6 @@ namespace {
 
 constexpr int kBlock = 128;
 
-struct F3 { float x, y, z; };
-
-__device__ __forceinline__ float fm(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float fa(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float fs(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float fd(float a, float b) { return __fdiv_rn(a, b); }
 __device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double ds(double a, double b) { return __dsub_rn(a, b); }
@@ -111,14 +106,6 @@ __device__ __forceinline__ void inv4(const float* T, float* Ti) {
         for (int j = 0; j < 3; j++) Ti[i * 4 + j] = RT[i * 3 + j];
         Ti[i * 4 + 3] = gemm3_elem(RT, 3, i, t, 1, 0, -1.0);
     }
-}
-
-// cvu::se3map: Matx33f * Point3f (float sums from 0) + t
-__device__ __forceinline__ F3 se3map(const float* T, F3 p) {
-    float r[3];
-#pragma unroll
-    for (int i = 0; i < 3; i++) r[i] = fa(fa(fa(0.f, fm(T[i * 4], p.x)), fm(T[i * 4 + 1], p.y)), fm(T[i * 4 + 2], p.z));
-    return {fa(r[0], T[3]), fa(r[1], T[7]), fa(r[2], T[11])};
 }
 
 // cv::SVD::compute(A, w, u, vt, MODIFY_A|FULL_UV) on a 4x4 float matrix: OpenCV's one-sided Jacobi (JacobiSVDImpl_<float>)

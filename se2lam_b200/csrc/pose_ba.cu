@@ -37,12 +37,12 @@ struct Params {
     int iterations;
 };
 
-__global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, const int* __restrict__ edge_ptr,
-                                                      const float* __restrict__ xyz, const float* __restrict__ uv,
-                                                      const float* __restrict__ info, Params p, int min_edges,
-                                                      se2gpu_ba_iter_stats* __restrict__ stats, int* __restrict__ iters,
-                                                      int* __restrict__ status, double* __restrict__ pose_out,
-                                                      double* __restrict__ trace) {
+__global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, const int* __restrict__ edge_ptr, int edge_slot,
+                                                      const int* __restrict__ skip, const float* __restrict__ xyz,
+                                                      const float* __restrict__ uv, const float* __restrict__ info, Params p,
+                                                      int min_edges, se2gpu_ba_iter_stats* __restrict__ stats,
+                                                      int* __restrict__ iters, int* __restrict__ status,
+                                                      double* __restrict__ pose_out, double* __restrict__ trace) {
     extern __shared__ float s_stage[];  // [kStageMax*3] xyz, [kStageMax*2] uv, [kStageMax] info
     __shared__ double s_red[kWarps][kAcc];
     __shared__ double s_H[36], s_b[6], s_info[36], s_sum[kAcc];
@@ -51,12 +51,14 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
     __shared__ int s_ok2, s_more, s_stop;
 
     const int pb = blockIdx.x, tid = threadIdx.x;
-    const int e0 = edge_ptr[pb], E = edge_ptr[pb + 1] - e0;
+    // edge_slot 0: problem pb's edges are edge_ptr[pb] .. edge_ptr[pb+1]-1; otherwise the first edge_ptr[pb] of its slot
+    const int e0 = edge_slot ? pb * edge_slot : edge_ptr[pb], E = edge_slot ? edge_ptr[pb] : edge_ptr[pb + 1] - e0;
+    const int sk = skip ? skip[pb] : 0;  // 1: gated by the caller, 2: not run
     float* T16 = Tcw + 16 * (size_t)pb;
-    if (E <= 0 || E <= min_edges) {  // nothing to refine against: the pose is left as it is
+    if (E <= 0 || E <= min_edges || sk) {  // nothing to refine against: the pose is left as it is
         if (tid == 0) {
             if (iters) iters[pb] = 0;
-            if (status) status[pb] = E <= 0 ? SE2GPU_POSE_BA_NO_EDGES : SE2GPU_POSE_BA_GATED;
+            if (status) status[pb] = (sk == 1 || (E > 0 && sk == 0)) ? SE2GPU_POSE_BA_GATED : SE2GPU_POSE_BA_NO_EDGES;
             if (pose_out) store_pose(se3_from_f32(T16), pose_out + 7 * (size_t)pb);
         }
         return;
@@ -168,21 +170,34 @@ __global__ void __launch_bounds__(kThreads) k_pose_ba(float* __restrict__ Tcw, c
     }
 }
 
-// Localizer::DoLocalBA's edge list from MatchByProjection's device output, in ascending map-point index: map point j is an
-// edge when some keypoint i < n matched it (the highest such i, as repeated KeyFrame::addObservation leaves it) and use[j];
-// every edge's information is inv_sigma2[kp[0].octave] (MapPoint::getOctave on a keyframe it never observed). One CTA.
-__global__ void __launch_bounds__(1024) k_localizer_edges(const se2gpu_keypoint* __restrict__ kp, int n_kf, const int* __restrict__ d_n_kf,
+// Localizer::DoLocalBA's edge lists for B streams (one CTA each), in ascending map-point index: map point j is an edge of
+// stream b when some keypoint i < n[b] of b matched it (the highest such i, as repeated KeyFrame::addObservation leaves it)
+// and use[j]; every edge's information is inv_sigma2[kp[0].octave] (MapPoint::getOctave on a keyframe it never observed).
+// Stream b reads kp / matches + b * cap_kf and writes best + b * n_mp, xyz / uv / w at b * edge_slot (edge_slot 0: one
+// stream, edge_ptr = {0, count}; otherwise edge_ptr[b] = count). The count of distinct matched map points, used or not,
+// is getSizeObsMP(): with run (may be NULL) and min_obs >= 0, skip[b] is 2 when !run[b] (no edges) and 1 when that count
+// is min_obs or less (DoLocalBA's gate); n_obs (may be NULL) receives it.
+__global__ void __launch_bounds__(1024) k_localizer_edges(const se2gpu_keypoint* __restrict__ kp, int cap_kf, const int* __restrict__ d_n_kf,
                                                           const int* __restrict__ matches, int n_mp, const float* __restrict__ mp_xyz,
                                                           const uint8_t* __restrict__ mp_use, const float* __restrict__ inv_sigma2,
-                                                          int nlevels, int* __restrict__ best, float* __restrict__ xyz,
-                                                          float* __restrict__ uv, float* __restrict__ w, int* __restrict__ edge_ptr,
-                                                          int* __restrict__ n_edges) {
-    __shared__ int s_wcount[32];
-    __shared__ int s_base;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n = d_n_kf ? min(max(*d_n_kf, 0), n_kf) : n_kf;
+                                                          int nlevels, const int* __restrict__ run, int min_obs, int edge_slot,
+                                                          int* __restrict__ best_all, float* __restrict__ xyz_all,
+                                                          float* __restrict__ uv_all, float* __restrict__ w_all,
+                                                          int* __restrict__ edge_ptr, int* __restrict__ n_edges,
+                                                          int* __restrict__ skip, int* __restrict__ n_obs) {
+    __shared__ int s_wcount[32], s_wobs[32];
+    __shared__ int s_base, s_obs;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const bool go = !run || run[b];
+    kp += (size_t)b * cap_kf; matches += (size_t)b * cap_kf;
+    int* best = best_all + (size_t)b * n_mp;
+    const size_t eo = (size_t)b * edge_slot;
+    float* xyz = xyz_all + 3 * eo;
+    float* uv = uv_all + 2 * eo;
+    float* w = w_all + eo;
+    const int n = go ? count_of(d_n_kf ? d_n_kf + b : nullptr, cap_kf) : 0;
     for (int j = tid; j < n_mp; j += blockDim.x) best[j] = -1;
-    if (tid == 0) s_base = 0;
+    if (tid == 0) { s_base = 0; s_obs = 0; }
     __syncthreads();
     for (int i = tid; i < n; i += blockDim.x) {
         const int m = matches[i];
@@ -195,7 +210,8 @@ __global__ void __launch_bounds__(1024) k_localizer_edges(const se2gpu_keypoint*
         const int k = j < n_mp ? best[j] : -1;
         const bool take = k >= 0 && mp_use[j];
         const unsigned bal = __ballot_sync(0xffffffffu, take);
-        if (lane == 0) s_wcount[warp] = __popc(bal);
+        const unsigned bobs = __ballot_sync(0xffffffffu, k >= 0);
+        if (lane == 0) { s_wcount[warp] = __popc(bal); s_wobs[warp] = __popc(bobs); }
         __syncthreads();
         int off = s_base;
         for (int v = 0; v < warp; ++v) off += s_wcount[v];
@@ -207,16 +223,23 @@ __global__ void __launch_bounds__(1024) k_localizer_edges(const se2gpu_keypoint*
         }
         __syncthreads();
         if (tid == 0) {
-            int tot = 0;
-            for (int v = 0; v < (int)(blockDim.x >> 5); ++v) tot += s_wcount[v];
+            int tot = 0, obs = 0;
+            for (int v = 0; v < (int)(blockDim.x >> 5); ++v) { tot += s_wcount[v]; obs += s_wobs[v]; }
             s_base += tot;
+            s_obs += obs;
         }
         __syncthreads();
     }
     if (tid == 0) {
-        edge_ptr[0] = 0;
-        edge_ptr[1] = s_base;
-        if (n_edges) *n_edges = s_base;
+        if (edge_slot) {
+            edge_ptr[b] = s_base;
+        } else {
+            edge_ptr[0] = 0;
+            edge_ptr[1] = s_base;
+        }
+        if (n_edges) n_edges[b] = s_base;
+        if (skip) skip[b] = !go ? 2 : (min_obs >= 0 && s_obs <= min_obs ? 1 : 0);
+        if (n_obs) n_obs[b] = s_obs;
     }
 }
 
@@ -232,12 +255,12 @@ int check_params(const se2gpu_pose_ba_params* prm, Params* p) {
 
 constexpr size_t kStageBytes = sizeof(float) * 6 * kStageMax;
 
-int launch(int B, float* d_Tcw, const int* d_edge_ptr, const float* d_xyz, const float* d_uv, const float* d_info, const Params& p,
-           int min_edges, se2gpu_ba_iter_stats* d_stats, int* d_iters, int* d_status, double* d_pose, double* d_trace,
-           cudaStream_t stream) {
+int launch(int B, float* d_Tcw, const int* d_edge_ptr, int edge_slot, const int* d_skip, const float* d_xyz, const float* d_uv,
+           const float* d_info, const Params& p, int min_edges, se2gpu_ba_iter_stats* d_stats, int* d_iters, int* d_status,
+           double* d_pose, double* d_trace, cudaStream_t stream) {
     SE2_NVTX("se2gpu_pose_ba");
-    SE2_LAUNCH(k_pose_ba, B, kThreads, kStageBytes, stream, d_Tcw, d_edge_ptr, d_xyz, d_uv, d_info, p, min_edges, d_stats, d_iters,
-               d_status, d_pose, d_trace);
+    SE2_LAUNCH(k_pose_ba, B, kThreads, kStageBytes, stream, d_Tcw, d_edge_ptr, edge_slot, d_skip, d_xyz, d_uv, d_info, p, min_edges,
+               d_stats, d_iters, d_status, d_pose, d_trace);
     SE2_CUDA(cudaGetLastError());
     return SE2GPU_OK;
 }
@@ -270,7 +293,7 @@ int host_run(int B, float* Tcw, const int* edge_ptr, const float* xyz, const flo
     if (dst) st.check(cudaMemset(dst, 0, sizeof(se2gpu_ba_iter_stats) * B * it), "cudaMemset");
     if (dtr) st.check(cudaMemset(dtr, 0, sizeof(double) * 7 * B * it), "cudaMemset");
     if (const int rc = st.status()) return rc;
-    { const int rc = launch(B, dT, dptr, dx, du, dw, p, 0, dst, dit, dsts, dpose, dtr, nullptr); if (rc) return rc; }
+    { const int rc = launch(B, dT, dptr, 0, nullptr, dx, du, dw, p, 0, dst, dit, dsts, dpose, dtr, nullptr); if (rc) return rc; }
     return st.finish();
 }
 
@@ -327,7 +350,7 @@ int se2gpu_pose_ba_device(int B, float* d_Tcw, const int* d_edge_ptr, const floa
     if (B < 0 || (B && (!d_Tcw || !d_edge_ptr))) return fail(SE2GPU_ERR_INVALID, "bad arguments");
     { const int rc = require_device(); if (rc) return rc; }
     if (B == 0) return SE2GPU_OK;
-    return launch(B, d_Tcw, d_edge_ptr, d_xyz, d_uv, d_info, p, 0, d_stats, d_iterations, d_status, d_pose, nullptr, (cudaStream_t)stream);
+    return launch(B, d_Tcw, d_edge_ptr, 0, nullptr, d_xyz, d_uv, d_info, p, 0, d_stats, d_iterations, d_status, d_pose, nullptr, (cudaStream_t)stream);
 }
 
 int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_kp, int n_kf, const int* d_n_kf,
@@ -343,8 +366,24 @@ int se2gpu_localizer_ba_device(se2gpu_localizer* h, const se2gpu_keypoint* d_kf_
     if (n_mp > h->max_mp) return fail(SE2GPU_ERR_CAPACITY, "n_mp = %d exceeds the context's %d map points", n_mp, h->max_mp);
     SE2_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = (cudaStream_t)stream;
+    // the B = 1 call of the batched edge kernel se2gpu_loc_step runs
     SE2_LAUNCH(k_localizer_edges, 1, 1024, 0, s, d_kf_kp, n_kf, d_n_kf, d_matches_idx_mp, n_mp, d_mp_xyz, d_mp_use, d_inv_sigma2,
-               nlevels, h->best, h->xyz, h->uv, h->w, h->edge_ptr, d_n_edges);
+               nlevels, nullptr, -1, 0, h->best, h->xyz, h->uv, h->w, h->edge_ptr, d_n_edges, nullptr, nullptr);
     SE2_CUDA(cudaGetLastError());
-    return launch(1, d_Tcw, h->edge_ptr, h->xyz, h->uv, h->w, p, min_edges, d_stats, d_iterations, d_status, d_pose, nullptr, s);
+    return launch(1, d_Tcw, h->edge_ptr, 0, nullptr, h->xyz, h->uv, h->w, p, min_edges, d_stats, d_iterations, d_status, d_pose,
+                  nullptr, s);
+}
+
+// DoLocalBA for B streams of the localization handle (loc.cu): edges at stream b's slot of edge_slot entries, run / gate as
+// k_localizer_edges above, then the batched solve with min_edges 0 (a stream without edges keeps its pose).
+int se2gpu::loc_local_ba(int B, const se2gpu_keypoint* d_kp, int cap_kf, const int* d_n, const int* d_obs_mp, int n_mp,
+                         const float* d_mp_xyz, const uint8_t* d_mp_use, const float* d_inv_sigma2, int nlevels, const int* d_run,
+                         int min_obs, int* d_best, float* d_xyz, float* d_uv, float* d_w, int* d_edges, int* d_skip, int* d_n_obs,
+                         float* d_Tcw, const se2gpu_pose_ba_params* params, int* d_iterations, int* d_status, cudaStream_t s) {
+    Params p;
+    { const int rc = check_params(params, &p); if (rc) return rc; }
+    SE2_LAUNCH(k_localizer_edges, B, 1024, 0, s, d_kp, cap_kf, d_n, d_obs_mp, n_mp, d_mp_xyz, d_mp_use, d_inv_sigma2, nlevels, d_run,
+               min_obs, cap_kf, d_best, d_xyz, d_uv, d_w, d_edges, nullptr, d_skip, d_n_obs);
+    SE2_CUDA(cudaGetLastError());
+    return launch(B, d_Tcw, d_edges, cap_kf, d_skip, d_xyz, d_uv, d_w, p, 0, nullptr, d_iterations, d_status, nullptr, nullptr, s);
 }
