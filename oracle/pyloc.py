@@ -136,7 +136,8 @@ class LocOracle:
         odom = np.asarray(odom, F)
         if Tcw_prev is not None:
             self.Tcw = np.asarray(Tcw_prev, F).copy()
-        self.kp, self.desc = self.orb.extract(img)                         # ReadFrameInfo
+        img = pyoracle.frame_image(img, self.cfg["K"], self.cfg.get("dist", ()))   # ReadFrameInfo builds a Frame, which undistorts
+        self.kp, self.desc = self.orb.extract(img)
         self.obs_mp = np.full(len(self.kp), -1, np.int32)
         self.covis = np.zeros(self.K, np.uint8)
         r = dict(tracked=0, first=0, n_keypoints=len(self.kp), n_matched=0, n_obs_mp=0, ba_status=1, ba_iterations=0,

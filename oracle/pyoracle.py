@@ -135,6 +135,13 @@ def undistort(img, K, dist):
     return out
 
 
+def frame_image(img, K, dist):
+    """the image a Frame extracts from (reference src/Frame.cpp:22): cv::undistort(img, K, dist) when dist has
+    coefficients, img itself when it is empty. The tracker and localizer oracles both read their frames through this."""
+    d = np.asarray(() if dist is None else dist, np.float32).ravel()
+    return undistort(img, K, d) if len(d) else img
+
+
 def undistort_map(K, dist, w, h):
     K = np.ascontiguousarray(K, np.float32).reshape(9)
     dist = np.ascontiguousarray(dist, np.float32).ravel()

@@ -88,10 +88,7 @@ class TrackOracle:
         self.good = np.zeros(self.cap, np.uint8)
 
     def _extract(self, img):
-        d = np.asarray(self.cfg.get("dist", ()), np.float32)
-        if len(d):
-            img = pyoracle.undistort(img, np.asarray(self.cfg["K"], np.float32), d)
-        return self.orb.extract(img)
+        return self.orb.extract(pyoracle.frame_image(img, self.cfg["K"], self.cfg.get("dist", ())))
 
     def first(self, img, odom):
         self.has_ref, self.next_id = False, 0

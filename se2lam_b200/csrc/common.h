@@ -372,9 +372,10 @@ int loc_local_ba(int B, const se2gpu_keypoint* d_kp, int cap_kf, const int* d_n,
                  const se2gpu_pose_ba_params* params, int* d_iterations, int* d_status, cudaStream_t s);
 // The set-up a stream capture must not contain, done ahead of one: the extractor's geometry tables and undistortion map for
 // a w x hgt frame (orb.cu), the outlier kernel's table and shared-memory limit (fundam.cu); and whether MatchByWindow on
-// cap1 x cap2 keypoints takes the shared-memory resolve, whose launches hold no host-to-device copy (matcher.cu).
+// cap1 x cap2 keypoints on `device` takes the shared-memory resolve, whose launches hold no host-to-device copy (matcher.cu;
+// answered before any matcher is made, so a refused handle allocates nothing for it).
 int orb_prepare_shape(se2gpu_orb* h, int w, int hgt, cudaStream_t s);
 int fundam_prepare();
-bool matcher_window_capturable(const se2gpu_matcher* m, int cap1, int cap2);
+bool matcher_window_capturable(int device, int cap1, int cap2);
 
 }  // namespace se2gpu

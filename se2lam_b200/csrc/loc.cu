@@ -407,6 +407,11 @@ se2gpu_loc* se2gpu_loc_create(int max_streams, int max_w, int max_h, const se2gp
     if (max_streams > 65535) { fail(SE2GPU_ERR_CAPACITY, "%d streams: at most 65535", max_streams); return nullptr; }
     if (map_ok(map, params->nlevels)) return nullptr;
     if (select_device(device) != SE2GPU_OK) return nullptr;
+    if (!matcher_window_capturable(device, params->max_local_mps, params->nfeatures)) {
+        fail(SE2GPU_ERR_CAPACITY, "%d local map points x %d features are too many for the matcher's shared-memory resolve",
+             params->max_local_mps, params->nfeatures);
+        return nullptr;
+    }
     se2gpu_loc* h = new se2gpu_loc;
     h->device = device; h->S = max_streams; h->C = params->nfeatures; h->Q = params->max_local_mps; h->max_w = max_w; h->max_h = max_h;
     h->p = *params;
@@ -421,10 +426,6 @@ se2gpu_loc* se2gpu_loc_create(int max_streams, int max_w, int max_h, const se2gp
     if (se2gpu_orb_set_undistort(h->orb, params->ndist ? params->K : nullptr, params->dist, params->ndist) != SE2GPU_OK) { delete h; return nullptr; }
     h->matcher = se2gpu_matcher_create_batch(h->Q, h->C, max_streams, device);
     if (!h->matcher) { delete h; return nullptr; }
-    if (!matcher_window_capturable(h->matcher, h->Q, h->C)) {
-        fail(SE2GPU_ERR_CAPACITY, "%d local map points x %d features are too many for the matcher's shared-memory resolve", h->Q, h->C);
-        delete h; return nullptr;
-    }
     const size_t S = max_streams, C = h->C, Q = h->Q, Kn = std::max(K, 1), Mn = std::max(M, 1);
     const size_t nkp = std::max(map->kf_kp_ptr[K], 1), nobs = std::max(map->kf_obs_ptr[K], 1), ncov = std::max(map->kf_cov_ptr[K], 1);
     bool ok = true;

@@ -608,9 +608,9 @@ int launch_grid(se2gpu_matcher* m, int B, const se2gpu_keypoint* d_kp, int n, co
 
 size_t resolve_smem(int nq, int n2, int K) { return ((size_t)n2 * (2 + K) + 2 * (size_t)nq) * sizeof(int); }
 
-int pick_K(const se2gpu_matcher* m, int nq, int n2) {
+int pick_K(int smem_max, int nq, int n2) {
     for (int K = 16; K >= 2; K -= 2)
-        if (resolve_smem(nq, n2, K) <= (size_t)m->resolve_smem_max) return K;
+        if (resolve_smem(nq, n2, K) <= (size_t)smem_max) return K;
     return 0;
 }
 
@@ -618,7 +618,7 @@ int pick_K(const se2gpu_matcher* m, int nq, int n2) {
 // so it is the same for every pair.
 template <int MODE>
 int launch_resolve(se2gpu_matcher* m, int B, ResolveArgs ra, const se2gpu_keypoint* kp1, cudaStream_t s) {
-    const int K = (ra.nq_cap < 65536) ? pick_K(m, ra.nq_cap, ra.n2_cap) : 0;
+    const int K = (ra.nq_cap < 65536) ? pick_K(m->resolve_smem_max, ra.nq_cap, ra.n2_cap) : 0;
     ra.scr_q = m->max_q;
     m->last_batch = B;
     SE2_CUDA(cudaMemsetAsync(m->flags, 0, 2 * sizeof(int) * B, s));
@@ -643,8 +643,15 @@ se2gpu_matcher* g_default[se2gpu::kMaxDevices] = {};
 
 }  // namespace
 
-bool se2gpu::matcher_window_capturable(const se2gpu_matcher* m, int cap1, int cap2) {
-    return cap1 < 65536 && pick_K(m, cap1, cap2) >= 2;
+// the dynamic shared memory k_resolve may use on `device` (what se2gpu_matcher_create_batch opts into)
+static int resolve_smem_limit(int device) {
+    int optin = 0;
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    return optin > 0 ? optin - 2048 : 46 * 1024;
+}
+
+bool se2gpu::matcher_window_capturable(int device, int cap1, int cap2) {
+    return cap1 < 65536 && pick_K(resolve_smem_limit(device), cap1, cap2) >= 2;
 }
 
 extern "C" {
@@ -678,9 +685,7 @@ se2gpu_matcher* se2gpu_matcher_create_batch(int max_queries, int max_db, int max
     ok = ok && m->pin.reserve(m->pin_bytes);
     ok = ok && cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) == cudaSuccess;
     if (ok) {
-        int optin = 0;
-        cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
-        m->resolve_smem_max = optin > 0 ? optin - 2048 : 46 * 1024;
+        m->resolve_smem_max = resolve_smem_limit(device);
         ok = cudaFuncSetAttribute(k_resolve<MODE_WINDOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->resolve_smem_max) == cudaSuccess &&
              cudaFuncSetAttribute(k_resolve<MODE_PROJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->resolve_smem_max) == cudaSuccess &&
              cudaFuncSetAttribute(k_resolve<MODE_BOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, m->resolve_smem_max) == cudaSuccess;

@@ -322,6 +322,10 @@ se2gpu_tracker* se2gpu_tracker_create(int max_streams, int max_w, int max_h, con
     if (max_streams <= 0 || max_w <= 0 || max_h <= 0 || !params_ok(params)) { fail(SE2GPU_ERR_INVALID, "bad arguments"); return nullptr; }
     if (max_streams > 65535) { fail(SE2GPU_ERR_CAPACITY, "%d streams: at most 65535", max_streams); return nullptr; }
     if (select_device(device) != SE2GPU_OK) return nullptr;
+    if (!matcher_window_capturable(device, params->nfeatures, params->nfeatures)) {
+        fail(SE2GPU_ERR_CAPACITY, "%d features per frame are too many for the matcher's shared-memory resolve", params->nfeatures);
+        return nullptr;
+    }
     se2gpu_tracker* t = new se2gpu_tracker;
     t->device = device; t->S = max_streams; t->cap = params->nfeatures; t->max_w = max_w; t->max_h = max_h; t->p = *params;
     t->st.resize(max_streams);
@@ -331,10 +335,6 @@ se2gpu_tracker* se2gpu_tracker_create(int max_streams, int max_w, int max_h, con
     if (se2gpu_orb_set_undistort(t->orb, params->ndist ? params->K : nullptr, params->dist, params->ndist) != SE2GPU_OK) { delete t; return nullptr; }
     t->matcher = se2gpu_matcher_create_batch(params->nfeatures, params->nfeatures, max_streams, device);
     if (!t->matcher) { delete t; return nullptr; }
-    if (!matcher_window_capturable(t->matcher, t->cap, t->cap)) {
-        fail(SE2GPU_ERR_CAPACITY, "%d features per frame are too many for the matcher's shared-memory resolve", t->cap);
-        delete t; return nullptr;
-    }
     const size_t S = max_streams, C = t->cap;
     bool ok = true;
     auto A = [&](auto** p, size_t count) { ok = ok && t->bufs.alloc(p, count) == cudaSuccess; };

@@ -16,7 +16,7 @@ import numpy as np
 
 from ._capi import (KP_DTYPE, LOC_RESULT_FIELDS, GridParams, LocMap, LocParams, LocResult, LocStreamState, PoseBAParams, check,
                     lib, ptr)
-from .track import _to_host
+from .track import _to_host, frame_layout
 
 RESULT_DTYPE = np.dtype([(n, np.int32) for n in LOC_RESULT_FIELDS] + [("Tcw", np.float32, (4, 4))])
 MAP_FIELDS = {"kf_Tcw": np.float32, "kf_kp_ptr": np.int32, "kf_obs_mp": np.int32, "kf_obs_ptr": np.int32, "kf_obs": np.int32,
@@ -93,14 +93,12 @@ class Localizer:
     __del__ = close
 
     def step(self, frames, odom):
-        """one frame per stream 0 .. B-1: frames uint8 [B, h, w] (numpy or a CUDA tensor), odom [B, 3]"""
-        on_dev = hasattr(frames, "data_ptr")
-        if not on_dev:
-            frames = np.ascontiguousarray(frames, np.uint8)
-        B, hgt, w = frames.shape
+        """one frame per stream 0 .. B-1, the other streams left as they are: frames [B, h, w] (numpy or a CUDA tensor,
+        read in place with its own strides when they allow it: se2lam_b200.track.frame_layout), odom [B, 3]"""
+        frames, on_dev, B, hgt, w, stride, fstride = frame_layout(frames)
         odom = np.ascontiguousarray(odom, np.float32).reshape(B, 3)
         out = (LocResult * B)()
-        check(lib().se2gpu_loc_step(self.h, B, ptr(frames), int(on_dev), w, hgt, w, w * hgt, ptr(odom), out), "se2gpu_loc_step")
+        check(lib().se2gpu_loc_step(self.h, B, ptr(frames), on_dev, w, hgt, stride, fstride, ptr(odom), out), "se2gpu_loc_step")
         return _results(out, B)
 
     def relocalize(self, streams, kf_loop, matches):

@@ -3,7 +3,8 @@ independent camera streams whose tracking state (reference frame, mPrevMatched, 
 on the device between frames. One `step` takes one frame and one odometry reading per stream and returns the per-stream
 record (counts and the two needNewKF flags); the caller makes the keyframes and calls `reset` for those streams.
 
-Frames are uint8 arrays [B, h, w]: numpy (host) or torch CUDA tensors (device). The keyframe side of stream b is a dict
+Frames are uint8 arrays [B, h, w]: numpy (host) or torch CUDA tensors (device), read in place with their own row and
+frame strides when the last axis has unit stride (frame_layout), packed into a copy otherwise. The keyframe side of stream b is a dict
     observed: device uint8 [nfeatures] (mpKF->hasObservation), view_mp: device float32 [nfeatures, 3] (mpKF->mViewMPs),
     n_obs_mp: int (getSizeObsMP), accept: bool (acceptNewKF), odom: (x, y, theta) (mpKF->odom)
 """
@@ -54,6 +55,38 @@ def _results(out, B):
     return np.frombuffer(bytes(out), RESULT_DTYPE, count=B).copy()
 
 
+def frame_layout(frames):
+    """(frames, on_device, B, h, w, stride, frame_stride) for a batch of frames [B, h, w]: a numpy array (host) or a torch
+    CUDA tensor (device). A uint8 array whose last axis has unit stride, whose rows do not overlap and whose frames do not
+    overlap (B = 1: any frame stride) is passed as it is, with its own row stride and frame stride in bytes, so a view
+    such as big[:, y0:y0 + h, x0:x0 + w] is read where it lies. Any other array is first made a packed uint8 copy (a
+    torch CPU tensor becomes a numpy array)."""
+    if hasattr(frames, "data_ptr") and not frames.is_cuda:
+        frames = frames.numpy()
+    on_dev = hasattr(frames, "data_ptr")
+    if on_dev:
+        import torch
+        ok = frames.dtype == torch.uint8 and frames.dim() == 3
+        strides = frames.stride() if ok else ()
+    else:
+        frames = np.asarray(frames)
+        ok = frames.dtype == np.uint8 and frames.ndim == 3
+        strides = frames.strides if ok else ()
+    if ok:
+        B, hgt, w = frames.shape
+        fs, rs, cs = strides
+        ok = cs == 1 and rs >= w and (B == 1 or fs >= rs * (hgt - 1) + w) and fs >= 0
+    if not ok:
+        if on_dev:
+            import torch
+            frames = frames.to(torch.uint8).contiguous()
+        else:
+            frames = np.ascontiguousarray(frames, np.uint8)
+        B, hgt, w = frames.shape
+        fs, rs = w * hgt, w
+    return frames, int(on_dev), B, hgt, w, int(rs), int(fs)
+
+
 class Tracker:
     def __init__(self, max_streams, max_w, max_h, p: TrackerParams, device=0):
         self.p, self.cap, self.S = p, p.nfeatures, max_streams
@@ -68,25 +101,20 @@ class Tracker:
 
     __del__ = close
 
-    @staticmethod
-    def _frames(frames):
-        on_dev = hasattr(frames, "data_ptr")
-        if not on_dev:
-            frames = np.ascontiguousarray(frames, np.uint8)
-        B, hgt, w = frames.shape
-        return frames, int(on_dev), B, w, hgt
-
     def first(self, frames, odom):
-        """mCreateFrame for streams 0 .. B-1 (their reference frames dropped, frame ids restarted)"""
-        frames, on_dev, B, w, hgt = self._frames(frames)
+        """mCreateFrame for streams 0 .. B-1 (their reference frames dropped, frame ids restarted); frames as for
+        frame_layout. The other streams are left as they are."""
+        frames, on_dev, B, hgt, w, stride, fstride = frame_layout(frames)
         odom = np.ascontiguousarray(odom, np.float32).reshape(B, 3)
         out = (TrackResult * B)()
-        check(lib().se2gpu_tracker_first(self.h, B, ptr(frames), on_dev, w, hgt, w, w * hgt, ptr(odom), out), "se2gpu_tracker_first")
+        check(lib().se2gpu_tracker_first(self.h, B, ptr(frames), on_dev, w, hgt, stride, fstride, ptr(odom), out),
+              "se2gpu_tracker_first")
         return _results(out, B)
 
     def step(self, frames, odom, kf=None):
-        """one frame per stream 0 .. B-1; kf: one dict per stream (None for streams without a reference frame)"""
-        frames, on_dev, B, w, hgt = self._frames(frames)
+        """one frame per stream 0 .. B-1 (frames as for frame_layout; the other streams are left as they are); kf: one
+        dict per stream (None for streams without a reference frame)"""
+        frames, on_dev, B, hgt, w, stride, fstride = frame_layout(frames)
         odom = np.ascontiguousarray(odom, np.float32).reshape(B, 3)
         kfs = None
         if kf is not None:
@@ -98,7 +126,7 @@ class Tracker:
                 kfs[b].n_obs_mp, kfs[b].accept_new_kf = int(k["n_obs_mp"]), int(bool(k["accept"]))
                 kfs[b].odom[:] = [float(v) for v in k["odom"]]
         out = (TrackResult * B)()
-        check(lib().se2gpu_tracker_step(self.h, B, ptr(frames), on_dev, w, hgt, w, w * hgt, ptr(odom), kfs, out),
+        check(lib().se2gpu_tracker_step(self.h, B, ptr(frames), on_dev, w, hgt, stride, fstride, ptr(odom), kfs, out),
               "se2gpu_tracker_step")
         return _results(out, B)
 

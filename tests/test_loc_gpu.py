@@ -35,28 +35,34 @@ def _map_arrays(m):
 
 
 class Harness:
-    """B streams through the handle and B oracles; stream b relocalizes at frame 1 against its start keyframe"""
+    """streams through a handle with one stream per stream given (frames up to max_w x max_h, default cfg's size) and one
+    oracle per stream; stream b relocalizes at its frame 1 against its start keyframe. Each stream keeps its own frame
+    counter, so a call may cover streams 0 .. B-1 only."""
 
-    def __init__(self, streams, cfg, m, oracle=True, eager=False, **kw):
+    def __init__(self, streams, cfg, m, oracle=True, eager=False, max_w=None, max_h=None, **kw):
         from se2lam_b200.loc import Localizer, inv_level_sigma2
         self.cfg, self.m, self.streams, self.B = dict(cfg, **kw), m, streams, len(streams)
-        self.h = Localizer(self.B, cfg["w"], cfg["h"], _params(cfg, **kw), _map_arrays(m))
+        self.h = Localizer(self.B, max_w or cfg["w"], max_h or cfg["h"], _params(cfg, **kw), _map_arrays(m))
         self.h.set_eager(eager)
         isig = inv_level_sigma2(cfg["scale_factor"], cfg["nlevels"])
         logic = pyloc.CppLogic(m)
         self.orc = [pyloc.LocOracle(self.cfg, m, isig, logic) for _ in streams] if oracle else None
-        self.k = 0
+        self.ks = [0] * self.B
 
-    def step(self):
-        k = self.k
-        frames = np.stack([s[0][k] for s in self.streams])
-        odom = np.stack([s[1][k] for s in self.streams])
-        prev = [self.h.state(b)["Tcw"] for b in range(self.B)]
-        rec = self.h.step(frames, odom)
+    def step(self, B=None, layout=None):
+        """one call over streams 0 .. B-1 (default all), each at its own next frame; layout(frames [B,h,w]) -> the array
+        handed to the binding"""
+        n = B or self.B
+        ks = self.ks[:n]
+        frames = np.stack([self.streams[b][0][ks[b]] for b in range(n)])
+        odom = np.stack([self.streams[b][1][ks[b]] for b in range(n)])
+        prev = [self.h.state(b)["Tcw"] for b in range(n)]
+        rec = self.h.step(layout(frames) if layout else frames, odom)
         ref = None
         if self.orc:
-            ref = [o.step(frames[b], odom[b], prev[b] if k else None) for b, o in enumerate(self.orc)]
-        self.k += 1
+            ref = [o.step(frames[b], odom[b], prev[b] if ks[b] else None) for b, o in enumerate(self.orc[:n])]
+        for b in range(n):
+            self.ks[b] += 1
         return rec, ref
 
     def relocalize(self, streams):
@@ -92,24 +98,36 @@ def compare(h, b, rec, ref, where):
         assert st["local_mps"].tolist() == o.local_mps[:h.cfg["max_local_mps"]], f"{where}: local map points"
 
 
-def run(B, frames=30, eager=False):
-    cfg, m = scene()
-    streams = [ls.stream(200 + b, m, cfg, frames, ls.KINDS[b % len(ls.KINDS)]) for b in range(B)]
-    h = Harness(streams, cfg, m, eager=eager)
+def check_step(h, rec, ref, k):
+    """the records and state of the streams a call covered against their oracles; a stream lost during this step refuses
+    a relocalization"""
+    for b in range(len(rec)):
+        compare(h, b, rec[b], ref[b], f"frame {k} stream {b}")
+        if h.orc[b].branches[-1] == "lost_now":   # lost during this step: no loop search before the next frame
+            with pytest.raises(Exception):
+                h.h.relocalize([b], [0], [[]])
+
+
+def check_relocalize(h, streams):
+    rr, first, rref = h.relocalize(streams)
+    for j, b in enumerate(streams):
+        want, ofirst = rref[j]
+        assert close(first[j], ofirst), f"stream {b}: pose after the first BA"
+        compare(h, b, rr[j], want, f"relocalize stream {b}")
+    return rr
+
+
+def run(B, frames=30, eager=False, cfg=None, m=None, streams=None, layout=None, **kw):
+    if cfg is None:
+        cfg, m = scene()
+    streams = streams or [ls.stream(200 + b, m, cfg, frames, ls.KINDS[b % len(ls.KINDS)]) for b in range(B)]
+    h = Harness(streams, cfg, m, eager=eager, **kw)
     seen = set()
     for k in range(frames):
-        rec, ref = h.step()
-        for b in range(B):
-            compare(h, b, rec[b], ref[b], f"frame {k} stream {b}")
-            if h.orc[b].branches[-1] == "lost_now":   # lost during this step: no loop search before the next frame
-                with pytest.raises(Exception):
-                    h.h.relocalize([b], [0], [[]])
+        rec, ref = h.step(layout=layout)
+        check_step(h, rec, ref, k)
         if k == 1:
-            rr, first, rref = h.relocalize(list(range(B)))
-            for j in range(B):
-                want, ofirst = rref[j]
-                assert close(first[j], ofirst), f"stream {j}: pose after the first BA"
-                compare(h, j, rr[j], want, f"relocalize stream {j}")
+            check_relocalize(h, list(range(B)))
     for o in h.orc:
         seen |= set(o.branches)
     return h, seen

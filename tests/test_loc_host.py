@@ -169,3 +169,21 @@ def test_set_logic_boundaries_cpp_equals_numpy():
     oa, ob = np.full(6, -1, np.int32), np.full(6, -1, np.int32)
     assert cpp.loop_close(lc, 0, pairs, oa) == loc_numpy.loop_close(lc, 0, pairs, ob) == (1, 2)
     assert oa.tobytes() == ob.tobytes() and oa.tolist() == [-1, -1, -1, 1, 1, -1]
+
+
+@pytest.mark.parametrize("n", sorted(ts.DISTORTION))
+def test_oracle_extracts_from_the_undistorted_frame(n):
+    """ReadFrameInfo builds a Frame, and Frame::Frame runs cv::undistort before extracting (reference Frame.cpp:22): with
+    4, 5, 8 and 12 coefficients, LocOracle's keypoints and descriptors after one step are those of the undistorted frame"""
+    from oracle import pyoracle
+    from se2lam_b200.loc import inv_level_sigma2
+    cfg = ls.config(dist=ts.DISTORTION[n])
+    img = ts.stream(40 + n, 2, "normal", cfg)[0][0]
+    o = pyloc.LocOracle(cfg, {"kf_kp_ptr": np.zeros(1, np.int32)}, inv_level_sigma2(cfg["scale_factor"], cfg["nlevels"]), "numpy")
+    o.step(img, np.zeros(3, np.float32))
+    orb = pyoracle.OrbOracle(cfg["nfeatures"], cfg["scale_factor"], cfg["nlevels"], cfg["fast_th"])
+    kp, desc = orb.extract(pyoracle.undistort(img, cfg["K"], np.asarray(cfg["dist"], np.float32)))
+    assert len(kp) > 100
+    assert o.kp.tobytes() == kp.tobytes() and o.desc.tobytes() == desc.tobytes()
+    raw, _ = orb.extract(img)                            # the distortion moves the keypoints: the comparison can tell
+    assert raw.tobytes() != kp.tobytes()

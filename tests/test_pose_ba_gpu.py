@@ -67,6 +67,12 @@ CASES = {
     "E31": dict(E=31, seed=13),
     "E300": dict(E=300, seed=14),
     "E1000": dict(E=1000, seed=15),
+    # either side of a CTA's 256 edges and of the 1536 edges the batched kernel stages in shared memory (kStageMax)
+    "E255": dict(E=255, seed=22),
+    "E256": dict(E=256, seed=23),
+    "E257": dict(E=257, seed=24),
+    "E1536": dict(E=1536, seed=27),
+    "E1537": dict(E=1537, seed=26),
     "E5000_streamed": dict(E=5000, seed=16),
     "yaw_near_pi": dict(E=300, seed=17, yaw=math.pi - 1e-4),
     "yaw_near_minus_pi": dict(E=300, seed=18, yaw=-math.pi + 1e-4),
@@ -184,6 +190,39 @@ def test_localizer_entry_matches_host_flattening(seed):
     # the gate: no more edges than min_edges leaves the pose and reports GATED
     g = pba.localizerBA(kp, m, p["xyz"], use, ps.INV_SIGMA2, p["Tcw"], prm(), min_edges=len(xyz))
     assert g["status"] == pba.GATED and g["n_edges"] == len(xyz) and g["Tcw"].tobytes() == p["Tcw"].tobytes()
+
+
+@pytest.mark.parametrize("seed", [3, 4])
+def test_localizer_entry_across_keypoint_rounds(seed):
+    """~3 000 keypoints, so the edge scan walks several rounds of 1 024 keypoints. A map point matched by two keypoints
+    takes the higher index's position: 1 024 apart (one thread, two rounds), 1 023 apart (neighbouring threads of two
+    warps, two rounds, no barrier between them) and 600 apart (two warps of one round). Match indices >= n_mp are
+    ignored, and kp[0] on the top octave sets every edge's information (the reference's octave quirk). Checked against
+    the host flattening and the oracle."""
+    p, kp, m, use = _localizer_case(50 + seed, n_mp=400, n_kf=3000)
+    n_mp = len(use)
+    pairs = {int(j): (lo, hi) for j, (lo, hi) in zip(np.flatnonzero(use)[seed:seed + 3],
+                                                    [(700 + seed, 1724 + seed), (1600, 2623), (1030, 1630)])}
+    for j, (lo, hi) in pairs.items():
+        m[m == j] = -1
+        m[[lo, hi]] = j
+        kp["x"][lo], kp["y"][lo] = p["uv"][j] + np.float32(40)
+        kp["x"][hi], kp["y"][hi] = p["uv"][j] + np.float32(0.5)
+    m[[5, 1500, 2999]] = [n_mp, n_mp + 7, 2 ** 30]
+    kp["octave"][0] = len(ps.INV_SIGMA2) - 1
+    xyz, uv, w = pba.localizer_edges(kp, m, p["xyz"], use, ps.INV_SIGMA2)
+    js = np.flatnonzero(use != 0)
+    for j, (lo, hi) in pairs.items():
+        e = int(np.searchsorted(js[np.isin(js, m)], j))
+        assert uv[e].tolist() == [kp["x"][hi], kp["y"][hi]], (lo, hi)
+    assert (w == ps.INV_SIGMA2[-1]).all() and len(xyz) > 30
+    r = pba.localizerBA(kp, m, p["xyz"], use, ps.INV_SIGMA2, p["Tcw"], prm(), min_edges=30)
+    assert r["n_edges"] == len(xyz)
+    h = pba.poseOnlyBA(p["Tcw"][None], [0, len(xyz)], xyz, uv, w, prm())
+    assert r["Tcw"].tobytes() == h["Tcw"][0].tobytes() and r["pose"].tobytes() == h["pose"][0].tobytes()
+    o = pypose.run(p["Tcw"], xyz, uv, w, ps.FX, ps.CX, ps.CY, ps.Tbc_f32(), DELTA, iterations=ITERS)
+    assert np.abs(r["Tcw"] - o["Tcw"]).max() <= 1e-5 * max(1.0, np.abs(o["Tcw"]).max())
+    assert r["status"] == o["status"]
 
 
 def test_device_chain_from_match_by_projection():

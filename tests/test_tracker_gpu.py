@@ -19,51 +19,60 @@ def _params(cfg):
 
 
 class Harness:
-    """drives a tracker of B streams and B oracles as Track::run and the caller's keyframe side would"""
+    """drives a tracker with one stream per stream given (frames up to max_w x max_h, default cfg's size) and one oracle
+    per stream as Track::run and the caller's keyframe side would. Each stream keeps its own frame counter, so a call may
+    cover streams 0 .. B-1 only."""
 
-    def __init__(self, streams, cfg, oracle=True, eager=False):
+    def __init__(self, streams, cfg, oracle=True, eager=False, max_w=None, max_h=None):
         from se2lam_b200.track import Tracker
         self.cfg, self.streams, self.B = cfg, streams, len(streams)
-        self.t = Tracker(self.B, ts.W, ts.H, _params(cfg))
+        self.t = Tracker(self.B, max_w or cfg["w"], max_h or cfg["h"], _params(cfg))
         self.t.set_eager(eager)
         self.orc = [pytrack.TrackOracle(cfg) for _ in streams] if oracle else None
         self.dev = [dict(observed=torch.from_numpy(s[2]["observed"]).cuda(), view_mp=torch.from_numpy(s[2]["view_mp"]).cuda())
                     for s in streams]
         self.kf_odom = [None] * self.B
-        self.k = 0
+        self.ks = [0] * self.B
 
     def kf(self, b):
         s = self.streams[b][2]
         if self.kf_odom[b] is None:
             return None
         return dict(observed=self.dev[b]["observed"], view_mp=self.dev[b]["view_mp"], n_obs_mp=s["n_obs_mp"],
-                    accept=bool(s["accept"][self.k]), odom=self.kf_odom[b])
+                    accept=bool(s["accept"][self.ks[b]]), odom=self.kf_odom[b])
 
-    def step(self, device_frames=False):
-        k = self.k
-        frames = np.stack([s[0][k] for s in self.streams])
-        odom = np.stack([s[1][k] for s in self.streams])
-        kfs = [self.kf(b) for b in range(self.B)]
-        fr = torch.from_numpy(frames).cuda() if device_frames else frames
-        rec = self.t.first(fr, odom) if k == 0 else self.t.step(fr, odom, kfs if any(x is not None for x in kfs) else None)
+    def step(self, device_frames=False, B=None, first=None, layout=None):
+        """one call over streams 0 .. B-1 (default all), each at its own next frame; first: se2gpu_tracker_first (default:
+        when every stream in the call is at its frame 0); layout(frames [B,h,w]) -> the array handed to the binding"""
+        n = B or self.B
+        ks = self.ks[:n]
+        first = all(k == 0 for k in ks) if first is None else first
+        frames = np.stack([self.streams[b][0][ks[b]] for b in range(n)])
+        odom = np.stack([self.streams[b][1][ks[b]] for b in range(n)])
+        if first:
+            self.kf_odom[:n] = [None] * n
+        kfs = [self.kf(b) for b in range(n)]
+        fr = layout(frames) if layout else torch.from_numpy(frames).cuda() if device_frames else frames
+        rec = self.t.first(fr, odom) if first else self.t.step(fr, odom, kfs if any(x is not None for x in kfs) else None)
         ref = None
         if self.orc:
             ref = []
-            for b, o in enumerate(self.orc):
+            for b, o in enumerate(self.orc[:n]):
                 kfo = None
                 if kfs[b] is not None:
                     s = self.streams[b][2]
                     kfo = dict(observed=s["observed"], view_mp=s["view_mp"], n_obs_mp=s["n_obs_mp"], accept=kfs[b]["accept"],
                                odom=self.kf_odom[b])
-                ref.append(o.first(frames[b], odom[b]) if k == 0 else o.step(frames[b], odom[b], kfo))
-        new = [b for b in range(self.B) if rec[b]["new_kf"]]
+                ref.append(o.first(frames[b], odom[b]) if first else o.step(frames[b], odom[b], kfo))
+        new = [b for b in range(n) if rec[b]["new_kf"]]
         if new:
             self.t.reset(new, [self.dev[b]["view_mp"] for b in new])
             for b in new:
                 self.kf_odom[b] = odom[b].copy()
                 if self.orc:
                     self.orc[b].reset(self.streams[b][2]["view_mp"])
-        self.k += 1
+        for b in range(n):
+            self.ks[b] += 1
         return rec, ref
 
 
@@ -85,20 +94,25 @@ def compare_state(h, b, where):
     assert st["pre_meas"].tobytes() == o.meas.tobytes() and st["pre_cov"].ravel(order="F").tobytes() == o.cov.tobytes(), f"{where}: preSE2"
 
 
-def run_against_oracle(streams, cfg, frames, device_frames=False, eager=False):
-    h = Harness(streams, cfg, eager=eager)
+def check_step(h, rec, ref, k, seen):
+    """records and the state of the streams a call covered against their oracles; counts the branches reached in seen"""
+    for b in range(len(rec)):
+        got = {n: int(rec[b][n]) for n in rec.dtype.names}
+        assert got == ref[b], f"frame {k} stream {b}: {got} != {ref[b]}"
+        compare_state(h, b, f"frame {k} stream {b}")
+        for key, hit in (("first_low", got["first"] and not got["new_kf"]), ("gated", not got["first"] and not got["triangulated"]),
+                         ("new_kf", got["new_kf"] and not got["first"]), ("abort", got["abort_ba"]),
+                         ("cleared", not got["first"] and got["n_matched"] > 0 and got["n_inlier"] == 0),
+                         ("c1c2", got["new_kf"] and got["n_good_prl"] > 40), ("empty", got["n_keypoints"] == 0)):
+            seen[key] = seen.get(key, 0) + bool(hit)
+
+
+def run_against_oracle(streams, cfg, frames, device_frames=False, eager=False, layout=None, h=None):
+    h = h or Harness(streams, cfg, eager=eager)
     seen = {}
     for k in range(frames):
-        rec, ref = h.step(device_frames)
-        for b in range(h.B):
-            got = {n: int(rec[b][n]) for n in rec.dtype.names}
-            assert got == ref[b], f"frame {k} stream {b}: {got} != {ref[b]}"
-            compare_state(h, b, f"frame {k} stream {b}")
-            for key, hit in (("first_low", got["first"] and not got["new_kf"]), ("gated", not got["first"] and not got["triangulated"]),
-                             ("new_kf", got["new_kf"] and not got["first"]), ("abort", got["abort_ba"]),
-                             ("cleared", not got["first"] and got["n_matched"] > 0 and got["n_inlier"] == 0),
-                             ("c1c2", got["new_kf"] and got["n_good_prl"] > 40), ("empty", got["n_keypoints"] == 0)):
-                seen[key] = seen.get(key, 0) + bool(hit)
+        rec, ref = h.step(device_frames, layout=layout)
+        check_step(h, rec, ref, k, seen)
     return h, seen
 
 

@@ -17,8 +17,10 @@ F32 = np.float32
 DEPTH = 3.0
 
 
-def config(nfeatures=500, w=ts.W, h=ts.H, max_local_mps=2048):
-    c = ts.config(nfeatures=nfeatures, w=w, h=h)
+def config(nfeatures=500, w=ts.W, h=ts.H, max_local_mps=2048, **camera):
+    """tools/track_scenes.config (camera: fx, dist, fast_th) plus the Localizer's image bounds, Huber width and local-map
+    capacity"""
+    c = ts.config(nfeatures=nfeatures, w=w, h=h, **camera)
     c.update(bounds=(0.0, float(w), 0.0, float(h)), huber=float(np.sqrt(5.991)), max_local_mps=max_local_mps, w=w, h=h)
     return c
 
