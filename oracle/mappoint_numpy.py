@@ -42,6 +42,7 @@ class Restatement:
     def __init__(self, kf, mp, params):
         self.kf, self.mp, self.p = kf, mp, params
         self.trace = []
+        self.pkf0 = []                                     # (m, q, j0) of every updateParallax that chose a pKF0
         self.sf = np.asarray(params["scale_factors"], f32)
 
     # ------------------------------------------------------------------ helpers over list entries (positions j of point m)
@@ -60,6 +61,8 @@ class Restatement:
         v = [j for j in obs if not kf["kf_null"][self._kf(m, j)]]
         if len(v) < len(obs):
             self._ev(m, "null_kf_skipped")
+        if len(v) <= 32 < int(mp["obs_ptr"][m + 1] - mp["obs_ptr"][m]):
+            self._ev(m, "short_median_of_long_list")
         if not v:
             return
         d = [kf["desc"][self._slot(m, j)] for j in v]
@@ -76,6 +79,8 @@ class Restatement:
             self._ev(m, "main_unchanged")
             return
         self._ev(m, "main_changed")
+        if len(self.sf) != 8:
+            self._ev(m, "range_of_other_nlevels")
         mp["main_kf"][m] = k
         o = int(kf["kp"]["octave"][s])
         mp["main_octave"][m] = o
@@ -103,6 +108,7 @@ class Restatement:
             if j0 is None or self._id(m, j) < self._id(m, j0):
                 j0 = j
         self._ev(m, "pkf0_self" if j0 == q else "pkf0_older")
+        self.pkf0.append((m, q, j0))
         if any(idn - self._id(m, j) > 6 for j in obs):
             self._ev(m, "observer_beyond_6")
         T0, T1 = self._T(m, j0), self._T(m, q)
@@ -164,6 +170,8 @@ class Restatement:
                 obs.append(q); obs.sort()
                 was_null = bool(mp["null"][m])
                 self._main(m, obs)
+                if ab[m] and not mp["good_prl"][m] and len(obs) > 2:
+                    self._ev(m, "parallax_after_abandon")
                 ab[m] |= self._parallax(m, obs, q)
                 nn = _unit(self.kf["view_mp"][self._slot(m, q)])
                 n = mp["normal"][m]
@@ -182,6 +190,8 @@ class Restatement:
             obs = list(range(int(mp["obs_ptr"][m + 1] - mp["obs_ptr"][m])))
             for q in [int(x) for x in upd_pos[upd_ptr[m]:upd_ptr[m + 1]]]:
                 npos = _unit(self.kf["view_mp"][self._slot(m, q)])
+                if mp["main_kf"][m] == self._kf(m, q):
+                    self._ev(m, "erase_main")
                 obs.remove(q)
                 if not mp["null"][m] and not obs:
                     self._ev(m, "erased_to_empty")

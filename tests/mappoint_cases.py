@@ -49,3 +49,33 @@ def split_updates(sc):
         u2 += [last] if last is not None else []; u2p.append(len(u2))
     i4 = lambda x: np.asarray(x, np.int32)
     return (i4(ptr1), i4(kf1), i4(idx1), i4(u1p), i4(u1)), (i4(u2p), i4(u2))
+
+
+# scenes of update sequences and list shapes the families above do not build, and the events they must reach
+def many_updates_scene():
+    """3 to 8 adds per point without good parallax: abandonments followed by enough re-adds for updateParallax to run
+    on the rebuilt list"""
+    return ms.scene(400, seed=111, updates=(3, 8), good_frac=0.0, lengths=np.arange(400) % 30 + 8)
+
+
+def erase_main_scene():
+    """every point erases its whole list, each time the entry of its current main keyframe"""
+    return ms.scene(150, seed=211, mode="erase", erase_main=True, lengths=np.arange(150) % 40 + 1, kf_null_frac=0.1)
+
+
+LIST_LENGTHS = (31, 32, 33, 255, 256, 257, 1000, 4000)
+
+
+def list_length_scene(mode="add", lengths=LIST_LENGTHS):
+    """lists on both sides of the 32-entry shared-memory list and long ones, with null keyframes and 3 to 8 updates (absent
+    positions while an add runs, erased ones while an erase runs); every update of a list of N recomputes an N x N median"""
+    lengths = np.repeat(lengths, [2 if L <= 257 else 1 for L in lengths])          # one each of the longest
+    return ms.scene(len(lengths), seed=311 if mode == "add" else 312, lengths=lengths, mode=mode, good_frac=0.0,
+                    updates=(3, 8), kf_null_frac=0.15)
+
+
+NLEVELS = (1, 5, 12, 32)
+
+
+def nlevels_scene(nlevels, mode="add"):
+    return ms.scene(300, seed=500 + nlevels, mode=mode, nlevels=nlevels, updates=(1, 4), good_frac=0.2)

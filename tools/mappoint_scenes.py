@@ -25,18 +25,23 @@ def keyframe_chain(n_kf, rng, step=0.12, null_frac=0.03):
     return Tcw.astype(np.float32), kf_id, kf_null
 
 
-def scene(M, seed=0, n_kf=None, lengths=None, n_upd=(0.15, 0.65, 0.2), mode="add", good_frac=0.3, null_frac=0.02):
+def scene(M, seed=0, n_kf=None, lengths=None, n_upd=(0.15, 0.65, 0.2), mode="add", good_frac=0.3, null_frac=0.02,
+          updates=None, erase_main=False, kf_null_frac=0.03, nlevels=NLEVELS):
     """M points. lengths: the list length of every point (default 1..40 with a few LONG_LISTS). n_upd: probabilities of 0, 1
     and 2 updates per point. mode "add" picks update positions among the list, "erase" the same.
+    updates=(lo, hi) draws lo..hi updates per point instead of n_upd. erase_main (mode "erase") makes every point erase its
+    whole list, each time the entry of its current main keyframe. kf_null_frac is the share of null keyframes, nlevels the
+    pyramid's level count (octaves and scale factors).
     Returns dict(kf, mp, upd_ptr, upd_pos, params) with params the arguments of mappoint.params."""
     rng = np.random.default_rng(seed)
+    sf = SCALE_FACTORS if nlevels == NLEVELS else (np.float32(1.2) ** np.arange(nlevels, dtype=np.float32)).astype(np.float32)
     if lengths is None:
         lengths = np.minimum(rng.geometric(0.12, M), 40).astype(np.int64)
         long = rng.random(M) < 0.01
         lengths[long] = rng.choice(LONG_LISTS, int(long.sum()))
     lengths = np.asarray(lengths, np.int64)
     n_kf = n_kf or int(max(64, lengths.max() + 8))
-    Tcw, kf_id, kf_null = keyframe_chain(n_kf, rng)
+    Tcw, kf_id, kf_null = keyframe_chain(n_kf, rng, null_frac=kf_null_frac)
     Twc = np.linalg.inv(Tcw.astype(np.float64))
 
     start = (rng.random(M) * (n_kf - lengths + 1)).astype(np.int64)
@@ -74,7 +79,7 @@ def scene(M, seed=0, n_kf=None, lengths=None, n_upd=(0.15, 0.65, 0.2), mode="add
 
     kp = np.zeros(S, KP_DTYPE)
     kp["x"] = rng.uniform(0, 640, S); kp["y"] = rng.uniform(0, 480, S)
-    kp["octave"] = rng.integers(0, NLEVELS, S); kp["size"] = 31; kp["angle"] = -1; kp["class_id"] = -1
+    kp["octave"] = rng.integers(0, nlevels, S); kp["size"] = 31; kp["angle"] = -1; kp["class_id"] = -1
     kp["x"][slot] = uv[:, 0]; kp["y"][slot] = uv[:, 1]
     base = rng.integers(0, 256, (M, 32), dtype=np.uint8)
     desc = rng.integers(0, 256, (S, 32), dtype=np.uint8)
@@ -92,31 +97,56 @@ def scene(M, seed=0, n_kf=None, lengths=None, n_upd=(0.15, 0.65, 0.2), mode="add
     normal = Xw - Twc[start][:, :3, 3]
     normal /= np.linalg.norm(normal, axis=1, keepdims=True)
     main_octave = kp["octave"][first].astype(np.int32)
-    level_scale = SCALE_FACTORS[main_octave]
+    level_scale = sf[main_octave]
     dist = np.linalg.norm(view_mp[first].astype(np.float64), axis=1).astype(np.float32)
     mp = dict(pos=(Xw + rng.normal(0, 0.02, (M, 3))).astype(np.float32),
               good_prl=(rng.random(M) < good_frac).astype(np.uint8), null=(rng.random(M) < null_frac).astype(np.uint8),
               main_kf=main_kf, main_desc=desc[first].copy(), main_octave=main_octave,
               main_measure=np.stack([kp["x"][first], kp["y"][first]], 1).astype(np.float32),
               level_scale=level_scale.astype(np.float32), normal=normal.astype(np.float32),
-              min_dist=(dist * level_scale / SCALE_FACTORS[-1]).astype(np.float32), max_dist=(dist * level_scale).astype(np.float32),
+              min_dist=(dist * level_scale / sf[-1]).astype(np.float32), max_dist=(dist * level_scale).astype(np.float32),
               obs_ptr=obs_ptr, obs_kf=obs_kf, obs_idx=obs_idx)
     kf = dict(kf_id=kf_id, kf_null=kf_null, Tcw=Tcw, kp_base=kp_base, kp=kp, desc=desc, view_mp=view_mp, view_info=view_info)
 
     # updates: 0, 1 or 2 distinct list positions per point; adds favour the newest keyframes
-    nu = np.minimum(rng.choice(3, M, p=n_upd), lengths)
+    nu = np.minimum(rng.choice(3, M, p=n_upd) if updates is None else rng.integers(updates[0], updates[1] + 1, M), lengths)
+    if erase_main:
+        nu = lengths.copy()
     upd_ptr = np.zeros(M + 1, np.int32); upd_ptr[1:] = np.cumsum(nu)
     upd_pos = np.zeros(int(upd_ptr[-1]), np.int32)
     for m in np.nonzero(nu)[0]:
         L = int(lengths[m])
-        if mode == "add" and rng.random() < 0.7:
+        if erase_main:
+            pos = _main_first_order(kf_null[obs_kf[obs_ptr[m]:obs_ptr[m + 1]]], desc[slot[obs_ptr[m]:obs_ptr[m + 1]]],
+                                    0 if main_kf[m] >= 0 else None)
+        elif mode == "add" and rng.random() < 0.7:
             kfs = obs_kf[obs_ptr[m]:obs_ptr[m + 1]]
             pos = np.argsort(-kfs, kind="stable")[:nu[m]][::-1]            # the newest observers, oldest first
         else:
             pos = rng.choice(L, nu[m], replace=False)
         upd_pos[upd_ptr[m]:upd_ptr[m + 1]] = pos
     return dict(kf=kf, mp=mp, upd_ptr=upd_ptr, upd_pos=upd_pos,
-                params=dict(K=K, lower_depth=LOWER_DEPTH, upper_depth=UPPER_DEPTH, fx=FX, scale_factors=SCALE_FACTORS))
+                params=dict(K=K, lower_depth=LOWER_DEPTH, upper_depth=UPPER_DEPTH, fx=FX, scale_factors=sf))
+
+
+def _main_first_order(kf_null, desc, main):
+    """list positions in the order that erases the main keyframe's entry each time: `main` first (None: no main keyframe),
+    then the entry updateMainKFandDescriptor picks among the rest (least median Hamming distance over the entries of
+    non-null keyframes, first on ties), and any entry once only null keyframes remain"""
+    left = list(range(len(kf_null)))
+    order = []
+    while left:
+        valid = [j for j in left if not kf_null[j]]
+        if main is None or main not in left:
+            main = left[0]
+            if valid:
+                bits = np.unpackbits(desc[valid], axis=1).astype(np.int32)
+                D = (bits[:, None, :] != bits[None, :, :]).sum(2)
+                med = np.sort(D, axis=1)[:, int(0.5 * (len(valid) - 1))]
+                main = valid[int(np.argmin(med))]
+        order.append(main)
+        left.remove(main)
+    return np.array(order, np.int64)
 
 
 def copy_tables(sc):
