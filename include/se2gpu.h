@@ -636,6 +636,27 @@ int se2gpu_ba_optimize(se2gpu_ba* h, int max_iters, const volatile unsigned char
 int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, const volatile unsigned char* stop_flag,
                             se2gpu_ba_iter_stats* stats, double* trace_poses, double* trace_points);
 
+/* Optimise B loaded windows together: window k is contexts[k] (distinct contexts, all on one device, world 1, a window
+ * loaded, n <= 156 unknowns). Same semantics per window as se2gpu_ba_optimize(contexts[k], max_iters, ...): LM from
+ * iteration 0, estimates and LM state left in the context, so get / get_f32 / reset work as after optimize.
+ * stop_flags [B] (array and entries may be NULL) are polled between trials like setForceStopFlag. iterations [B]
+ * receives each window's iteration count; stats [B * max_iters] (window k at k * max_iters), trace_poses [B] /
+ * trace_points [B] (arrays of host pointers, may be NULL) as for se2gpu_ba_optimize. Ordered after the work already
+ * enqueued on every context's stream; runs on contexts[0]'s stream and returns when all windows are done. Returns 0 or a
+ * negative error; on a refusal no context changes, and the message names the offending window:
+ *   SE2GPU_ERR_INVALID   a NULL or repeated context, contexts on different devices, a sharded context, no window loaded,
+ *                        a context in multi-launch mode (se2gpu_ba_set_mode 1: the batch runs the persistent kernel);
+ *   SE2GPU_ERR_CAPACITY  n > 156 unknowns (se2gpu_ba_optimize's band and envelope solvers take those), or max_iters above
+ *                        a context's stats capacity.
+ * Each window runs on one thread-block cluster of 8 CTAs (SE2GPU_BA_BATCH_CLUSTER: 2 or 4 for one context, for measuring),
+ * one launch per cluster size present; a window's result equals se2gpu_ba_optimize's under SE2GPU_BA_PK_GRID = that size, byte for
+ * byte, whatever it is batched with. Until the call returns, no other thread may use any of the contexts. */
+int se2gpu_ba_optimize_batch(se2gpu_ba* const* contexts, int B, int max_iters,
+                             const volatile unsigned char* const* stop_flags, int* iterations,
+                             se2gpu_ba_iter_stats* stats, double* const* trace_poses, double* const* trace_points);
+/* test hook: the cluster size the batched launch uses for the window loaded in h; changes nothing */
+int se2gpu_ba_batch_cluster(se2gpu_ba* h);
+
 /* restore the estimates loaded by the last se2gpu_ba_set_problem (device-side copy; lets a caller re-run
  * optimize on the same window without re-uploading it) */
 int se2gpu_ba_reset(se2gpu_ba* h);

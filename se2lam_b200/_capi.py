@@ -162,6 +162,7 @@ SYMBOLS = [
     "se2gpu_ba_set_shard", "se2gpu_ba_peer_export", "se2gpu_ba_peer_import", "se2gpu_ba_set_stream", "se2gpu_ba_debug_system", "se2gpu_ba_reset", "se2gpu_ba_profile",
     "se2gpu_ba_profile_read", "se2gpu_ba_set_mode", "se2gpu_ba_get_f32", "se2gpu_ba_build_information", "se2gpu_ba_optimize_from", "se2gpu_ba_peer_attach_local",
     "se2gpu_ba_debug_plan", "se2gpu_ba_set_problem_device", "se2gpu_ba_build_information_device", "se2gpu_ba_debug_structure",
+    "se2gpu_ba_optimize_batch", "se2gpu_ba_batch_cluster",
     "se2gpu_voc_create", "se2gpu_voc_destroy", "se2gpu_voc_transform", "se2gpu_voc_transform_device", "se2gpu_median_descriptor",
     "se2gpu_triangulate", "se2gpu_triangulate_device", "se2gpu_track_triangulate", "se2gpu_track_triangulate_device",
     "se2gpu_xyz_info", "se2gpu_xyz_info_device", "se2gpu_projection_observations", "se2gpu_projection_observations_device",
@@ -259,6 +260,8 @@ def lib():
     L.se2gpu_ba_get_f32.argtypes = [vp, vp, vp]
     L.se2gpu_ba_optimize_from.argtypes = [vp, i, i, vp, vp, vp, vp]
     L.se2gpu_ba_peer_attach_local.argtypes = [vp, i]
+    L.se2gpu_ba_optimize_batch.argtypes = [vp, i, i, vp, vp, vp, vp, vp]
+    L.se2gpu_ba_batch_cluster.argtypes = [vp]
     L.se2gpu_ba_build_information.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, i, f, f, f, vp, i]
     L.se2gpu_ba_set_problem_device.argtypes = [vp, i, i, i, i] + [vp] * 11 + [d, d, d, vp, d]
     L.se2gpu_ba_build_information_device.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, i, f, f, f, vp, vp]

@@ -122,6 +122,33 @@ class LocalBA:
         return (n, st[:n], tp[:n], tl[:n]) if trace else (n, st[:n])
 
     @staticmethod
+    def optimize_batch(bas, iters, trace=False, stop_flags=None):
+        """Optimise the windows loaded in the contexts `bas` together (se2gpu_ba_optimize_batch): one thread-block cluster per
+        window, one launch per cluster size. Returns, per window, what `optimize(iters, trace)` returns. stop_flags: None or
+        one uint8 array of length 1 (or None) per window."""
+        B = len(bas)
+        arr = (C.c_void_p * B)(*[b.h if b is not None else None for b in bas])
+        st = np.zeros((B, max(iters, 1)), BA_STATS_DTYPE)
+        its = np.zeros(B, np.int32)
+        flags = None if stop_flags is None else (C.c_void_p * B)(*[ptr(f) for f in stop_flags])
+        tp = tl = tpa = tla = None
+        if trace:          # a None context gets no trace buffer; the library refuses it and names the window
+            tp = [np.zeros((max(iters, 1), b.P, 3)) if b is not None else None for b in bas]
+            tl = [np.zeros((max(iters, 1), b.L, 3)) if b is not None else None for b in bas]
+            tpa = (C.c_void_p * B)(*[ptr(x) for x in tp])
+            tla = (C.c_void_p * B)(*[ptr(x) for x in tl])
+        check(lib().se2gpu_ba_optimize_batch(arr, B, int(iters), flags, ptr(its), ptr(st), tpa, tla), "se2gpu_ba_optimize_batch")
+        out = []
+        for k in range(B):
+            n = int(its[k])
+            out.append((n, st[k, :n], tp[k][:n], tl[k][:n]) if trace else (n, st[k, :n]))
+        return out
+
+    def batch_cluster(self):
+        """Cluster size (CTAs) optimize_batch runs the loaded window on (se2gpu_ba_batch_cluster)."""
+        return check(lib().se2gpu_ba_batch_cluster(self.h), "se2gpu_ba_batch_cluster")
+
+    @staticmethod
     def attach_local(bas):
         """Peer exchange between several contexts of THIS process (one per GPU, or several on one GPU): rank order."""
         arr = (C.c_void_p * len(bas))(*[b.h for b in bas])

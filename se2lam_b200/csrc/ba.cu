@@ -12,6 +12,8 @@
 //     phases separated by grid barriers, LM control evaluated redundantly by every CTA;
 //   * one kernel per phase (large windows, sharded runs without peer exchange, set_mode(1)), the reduced system of a
 //     sharded run summed through the all-reduce callback.
+// ba_persistent's body is a template over the team of CTAs that runs one window (GridTeam / ClusterTeam):
+// ba_persistent_cluster runs it on one thread-block cluster per window, many windows per launch (se2gpu_ba_optimize_batch).
 // Both modes call the same LM phase functions (section "LM phase functions" below): pk_landmark (EdgeSE2XYZ error, Huber
 // weighting, Hll/bl, Hpl/PH records), pk_odo (PreEdgeSE2), lm_damp (damping terms), pk_pose_item and pose_odo_gather
 // (pose-side gather), schur_pairs / schur_odo / schur_pose_sweep (Schur gathers of ba_schur and pk_phase_schur_par),
@@ -36,6 +38,8 @@
 #include <chrono>
 #include <vector>
 #include <algorithm>
+#include <mutex>
+#include <unordered_map>
 
 #include "ba_context.h"
 #include "lm.h"
@@ -83,7 +87,11 @@ __device__ __forceinline__ double normalize_theta(double theta) {
 // EdgeSE2XYZ::computeError / linearizeOplus (EdgeSE2XYZ.cpp:61-106), closed form:
 // lc = Rcb Rz(-theta) (lw - (x,y,0)) + tcb ; e = fx*(lc.xy/lc.z) + c - uv ; M = Jpi Rcw ;
 // J_pose = [-M[:,0:2] | M (d.y,-d.x,0)^T] ; J_point = M
-template <bool JAC>
+// EXPLICIT: the camera-frame point as the rounding sequence nvcc contracts it to when the camera is a kernel parameter
+// (ba_persistent): fma(Rcw2, d2, fma(Rcw0, d0, Rcw1 * d1)) + tcb. ba_persistent_cluster reads the camera from shared memory;
+// left to itself nvcc then hoists Rcb2 * d2 out of the edge loop and rounds it on its own in one copy, and the two kernels
+// would differ in the last bits for a camera whose extrinsic products are inexact.
+template <bool JAC, bool EXPLICIT = false>
 __device__ __forceinline__ void edge_xyz(const Cam& cam, const double* __restrict__ ps, const double* __restrict__ lw,
                                          double u, double v, double* err, double* A, double* B) {
     double s, c;
@@ -97,8 +105,14 @@ __device__ __forceinline__ void edge_xyz(const Cam& cam, const double* __restric
     }
     const double d0 = lw[0] - ps[0], d1 = lw[1] - ps[1], d2 = lw[2];
     double lc[3];
+    if (EXPLICIT) {
 #pragma unroll
-    for (int r = 0; r < 3; ++r) lc[r] = Rcw[r * 3] * d0 + Rcw[r * 3 + 1] * d1 + Rcw[r * 3 + 2] * d2 + cam.tcb[r];
+        for (int r = 0; r < 3; ++r)
+            lc[r] = __dadd_rn(__fma_rn(Rcw[r * 3 + 2], d2, __fma_rn(Rcw[r * 3], d0, __dmul_rn(Rcw[r * 3 + 1], d1))), cam.tcb[r]);
+    } else {
+#pragma unroll
+        for (int r = 0; r < 3; ++r) lc[r] = Rcw[r * 3] * d0 + Rcw[r * 3 + 1] * d1 + Rcw[r * 3 + 2] * d2 + cam.tcb[r];
+    }
     const double zi = 1.0 / lc[2];
     err[0] = lc[0] * zi * cam.fx + cam.cx - u;
     err[1] = lc[1] * zi * cam.fx + cam.cy - v;
@@ -204,7 +218,7 @@ __device__ __forceinline__ void lm_damp(const Dev& d, int j, int beg, int end, i
 // per-edge Hpl and pose-side records. lam_fuse >= 0: the damping of the coming trial is already known, and the damping-
 // dependent landmark terms are formed here from the sums every lane of the group holds (the persistent kernel saves its
 // lm_prep phase and grid barrier that way). Returns the lane's share of the robust chi2.
-template <bool JAC, int LANES>
+template <bool JAC, int LANES, bool EXPLICIT = false>
 __device__ __forceinline__ double pk_landmark(const Dev& d, const Cam& cam, const double* xp, const double* xl, int j, int sub, double lam_fuse) {
     static_assert(LANES == 1 || LANES == LPL, "group_sum sums over LPL lanes");
     double chi = 0, h00 = 0, h01 = 0, h02 = 0, h11 = 0, h12 = 0, h22 = 0, b0 = 0, b1 = 0, b2 = 0;
@@ -217,7 +231,7 @@ __device__ __forceinline__ double pk_landmark(const Dev& d, const Cam& cam, cons
             const int p = d.e_pose[e];
             const double ps[3] = {xp[3 * p], xp[3 * p + 1], xp[3 * p + 2]};
             double er[2], A[6], B[6];
-            edge_xyz<JAC>(cam, ps, lw, d.e_u[e], d.e_v[e], er, A, B);
+            edge_xyz<JAC, EXPLICIT>(cam, ps, lw, d.e_u[e], d.e_v[e], er, A, B);
             const double w00 = d.e_w00[e], w01 = d.e_w01[e], w11 = d.e_w11[e];
             const double we0 = w00 * er[0] + w01 * er[1], we1 = w01 * er[0] + w11 * er[1];
             const double c2 = er[0] * we0 + er[1] * we1;
@@ -862,20 +876,46 @@ __device__ __forceinline__ void ldlt_stage(const Dev& d, const double* S, unsign
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) { unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
-// Two-sided solve of the reduced system on CTAs 0 and 1 of the persistent kernel (both resident: cooperative launch).
+// The CTAs that run one window in the persistent kernel ("team"): the cooperative grid (ba_persistent) or one thread-block
+// cluster (ba_persistent_cluster). rank() / size() are the CTA's place among the window's CTAs and their number; sync() ends a
+// phase. Phase functions read them through the type, as unsigned like blockIdx.x / gridDim.x, so that the grid instantiation
+// compiles to the code the grid-only kernel had.
+namespace cg = cooperative_groups;
+struct GridTeam {
+    static constexpr bool kExplicitFma = false;   // camera in parameter space: edge_xyz as written (see there)
+    cg::grid_group g;
+    __device__ __forceinline__ GridTeam() : g(cg::this_grid()) {}
+    static __device__ __forceinline__ unsigned rank() { return blockIdx.x; }
+    static __device__ __forceinline__ unsigned size() { return gridDim.x; }
+    __device__ __forceinline__ void sync() { g.sync(); }
+};
+// Cluster barrier: barrier.cluster.arrive.release + wait.acquire, which sm_90a compiles to MEMBAR.ALL.GPU, UCGABAR_ARV,
+// UCGABAR_WAIT and CCTL.IVALL - the L1 invalidation lets plain loads after it see what the other CTAs of the cluster stored
+// before it. Cluster scope is enough: everything one phase hands to the next (part_*, S / bs, tw_buf / tw_flag, the LM state
+// and the per-landmark and per-edge arrays) belongs to the window, and only the window's own CTAs read it.
+struct ClusterTeam {
+    static constexpr bool kExplicitFma = true;    // camera in shared memory: edge_xyz's contraction spelled out (see there)
+    static __device__ __forceinline__ unsigned rank() { return cg::this_cluster().block_rank(); }
+    static __device__ __forceinline__ unsigned size() { return cg::this_cluster().num_blocks(); }
+    __device__ __forceinline__ void sync() { cg::this_cluster().sync(); }
+};
+
+// Two-sided solve of the reduced system on CTAs 0 and 1 of the persistent kernel (both resident: cooperative launch, or
+// one cluster, whose CTAs the hardware co-schedules).
 // The pivot chain - one dependent 3x3 inverse per pose block - is the critical path of the single-CTA solve; the envelope of a
 // local window is a narrow band, so the blocks split into top [0, m0), separator [m0, m0 + w) and bottom [m0 + w, nb) with no
 // top-bottom coupling. CTA 0 eliminates the top blocks of S[0 : 3(m0+w)) in place; CTA 1 eliminates the bottom blocks on the
 // index-reversed copy A1[r'][c'] = S[n-1-c'][n-1-r'] (lower triangle -> lower triangle, same code); its separator update goes to
 // CTA 0 through tw_buf, CTA 0 finishes the separator blocks, back-substitutes and hands the separator solution back as soon as it
 // exists. Chain length max(m0, nb - m0 - w) + w instead of nb. `seq` counts the solves of this launch from 1.
+template <class Team>
 __device__ void ldlt_twisted_solve(const Dev& d, const double* S, const double* bs, unsigned long long* bar, unsigned parity, unsigned seq) {
     extern __shared__ double sm[];
     __shared__ double xs[3 * TW_MAX_W];
     const int n = d.n, nb = n / 3, m0 = d.tw_m0, w = d.tw_w, m1 = nb - m0 - w, w3 = 3 * w;
     const int tid = threadIdx.x, nt = blockDim.x;
     double* T = d.tw_buf;
-    if (blockIdx.x == 0) {
+    if (Team::rank() == 0) {
         const int n0 = 3 * (m0 + w);
         // layout: A [n0 rows, leading dimension n] | y [n0] | W [3 n0] | pad [2] | cmax (int) [n0] | scratch
         double* y = sm + (size_t)n0 * n;
@@ -1059,7 +1099,6 @@ __global__ void __launch_bounds__(256) ba_decide(Dev d, int nb_scale, int phase,
 // control (rho test, lambda schedule, accept/reject, termination) is evaluated redundantly and identically by every
 // CTA from the same fixed-order partial sums, so no host round trip happens inside an optimize() call.
 // Per-landmark work is spread over LPL lanes (edges strided over the lanes, xor-tree over the lane group).
-namespace cg = cooperative_groups;
 constexpr int FALLBACK_CLOCK_KHZ = 1980000;   // H100 SXM maximum SM clock: cycle <-> time conversion if the device does not report one
 
 struct PKArgs {
@@ -1073,12 +1112,12 @@ struct PKArgs {
     int* abort_dev;           // [2] published copies (slot 0: written in phase A, slot 1: in phase F; read by all CTAs after the
                               // grid barrier that ends the phase - two slots so that a CTA running ahead into the next phase
                               // never overwrites a word a slower CTA has yet to read)
-    double* part_chi;         // [2][gridDim.x]: row 0 = phase A (linearisation at x_cur), row 1 = phase F (chi2 at the trial point)
-    double* part_scale;       // [gridDim.x]
-    double* part_max;         // [gridDim.x]
+    double* part_chi;         // [2][team size]: row 0 = phase A (linearisation at x_cur), row 1 = phase F (chi2 at the trial point)
+    double* part_scale;       // [team size]
+    double* part_max;         // [team size]
     long long* phase_cycles;  // [8] SM cycles CTA 0 spent per phase incl. the barrier that ends it (profiling aid)
     int dyn_smem_bytes;       // dynamic shared memory of the launch (arena size of the non-zero CTAs)
-    long long* cta_work;      // [gridDim.x][8] per-CTA busy cycles per phase (debug aid, null = off)
+    long long* cta_work;      // [team size][10] per-CTA busy cycles per phase (debug aid, null = off)
 };
 
 // Multi-GPU hooks of the persistent kernel (sharded runs on one NVLink node, se2gpu_ba_peer_import / _peer_attach_local): every
@@ -1103,6 +1142,13 @@ struct PKShard {
     const int* env_idx;                // linear indices (into [S | bs]) of the entries inside the envelope of S, then of bs
     int nenv;
 };
+// what one cluster of ba_persistent_cluster optimises (8-byte multiple: copied as 64-bit words)
+struct PKWindow {
+    Dev d;
+    Cam cam;
+    PKArgs pa;
+};
+static_assert(sizeof(PKWindow) % 8 == 0, "PKWindow is copied in 8-byte words");
 constexpr int XCH_HDR = 16;            // doubles: [0] S flag, [1] scalar flag (as long long), rest padding
 
 __device__ __forceinline__ void pk_publish(const PKShard& sh, int which, long long epoch) {     // CTA 0, thread 0, after a grid barrier
@@ -1111,9 +1157,10 @@ __device__ __forceinline__ void pk_publish(const PKShard& sh, int which, long lo
     __threadfence_system();
 }
 // all threads of all CTAs; returns false on peer timeout (uniform across the grid)
+template <class Team>
 __device__ bool pk_wait_peers(const PKShard& sh, int which, long long epoch) {
     __shared__ long long s_go;
-    if (blockIdx.x == 0) {
+    if (Team::rank() == 0) {
         int ok = 1;
         if ((int)threadIdx.x < sh.world && (int)threadIdx.x != sh.rank) {
             const volatile long long* f = reinterpret_cast<const volatile long long*>(sh.xch[threadIdx.x] + which);
@@ -1142,8 +1189,9 @@ __device__ bool pk_wait_peers(const PKShard& sh, int which, long long epoch) {
 // every CTA: ssum[e] = sum over ranks of red[r][e], rank order, for the entries e inside the envelope of the reduced system
 // (the lower triangle within colmax[] - everything the Schur phase can write - and the right-hand side): a few percent of the
 // dense n x n array for a local window, so the exchange moves kilobytes, not the whole buffer. ssum stays zero elsewhere.
+template <class Team>
 __device__ void pk_sum_partials(const PKShard& sh) {
-    const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gthreads = gridDim.x * blockDim.x;
+    const int gtid = Team::rank() * blockDim.x + threadIdx.x, gthreads = Team::size() * blockDim.x;
     for (int v = gtid; v < sh.nenv; v += gthreads) {
         const int e = sh.env_idx[v];
         double t[MAX_PEERS];
@@ -1171,9 +1219,10 @@ __device__ double cta_sum_array(const double* a, int n, double* sh) {
     return out;
 }
 // Landmark work of the persistent kernel: lane groups (LPL lanes per landmark) are dealt to the CTAs round-robin, so every
-// SM gets L / gridDim.x landmarks on its first warps instead of the first CTAs running all 16 warps while the rest
+// SM gets L / Team::size() landmarks on its first warps instead of the first CTAs running all 16 warps while the rest
 // idle (the phases are FP64-issue bound per SM). Whole warps iterate together (the lane-group shuffles need them): the
 // loop bound is the warp's first landmark; landmarks >= L are skipped inside the bodies.
+template <class Team>
 struct PKLmIter {
     int j, sub, step, j_warp;
     // In a sharded run only the landmarks j % world == rank carry work on this rank: the lane groups are dealt over THOSE (the
@@ -1182,26 +1231,26 @@ struct PKLmIter {
     __device__ __forceinline__ PKLmIter(const Dev& d) {
         const int lg = threadIdx.x / LPL;                       // lane group inside the CTA
         sub = threadIdx.x % LPL;
-        j = (lg * gridDim.x + blockIdx.x) * d.world + d.rank;
-        j_warp = ((threadIdx.x / 32) * (32 / LPL) * gridDim.x + blockIdx.x) * d.world + d.rank;
-        step = (blockDim.x / LPL) * gridDim.x * d.world;
+        j = (lg * Team::size() + Team::rank()) * d.world + d.rank;
+        j_warp = ((threadIdx.x / 32) * (32 / LPL) * Team::size() + Team::rank()) * d.world + d.rank;
+        step = (blockDim.x / LPL) * Team::size() * d.world;
     }
     __device__ __forceinline__ bool more(int L) const { return j_warp < L; }
     __device__ __forceinline__ void next() { j += step; j_warp += step; }
 };
 
-template <bool JAC>
+template <class Team, bool JAC>
 __device__ void pk_phase_linearize(const Dev& d, const Cam& cam, int xi, double* part, double* sh, double lam_fuse = -1.0) {
     const double* xp = d.xp[xi];
     const double* xl = d.xl[xi];
     double chi = 0;
-    for (PKLmIter it(d); it.more(d.L); it.next()) chi += pk_landmark<JAC, LPL>(d, cam, xp, xl, it.j, it.sub, lam_fuse);
+    for (PKLmIter<Team> it(d); it.more(d.L); it.next()) chi += pk_landmark<JAC, LPL, Team::kExplicitFma>(d, cam, xp, xl, it.j, it.sub, lam_fuse);
     // PreEdgeSE2 edges: one per CTA on the first lane of the last warp (idle unless a CTA holds > 60 landmarks), so that no CTA
     // serialises all of them behind its landmark work (they used to sit on CTA 0 and made it the slowest of the phase)
     if (threadIdx.x == blockDim.x - 32)
-        for (int o = blockIdx.x; o < d.O; o += gridDim.x) chi += pk_odo<JAC>(d, xp, o);
+        for (int o = Team::rank(); o < d.O; o += Team::size()) chi += pk_odo<JAC>(d, xp, o);
     const double tot = block_sum(chi, sh);
-    if (threadIdx.x == 0) part[blockIdx.x] = tot;
+    if (threadIdx.x == 0) part[Team::rank()] = tot;
 }
 
 // Static work lists of a persistent CTA, cached once per optimize() in its (otherwise unused) dynamic shared memory:
@@ -1419,9 +1468,10 @@ __device__ void pk_phase_schur_par(const Dev& d, double lam, const PKWork& w, co
     }
 }
 
+template <class Team>
 __device__ void pk_phase_lm_prep(const Dev& d, double lam) {
     const size_t L = d.L;
-    for (PKLmIter it(d); it.more(d.L); it.next()) {
+    for (PKLmIter<Team> it(d); it.more(d.L); it.next()) {
         const int j = it.j;
         if (j >= d.L) continue;
         const int beg = d.lm_ptr[j], end = d.lm_ptr[j + 1];
@@ -1435,6 +1485,7 @@ __device__ void pk_phase_lm_prep(const Dev& d, double lam) {
 // trial point (*chi_out), with no grid barrier in between. The chi2 of a landmark's edges needs the landmark's trial point (formed
 // by the same lane group a few instructions earlier) and the trial POSES: every CTA forms all of them itself first (P is a few
 // dozen; all CTAs store identical values, and a CTA reads back only what it stored itself before its block barrier).
+template <class Team>
 __device__ double pk_phase_backsub(const Dev& d, const Cam& cam, int cur, double lam, double lam_pose, double* chi_out) {
     const double* xp = d.xp[cur];
     const double* xl = d.xl[cur];
@@ -1444,7 +1495,7 @@ __device__ double pk_phase_backsub(const Dev& d, const Cam& cam, int cur, double
     double sc = 0, chi = 0;
     for (int t = threadIdx.x; t < d.P; t += blockDim.x) pose_oplus(d, t, xp, xpt);
     __syncthreads();
-    for (PKLmIter it(d); it.more(d.L); it.next()) {
+    for (PKLmIter<Team> it(d); it.more(d.L); it.next()) {
         const int j = it.j, sub = it.sub;
         int beg = 0, end = 0;
         if (j < d.L) { beg = d.lm_ptr[j]; end = d.lm_ptr[j + 1]; }
@@ -1472,22 +1523,24 @@ __device__ double pk_phase_backsub(const Dev& d, const Cam& cam, int cur, double
             xlt[3 * j] = xl[3 * j] + dl0; xlt[3 * j + 1] = xl[3 * j + 1] + dl1; xlt[3 * j + 2] = xl[3 * j + 2] + dl2;
         }
         __syncwarp();                                           // the group's other lanes read the trial point back
-        chi += pk_landmark<false, LPL>(d, cam, xpt, xlt, j, sub, -1.0);
+        chi += pk_landmark<false, LPL, Team::kExplicitFma>(d, cam, xpt, xlt, j, sub, -1.0);
     }
     // pose terms of computeScale and the PreEdgeSE2 chi2: one item per CTA on the first lane of the last warp (see pk_phase_linearize)
     if (threadIdx.x == blockDim.x - 32) {
-        for (int t = blockIdx.x; t < d.P; t += gridDim.x) {
+        for (int t = Team::rank(); t < d.P; t += Team::size()) {
             const int a = d.hidx[t];
             if (a >= 0) sc += pose_scale(d, a, lam_pose);
         }
-        for (int o = blockIdx.x; o < d.O; o += gridDim.x) chi += pk_odo<false>(d, xpt, o);
+        for (int o = Team::rank(); o < d.O; o += Team::size()) chi += pk_odo<false>(d, xpt, o);
     }
     *chi_out = chi;
     return sc;
 }
 
-__global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, PKArgs pa, PKShard shd) {
-    cg::grid_group grid = cg::this_grid();
+// The whole optimize() of one window on the CTAs of `team` (see GridTeam / ClusterTeam). The LM arguments are taken by value:
+// bound by reference to ba_persistent's parameter they cost it spill traffic (ptxas, sm_90a, CUDA 12.9).
+template <class Team>
+__device__ __forceinline__ void pk_optimize(Team& team, const Dev& d, const Cam& cam, const PKArgs pa, const PKShard& shd) {
     __shared__ double sh[32];
     __shared__ double shv[(PK_THREADS / 32) * 21];
     __shared__ __align__(8) unsigned long long stage_bar;
@@ -1502,10 +1555,10 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
     double* red_scratch = sm + (pa.dyn_smem_bytes - RED_SCRATCH_BYTES) / 8;      // worker CTAs only (CTA 0 keeps its arena for the solve)
     PKWork work;
     {
-        const int G = gridDim.x;
+        const int G = Team::size();
         const int nsolve = d.tw_m0 > 0 ? 2 : 1;             // CTAs that keep their shared memory for the reduced solve
         work.stride = G > 1 ? G - nsolve : 1;
-        work.first = G > 1 ? (int)blockIdx.x - nsolve : 0;  // < 0 for the solver CTAs of a multi-CTA grid
+        work.first = G > 1 ? (int)Team::rank() - nsolve : 0;  // < 0 for the solver CTAs of a multi-CTA grid
         work.own = own;
         work.arena = reinterpret_cast<const int*>(sm);
         int* arena = reinterpret_cast<int*>(sm);
@@ -1554,14 +1607,14 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
         }
     }
     __syncthreads();
-    const int n = d.n, nparts = gridDim.x;
+    const int n = d.n, nparts = Team::size();
     const bool shard = shd.world > 1;
     const double* Ssrc = shard ? shd.ssum : d.S;                   // what the solve stages: the rank-summed system in sharded runs
     const double* bsrc = shard ? shd.ssum + (size_t)n * n : d.bs;
     double lambda = d.st->lambda, ni = d.st->ni, chi_cur = d.st->chi_cur;   // continued from the previous call when first_iter > 0
     long long epoch = shd.epoch0;
     unsigned tw_seq = 0;
-    if (d.tw_m0 > 0 && blockIdx.x == 0 && threadIdx.x == 0) { d.tw_flag[0] = 0; d.tw_flag[1] = 0; d.tw_flag[2] = 0; }   // first use is several grid barriers away
+    if (d.tw_m0 > 0 && Team::rank() == 0 && threadIdx.x == 0) { d.tw_flag[0] = 0; d.tw_flag[1] = 0; d.tw_flag[2] = 0; }   // first use is several grid barriers away
     int cur = d.st->cur, done = 0;
     bool stop = false, peer_err = false;
     // scalar exchange of a sharded run: CTA 0 fills this rank's slot `epoch & 1` with v[0..nv) (+ the pose diagonal when
@@ -1576,22 +1629,22 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
         const int itg = pa.first_iter + it;                       // g2o's iteration number
         // ---- A: linearise at x_cur (computeActiveErrors + buildSystem). For itg > 0 the damping of the first trial is already
         // known, so the damping-dependent landmark terms are formed in the same pass (no phase B, one grid barrier less).
-        pk_phase_linearize<true>(d, cam, cur, pa.part_chi, sh, itg > 0 ? lambda : -1.0);
-        if (blockIdx.x == 0 && threadIdx.x == 0) pa.abort_dev[0] = *pa.abort_host;
+        pk_phase_linearize<Team, true>(d, cam, cur, pa.part_chi, sh, itg > 0 ? lambda : -1.0);
+        if (Team::rank() == 0 && threadIdx.x == 0) pa.abort_dev[0] = *pa.abort_host;
         PK_WORK(0);
-        grid.sync();
+        team.sync();
         PK_TICK(0);
         if (!shard && pa.abort_dev[0]) break;                      // sharded runs take the abort decision collectively (below)
         if (itg == 0) {
             // ---- B (first iteration only): pose-side gather and landmark diagonal maximum for lambda_0 = 1e-5 max|diag H|
             pk_phase_pose_reduce(d, work, shv);
             double m = 0;
-            for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < d.L; j += gridDim.x * blockDim.x)
+            for (int j = Team::rank() * blockDim.x + threadIdx.x; j < d.L; j += Team::size() * blockDim.x)
                 if (d.lm_ptr[j + 1] > d.lm_ptr[j]) m = fmax(m, diag_absmax(d.Hll, d.L, j));
             m = cta_max(m, sh);
-            if (threadIdx.x == 0) pa.part_max[blockIdx.x] = m;
+            if (threadIdx.x == 0) pa.part_max[Team::rank()] = m;
             PK_WORK(1);
-            grid.sync();
+            team.sync();
             PK_TICK(1);
         }
         if (!shard || it == 0) chi_cur = cta_sum_array(pa.part_chi, nparts, sh);   // sharded: afterwards the accepted trial's global chi2 is carried
@@ -1606,14 +1659,14 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
                 // lambda_0 needs the maximum over ALL landmarks and over the rank-SUMMED pose diagonal; chi2 and the abort flag ride along
                 m = cta_max(m, sh);
                 ++epoch;
-                if (blockIdx.x == 0) {
+                if (Team::rank() == 0) {
                     double* slot = shd.my_xch + XCH_HDR + (size_t)(epoch & 1) * shd.xslot;
                     if (threadIdx.x == 0) { slot[0] = chi_cur; slot[1] = 0.0; slot[2] = pa.abort_dev[0] ? 1.0 : 0.0; slot[3] = m; }
                     for (int a = threadIdx.x; a < d.nf; a += blockDim.x) { slot[8 + 3 * a] = d.Hpp[a]; slot[8 + 3 * a + 1] = d.Hpp[3 * nf + a]; slot[8 + 3 * a + 2] = d.Hpp[5 * nf + a]; }
                     __syncthreads();
                     if (threadIdx.x == 0) pk_publish(shd, 1, epoch);
                 }
-                if (!pk_wait_peers(shd, 1, epoch)) { peer_err = true; break; }
+                if (!pk_wait_peers<Team>(shd, 1, epoch)) { peer_err = true; break; }
                 double chi = 0, ab = 0, mm = 0;
                 for (int r = 0; r < shd.world; ++r) { const double* sl = xslot_of(r, epoch); chi += __ldcv(sl); ab += __ldcv(sl + 2); mm = fmax(mm, __ldcv(sl + 3)); }
                 for (int q = threadIdx.x; q < 3 * d.nf; q += blockDim.x) {
@@ -1629,12 +1682,12 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
         } else if (shard && it == 0) {
             // continuation call of a sharded run: this rank's chi2 partial -> global (one scalar exchange)
             ++epoch;
-            if (blockIdx.x == 0 && threadIdx.x == 0) {
+            if (Team::rank() == 0 && threadIdx.x == 0) {
                 double* slot = shd.my_xch + XCH_HDR + (size_t)(epoch & 1) * shd.xslot;
                 slot[0] = chi_cur; slot[1] = 0.0; slot[2] = pa.abort_dev[0] ? 1.0 : 0.0; slot[3] = 0.0;
                 pk_publish(shd, 1, epoch);
             }
-            if (!pk_wait_peers(shd, 1, epoch)) { peer_err = true; break; }
+            if (!pk_wait_peers<Team>(shd, 1, epoch)) { peer_err = true; break; }
             double chi = 0, ab = 0;
             for (int r = 0; r < shd.world; ++r) { const double* sl = xslot_of(r, epoch); chi += __ldcv(sl); ab += __ldcv(sl + 2); }
             chi_cur = chi;
@@ -1648,54 +1701,54 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
             // ---- P: damping-dependent per-landmark terms (first trial of itg > 0: already formed in phase A)
             PK_TICK(6);
             if (itg == 0 || trials > 0) {
-                pk_phase_lm_prep(d, lambda);
+                pk_phase_lm_prep<Team>(d, lambda);
                 PK_WORK(2);
-                grid.sync();
+                team.sync();
             }
             PK_TICK(2);
             // ---- C: Schur complement gather
             if (s_plan_ok) pk_phase_schur_par(d, lambda * lam_pose_mask, work, plan_w0, plan_nw, shv, red_scratch, pa.cta_work ? wacc : nullptr);
             else pk_phase_schur(d, lambda * lam_pose_mask, work, shv);
             PK_WORK(3);
-            grid.sync();
+            team.sync();
             PK_TICK(3);
             if (shard) {
                 // ---- X1: the all-reduce of the reduced system, inside the kernel: publish, wait for the peers, sum the ranks' buffers
                 ++epoch;
-                if (blockIdx.x == 0 && threadIdx.x == 0) pk_publish(shd, 0, epoch);
-                if (!pk_wait_peers(shd, 0, epoch)) { peer_err = true; break; }
-                pk_sum_partials(shd);
-                grid.sync();
+                if (Team::rank() == 0 && threadIdx.x == 0) pk_publish(shd, 0, epoch);
+                if (!pk_wait_peers<Team>(shd, 0, epoch)) { peer_err = true; break; }
+                pk_sum_partials<Team>(shd);
+                team.sync();
                 PK_TICK(1);
             }
             // ---- D: reduced solve (one CTA; S staged into its shared memory)
             if (d.tw_m0 > 0) {
                 ++tw_seq;
-                if (blockIdx.x < 2) ldlt_twisted_solve(d, Ssrc, bsrc, &stage_bar, stage_parity, tw_seq);
+                if (Team::rank() < 2) ldlt_twisted_solve<Team>(d, Ssrc, bsrc, &stage_bar, stage_parity, tw_seq);
                 stage_parity ^= 1;
-            } else if (blockIdx.x == 0) {
+            } else if (Team::rank() == 0) {
                 ldlt_stage(d, Ssrc, &stage_bar, stage_parity);
                 stage_parity ^= 1;
                 PK_TICK(7);
                 ldlt_block_solve<true>(nullptr, nullptr, n, nullptr, bsrc, d.dxp, d.st);
             }
             PK_WORK(4);
-            grid.sync();
+            team.sync();
             PK_TICK(4);
             const int solve_ok = d.st->solve_ok;
             // ---- E: back-substitution, oplus into the trial buffers, computeScale partials
             //      + F: robust chi2 at the trial point (same phase, see pk_phase_backsub)
             {
                 double chi_part;
-                const double sc = pk_phase_backsub(d, cam, cur, lambda, lambda * lam_pose_mask, &chi_part);
+                const double sc = pk_phase_backsub<Team>(d, cam, cur, lambda, lambda * lam_pose_mask, &chi_part);
                 const double tot = block_sum(sc, sh);
-                if (threadIdx.x == 0) pa.part_scale[blockIdx.x] = tot;
+                if (threadIdx.x == 0) pa.part_scale[Team::rank()] = tot;
                 const double totc = block_sum(chi_part, sh);
-                if (threadIdx.x == 0) pa.part_chi[nparts + blockIdx.x] = totc;
+                if (threadIdx.x == 0) pa.part_chi[nparts + Team::rank()] = totc;
             }
-            if (blockIdx.x == 0 && threadIdx.x == 0) pa.abort_dev[1] = *pa.abort_host;
+            if (Team::rank() == 0 && threadIdx.x == 0) pa.abort_dev[1] = *pa.abort_host;
             PK_WORK(5);
-            grid.sync();
+            team.sync();
             PK_TICK(5);
             // ---- LM decision (identical in every CTA, and in every rank)
             double tempChi = cta_sum_array(pa.part_chi + nparts, nparts, sh);
@@ -1704,12 +1757,12 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
             if (shard) {
                 // ---- X2: [chi2, scale, abort] summed over the ranks
                 ++epoch;
-                if (blockIdx.x == 0 && threadIdx.x == 0) {
+                if (Team::rank() == 0 && threadIdx.x == 0) {
                     double* slot = shd.my_xch + XCH_HDR + (size_t)(epoch & 1) * shd.xslot;
                     slot[0] = tempChi; slot[1] = scale; slot[2] = ab; slot[3] = 0.0;
                     pk_publish(shd, 1, epoch);
                 }
-                if (!pk_wait_peers(shd, 1, epoch)) { peer_err = true; break; }
+                if (!pk_wait_peers<Team>(shd, 1, epoch)) { peer_err = true; break; }
                 tempChi = 0; scale = 0; ab = 0;
                 for (int r = 0; r < shd.world; ++r) { const double* sl = xslot_of(r, epoch); tempChi += __ldcv(sl); scale += __ldcv(sl + 1); ab += __ldcv(sl + 2); }
             }
@@ -1719,21 +1772,40 @@ __global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, P
         } while (lm_retry(rho, trials) && !stop);
         if (peer_err) break;
         const se2gpu_ba_iter_stats o = lm_iter_stats(chi_before, chi_cur, lambda, rho, trials, accepted);
-        if (blockIdx.x == 0 && threadIdx.x == 0 && pa.stats) pa.stats[it] = o;
-        if (pa.trace_p) for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * d.P; i += gridDim.x * blockDim.x) pa.trace_p[(size_t)it * 3 * d.P + i] = d.xp[cur][i];
-        if (pa.trace_l) for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * d.L; i += gridDim.x * blockDim.x) pa.trace_l[(size_t)it * 3 * d.L + i] = d.xl[cur][i];
+        if (Team::rank() == 0 && threadIdx.x == 0 && pa.stats) pa.stats[it] = o;
+        if (pa.trace_p) for (int i = Team::rank() * blockDim.x + threadIdx.x; i < 3 * d.P; i += Team::size() * blockDim.x) pa.trace_p[(size_t)it * 3 * d.P + i] = d.xp[cur][i];
+        if (pa.trace_l) for (int i = Team::rank() * blockDim.x + threadIdx.x; i < 3 * d.L; i += Team::size() * blockDim.x) pa.trace_l[(size_t)it * 3 * d.L + i] = d.xl[cur][i];
         ++done;
         if (o.terminate) stop = true;
     }
     PK_TICK(6);
 #undef PK_TICK
 #undef PK_WORK
-    if (pa.cta_work && threadIdx.x == 0) for (int g = 0; g < 10; ++g) pa.cta_work[blockIdx.x * 10 + g] = wacc[g];
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (pa.cta_work && threadIdx.x == 0) for (int g = 0; g < 10; ++g) pa.cta_work[Team::rank() * 10 + g] = wacc[g];
+    if (Team::rank() == 0 && threadIdx.x == 0) {
         LMState& s = *d.st;
         s.cur = cur; s.lambda = lambda; s.ni = ni; s.chi_cur = chi_cur; s.iter = done; s.epoch = epoch; s.error = peer_err ? 1 : 0;
         if (pa.phase_cycles) for (int g = 0; g < 8; ++g) pa.phase_cycles[g] += tacc[g];
     }
+}
+
+__global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent(Dev d, Cam cam, PKArgs pa, PKShard shd) {
+    GridTeam team;
+    pk_optimize(team, d, cam, pa, shd);
+}
+
+// One window per thread-block cluster: cluster k optimises window k of the launch. The descriptor is copied once into shared
+// memory from a device array the host fills per call (a parameter block would bound the batch by the 32 KB parameter limit:
+// a descriptor is about 0.8 KB); the phases then read it as ba_persistent reads its parameters.
+__global__ void __launch_bounds__(PK_THREADS, 1) ba_persistent_cluster(const PKWindow* __restrict__ windows) {
+    __shared__ PKWindow w;
+    const PKWindow* src = windows + blockIdx.x / ClusterTeam::size();
+    for (int i = threadIdx.x; i < (int)(sizeof(PKWindow) / 8); i += blockDim.x)
+        reinterpret_cast<unsigned long long*>(&w)[i] = reinterpret_cast<const unsigned long long*>(src)[i];
+    __syncthreads();
+    ClusterTeam team;
+    const PKShard shd{};    // world 0: the batch runs unsharded windows only
+    pk_optimize(team, w.d, w.cam, w.pa, shd);
 }
 
 // Map::optimizeLocalGraph write-back (Map.cpp:768-779): KeyFrame::setPose(Se2(vp(0), vp(1), vp(2))) narrows the pose to float
@@ -1761,6 +1833,7 @@ Switches read_switches() {
     sw.debug = getenv("SE2GPU_BA_DEBUG") != nullptr;
     sw.no_band = getenv("SE2GPU_BA_NO_BAND") != nullptr;
     sw.no_twist = getenv("SE2GPU_BA_NO_TWIST") != nullptr;
+    if (const char* c = getenv("SE2GPU_BA_BATCH_CLUSTER")) { const int v = atoi(c); if (v == 2 || v == 4 || v == 8) sw.batch_cluster = v; }
     return sw;
 }
 
@@ -2022,6 +2095,7 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
             SE2_CUDA(h->bufs.regrow(&h->trace_l, (size_t)max_iters * 3 * h->L));
             h->trace_cap_l = (size_t)max_iters * 3 * h->L;
         }
+        if (const int rc = plan_for_grid(h, h->pk_grid)) return rc;     // after a batched optimize the plan was made for a cluster
         *h->abort_host = (stop_flag && *stop_flag) ? 1 : 0;
         PKShard shd{};
         shd.world = h->world; shd.rank = h->rank;
@@ -2137,6 +2211,162 @@ int se2gpu_ba_optimize_from(se2gpu_ba* h, int first_iteration, int max_iters, co
     }
     SE2_CUDA(cudaStreamSynchronize(s));
     return done;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Cluster size of the batched launch: 8 CTAs for every window. Measured against 2 and 4 on windows of 9, 19 and 49 free poses
+// at B = 1 to 64 (tools/ba_batch_bench.py, DESIGN.md section 3 "Batches of windows"), 8 was the fastest on every workload, so
+// no rule depends on the window. It never depends on the batch, so a window's bytes do not depend on its batchmates.
+// SE2GPU_BA_BATCH_CLUSTER sets another size per context, for measuring.
+constexpr int kBatchCluster = 8;
+int batch_cluster_size(const se2gpu_ba* h) { return h->sw.batch_cluster ? h->sw.batch_cluster : kBatchCluster; }
+
+// At first use of a cluster size on a device: the launch attribute for the largest window and the scheduling check. A size
+// the device cannot schedule is an error; another size would give other results.
+int check_cluster_size(int device, int C) {
+    static std::mutex mu;
+    static bool ok[se2gpu::kMaxDevices][9] = {};
+    if (device < 0 || device >= se2gpu::kMaxDevices) return fail(SE2GPU_ERR_INVALID, "device %d", device);
+    std::lock_guard<std::mutex> lock(mu);
+    if (ok[device][C]) return SE2GPU_OK;
+    const int smem_max = (int)pk_dyn_smem_bytes(SMEM_CHOL_MAX_N);
+    SE2_CUDA(cudaFuncSetAttribute(ba_persistent_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = C; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(C); cfg.blockDim = dim3(PK_THREADS); cfg.dynamicSmemBytes = smem_max; cfg.attrs = &attr; cfg.numAttrs = 1;
+    int clusters = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveClusters(&clusters, (void*)ba_persistent_cluster, &cfg);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(SE2GPU_ERR_CUDA, "cudaOccupancyMaxActiveClusters for clusters of %d CTAs: %s", C, cudaGetErrorString(e)); }
+    if (clusters < 1) return fail(SE2GPU_ERR_CUDA, "device %d cannot schedule a cluster of %d CTAs of %d threads and %d bytes of shared memory", device, C, PK_THREADS, smem_max);
+    ok[device][C] = true;
+    return SE2GPU_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int se2gpu_ba_batch_cluster(se2gpu_ba* h) {
+    if (!h || !h->loaded) return fail(SE2GPU_ERR_INVALID, "no problem loaded");
+    return batch_cluster_size(h);
+}
+
+int se2gpu_ba_optimize_batch(se2gpu_ba* const* hs, int B, int max_iters, const volatile unsigned char* const* stop_flags, int* iterations,
+                             se2gpu_ba_iter_stats* stats, double* const* trace_poses, double* const* trace_points) {
+    if (!hs || B < 1) return fail(SE2GPU_ERR_INVALID, "no contexts");
+    if (max_iters < 0) return fail(SE2GPU_ERR_INVALID, "negative iteration count");
+    SE2_NVTX("se2gpu.ba.optimize_batch");
+    // every refusal comes before anything changes
+    std::unordered_map<const se2gpu_ba*, int> seen;
+    for (int k = 0; k < B; ++k) {
+        se2gpu_ba* h = hs[k];
+        if (!h) return fail(SE2GPU_ERR_INVALID, "window %d: null context", k);
+        const auto at = seen.emplace(h, k);
+        if (!at.second) return fail(SE2GPU_ERR_INVALID, "window %d: the context of window %d again", k, at.first->second);
+        if (h->device != hs[0]->device) return fail(SE2GPU_ERR_INVALID, "window %d: device %d, window 0 is on device %d", k, h->device, hs[0]->device);
+        if (h->world != 1) return fail(SE2GPU_ERR_INVALID, "window %d: sharded context (rank %d of %d)", k, h->rank, h->world);
+        if (!h->loaded) return fail(SE2GPU_ERR_INVALID, "window %d: no problem loaded", k);
+        if (h->pk_grid <= 0) return fail(SE2GPU_ERR_INVALID, "window %d: the persistent kernel is unavailable on this context", k);
+        if (h->mode == 1) return fail(SE2GPU_ERR_INVALID, "window %d: context in multi-launch mode (se2gpu_ba_set_mode 1); the batch runs the persistent kernel", k);
+        if (h->d.n > SMEM_CHOL_MAX_N) return fail(SE2GPU_ERR_CAPACITY, "window %d: %d unknowns > %d (se2gpu_ba_optimize runs it)", k, h->d.n, SMEM_CHOL_MAX_N);
+        if (max_iters > h->max_stats) return fail(SE2GPU_ERR_CAPACITY, "window %d: max_iters > %d", k, h->max_stats);
+    }
+    const int device = hs[0]->device;
+    SE2_CUDA(cudaSetDevice(device));
+    // windows whose stop flag is already set do no iteration (as se2gpu_ba_optimize) and stay out of the launch
+    std::vector<int> active;
+    for (int k = 0; k < B; ++k) {
+        if (iterations) iterations[k] = 0;
+        if (max_iters > 0 && !(stop_flags && stop_flags[k] && *stop_flags[k])) active.push_back(k);
+    }
+    if (active.empty()) return SE2GPU_OK;
+    for (int k : active) if (const int rc = check_cluster_size(device, batch_cluster_size(hs[k]))) return rc;
+    // per window: trace capacity, the plan for its cluster, the abort word; then everything enqueued on its stream is waited
+    // for, which orders the launch after it
+    for (int k : active) {
+        se2gpu_ba* h = hs[k];
+        const bool tp = trace_poses && trace_poses[k], tl = trace_points && trace_points[k];
+        if (tp && h->trace_cap_p < (size_t)max_iters * 3 * h->P) {
+            h->trace_cap_p = 0;
+            SE2_CUDA(h->bufs.regrow(&h->trace_p, (size_t)max_iters * 3 * h->P));
+            h->trace_cap_p = (size_t)max_iters * 3 * h->P;
+        }
+        if (tl && h->trace_cap_l < (size_t)max_iters * 3 * h->L) {
+            h->trace_cap_l = 0;
+            SE2_CUDA(h->bufs.regrow(&h->trace_l, (size_t)max_iters * 3 * h->L));
+            h->trace_cap_l = (size_t)max_iters * 3 * h->L;
+        }
+        if (const int rc = plan_for_grid(h, batch_cluster_size(h))) return rc;
+        *h->abort_host = 0;
+        SE2_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    // descriptors grouped by cluster size, one launch per size present
+    se2gpu_ba* h0 = hs[0];
+    cudaStream_t s = h0->stream;
+    std::vector<PKWindow> desc;
+    desc.reserve(active.size());
+    struct Group { int C, first, count; size_t smem; };
+    std::vector<Group> groups;
+    for (int C : {2, 4, 8}) {
+        Group g{C, (int)desc.size(), 0, 0};
+        for (int k : active) {
+            se2gpu_ba* h = hs[k];
+            if (batch_cluster_size(h) != C) continue;
+            const size_t smem = pk_dyn_smem_bytes(h->d.n);     // the window's own arena: its Schur blocks are cached as on one context
+            const bool tp = trace_poses && trace_poses[k], tl = trace_points && trace_points[k];
+            PKArgs pa{max_iters, 0, h->stats_dev, tp ? h->trace_p : nullptr, tl ? h->trace_l : nullptr, h->abort_host_dev, h->abort_dev,
+                      h->pk_part_chi, h->pk_part_scale, h->pk_part_max, nullptr, (int)smem, nullptr};
+            desc.push_back(PKWindow{h->d, h->cam, pa});
+            g.count++; g.smem = std::max(g.smem, smem);
+        }
+        if (g.count) groups.push_back(g);
+    }
+    const size_t words = desc.size() * sizeof(PKWindow) / 8;
+    if (h0->bdesc_cap < words) {
+        h0->bdesc_cap = 0;
+        SE2_CUDA(h0->bufs.regrow(&h0->bdesc, words));
+        h0->bdesc_cap = words;
+    }
+    h0->arena.reserve(words * 8 + 64);     // on failure the upload falls back to a pageable copy
+    if (const int rc = h0->arena.up(h0->bdesc, reinterpret_cast<const unsigned long long*>(desc.data()), words, s)) return rc;
+    const PKWindow* dev_desc = reinterpret_cast<const PKWindow*>(h0->bdesc);
+    for (const Group& g : groups) {
+        cudaLaunchAttribute attr{};
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = g.C; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(g.count * g.C); cfg.blockDim = dim3(PK_THREADS); cfg.dynamicSmemBytes = g.smem; cfg.stream = s;
+        cfg.attrs = &attr; cfg.numAttrs = 1;
+        const cudaError_t e = cudaLaunchKernelEx(&cfg, ba_persistent_cluster, dev_desc + g.first);
+        if (e != cudaSuccess) {
+            cudaStreamSynchronize(s);       // the launches already made finish before the error returns
+            cudaGetLastError();
+            return fail(SE2GPU_ERR_CUDA, "launch of the clusters of %d CTAs failed: %s", g.C, cudaGetErrorString(e));
+        }
+        se2gpu::g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    for (int k : active) SE2_CUDA(cudaMemcpyAsync(hs[k]->st_host, hs[k]->d.st, sizeof(LMState), cudaMemcpyDeviceToHost, s));
+    if (stop_flags) {   // the host forwards the stop flags while the windows run (setForceStopFlag)
+        while (cudaStreamQuery(s) == cudaErrorNotReady)
+            for (int k : active) if (stop_flags[k] && *stop_flags[k]) *(volatile int*)hs[k]->abort_host = 1;
+    }
+    SE2_CUDA(cudaStreamSynchronize(s));
+    for (int k : active) {
+        se2gpu_ba* h = hs[k];
+        const int done = h->st_host->iter;
+        if (iterations) iterations[k] = done;
+        if (done <= 0) continue;
+        if (stats) SE2_CUDA(cudaMemcpyAsync(stats + (size_t)k * max_iters, h->stats_dev, sizeof(se2gpu_ba_iter_stats) * done, cudaMemcpyDeviceToHost, s));
+        if (trace_poses && trace_poses[k]) SE2_CUDA(cudaMemcpyAsync(trace_poses[k], h->trace_p, sizeof(double) * (size_t)done * 3 * h->P, cudaMemcpyDeviceToHost, s));
+        if (trace_points && trace_points[k]) SE2_CUDA(cudaMemcpyAsync(trace_points[k], h->trace_l, sizeof(double) * (size_t)done * 3 * h->L, cudaMemcpyDeviceToHost, s));
+    }
+    SE2_CUDA(cudaStreamSynchronize(s));
+    return SE2GPU_OK;
 }
 
 int se2gpu_ba_reset(se2gpu_ba* h) {

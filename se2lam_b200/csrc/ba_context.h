@@ -80,6 +80,8 @@ struct Switches {
     bool debug = false;             // SE2GPU_BA_DEBUG: set_problem timings and per-CTA phase cycles to stderr
     bool no_band = false;           // SE2GPU_BA_NO_BAND: large windows take the global-memory envelope solver
     bool no_twist = false;          // SE2GPU_BA_NO_TWIST: the persistent kernel's reduced solve stays on one CTA
+    int batch_cluster = 0;          // SE2GPU_BA_BATCH_CLUSTER: cluster size (2, 4, 8) of the window in se2gpu_ba_optimize_batch
+                                    // instead of 8; for measuring the sizes against each other (tools/ba_batch_bench.py)
 };
 
 // What se2gpu_ba_set_problem_device keeps between calls (ba_loader.cu): the loaded topology as device copies, the
@@ -156,10 +158,18 @@ struct se2gpu_ba {
     int smem_optin = 0;
     int plan[SE2GPU_BA_PLAN_FIELDS] = {};   // host-side decisions of the last full set_problem (se2gpu_ba_debug_plan)
     se2ba::DevLoad dl;                      // se2gpu_ba_set_problem_device
+    // decide()'s inputs for the loaded window - bmax [nf] | pairs per block [nblk] | pose edges per diagonal block [nblk] - and
+    // the grid the uploaded plan (tw_*, blk_order) was made for: a batched optimize runs a window on a cluster of another size
+    std::vector<int> plan_in;
+    int plan_grid = 0;
+    unsigned long long* bdesc = nullptr; size_t bdesc_cap = 0;   // se2gpu_ba_optimize_batch: window descriptors, in 8-byte words
     long long struct_len[SE2GPU_BA_STRUCT_COUNT] = {};   // element count of each se2gpu_ba_debug_structure array
 };
 
 namespace se2ba {
+
+// Makes the uploaded plan the one decide() makes for `grid` CTAs (ba_loader.cu); enqueued on the context's stream
+int plan_for_grid(se2gpu_ba* h, int grid);
 
 // LM scalars of a freshly loaded (or reset) window, enqueued on the context's stream
 inline int reset_lm_state(se2gpu_ba* h) {

@@ -150,6 +150,7 @@ struct WindowPlan : Decisions {   // everything derived from the graph structure
     bool sorted_structure = false;   // block and pair lists by comparison sort (nf^2 beyond the dense table)
     std::vector<int> hidx, lm_ptr, perm, pose_ptr, pose_edges, pose_odo_ptr, pose_odo;
     std::vector<int> blk_a, blk_b, blk_pair_ptr, blk_odo_ptr, blk_odo, bmax;
+    std::vector<int> plan_in;        // decide()'s inputs: bmax | np | ne
     int *e_pose, *e_hidx, *pair_e1, *pair_e2;   // [El], [El], [npairs], [npairs]
     std::vector<int> pageable[4];
 };
@@ -368,6 +369,9 @@ WindowPlan plan_window(PinnedArena& built, int P, int L, int E, int O, const uin
         ne[b] = blk_a[b] == blk_b[b] ? pose_ptr[blk_a[b] + 1] - pose_ptr[blk_a[b]] : 0;
     }
     decide(w, nf, bmax.data(), np.data(), ne.data(), nblk, world, pk_grid, sw);
+    w.plan_in = bmax;
+    w.plan_in.insert(w.plan_in.end(), np.begin(), np.end());
+    w.plan_in.insert(w.plan_in.end(), ne.begin(), ne.end());
     return w;
 }
 
@@ -594,6 +598,7 @@ int load_window(se2gpu_ba* h, int P, int L, int E, int O, const double* poses, c
     h->t_edge_pose.assign(edge_pose, edge_pose + E); h->t_edge_point.assign(edge_point, edge_point + E); h->t_odo_i.assign(odo_i, odo_i + O);
     h->t_odo_j.assign(odo_j, odo_j + O); h->t_fixed.assign(fixed, fixed + P); h->t_rank = h->rank; h->t_world = h->world;
     set_struct_len(h, (int)w.pose_edges.size(), (int)w.pose_odo.size(), w.npairs, (int)w.blk_odo.size(), w.tw_cmax1.size(), w.blk_order.size());
+    h->plan_in = w.plan_in; h->plan_grid = h->pk_grid;
     h->loaded = true;
     return SE2GPU_OK;
 }
@@ -1268,12 +1273,40 @@ int load_window_device(se2gpu_ba* h, int P, int L, int E, int O, const double* p
     h->P = P; h->L = L; h->E = E; h->O = O;
     h->t_rank = h->rank; h->t_world = h->world;
     set_struct_len(h, sc[DL_NPE], sc[DL_NPO], npairs, nodob, w.tw_cmax1.size(), w.blk_order.size());
+    h->plan_in.assign(g.planin_host.begin(), g.planin_host.begin() + nplan); h->plan_grid = h->pk_grid;
     g.valid = true;
     h->loaded = true;
     return SE2GPU_OK;
 }
 
 }  // namespace
+
+namespace se2ba {
+
+// The decisions that depend on the number of CTAs - the two-sided split and the serving order of the Schur blocks - made again
+// by the one planner from the inputs the load kept, and their O(nf + nblk) results uploaded. The envelope and the sharded
+// exchange list do not depend on it. A serving order of W workers has at most max(12 W, nblk + W) positions; ensure_cap
+// leaves the block lists room for nblk + 1024, so clusters of up to 8 CTAs always fit (the check below is a guard).
+int plan_for_grid(se2gpu_ba* h, int grid) {
+    if (h->plan_grid == grid) return SE2GPU_OK;
+    Dev& d = h->d;
+    const int nf = d.nf, nblk = d.nblk;
+    const int* in = h->plan_in.data();
+    Decisions w;
+    decide(w, nf, in, in + nf, in + nf + nblk, nblk, h->world, grid, h->sw);
+    if (w.blk_order.size() > h->cap_blk) return fail(SE2GPU_ERR_CAPACITY, "serving order of %zu positions exceeds the block lists", w.blk_order.size());
+    h->arena.reserve(sizeof(int) * (w.tw_cmax1.size() + w.blk_order.size()) + 256);   // on failure the uploads fall back to pageable copies
+    int rc = up(h, d.tw_cmax1, w.tw_cmax1.data(), w.tw_cmax1.size());
+    if (rc == SE2GPU_OK) rc = up(h, d.blk_order, w.blk_order.data(), w.blk_order.size());
+    if (rc != SE2GPU_OK) return rc;
+    d.nord = (int)w.blk_order.size(); d.tw_m0 = w.tw_m0; d.tw_w = w.tw_w;
+    h->struct_len[SE2GPU_BA_STRUCT_TW_CMAX1] = (long long)w.tw_cmax1.size();   // se2gpu_ba_debug_structure shows the plan in use
+    h->struct_len[SE2GPU_BA_STRUCT_BLK_ORDER] = (long long)w.blk_order.size();
+    h->plan_grid = grid;
+    return SE2GPU_OK;
+}
+
+}  // namespace se2ba
 
 extern "C" {
 
