@@ -29,6 +29,12 @@ class BowKF(C.Structure):
                 ("node", C.c_void_p), ("n_node", C.c_int), ("ptr", C.c_void_p), ("feat", C.c_void_p)]
 
 
+class BowBatchKF(C.Structure):
+    """se2gpu_bow_batch_kf: one side of se2gpu_search_by_bow_batch_device (device pointers)"""
+    _fields_ = [("kp", C.c_void_p), ("desc", C.c_void_p), ("has_mp", C.c_void_p), ("cap", C.c_int), ("node", C.c_void_p),
+                ("ptr", C.c_void_p), ("feat", C.c_void_p), ("n_node", C.c_void_p)]
+
+
 class PoseBAParams(C.Structure):
     _fields_ = [("fx", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("Tbc", C.c_float * 16), ("huber_delta", C.c_float),
                 ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float), ("iterations", C.c_int)]
@@ -157,13 +163,14 @@ SYMBOLS = [
     "se2gpu_match_by_projection_device", "se2gpu_matcher_match_by_window", "se2gpu_matcher_match_by_projection",
     "se2gpu_matcher_search_by_bow", "se2gpu_matcher_profile", "se2gpu_matcher_profile_read", "se2gpu_matcher_last_rounds",
     "se2gpu_matcher_create_batch", "se2gpu_match_by_window_batch_device", "se2gpu_match_by_projection_batch_device",
-    "se2gpu_matcher_last_rounds_batch",
+    "se2gpu_matcher_last_rounds_batch", "se2gpu_search_by_bow_batch_device",
     "se2gpu_ba_create", "se2gpu_ba_destroy", "se2gpu_ba_set_problem", "se2gpu_ba_optimize", "se2gpu_ba_get",
     "se2gpu_ba_set_shard", "se2gpu_ba_peer_export", "se2gpu_ba_peer_import", "se2gpu_ba_set_stream", "se2gpu_ba_debug_system", "se2gpu_ba_reset", "se2gpu_ba_profile",
     "se2gpu_ba_profile_read", "se2gpu_ba_set_mode", "se2gpu_ba_get_f32", "se2gpu_ba_build_information", "se2gpu_ba_optimize_from", "se2gpu_ba_peer_attach_local",
     "se2gpu_ba_debug_plan", "se2gpu_ba_set_problem_device", "se2gpu_ba_build_information_device", "se2gpu_ba_debug_structure",
     "se2gpu_ba_optimize_batch", "se2gpu_ba_batch_cluster",
-    "se2gpu_voc_create", "se2gpu_voc_destroy", "se2gpu_voc_transform", "se2gpu_voc_transform_device", "se2gpu_median_descriptor",
+    "se2gpu_voc_create", "se2gpu_voc_destroy", "se2gpu_voc_transform", "se2gpu_voc_transform_device", "se2gpu_voc_compute_bow_device",
+    "se2gpu_median_descriptor",
     "se2gpu_triangulate", "se2gpu_triangulate_device", "se2gpu_track_triangulate", "se2gpu_track_triangulate_device",
     "se2gpu_xyz_info", "se2gpu_xyz_info_device", "se2gpu_projection_observations", "se2gpu_projection_observations_device",
     "se2gpu_debug_svd4", "se2gpu_remove_outliers", "se2gpu_remove_outliers_device", "se2gpu_fundam_niters_table",
@@ -247,6 +254,7 @@ def lib():
     L.se2gpu_matcher_profile_read.argtypes = [vp, vp, vp]
     L.se2gpu_matcher_last_rounds.argtypes = [vp, C.POINTER(i), C.POINTER(i)]
     L.se2gpu_matcher_last_rounds_batch.argtypes = [vp, i, vp, vp]
+    L.se2gpu_search_by_bow_batch_device.argtypes = [vp, i, C.POINTER(BowBatchKF), C.POINTER(BowBatchKF), vp, i, f, i, vp, vp, vp]
     L.se2gpu_ba_create.restype = vp
     L.se2gpu_ba_create.argtypes = [i, i, i, i, i]
     L.se2gpu_ba_destroy.argtypes = [vp]
@@ -271,6 +279,7 @@ def lib():
     L.se2gpu_voc_destroy.argtypes = [vp]
     L.se2gpu_voc_transform.argtypes = [vp, vp, i, i, vp, vp, vp]
     L.se2gpu_voc_transform_device.argtypes = [vp, vp, i, i, vp, vp, vp, vp]
+    L.se2gpu_voc_compute_bow_device.argtypes = [vp, i, vp, i, vp, i] + [vp] * 8
     L.se2gpu_median_descriptor.argtypes = [vp, vp, i, vp, vp, i]
     L.se2gpu_triangulate.argtypes = [i, vp, vp, vp, i, vp, vp, vp, i]
     L.se2gpu_triangulate_device.argtypes = [i] + [vp] * 7

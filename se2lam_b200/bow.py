@@ -4,8 +4,11 @@
 (reference Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1150-1216) as KeyFrame::ComputeBoW calls it
 (src/KeyFrame.cpp:244-254): the per-descriptor tree descent runs on the GPU, the BowVector / FeatureVector assembly (a
 sorted-map accumulation in feature order + L1 normalisation, TF_IDF weighting: the ORBvoc settings) on the host.
+`Vocabulary.compute_bow_device` runs both halves on the device for a batch of keyframes (se2gpu_voc_compute_bow_device).
 """
 from __future__ import annotations
+
+import ctypes as C
 
 import numpy as np
 
@@ -57,6 +60,16 @@ class Vocabulary:
             for k in v:
                 v[k] /= norm
         return dict(sorted(v.items())), dict(sorted(fv.items()))
+
+    def compute_bow_device(self, B, d_desc, cap, d_fv_node, d_fv_ptr, d_fv_feat, d_fv_n, d_bow_word=None, d_bow_value=None,
+                           d_bow_n=None, d_n=None, levelsup=4, stream=0):
+        """KeyFrame::ComputeBoW for B keyframes on device buffers (CUDA pointers: ints or torch tensors), asynchronous on
+        `stream`. Keyframe b: descriptors d_desc + b*cap*32, d_n[b] of them (None: cap); BowVector d_bow_word / d_bow_value
+        (float64) + b*cap, d_bow_n[b] words (all three None: FeatureVector only); FeatureVector d_fv_node + b*cap ascending,
+        d_fv_ptr + b*(cap+1), d_fv_feat + b*cap, d_fv_n[b] nodes. See se2gpu_voc_compute_bow_device."""
+        check(lib().se2gpu_voc_compute_bow_device(self.h, int(B), ptr(d_desc), int(cap), ptr(d_n), int(levelsup), ptr(d_bow_word),
+                                                  ptr(d_bow_value), ptr(d_bow_n), ptr(d_fv_node), ptr(d_fv_ptr), ptr(d_fv_feat),
+                                                  ptr(d_fv_n), C.c_void_p(int(stream) if stream else 0)), "se2gpu_voc_compute_bow_device")
 
 
 def median_descriptor(desc, ptr_, device=0):

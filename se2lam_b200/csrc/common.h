@@ -340,6 +340,28 @@ inline int check_se3_links(int N, int n, const int* from, const int* to, const f
 // number of valid entries: *d_n clamped to [0, cap], or cap when there is no device-side count
 __device__ __forceinline__ int count_of(const int* d_n, int cap) { return d_n ? min(max(*d_n, 0), cap) : cap; }
 
+// exclusive prefix sum over the CTA of one value per thread (blockDim.x a multiple of 32); `total` receives the sum.
+// s_warp: [32] ints of shared memory. Every thread of the CTA calls it; it ends with a barrier, so s_warp may be reused.
+__device__ __forceinline__ int block_exclusive_sum(int x, int& total, int* s_warp) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int inc = x;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+    if (lane == 31) s_warp[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+        int v = lane < nw ? s_warp[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+        if (lane < nw) s_warp[lane] = v;
+    }
+    __syncthreads();
+    const int excl = (w ? s_warp[w - 1] : 0) + inc - x;
+    total = s_warp[nw - 1];
+    __syncthreads();
+    return excl;
+}
+
 // Hamming distance of two 256-bit ORB descriptors (8 x 32 bit, 16-byte aligned)
 __device__ __forceinline__ int hamming256(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b) {
     const uint4 a0 = *reinterpret_cast<const uint4*>(a), a1 = *reinterpret_cast<const uint4*>(a + 4);

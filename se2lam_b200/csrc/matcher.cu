@@ -23,6 +23,8 @@
 // The device entry points take a batch of B independent frame pairs (se2gpu_match_by_*_batch_device; the single-pair entry
 // points are B = 1): the grid and candidate kernels take the pair from blockIdx.y, k_resolve runs one CTA and k_fallback_*
 // one warp per pair, and every pair works in its own slice of the context's scratch. The launch count does not depend on B.
+// se2gpu_search_by_bow_batch_device puts k_bow_walk in front, one CTA per pair: the node walk of SearchByBoW (:160-247) over
+// the two device FeatureVectors, which writes the pair's queries for k_candidates_bow.
 #include <climits>
 #include <cstring>
 #include <mutex>
@@ -41,6 +43,7 @@ struct se2gpu_matcher {
     int* work = nullptr;                // fallback: [2 * max_db + max_q]
     int* flags = nullptr;               // [0] fallback needed, [1] rounds of the last resolve
     int* nm = nullptr;                  // match count of the last call
+    int *bow_q = nullptr, *bow_nq = nullptr;   // SearchByBoW batch: [max_batch][3][max_q] (feature, KF2 range), [max_batch] count
     std::vector<int> seq_flags;         // [max_batch][2] = {1, 0}: the flags of every pair when the sequential kernel runs alone
     int last_batch = 0;                 // pairs of the last resolve
     // device + pinned staging of the host entry points
@@ -231,31 +234,86 @@ __global__ void __launch_bounds__(256) k_candidates(CandArgs a) {
 }
 
 // SearchByBoW candidates (ORBmatcher.cpp:166-204): query q = feature qidx[q] of KF1 (node-walk order), its candidates are
-// the features of the same vocabulary node in KF2, in the node's feature order.
-__global__ void __launch_bounds__(256) k_candidates_bow(int nq, const int* __restrict__ qidx, const int* __restrict__ qb0, const int* __restrict__ qb1,
-                                                        const uint32_t* __restrict__ d1, const uint8_t* __restrict__ mp1,
-                                                        const int* __restrict__ feat2, const uint32_t* __restrict__ d2, const uint8_t* __restrict__ mp2,
-                                                        int mp_only, int cap, int2* __restrict__ cand, int* __restrict__ ncand) {
+// the features of the same vocabulary node in KF2, in the node's feature order. Pair = blockIdx.y: KF1 at b * cap1, KF2 at
+// slot2[b] * cap2 (slot2 NULL: b), the queries at b * qstride and the candidate rows in the pair's scratch slice.
+struct BowCandArgs {
+    int nq_cap; const int* d_nq;                       // queries per pair: capacity and device count (NULL: nq_cap)
+    const int* qidx; const int* qb0; const int* qb1;   // KF1 feature and its KF2 feat range [qb0, qb1), per query
+    int qstride;
+    const uint32_t* d1; const uint8_t* mp1; int cap1;
+    const int* feat2; const uint32_t* d2; const uint8_t* mp2; int cap2; const int* slot2;
+    int mp_only;
+    int cap; int2* cand; int* ncand; int scr_q;
+};
+__device__ __forceinline__ void pair_slice(BowCandArgs& a, int b) {
+    const size_t s2 = (size_t)(a.slot2 ? a.slot2[b] : b) * a.cap2, q = (size_t)b * a.qstride;
+    if (a.d_nq) a.d_nq += b;
+    a.qidx += q; a.qb0 += q; a.qb1 += q;
+    a.d1 += 8 * (size_t)b * a.cap1; if (a.mp1) a.mp1 += (size_t)b * a.cap1;
+    a.feat2 += s2; a.d2 += 8 * s2; if (a.mp2) a.mp2 += s2;
+    a.cand += (size_t)b * a.scr_q * a.cap; a.ncand += (size_t)b * a.scr_q;
+}
+__global__ void __launch_bounds__(256) k_candidates_bow(BowCandArgs a) {
+    pair_slice(a, blockIdx.y);
     const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (q >= nq) return;
-    const int idx1 = qidx[q];
+    if (q >= count_of(a.d_nq, a.nq_cap)) return;
+    const int idx1 = a.qidx[q];
     int count = 0;
-    if (!(mp_only && !mp1[idx1])) {
-        const int b0 = qb0[q], b1 = qb1[q];
+    if (!(a.mp_only && !a.mp1[idx1])) {
+        const int b0 = a.qb0[q], b1 = a.qb1[q];
         for (int k0 = b0; k0 < b1; k0 += 32) {
             const int k = k0 + lane;
             bool hit = false;
             int idx2 = -1;
-            if (k < b1) { idx2 = feat2[k]; hit = !(mp_only && !mp2[idx2]); }
+            if (k < b1) { idx2 = a.feat2[k]; hit = !(a.mp_only && !a.mp2[idx2]); }
             const unsigned bal = __ballot_sync(0xffffffffu, hit);
             if (hit) {
                 const int pos = count + __popc(bal & ((1u << lane) - 1));
-                if (pos < cap) cand[(size_t)q * cap + pos] = make_int2(idx2, hamming256(d1 + 8 * (size_t)idx1, d2 + 8 * (size_t)idx2));
+                if (pos < a.cap) a.cand[(size_t)q * a.cap + pos] = make_int2(idx2, hamming256(a.d1 + 8 * (size_t)idx1, a.d2 + 8 * (size_t)idx2));
             }
             count += __popc(bal);
         }
     }
-    if (lane == 0) ncand[q] = min(count, cap);
+    if (lane == 0) a.ncand[q] = min(count, a.cap);
+}
+
+// The two-iterator walk of SearchByBoW over the ascending node ids (:160-247) for pair blockIdx.x, on the FeatureVectors
+// se2gpu_voc_compute_bow_device writes: every KF1 node is looked up in KF2's node list by binary search (both lists are
+// ascending and free of repeats, so a node is common exactly when the walk stops on it), and the features of the common
+// nodes become the queries, numbered in walk order by an exclusive sum over the nodes in ascending order.
+struct BowWalkArgs {
+    const int* node1; const int* ptr1; const int* feat1; const int* n_node1; int cap1;
+    const int* node2; const int* ptr2; const int* n_node2; int cap2; const int* slot2;
+    int* qidx; int* qb0; int* qb1; int qstride; int* nq;
+};
+__global__ void __launch_bounds__(256) k_bow_walk(BowWalkArgs a) {
+    __shared__ int s_warp[32];
+    const int b = blockIdx.x, s2 = a.slot2 ? a.slot2[b] : b;
+    const int* node1 = a.node1 + (size_t)b * a.cap1; const int* ptr1 = a.ptr1 + (size_t)b * (a.cap1 + 1);
+    const int* feat1 = a.feat1 + (size_t)b * a.cap1;
+    const int* node2 = a.node2 + (size_t)s2 * a.cap2; const int* ptr2 = a.ptr2 + (size_t)s2 * (a.cap2 + 1);
+    const int n1 = min(max(a.n_node1[b], 0), a.cap1), n2 = min(max(a.n_node2[s2], 0), a.cap2);
+    const size_t qo = (size_t)b * a.qstride;
+    int *qidx = a.qidx + qo, *qb0 = a.qb0 + qo, *qb1 = a.qb1 + qo;
+    int base = 0;
+    for (int a0 = 0; a0 < n1; a0 += blockDim.x) {
+        const int i = a0 + threadIdx.x;
+        int c = 0, j = -1;
+        if (i < n1) {
+            const int nd = node1[i];
+            int lo = 0, hi = n2;
+            while (lo < hi) { const int mid = (lo + hi) >> 1; if (node2[mid] < nd) lo = mid + 1; else hi = mid; }
+            if (lo < n2 && node2[lo] == nd) { j = lo; c = ptr1[i + 1] - ptr1[i]; }
+        }
+        int total;
+        const int off = base + se2gpu::block_exclusive_sum(c, total, s_warp);
+        if (c > 0) {
+            const int p1 = ptr1[i], b0 = ptr2[j], b1 = ptr2[j + 1];
+            for (int k = 0; k < c && off + k < a.cap1; ++k) { qidx[off + k] = feat1[p1 + k]; qb0[off + k] = b0; qb1[off + k] = b1; }
+        }
+        base += total;
+    }
+    if (threadIdx.x == 0) a.nq[b] = min(base, a.cap1);
 }
 
 __device__ void three_maxima(const int* hist, int& ind1, int& ind2, int& ind3) {  // ORBmatcher.cpp:64-105
@@ -288,7 +346,9 @@ struct ResolveArgs {
     int K;                            // claim slots per database item in shared memory
     // rotation histogram inputs (angle of query q at ang1[qid(q) * stride1], of database item j at ang2[j * stride2])
     const float* ang1; int stride1; const float* ang2; int stride2; int check_ori;
-    const int* qid;                   // BOW: feature index of query q; null: q
+    const int* qid;                   // BOW: feature index of query q (pair stride qstride); null: q
+    int qstride;
+    const int* slot2;                 // BOW batch: pair b's database is slot2[b] of the side-2 arrays; null: b
     const se2gpu_keypoint* kp2;       // WINDOW: database keypoints (vbPrevMatched update)
     int* out; int n_out;              // WINDOW: matches12[n1]; PROJ: vMatchesIdxMP[n_kf]; BOW: matches12[n1]
     float* prev;                      // WINDOW: vbPrevMatched, updated in place
@@ -296,10 +356,12 @@ struct ResolveArgs {
     int scr_q;                        // max_queries: per-pair rows of cand (each `cap` wide) and entries of ncand
 };
 
-// pair b's slice (WINDOW / PROJ; SearchByBoW runs one pair): queries and database items are strided by nq_cap / n2_cap,
-// outputs by n_out, the context scratch by its capacities; work is the fallback's [2 * cap + scr_q] per pair
+// pair b's slice: queries and database items are strided by nq_cap / n2_cap (BOW: the angles are per feature and nq_cap
+// is KF1's feature capacity), outputs by n_out, the context scratch by its capacities; work is the fallback's
+// [2 * cap + scr_q] per pair
 __device__ __forceinline__ void pair_slice(ResolveArgs& a, int b) {
-    const size_t q = (size_t)b * a.nq_cap, d = (size_t)b * a.n2_cap;
+    const size_t q = (size_t)b * a.nq_cap, d = (size_t)(a.slot2 ? a.slot2[b] : b) * a.n2_cap;
+    if (a.qid) a.qid += (size_t)b * a.qstride;
     if (a.d_nq) a.d_nq += b;
     if (a.d_n2) a.d_n2 += b;
     a.cand += (size_t)b * a.scr_q * a.cap; a.ncand += (size_t)b * a.scr_q;
@@ -322,7 +384,7 @@ __global__ void __launch_bounds__(1024) k_resolve(ResolveArgs a) {
     __shared__ int s_over, s_nm, s_top[3];
     // pair 0 needs no offsets; skipping them keeps a single pair's prologue as short as it was (one CTA on one SM runs the
     // whole resolve, so every per-thread instruction before the rounds is on the critical path)
-    if (blockIdx.x != 0) pair_slice(a, blockIdx.x);
+    if (blockIdx.x != 0 || (MODE == MODE_BOW && a.slot2)) pair_slice(a, blockIdx.x);
     const int tid = threadIdx.x, nt = blockDim.x;
     const int nq = count_of(a.d_nq, a.nq_cap), n2 = count_of(a.d_n2, a.n2_cap);
     const int K = a.K;
@@ -541,10 +603,13 @@ __global__ void __launch_bounds__(32) k_fallback_projection(ResolveArgs a, int* 
 
 // SearchByBoW's sequential loop (:166-246) over the precomputed candidate lists. work: [n2] vbMatched2, [nq] bin_of
 __global__ void __launch_bounds__(32) k_fallback_bow(ResolveArgs a, int* __restrict__ work) {
-    if (a.flags[0] == 0) return;
+    const int b = blockIdx.x;
+    if (a.flags[2 * b] == 0) return;
+    pair_slice(a, b);
+    work = work_slice(a, work, b);
     __shared__ int hist[HISTO_LENGTH];
     const int lane = threadIdx.x;
-    const int nq = a.nq_cap, n2 = a.n2_cap;
+    const int nq = count_of(a.d_nq, a.nq_cap), n2 = a.n2_cap;
     int* matched2 = work; int* bin_of = work + n2;
     for (int i = lane; i < n2; i += 32) matched2[i] = 0;
     for (int i = lane; i < a.n_out; i += 32) a.out[i] = -1;
@@ -614,7 +679,7 @@ int pick_K(int smem_max, int nq, int n2) {
     return 0;
 }
 
-// common tail of the three device paths for B pairs (SearchByBoW: 1): resolve + guarded fallback. K depends on the caps only,
+// common tail of the device paths for B pairs: resolve + guarded fallback. K depends on the caps only,
 // so it is the same for every pair.
 template <int MODE>
 int launch_resolve(se2gpu_matcher* m, int B, ResolveArgs ra, const se2gpu_keypoint* kp1, cudaStream_t s) {
@@ -633,7 +698,7 @@ int launch_resolve(se2gpu_matcher* m, int B, ResolveArgs ra, const se2gpu_keypoi
     m->prof.begin(3, s);
     if (MODE == MODE_WINDOW) SE2_LAUNCH(k_fallback_window, B, 32, 0, s, ra, kp1, m->work);
     else if (MODE == MODE_PROJ) SE2_LAUNCH(k_fallback_projection, B, 32, 0, s, ra, m->work);
-    else SE2_LAUNCH(k_fallback_bow, 1, 32, 0, s, ra, m->work);
+    else SE2_LAUNCH(k_fallback_bow, B, 32, 0, s, ra, m->work);
     m->prof.end(s);
     return SE2GPU_OK;
 }
@@ -677,6 +742,7 @@ se2gpu_matcher* se2gpu_matcher_create_batch(int max_queries, int max_db, int max
     auto A = [&](auto** p, size_t count) { ok = ok && m->bufs.alloc(p, count) == cudaSuccess; };
     A(&m->cell, P * D); A(&m->order, P * D); A(&m->nvalid, P);
     A(&m->cand, P * Q * D); A(&m->ncand, P * Q); A(&m->work, P * (2 * D + Q)); A(&m->flags, 2 * P); A(&m->nm, P);
+    A(&m->bow_q, P * 3 * Q); A(&m->bow_nq, P);
     A(&m->d_kp1, N); A(&m->d_kp2, N); A(&m->d_desc1, N * 32); A(&m->d_desc2, N * 32);
     A(&m->d_u8a, N); A(&m->d_u8b, N); A(&m->d_f1, 2 * N); A(&m->d_f2, 2 * N);
     A(&m->d_i1, N + 1); A(&m->d_i2, N + 1); A(&m->d_i3, N + 1); A(&m->d_i4, N + 1); A(&m->d_out, N);
@@ -837,6 +903,51 @@ int se2gpu_match_by_projection_batch_device(se2gpu_matcher* m, int B, const se2g
     return launch_resolve<MODE_PROJ>(m, B, ra, nullptr, s);
 }
 
+int se2gpu_search_by_bow_batch_device(se2gpu_matcher* m, int B, const se2gpu_bow_batch_kf* kf1, const se2gpu_bow_batch_kf* kf2,
+                                      const int* d_slot2, int mp_only, float nnratio, int check_orientation, int* d_matches12,
+                                      int* d_nmatches, void* stream) {
+    if (!m) return fail(SE2GPU_ERR_INVALID, "null handle");
+    if (!kf1 || !kf2) return fail(SE2GPU_ERR_INVALID, "null keyframe side");
+    const int cap1 = kf1->cap, cap2 = kf2->cap;
+    if (B < 0 || cap1 < 0 || cap2 < 0) return fail(SE2GPU_ERR_INVALID, "negative sizes");
+    if (B > m->max_batch || cap1 > m->max_q || cap2 > m->max_db)
+        return fail(SE2GPU_ERR_CAPACITY, "%d pairs of %d x %d exceed the matcher's capacity %d pairs of %d x %d", B, cap1, cap2, m->max_batch, m->max_q, m->max_db);
+    SE2_NVTX("se2gpu.search_by_bow_batch");
+    if (B == 0) return SE2GPU_OK;
+    auto missing = [&](const se2gpu_bow_batch_kf* k) {
+        return !k->kp || !k->desc || (mp_only && !k->has_mp) || !k->node || !k->ptr || !k->feat || !k->n_node;
+    };
+    if ((cap1 && (missing(kf1) || !d_matches12)) || (cap2 && missing(kf2))) return fail(SE2GPU_ERR_INVALID, "null argument");
+    SE2_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    int* nm = d_nmatches ? d_nmatches : m->nm;
+    if (cap1 == 0 || cap2 == 0) {
+        if (cap1) SE2_CUDA(cudaMemsetAsync(d_matches12, 0xff, sizeof(int) * cap1 * B, s));
+        SE2_CUDA(cudaMemsetAsync(nm, 0, sizeof(int) * B, s));
+        return SE2GPU_OK;
+    }
+    // pair b's queries at b * 3 max_q of bow_q: features, then the starts and ends of their KF2 ranges
+    const int qstride = 3 * m->max_q;
+    int *qidx = m->bow_q, *qb0 = qidx + m->max_q, *qb1 = qidx + 2 * m->max_q;
+    BowWalkArgs wa{kf1->node, kf1->ptr, kf1->feat, kf1->n_node, cap1, kf2->node, kf2->ptr, kf2->n_node, cap2, d_slot2,
+                   qidx, qb0, qb1, qstride, m->bow_nq};
+    BowCandArgs ca{};
+    ca.nq_cap = cap1; ca.d_nq = m->bow_nq; ca.qidx = qidx; ca.qb0 = qb0; ca.qb1 = qb1; ca.qstride = qstride;
+    ca.d1 = reinterpret_cast<const uint32_t*>(kf1->desc); ca.mp1 = kf1->has_mp; ca.cap1 = cap1;
+    ca.feat2 = kf2->feat; ca.d2 = reinterpret_cast<const uint32_t*>(kf2->desc); ca.mp2 = kf2->has_mp; ca.cap2 = cap2; ca.slot2 = d_slot2;
+    ca.mp_only = mp_only; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand; ca.scr_q = m->max_q;
+    m->prof.begin(1, s);
+    SE2_LAUNCH(k_bow_walk, B, 256, 0, s, wa);
+    SE2_LAUNCH(k_candidates_bow, dim3((cap1 * 32 + 255) / 256, B), 256, 0, s, ca);
+    m->prof.end(s);
+    ResolveArgs ra{};
+    ra.nq_cap = cap1; ra.d_nq = m->bow_nq; ra.n2_cap = cap2; ra.d_n2 = nullptr; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand;
+    ra.nnratio = nnratio; ra.ang1 = &kf1->kp->angle; ra.stride1 = sizeof(se2gpu_keypoint) / 4; ra.ang2 = &kf2->kp->angle;
+    ra.stride2 = sizeof(se2gpu_keypoint) / 4; ra.check_ori = check_orientation; ra.qid = qidx; ra.qstride = qstride; ra.slot2 = d_slot2;
+    ra.out = d_matches12; ra.n_out = cap1; ra.nmatches = nm; ra.flags = m->flags;
+    return launch_resolve<MODE_BOW>(m, B, ra, nullptr, s);
+}
+
 }  // extern "C"
 
 namespace {
@@ -962,9 +1073,13 @@ int se2gpu_matcher_search_by_bow(se2gpu_matcher* m, const se2gpu_bow_kf* k1, con
         st.up(m->d_f2, k2->angle, k2->n, s) || st.up(m->d_i1, qidx.data(), nq, s) || st.up(m->d_i2, qb0.data(), nq, s) ||
         st.up(m->d_i3, qb1.data(), nq, s) || st.up(m->d_i4, k2->feat, nf2, s))
         return SE2GPU_ERR_CUDA;
+    BowCandArgs ca{};
+    ca.nq_cap = nq; ca.d_nq = nullptr; ca.qidx = m->d_i1; ca.qb0 = m->d_i2; ca.qb1 = m->d_i3;
+    ca.d1 = reinterpret_cast<const uint32_t*>(m->d_desc1); ca.mp1 = m->d_u8a; ca.feat2 = m->d_i4;
+    ca.d2 = reinterpret_cast<const uint32_t*>(m->d_desc2); ca.mp2 = m->d_u8b;
+    ca.mp_only = mp_only; ca.cap = m->max_db; ca.cand = m->cand; ca.ncand = m->ncand; ca.scr_q = m->max_q;
     m->prof.begin(1, s);
-    SE2_LAUNCH(k_candidates_bow, (nq * 32 + 255) / 256, 256, 0, s, nq, m->d_i1, m->d_i2, m->d_i3, reinterpret_cast<const uint32_t*>(m->d_desc1), m->d_u8a,
-               m->d_i4, reinterpret_cast<const uint32_t*>(m->d_desc2), m->d_u8b, mp_only, m->max_db, m->cand, m->ncand);
+    SE2_LAUNCH(k_candidates_bow, (nq * 32 + 255) / 256, 256, 0, s, ca);
     m->prof.end(s);
     ResolveArgs ra{};
     ra.nq_cap = nq; ra.d_nq = nullptr; ra.n2_cap = k2->n; ra.d_n2 = nullptr; ra.cap = m->max_db; ra.cand = m->cand; ra.ncand = m->ncand; ra.nnratio = nnratio;

@@ -11,7 +11,7 @@ import dataclasses
 import numpy as np
 
 from . import _capi
-from ._capi import BowKF, GridParams, KP_DTYPE, check, lib, ptr
+from ._capi import BowBatchKF, BowKF, GridParams, KP_DTYPE, check, lib, ptr
 
 FRAME_GRID_ROWS, FRAME_GRID_COLS = 48, 64   # Frame.h:26-27
 
@@ -103,6 +103,22 @@ class ORBmatcher:
                                                             self.mfNNratio, ptr(d_matches_idx_mp), ptr(d_nmatches),
                                                             C.c_void_p(int(stream) if stream else 0)),
               "se2gpu_match_by_projection_batch_device")
+
+    @staticmethod
+    def BowBatchSide(kp, desc, cap, fv_node, fv_ptr, fv_feat, fv_n, has_mp=None) -> BowBatchKF:
+        """One side of SearchByBoWBatchDevice: keyframe k's keypoints, descriptors and has_mp in slot k of `cap`, and its
+        FeatureVector as Vocabulary.compute_bow_device writes it (device pointers: ints or torch tensors)."""
+        v = lambda a: ptr(a).value if a is not None else None
+        return BowBatchKF(v(kp), v(desc), v(has_mp), int(cap), v(fv_node), v(fv_ptr), v(fv_feat), v(fv_n))
+
+    def SearchByBoWBatchDevice(self, B, kf1: BowBatchKF, kf2: BowBatchKF, d_matches12, d_nmatches=None, d_slot2=None, bIfMPOnly=True,
+                               stream=0):
+        """SearchByBoW for B keyframe pairs: keyframe b of kf1 against keyframe d_slot2[b] of kf2 (None: b). Writes
+        d_matches12 + b*kf1.cap (-1 = none) and d_nmatches[b]; asynchronous on `stream` (se2gpu_search_by_bow_batch_device)."""
+        assert self.h, "device entry points need an owned context (pass max_queries / max_db)"
+        check(lib().se2gpu_search_by_bow_batch_device(self.h, int(B), C.byref(kf1), C.byref(kf2), ptr(d_slot2), int(bIfMPOnly),
+                                                      self.mfNNratio, int(self.mbCheckOrientation), ptr(d_matches12), ptr(d_nmatches),
+                                                      C.c_void_p(int(stream) if stream else 0)), "se2gpu_search_by_bow_batch_device")
 
     def profile(self, enable=True):
         check(lib().se2gpu_matcher_profile(self.h, int(enable)), "se2gpu_matcher_profile")
