@@ -50,6 +50,11 @@
  *   se2gpu_global_ba[_device]        GlobalMapper::GlobalBA's pose graph and optimize(GLOBAL_ITER)  src/GlobalMapper.cpp:328-504
  *                                    (addVertexSE3PlaneMotion src/optimizer.cpp:337-468, addEdgeSE3 :375-419)
  *   se2gpu_global_ba_update_points[_device]  GlobalBA's map-point write-back  src/GlobalMapper.cpp:506-531
+ *   se2gpu_detect_loop_device        GlobalMapper::DetectLoopClose / Localizer::DetectLoopClose (DBoW2 L1Scoring::score)
+ *                                    src/GlobalMapper.cpp:201-254, src/Localizer.cpp:337-392,
+ *                                    Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-68
+ *   se2gpu_verify_loop_device        GlobalMapper::VerifyLoopClose / Localizer::VerifyLoopClose  src/GlobalMapper.cpp:256-326,
+ *                                    (RemoveMatchOutlierRansac :1207-1248, RemoveKPMatch :1251-1276) src/Localizer.cpp:394-431
  */
 #ifndef SE2GPU_H
 #define SE2GPU_H
@@ -283,7 +288,8 @@ typedef struct se2gpu_bow_batch_kf {
  * B < 0, a negative cap or a NULL required pointer is SE2GPU_ERR_INVALID; B == 0 does nothing. Like every device entry,
  * it trusts the contents of device memory: the FeatureVectors must be well formed (ascending, unrepeated node ids, ptr
  * ascending within [0, cap], feature indices below cap, each feature in at most one node) and every d_slot2[b] a slot of
- * kf2's arrays. Calls on one context are ordered like the other device entries (its scratch is shared). */
+ * kf2's arrays or negative. A negative d_slot2[b] makes pair b empty: no queries, d_matches12 + b*kf1->cap all -1,
+ * d_nmatches[b] = 0, and nothing of kf2 is read for it. Calls on one context are ordered like the other device entries (its scratch is shared). */
 int se2gpu_search_by_bow_batch_device(se2gpu_matcher* m, int B, const se2gpu_bow_batch_kf* kf1, const se2gpu_bow_batch_kf* kf2,
                                       const int* d_slot2, int mp_only, float nnratio, int check_orientation, int* d_matches12,
                                       int* d_nmatches, void* stream);
@@ -537,6 +543,74 @@ int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const
  * and se2gpu_fundam_debug_niters evaluates the device lookup for ep = (n[i] - good[i]) / n[i] (HOST buffers). */
 void se2gpu_fundam_niters_table(double* thresholds);
 int se2gpu_fundam_debug_niters(int count, const int* n, const int* good, const int* max_iters, int* out, int device);
+
+/* ------------------------------------------------------------------------------------------ loop closure */
+/* DetectLoopClose's parameters: a database keyframe with |db_id - q_id| < min_id_offset is not selected
+ * (GM_DCL_MIN_KFID_OFFSET), and a loop is detected when the best score is > min_score (GM_DCL_MIN_SCORE_BEST). */
+typedef struct se2gpu_loop_detect_params {
+    int min_id_offset;
+    double min_score;
+} se2gpu_loop_detect_params;
+#define SE2GPU_LOOP_DETECT_GLOBAL_MAPPER {20, 0.005}  /* src/Config.cpp:80-81 */
+#define SE2GPU_LOOP_DETECT_LOCALIZER {0, 0.05}        /* src/Localizer.cpp:341; its current keyframe is not in the map */
+
+/* GlobalMapper::DetectLoopClose (src/GlobalMapper.cpp:201-254) and Localizer::DetectLoopClose (src/Localizer.cpp:337-392)
+ * for B query keyframes against N database keyframes, on DEVICE buffers, asynchronous on `stream`, on the current device.
+ * BowVectors in the layout se2gpu_voc_compute_bow_device writes: query b's words d_q_word + b*cap_q (ascending), values
+ * d_q_value + b*cap_q, d_q_n[b] of them; database keyframe n's at n*cap_db with d_db_n[n]. The database slots are
+ * Map::getAllKF()'s order (ascending mIdKF), so that among equal scores the first keyframe wins as in the reference.
+ *   d_scores [B*N]  score(q_b, db_n) at b*N + n = DBoW2's L1Scoring::score (Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-68)
+ *                   bit for bit: the terms fabs(vi - wi) - fabs(vi) - fabs(wi) of the common words added in ascending word
+ *                   order in double, then -score / 2.0 (an empty intersection gives -0.0). Every score is written,
+ *                   including those of excluded keyframes.
+ *   d_loop [B]      the selected database slot or -1; d_best [B] scoreBest.
+ * Selection as the reference: scoreBest starts at 0.0; a keyframe that |d_db_id[n] - d_q_id[b]| < min_id_offset does not
+ * exclude replaces the best only on score > scoreBest, so scores <= 0 never win and the first of equal scores does; a loop
+ * is detected when a best exists and scoreBest > min_score. d_q_id / d_db_id are read only when min_id_offset > 0.
+ * Two launches whatever B and N are; no allocation and no host synchronisation, so a CUDA graph may capture it. Checked
+ * on the host: B, N, cap_q, cap_db < 0, NULL params or a NULL required pointer is SE2GPU_ERR_INVALID; cap_q above the
+ * query's shared memory (12 bytes per word: 19 370 words on an H100) or N > 1 048 560 is SE2GPU_ERR_CAPACITY; a refused call writes
+ * nothing. B == 0 does nothing. Like every device entry, it trusts the contents of device memory: counts within [0, cap]
+ * (clamped) and ascending, unrepeated word ids. */
+int se2gpu_detect_loop_device(int B, const int* d_q_word, const double* d_q_value, const int* d_q_n, int cap_q, int N,
+                              const int* d_db_word, const double* d_db_value, const int* d_db_n, int cap_db, const int* d_q_id,
+                              const int* d_db_id, const se2gpu_loop_detect_params* params, double* d_scores, int* d_loop,
+                              double* d_best, void* stream);
+
+/* VerifyLoopClose's verdict. GlobalMapper (localizer = 0) accepts when nMP >= min_match_mp && nGood >= min_match_kp &&
+ * nMP * 1.0 / numMPsCurrent >= ratio_min_match_mp (GM_VCL_*, src/Config.cpp:76-78); the Localizer (localizer = 1) when
+ * nGood >= min_match_kp (numMinMatch = 45). */
+typedef struct se2gpu_loop_verify_params {
+    int localizer;
+    int min_match_mp;
+    int min_match_kp;
+    double ratio_min_match_mp;
+} se2gpu_loop_verify_params;
+#define SE2GPU_LOOP_VERIFY_GLOBAL_MAPPER {0, 15, 30, 0.05}
+#define SE2GPU_LOOP_VERIFY_LOCALIZER {1, 0, 45, 0.0}
+
+/* GlobalMapper::VerifyLoopClose (src/GlobalMapper.cpp:256-326) and Localizer::VerifyLoopClose (src/Localizer.cpp:394-431)
+ * for B pairs, on DEVICE buffers, asynchronous on `stream`: pair b is keyframe b of `cur` against keyframe d_loop[b] of
+ * `map` (d_loop as se2gpu_detect_loop_device writes it; -1 gives an empty pair, which is never verified).
+ *   1. d_raw + b*cur->cap   SearchByBoW(cur, loop, mapMatch, false) with ORBmatcher()'s nnratio 0.6 and orientation check
+ *                           (se2gpu_search_by_bow_batch_device on m, mp_only = 0), -1 = none.
+ *   2. d_good + b*cur->cap  RemoveMatchOutlierRansac (:1207-1248): fewer than 10 raw matches clear everything; otherwise
+ *                           cv::findFundamentalMat(FM_RANSAC, 3, 0.99) on keyPointsUn in ascending current-index order
+ *                           (LMedS below 15, as OpenCV), the matches its mask keeps (none when it finds no model).
+ *   3. d_mp + b*cur->cap    GlobalMapper only: RemoveKPMatch (:1251-1276) keeps a good match when
+ *                           cur->has_mp[i] && map->has_mp[match]; all -1 for the Localizer, which does not call it.
+ *                           In this entry has_mp is read as KeyFrame::hasObservation(idx) (mDualObservations), not
+ *                           SearchByBoW's "map point non-null": step 1 runs with mp_only = 0 and never reads it.
+ *   d_counts [B*3] (raw, good, MP) and d_verified [B] (1 = accepted, one byte per pair). d_n_mps_cur [B] is numMPsCurrent
+ *   (getAllObsMPs().size()); it is read, like has_mp, only for the GlobalMapper verdict.
+ * Launches: SearchByBoW's, one device-to-device copy, the outlier kernel and the verdict kernel, the same whatever B is; no
+ * allocation and no host synchronisation. Checked on the host before anything is written:
+ * B > the matcher's max_batch, cur->cap > max_queries or 8192 (the outlier kernel), map->cap > max_db is
+ * SE2GPU_ERR_CAPACITY; a NULL handle, side, params or required pointer, or negative sizes, is SE2GPU_ERR_INVALID. B == 0
+ * does nothing. Calls on one matcher are ordered like its other device entries. */
+int se2gpu_verify_loop_device(se2gpu_matcher* m, int B, const se2gpu_bow_batch_kf* cur, const se2gpu_bow_batch_kf* map,
+                              const int* d_loop, const int* d_n_mps_cur, const se2gpu_loop_verify_params* params, int* d_raw,
+                              int* d_good, int* d_mp, int* d_counts, uint8_t* d_verified, void* stream);
 
 /* ------------------------------------------------------------------------------------------ tracking */
 /* Track::mTrack (reference src/Track.cpp:124-160) for up to max_streams independent camera streams, with the tracking state

@@ -35,6 +35,16 @@ class BowBatchKF(C.Structure):
                 ("ptr", C.c_void_p), ("feat", C.c_void_p), ("n_node", C.c_void_p)]
 
 
+class LoopDetectParams(C.Structure):
+    """se2gpu_loop_detect_params"""
+    _fields_ = [("min_id_offset", C.c_int), ("min_score", C.c_double)]
+
+
+class LoopVerifyParams(C.Structure):
+    """se2gpu_loop_verify_params"""
+    _fields_ = [("localizer", C.c_int), ("min_match_mp", C.c_int), ("min_match_kp", C.c_int), ("ratio_min_match_mp", C.c_double)]
+
+
 class PoseBAParams(C.Structure):
     _fields_ = [("fx", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("Tbc", C.c_float * 16), ("huber_delta", C.c_float),
                 ("xrot_info", C.c_float), ("yrot_info", C.c_float), ("z_info", C.c_float), ("iterations", C.c_int)]
@@ -163,7 +173,7 @@ SYMBOLS = [
     "se2gpu_match_by_projection_device", "se2gpu_matcher_match_by_window", "se2gpu_matcher_match_by_projection",
     "se2gpu_matcher_search_by_bow", "se2gpu_matcher_profile", "se2gpu_matcher_profile_read", "se2gpu_matcher_last_rounds",
     "se2gpu_matcher_create_batch", "se2gpu_match_by_window_batch_device", "se2gpu_match_by_projection_batch_device",
-    "se2gpu_matcher_last_rounds_batch", "se2gpu_search_by_bow_batch_device",
+    "se2gpu_matcher_last_rounds_batch", "se2gpu_search_by_bow_batch_device", "se2gpu_detect_loop_device", "se2gpu_verify_loop_device",
     "se2gpu_ba_create", "se2gpu_ba_destroy", "se2gpu_ba_set_problem", "se2gpu_ba_optimize", "se2gpu_ba_get",
     "se2gpu_ba_set_shard", "se2gpu_ba_peer_export", "se2gpu_ba_peer_import", "se2gpu_ba_set_stream", "se2gpu_ba_debug_system", "se2gpu_ba_reset", "se2gpu_ba_profile",
     "se2gpu_ba_profile_read", "se2gpu_ba_set_mode", "se2gpu_ba_get_f32", "se2gpu_ba_build_information", "se2gpu_ba_optimize_from", "se2gpu_ba_peer_attach_local",
@@ -255,6 +265,9 @@ def lib():
     L.se2gpu_matcher_last_rounds.argtypes = [vp, C.POINTER(i), C.POINTER(i)]
     L.se2gpu_matcher_last_rounds_batch.argtypes = [vp, i, vp, vp]
     L.se2gpu_search_by_bow_batch_device.argtypes = [vp, i, C.POINTER(BowBatchKF), C.POINTER(BowBatchKF), vp, i, f, i, vp, vp, vp]
+    L.se2gpu_detect_loop_device.argtypes = [i, vp, vp, vp, i, i, vp, vp, vp, i, vp, vp, C.POINTER(LoopDetectParams), vp, vp, vp, vp]
+    L.se2gpu_verify_loop_device.argtypes = [vp, i, C.POINTER(BowBatchKF), C.POINTER(BowBatchKF), vp, vp, C.POINTER(LoopVerifyParams),
+                                            vp, vp, vp, vp, vp, vp]
     L.se2gpu_ba_create.restype = vp
     L.se2gpu_ba_create.argtypes = [i, i, i, i, i]
     L.se2gpu_ba_destroy.argtypes = [vp]

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libse2gpu.so")
-SOURCES = ["common.cu", "ba.cu", "ba_band.cu", "ba_loader.cu", "orb.cu", "matcher.cu", "bow.cu", "geom.cu", "fundam.cu", "pose_ba.cu", "feat_edge.cu", "global_ba.cu", "se3_ba.cu", "track.cu", "loc.cu"]
+SOURCES = ["common.cu", "ba.cu", "ba_band.cu", "ba_loader.cu", "orb.cu", "matcher.cu", "bow.cu", "geom.cu", "fundam.cu", "pose_ba.cu", "feat_edge.cu", "global_ba.cu", "se3_ba.cu", "track.cu", "loc.cu", "loop.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 (Hopper)
 NVCC_FLAGS = ["-O3", "-std=c++17", *GENCODE, "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-cudart", "static"]

@@ -398,6 +398,13 @@ int loc_local_ba(int B, const se2gpu_keypoint* d_kp, int cap_kf, const int* d_n,
 // answered before any matcher is made, so a refused handle allocates nothing for it).
 int orb_prepare_shape(se2gpu_orb* h, int w, int hgt, cudaStream_t s);
 int fundam_prepare();
+// GlobalMapper::RemoveMatchOutlierRansac (src/GlobalMapper.cpp:1207-1248) for `batch` keyframe pairs (fundam.cu): pair b's
+// current keypoints at d_kp1 + b * cap1, its loop keyframe's at d_kp2 + d_slot2[b] * cap2 (negative: an empty pair), the
+// matches d_matches12 + b * cap1 kept where cv::findFundamentalMat's mask is 1, all cleared when fewer than 10 are given.
+// cap1 <= kFundamMaxPairs, checked by the caller.
+constexpr int kFundamMaxPairs = 8192;
+int remove_outliers_loop(int batch, const se2gpu_keypoint* d_kp1, int cap1, const se2gpu_keypoint* d_kp2, int cap2,
+                         const int* d_slot2, int* d_matches12, cudaStream_t s);
 bool matcher_window_capturable(int device, int cap1, int cap2);
 
 }  // namespace se2gpu

@@ -27,7 +27,7 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kWave = 32;           // hypotheses drawn and scored per round
 constexpr int kModelPoints = 7;
-constexpr int kMaxPairs = 8192;     // keypoint capacity of frame 1 (shared memory: 20 bytes per pair)
+constexpr int kMaxPairs = kFundamMaxPairs;   // keypoint capacity of frame 1 (shared memory: 20 bytes per pair)
 constexpr int kNitersTable = 1000;  // RANSACUpdateNumIters never exceeds maxIters = 1000
 
 // c_niters[k - 1] = the least ep in [0, 1] with RANSACUpdateNumIters(0.99, ep, 7, 1000) >= k (glibc log / pow)
@@ -313,11 +313,20 @@ struct Wave {
     int score_i[kWave * 3];             // RANSAC inlier count of each model
 };
 
-// One CTA per frame pair. Dynamic shared memory: float2 p1[cap1], float2 p2[cap1], int idx[cap1].
-__global__ void __launch_bounds__(kThreads) k_remove_outliers(
+// What a call does with few matches. TRACK: Track::removeOutliers clears every match when fewer than 10 inliers remain after
+// the estimate. LOOP: GlobalMapper::RemoveMatchOutlierRansac (src/GlobalMapper.cpp:1207-1248) clears every match when
+// fewer than 10 are given and does not estimate; after an estimate it keeps the mask whatever its count.
+enum Gate { TRACK, LOOP };
+
+// One CTA per frame pair. Dynamic shared memory: float2 p1[cap1], float2 p2[cap1], int idx[cap1]. Pair b's frame-2
+// keypoints are slot2[b] of kp2_all / n2_all (slot2 NULL: b); a negative slot2[b] makes the pair's frame 2 empty.
+// ninliers may be NULL. The two gates are two kernels, k_remove_outliers (TRACK) and k_remove_outliers_loop (LOOP).
+template <Gate G>
+__device__ __forceinline__ void remove_outliers(
         const se2gpu_keypoint* __restrict__ kp1_all, const int* __restrict__ n1_all, int cap1,
-        const se2gpu_keypoint* __restrict__ kp2_all, const int* __restrict__ n2_all, int cap2, int* __restrict__ m12_all,
-        int* __restrict__ ninliers, double* __restrict__ F_out, int* __restrict__ iters_out, int lmeds_niters) {
+        const se2gpu_keypoint* __restrict__ kp2_all, const int* __restrict__ n2_all, int cap2, const int* __restrict__ slot2,
+        int* __restrict__ m12_all, int* __restrict__ ninliers, double* __restrict__ F_out, int* __restrict__ iters_out,
+        int lmeds_niters) {
     extern __shared__ __align__(16) unsigned char smem[];
     float2* p1 = reinterpret_cast<float2*>(smem);
     float2* p2 = p1 + cap1;
@@ -330,10 +339,11 @@ __global__ void __launch_bounds__(kThreads) k_remove_outliers(
     __shared__ uint64_t s_rng;
 
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int s2 = slot2 ? slot2[b] : b;
     const int n1 = n1_all ? min(max(n1_all[b], 0), cap1) : cap1;
-    const int n2 = n2_all ? min(max(n2_all[b], 0), cap2) : cap2;
+    const int n2 = s2 < 0 ? 0 : n2_all ? min(max(n2_all[s2], 0), cap2) : cap2;
     const se2gpu_keypoint* kp1 = kp1_all + (size_t)b * cap1;
-    const se2gpu_keypoint* kp2 = kp2_all + (size_t)b * cap2;
+    const se2gpu_keypoint* kp2 = kp2_all + (size_t)max(s2, 0) * cap2;
     int* m12 = m12_all + (size_t)b * cap1;
 
     // gather the matched pairs in ascending keypoint order (matches past n2 count as unmatched)
@@ -355,6 +365,16 @@ __global__ void __launch_bounds__(kThreads) k_remove_outliers(
         }
         n += tot;
         __syncthreads();
+    }
+
+    if (G == LOOP && n < 10) {
+        for (int i = tid; i < n1; i += kThreads) m12[i] = -1;
+        if (tid == 0) {
+            if (ninliers) ninliers[b] = 0;
+            if (iters_out) iters_out[b] = 0;
+        }
+        if (F_out && tid < 9) F_out[9 * (size_t)b + tid] = 0.;
+        return;
     }
 
     const bool lmeds = n < 15;
@@ -451,7 +471,7 @@ __global__ void __launch_bounds__(kThreads) k_remove_outliers(
         __syncthreads();
     }
 
-    // apply the mask (never written when no model was found: every pair is an outlier) and the < 10 rule
+    // apply the mask (never written when no model was found: every pair is an outlier) and Track's < 10 rule
     const bool have = s_have != 0;
     const float thr = __int_as_float(s_thresh_bits);
     int nin = 0;
@@ -465,16 +485,30 @@ __global__ void __launch_bounds__(kThreads) k_remove_outliers(
     // a false LMedS result (fewer than 7 inliers) returns an empty F; the mask stays written
     const bool f_out = n == kModelPoints || (have && !(lmeds && nin < kModelPoints));
     if (n == kModelPoints) nin = kModelPoints;
-    if (nin < 10) {
+    if (G == TRACK && nin < 10) {
         nin = 0;
         for (int i = tid; i < n1; i += kThreads) m12[i] = -1;
     }
     if (tid == 0) {
-        ninliers[b] = nin;
+        if (ninliers) ninliers[b] = nin;
         if (iters_out) iters_out[b] = s_iter;
     }
     if (F_out && tid < 9) F_out[9 * (size_t)b + tid] = f_out ? s_best[tid] : 0.;
 }
+
+#define SE2_REMOVE_OUTLIERS_PARAMS                                                                                            \
+    const se2gpu_keypoint* __restrict__ kp1_all, const int* __restrict__ n1_all, int cap1,                                    \
+    const se2gpu_keypoint* __restrict__ kp2_all, const int* __restrict__ n2_all, int cap2, const int* __restrict__ slot2,      \
+    int* __restrict__ m12_all, int* __restrict__ ninliers, double* __restrict__ F_out, int* __restrict__ iters_out, int lmeds_niters
+#define SE2_REMOVE_OUTLIERS_ARGS kp1_all, n1_all, cap1, kp2_all, n2_all, cap2, slot2, m12_all, ninliers, F_out, iters_out, lmeds_niters
+__global__ void __launch_bounds__(kThreads) k_remove_outliers(SE2_REMOVE_OUTLIERS_PARAMS) {
+    remove_outliers<TRACK>(SE2_REMOVE_OUTLIERS_ARGS);
+}
+__global__ void __launch_bounds__(kThreads) k_remove_outliers_loop(SE2_REMOVE_OUTLIERS_PARAMS) {
+    remove_outliers<LOOP>(SE2_REMOVE_OUTLIERS_ARGS);
+}
+#undef SE2_REMOVE_OUTLIERS_PARAMS
+#undef SE2_REMOVE_OUTLIERS_ARGS
 
 __global__ void k_debug_niters(int count, const int* n, const int* good, const int* max_iters, int* out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -528,13 +562,30 @@ int prepare_device() {
     if (dev < kMaxDevices && ready[dev]) return SE2GPU_OK;
     SE2_CUDA(cudaMemcpyToSymbol(c_niters, niters_table(), sizeof(double) * kNitersTable));
     SE2_CUDA(cudaFuncSetAttribute(k_remove_outliers, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * kMaxPairs));
+    SE2_CUDA(cudaFuncSetAttribute(k_remove_outliers_loop, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * kMaxPairs));
     if (dev < kMaxDevices) ready[dev] = true;
     return SE2GPU_OK;
+}
+
+// OpenCV's LMedS iteration count (RANSACUpdateNumIters(0.99, 0.45, 7, 1000), at least 3)
+int lmeds_niters() {
+    static const int v = [] { const int n = update_num_iters_host(0.99, 0.45, kModelPoints, 1000); return n < 3 ? 3 : n; }();
+    return v;
 }
 
 }  // namespace
 
 int se2gpu::fundam_prepare() { return prepare_device(); }
+
+int se2gpu::remove_outliers_loop(int batch, const se2gpu_keypoint* d_kp1, int cap1, const se2gpu_keypoint* d_kp2, int cap2,
+                                 const int* d_slot2, int* d_matches12, cudaStream_t s) {
+    if (batch == 0) return SE2GPU_OK;
+    { const int rc = prepare_device(); if (rc) return rc; }
+    SE2_LAUNCH(k_remove_outliers_loop, batch, kThreads, (size_t)20 * cap1, s, d_kp1, nullptr, cap1, d_kp2, nullptr, cap2, d_slot2,
+               d_matches12, nullptr, nullptr, nullptr, lmeds_niters());
+    SE2_CUDA(cudaGetLastError());
+    return SE2GPU_OK;
+}
 
 int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const int* d_n1, int cap1, const se2gpu_keypoint* d_kp2,
                                   const int* d_n2, int cap2, int* d_matches12, int* d_ninliers, double* d_F, int* d_iters,
@@ -546,10 +597,9 @@ int se2gpu_remove_outliers_device(int batch, const se2gpu_keypoint* d_kp1, const
     { const int rc = require_device(); if (rc) return rc; }
     if (batch == 0) return SE2GPU_OK;
     { const int rc = prepare_device(); if (rc) return rc; }
-    static const int lmeds_niters = [] { const int v = update_num_iters_host(0.99, 0.45, kModelPoints, 1000); return v < 3 ? 3 : v; }();
     SE2_NVTX("se2gpu_remove_outliers");
     SE2_LAUNCH(k_remove_outliers, batch, kThreads, (size_t)20 * cap1, (cudaStream_t)stream, d_kp1, d_n1, cap1, d_kp2, d_n2, cap2,
-               d_matches12, d_ninliers, d_F, d_iters, lmeds_niters);
+               nullptr, d_matches12, d_ninliers, d_F, d_iters, lmeds_niters());
     SE2_CUDA(cudaGetLastError());
     return SE2GPU_OK;
 }

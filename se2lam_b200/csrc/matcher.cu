@@ -24,7 +24,8 @@
 // points are B = 1): the grid and candidate kernels take the pair from blockIdx.y, k_resolve runs one CTA and k_fallback_*
 // one warp per pair, and every pair works in its own slice of the context's scratch. The launch count does not depend on B.
 // se2gpu_search_by_bow_batch_device puts k_bow_walk in front, one CTA per pair: the node walk of SearchByBoW (:160-247) over
-// the two device FeatureVectors, which writes the pair's queries for k_candidates_bow.
+// the two device FeatureVectors, which writes the pair's queries for k_candidates_bow. A negative d_slot2[b] makes pair b empty:
+// k_bow_walk gives it no queries, so no later kernel reads its side 2, and the side-2 offsets are formed from slot 0.
 #include <climits>
 #include <cstring>
 #include <mutex>
@@ -245,8 +246,10 @@ struct BowCandArgs {
     int mp_only;
     int cap; int2* cand; int* ncand; int scr_q;
 };
+// side-2 keyframe of pair b; a negative slot (an empty pair) is mapped to 0, whose arrays its kernels then never read
+__device__ __forceinline__ int side2_slot(const int* slot2, int b) { return slot2 ? max(slot2[b], 0) : b; }
 __device__ __forceinline__ void pair_slice(BowCandArgs& a, int b) {
-    const size_t s2 = (size_t)(a.slot2 ? a.slot2[b] : b) * a.cap2, q = (size_t)b * a.qstride;
+    const size_t s2 = (size_t)side2_slot(a.slot2, b) * a.cap2, q = (size_t)b * a.qstride;
     if (a.d_nq) a.d_nq += b;
     a.qidx += q; a.qb0 += q; a.qb1 += q;
     a.d1 += 8 * (size_t)b * a.cap1; if (a.mp1) a.mp1 += (size_t)b * a.cap1;
@@ -288,11 +291,12 @@ struct BowWalkArgs {
 };
 __global__ void __launch_bounds__(256) k_bow_walk(BowWalkArgs a) {
     __shared__ int s_warp[32];
-    const int b = blockIdx.x, s2 = a.slot2 ? a.slot2[b] : b;
+    const int b = blockIdx.x, s2 = side2_slot(a.slot2, b);
+    const bool empty = a.slot2 && a.slot2[b] < 0;
     const int* node1 = a.node1 + (size_t)b * a.cap1; const int* ptr1 = a.ptr1 + (size_t)b * (a.cap1 + 1);
     const int* feat1 = a.feat1 + (size_t)b * a.cap1;
     const int* node2 = a.node2 + (size_t)s2 * a.cap2; const int* ptr2 = a.ptr2 + (size_t)s2 * (a.cap2 + 1);
-    const int n1 = min(max(a.n_node1[b], 0), a.cap1), n2 = min(max(a.n_node2[s2], 0), a.cap2);
+    const int n1 = min(max(a.n_node1[b], 0), a.cap1), n2 = empty ? 0 : min(max(a.n_node2[s2], 0), a.cap2);
     const size_t qo = (size_t)b * a.qstride;
     int *qidx = a.qidx + qo, *qb0 = a.qb0 + qo, *qb1 = a.qb1 + qo;
     int base = 0;
@@ -360,7 +364,7 @@ struct ResolveArgs {
 // is KF1's feature capacity), outputs by n_out, the context scratch by its capacities; work is the fallback's
 // [2 * cap + scr_q] per pair
 __device__ __forceinline__ void pair_slice(ResolveArgs& a, int b) {
-    const size_t q = (size_t)b * a.nq_cap, d = (size_t)(a.slot2 ? a.slot2[b] : b) * a.n2_cap;
+    const size_t q = (size_t)b * a.nq_cap, d = (size_t)side2_slot(a.slot2, b) * a.n2_cap;
     if (a.qid) a.qid += (size_t)b * a.qstride;
     if (a.d_nq) a.d_nq += b;
     if (a.d_n2) a.d_n2 += b;
