@@ -176,10 +176,10 @@ def verify_cases():
     return pairs
 
 
-def run_verify(mt, pairs, loop, params, n_mps):
+def run_verify(mt, pairs, loop, params, n_mps, cap1=None, cap2=None):
     import torch
     B = len(pairs)
-    cap1 = max(len(p[0]["angle"]) for p in pairs); cap2 = max(len(p[1]["angle"]) for p in pairs)
+    cap1 = cap1 or max(len(p[0]["angle"]) for p in pairs); cap2 = cap2 or max(len(p[1]["angle"]) for p in pairs)
     s1 = verify_side([p[0] for p in pairs], cap1, 1)
     map_kfs = [pairs[j][1] for j in range(B)]
     s2 = verify_side(map_kfs, cap2, 2)
